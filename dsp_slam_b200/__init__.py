@@ -1,4 +1,4 @@
-"""dsp_slam_b200: DSP-SLAM's per-object shape-prior Gauss-Newton reconstruction, B200-native.
+"""dsp_slam_b200: DSP-SLAM's per-object shape-prior Gauss-Newton reconstruction, H100-native.
 
 Public surface (mirrors reconstruct/optimizer.py of the reference):
     from dsp_slam_b200.optimizer import Optimizer, MeshExtractor

@@ -1,6 +1,6 @@
 """ctypes binding of libdspgn.so (C ABI declared in include/dspgn.h).
 
-The product path has no CPU fallback: if the CUDA library is missing or no sm_100 GPU is present,
+The product path has no CPU fallback: if the CUDA library is missing or no sm_90 GPU is present,
 loading / creating handles raises.  Nothing here imports oracle/.
 """
 import ctypes as C
@@ -123,7 +123,7 @@ def load():
     if not os.path.isfile(LIB_PATH):
         raise DspgnError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, res, args in SYMBOLS:
         fn = getattr(lib, name)          # AttributeError if the export is missing

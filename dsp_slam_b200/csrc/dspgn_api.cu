@@ -199,7 +199,7 @@ int dspgn_decoder_create_ex(const DspgnDecoderSpec* spec, const float* const* W,
   CU(cudaSetDevice(device));
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_100a (B200) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
   DspgnDecoder* d = new (std::nothrow) DspgnDecoder();
   if (!d) return fail(DSPGN_E_ALLOC, "oom");
   d->device = device;
@@ -249,7 +249,7 @@ int dspgn_decoder_create_ex(const DspgnDecoderSpec* spec, const float* const* W,
       d->has_ln = true;
     }
   }
-  if (!rc && !generic) rc = tc_pack_decoder(*spec, W, b, d->tc, &dv, g_err);     // the tcgen05 engine covers the plain shape
+  if (!rc && !generic) rc = tc_pack_decoder(*spec, W, b, d->tc, &dv, g_err);     // the tensor-core engine covers the plain shape
   if (rc) { dspgn_decoder_destroy(d); return rc; }
   *out = d;
   return 0;
@@ -1142,7 +1142,7 @@ int dspgn_tc_selftest(int device, int n_mma, int k_steps, const float* A, const 
   if (dA.reserve(4 * (size_t)128 * K) || dB.reserve(blob.size()) || dD.reserve(4 * (size_t)128 * n_mma)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
   CU(cudaMemcpy(dA.p, A, 4 * (size_t)128 * K, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(dB.p, blob.data(), blob.size(), cudaMemcpyHostToDevice));
-  k_tc_selftest<<<1, 128, 2 * kTcStageBytes + 1024>>>(dA.as<float>(), K, dB.as<unsigned char>(), n_mma, k_steps, dD.as<float>());
+  k_tc_selftest<<<1, kTcThreads, kTcSelftestSmem>>>(dA.as<float>(), K, dB.as<unsigned char>(), n_mma, k_steps, dD.as<float>());
   cudaError_t e = cudaDeviceSynchronize();
   if (e == cudaSuccess) e = cudaMemcpy(D, dD.p, 4 * (size_t)128 * n_mma, cudaMemcpyDeviceToHost);
   dA.release(); dB.release(); dD.release();

@@ -1,4 +1,4 @@
-// Shared device-side structures and small closed forms for libdspgn (sm_100a).
+// Shared device-side structures and small closed forms for libdspgn (sm_90a).
 // Reference arithmetic being restated is cited per function (paths relative to the DSP-SLAM repo).
 #pragma once
 #include <cuda_runtime.h>
@@ -13,8 +13,8 @@ constexpr int kPInt = 72;                      // internal Jacobian row stride: 
 constexpr int kAccStride = kPInt * kPInt + kPInt + 8;  // floats per tile partial: H (upper) | b | {loss_sum, rows, ...}
 constexpr int kAccB = kPInt * kPInt;
 // H partials are stored as the PACKED upper triangle of the internal 72x72 matrix, row-major: entry (r, c), r <= c, at
-// tri_index(r, c) in [0, kTriInt).  The solve reads entry  tid + q*256  -> perfectly coalesced (the former r*72+c
-// addressing cost one 32-byte sector per lane: 2.7 us per tile, 43 us of a 76 us solve on 16 tiles).
+// tri_index(r, c) in [0, kTriInt).  The solve reads entry  tid + q*256  -> perfectly coalesced (r*72+c
+// addressing would cost one 32-byte sector per lane).
 constexpr int kTriInt = kPInt * (kPInt + 1) / 2;
 __host__ __device__ __forceinline__ int tri_index(int r, int c) { return r * kPInt - (r * (r - 1)) / 2 + (c - r); }
 constexpr int kAccLoss = kAccB + kPInt;        // +0 loss sum, +1 row count
@@ -49,14 +49,14 @@ struct ObjState {
   float zb0[256];
 };
 
-// ---- tcgen05 engine plan (dspgn_tc.cuh): one entry per GEMM step of a tile -----------------------
+// ---- tensor-core engine plan (dspgn_tc.cuh): one entry per GEMM step of a tile -----------------------
 constexpr int kTcMaxSteps = 18;
 enum { TK_FWD_HIDDEN = 0, TK_FWD_PENULT = 1, TK_BWD_MID = 2, TK_BWD_FIRST = 3 };   // PENULT: last hidden layer + the final Linear(.,1) on the CUDA cores
 struct TcStep {
   int kind;
-  int n_mma;         // UMMA N (multiple of 16, <= 256)
+  int n_mma;         // real output width rounded up to 16 (<= 256; the wgmma itself always runs N = 256)
   int k_steps;       // K=16 steps of the reduction
-  int a_reg, d_reg;  // TMEM region (0/1 -> column 0/256) of the A operand and of the accumulator
+  int a_reg, d_reg;  // operand / accumulator ping-pong slot of the step (plan bookkeeping)
   unsigned w_off;    // byte offset of this step's first weight image in the blob
   int layer;         // decoder layer (bias / ReLU-mask slot)
   int n_real;        // real output columns (the rest is zero padding)

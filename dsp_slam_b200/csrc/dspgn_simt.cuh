@@ -1,6 +1,6 @@
 // fp32 SIMT decoder engine: fused  transform -> DeepSDF forward -> backward-to-input -> Jacobian rows
 // -> per-tile partial sums of J^T J / J^T r  for one 64-row tile per CTA iteration.  This engine is the on-device ground truth
-// (plain FFMA, fp32 accumulation in k order) against which the tcgen05 engine is checked.
+// (plain FFMA, fp32 accumulation in k order) against which the tensor-core engine is checked.
 //
 // Restates: loss.py:22-43 (SDF term), loss.py:143-150 (band rows of the render term),
 // loss_utils.py:51-103 (decode / input Jacobian), deep_sdf_decoder.py:75-110, optimizer.py:161-167.
@@ -27,7 +27,7 @@ struct DecoderDev {
   const float* ln_gamma[DSPGN_MAX_LINEAR]; // LayerNorm after layer k (nullptr = none), [256] zero padded
   const float* ln_beta[DSPGN_MAX_LINEAR];
   int use_tanh, generic;                   // generic = any variant in use
-  // tcgen05 engine images (dspgn_tc.cuh): pre-swizzled fp16 hi/lo weight chunks + step plan
+  // tensor-core engine images (dspgn_tc.cuh): pre-swizzled fp16 hi/lo weight chunks + step plan
   const unsigned char* tc_blob;
   TcPlan tc_plan;
 };

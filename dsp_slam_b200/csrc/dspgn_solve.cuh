@@ -164,8 +164,8 @@ __global__ void k_build_inputs(BuildArgs a) {
 // (|u d + t| < 1 with u = R_oc q) brackets the hull to within a fraction of a sample, the search window is that bracket
 // +- 2 samples, found ends are extended outwards while the neighbour is valid, and a ray with an empty window is scanned
 // completely unless its line misses the ball by more than 1 % of the radius -- so the result is the hull of the exhaustive
-// test (`exact` = 1, env DSPGN_VPRE_EXACT: no bracket, the whole sample range is searched from both ends; testing all D
-// samples of every ray cost 12 us per solve on 450 rays).
+// test (`exact` = 1, env DSPGN_VPRE_EXACT: no bracket, the whole sample range is searched from both ends, which tests all D
+// samples of every ray).
 // Called by all `nthreads` (multiple of 32, <= 1024) threads; s_wsum: 32 ints of shared memory.  Returns the total.
 __device__ __forceinline__ int vpre_base(const ObjMeta& M, int o) { return M.ray_off + o; }
 template <bool NAMED_BAR>
@@ -267,7 +267,6 @@ struct InitArgs {
 };
 
 // zb0 = b0 + W0[:, :L] z   (fp32 FMA chain in i order; all threads of the calling CTA / epilogue)
-// (a variant with the code staged in shared memory and __ldg weight reads measured SLOWER: +9 us per solve, +12 us k_init)
 __device__ __forceinline__ void refresh_zb0(ObjState& st, const DecoderDev& dec, int tid, int nthreads) {
   const float* __restrict__ W = dec.Wf[0];      // reduction-major [in][256]
   const float* __restrict__ b = dec.bias[0];
@@ -420,7 +419,7 @@ __device__ __forceinline__ void gj_pivots(const int k0, const int k1, const int 
     const float pb = buf[(kPMax + 1) / 4].x;
     const float piv = pr[0];
     if (!(piv > 0.f) || !(piv < 3.0e38f)) bad_pivot = 1;        // every thread sees the same pivot
-    const float l = (tid == k) ? 0.f : __fdividef(arow[0], piv);        // MUFU.RCP path: 47 vs 112 cycles per pivot for __frcp_rn (tools/probes/solve_probe.cu)
+    const float l = (tid == k) ? 0.f : __fdividef(arow[0], piv);        // MUFU.RCP path, shorter than __frcp_rn (tools/probes/solve_probe.cu)
 #pragma unroll
     for (int j = 1; j < NE; ++j) arow[j - 1] = fmaf(-l, pr[j], arow[j]);
     brow = fmaf(-l, pb, brow);

@@ -1,26 +1,26 @@
-// tcgen05 tensor-core decoder engine for B200 (sm_100a).
+// wgmma tensor-core decoder engine for H100 (sm_90a).
 //
 // One persistent CTA per SM walks 128-row tiles.  For each tile the whole DeepSDF forward chain, the
 // backward-to-input chain and the Jacobian / J^T J reduction run without leaving the SM:
 //
-//   * accumulators AND the next layer's A operand live in TMEM (two 256-column regions, ping-pong):
-//     the epilogue warps read a finished accumulator (tcgen05.ld), apply bias/ReLU (forward) or the saved
-//     ReLU mask (backward), split every fp32 value into fp16 hi + fp16 lo and write the packed pairs back
-//     IN PLACE (tcgen05.st); the next GEMM consumes them as a TMEM A operand (tcgen05.mma, A from TMEM);
-//   * weights are pre-split (hi/lo fp16), pre-swizzled (128B swizzle, K-major) on the host into exactly
-//     the shared-memory image the UMMA descriptor expects, and streamed from L2 through a 4 x 32 KB ring
-//     with 1-D bulk copies (cp.async.bulk -> UBLKCP) signalling mbarriers;
+//   * two consumer warpgroups own 64 tile rows each; their accumulators (64 x 256 fp32) live in registers.  The
+//     epilogue works on the accumulator fragment in place: bias/ReLU (forward) or the saved ReLU mask (backward), then
+//     every fp32 value is split into fp16 hi + fp16 lo.  The wgmma accumulator fragment of columns [16t, 16t+16) is
+//     exactly the register A fragment of K-step t, so the hi halves stay in registers as the next GEMM's A operand and
+//     the lo halves go to a 128B-swizzled shared-memory image (A from a descriptor);
+//   * weights are pre-split (hi/lo fp16), pre-swizzled (128B swizzle, K-major, padded to 256 rows) on the host into
+//     exactly the shared-memory image the wgmma descriptor expects, and streamed from L2 through a 2 x 32 KB ring with
+//     1-D bulk copies (cp.async.bulk) signalling mbarriers;
 //   * every product is formed as  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo  (3 fp16 MMAs, fp32 accumulate):
 //     ~2^-21 relative error per product, which keeps the Gauss-Newton iteration inside the fp32 noise
 //     floor of the reference (SURVEY.md B.3: >= 15 mantissa bits needed; bf16/tf32 single pass is not);
 //   * only the hidden width x width layers are GEMM steps (14 per fwd+bwd tile of the 8 x 256 decoder): layer 0, with
 //     its latent part folded into a per-object bias, is 3 FMAs per output while the first operand is built, and the
 //     final Linear(width, 1) + tanh is a per-row dot product in the epilogue of the last hidden layer;
-//   * J^T J / J^T r of the tile on the CUDA cores with packed fp32 FMAs (FFMA2), written as per-tile partials.
+//   * J^T J / J^T r of the tile on the CUDA cores, written as per-tile partials.
 //
-// Warp roles (320 threads): warps 0-3 / 4-7 = epilogue groups (thread = tile row; group g owns accumulator
-// columns [128g, 128g+128)), warp 8 = MMA issuer (one elected lane), warp 9 = weight producer and, in the persistent
-// kernels, the CTA's scheduler (pops the device work queue).
+// Warp roles (288 threads): warps 0-3 / 4-7 = consumer warpgroups (MMA issue + epilogue, rows [64g, 64g+64)), warp 8 =
+// weight producer and, in the persistent kernels, the CTA's scheduler (pops the device work queue).
 //
 // Three schedules share this body (template SCHED): 0 = one launch per term and iteration (k_decoder_tc), 1 = persistent
 // kernel with SDF tiles only (k_gn_persistent), 2 = persistent kernel with the render term: ray-sample tiles (only the run
@@ -40,10 +40,12 @@
 namespace dspgn {
 
 constexpr int kTcRows = 128;
-constexpr int kTcThreads = 320;
+constexpr int kTcThreads = 288;
 constexpr int kTcEpiThreads = 256;
-constexpr int kTcStages = 4;
-constexpr int kTcStageBytes = 32768;
+constexpr int kTcStages = 2;
+constexpr int kTcStageBytes = 32768;      // one weight image: 256 rows x 64 K x fp16
+constexpr int kTcN = 256;                 // wgmma N of every GEMM step (weight images are zero padded to 256 rows)
+constexpr int kTcAloBytes = 32768;        // lo halves of one warpgroup's A operand: 4 x (64 rows x 128 B)
 
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -77,81 +79,38 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// generic-proxy shared-memory writes (the A lo image) before the async proxy (wgmma) reads them
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// the 128 threads of consumer warpgroup g (ids 1 / 2 are taken by the epilogue and the solve step)
+__device__ __forceinline__ void wg_bar_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(3 + g) : "memory"); }
 
-__device__ __forceinline__ void tc_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T, kind::f16 (fp16 inputs, fp32 accumulate)
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// whole-warp variants: called converged by all 32 lanes, one elected lane issues.  Keeping the control flow
-// warp-uniform lets the compiler hold descriptors in uniform registers instead of R2UR moves per operand.
-__device__ __forceinline__ void tc_mma_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t"
-      "}" ::"r"(smem_u32(bar)) : "memory");
-}
-#define DSPGN_R8(v, o) "=r"(v[o + 0]), "=r"(v[o + 1]), "=r"(v[o + 2]), "=r"(v[o + 3]), "=r"(v[o + 4]), "=r"(v[o + 5]), "=r"(v[o + 6]), "=r"(v[o + 7])
-#define DSPGN_W8(v, o) "r"(v[o + 0]), "r"(v[o + 1]), "r"(v[o + 2]), "r"(v[o + 3]), "r"(v[o + 4]), "r"(v[o + 5]), "r"(v[o + 6]), "r"(v[o + 7])
+#define DSPGN_D8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+#define DSPGN_D128                                                                                                    \
+  DSPGN_D8(0), DSPGN_D8(8), DSPGN_D8(16), DSPGN_D8(24), DSPGN_D8(32), DSPGN_D8(40), DSPGN_D8(48), DSPGN_D8(56),         \
+      DSPGN_D8(64), DSPGN_D8(72), DSPGN_D8(80), DSPGN_D8(88), DSPGN_D8(96), DSPGN_D8(104), DSPGN_D8(112), DSPGN_D8(120)
+#define DSPGN_ACC_OPS "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
 
-// 32 consecutive columns of this thread's TMEM lane (warp w%4 owns lanes 32(w%4)..+31)
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+// D[64 x 256] += A[64 x 16] * B[256 x 16]^T, kind f16 (fp32 accumulate); A from registers (fragment of K-step t)
+__device__ __forceinline__ void wgmma_rs(float (&d)[128], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : DSPGN_R8(v, 0), DSPGN_R8(v, 8), DSPGN_R8(v, 16), DSPGN_R8(v, 24)
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " DSPGN_ACC_OPS
+      "{%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
+      : DSPGN_D128
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(1)
       : "memory");
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+// same with A from a shared-memory descriptor
+__device__ __forceinline__ void wgmma_ss(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : DSPGN_R8(v, 0), DSPGN_R8(v, 8)
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t tc_ld1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
-}
-__device__ __forceinline__ void tc_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      DSPGN_W8(v, 0), DSPGN_W8(v, 8), DSPGN_W8(v, 16), DSPGN_W8(v, 24)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " DSPGN_ACC_OPS
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : DSPGN_D128
+      : "l"(a_desc), "l"(b_desc), "r"(1)
       : "memory");
 }
 
@@ -165,21 +124,16 @@ constexpr int kClkSlots = 8, kClkTiles = 4;
 
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// K-major, 128B-swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm100):
-// start>>4 [0,14) | LBO>>4 [16,30) = 1 | SBO>>4 [32,46) = 64 (8 rows x 128 B) | version [46,48) = 1 |
-// layout [61,64) = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
+// K-major, 128B-swizzled shared-memory matrix descriptor (sm90 GMMA descriptor):
+// start>>4 [0,14) | LBO>>4 [16,30) = 1 (unused for swizzled K-major) | SBO>>4 [32,46) = 64 (8 rows x 128 B) |
+// base offset [49,52) = 0 (1024 B aligned atoms) | layout [62,64) = 1 (SWIZZLE_128B)
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)64 << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=f16, K-major both, M=128
-__host__ __device__ __forceinline__ uint32_t make_idesc(int n_mma) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(n_mma >> 3) << 17) | ((128u >> 4) << 24);
 }
 
 // fp32 -> (fp16 hi, fp16 lo) for two consecutive K elements, packed low half = even element
@@ -197,19 +151,17 @@ __device__ __forceinline__ void split_pack(float a, float b, uint32_t& hi, uint3
 constexpr int kJpStride = 76;             // floats per row of the point-major Jacobian tile (72 + pad, 16B aligned)
 struct TcSmemTail {
   float Jp[kTcRows * kJpStride];          // [row][72+4]: J row of each point; cols 0..66 double as latent_in skip gradient
-  uint32_t maskw[8 * 8 * kTcRows];        // ReLU masks [layer][32-col word][row]
+  uint32_t maskw[8 * 4 * kTcEpiThreads];  // ReLU masks [layer][word][consumer thread]: bit e of word w = fragment element 32w+e
   float bias[9 * kHid];
   float wlast[kHid];
   float w0x[3 * kHid];                    // xyz rows of the layer-0 matrix (the latent rows are folded into ObjState.zb0)
   float zs[kMaxCode + 16];                // latent code of the tile's object (zero padded)
   float xr[3 * kTcRows];                  // object-frame point of every row
   float rr[kTcRows], rsc[kTcRows];
+  float yrow[kTcRows], scr[kTcRows];      // decoder output and row weight (0 = inactive row) of every row
   int prefix[kMaxObjScan + 1];
   int warp_tmp[32];
   uint64_t w_full[kTcStages], w_empty[kTcStages];
-  uint64_t acc_full[4];                   // accumulator quarter q (64 columns) of the current step is complete
-  uint64_t a_ready[8];                    // 32-column unit u of the next A operand has been written
-  uint32_t tmem_base;
   int cur_class;
   int fifo[4]; int fifo_pub; int epi_seq; int last_flag;   // persistent mode: CTA-local tile FIFO (scheduler = producer warp)
   TcPlan plans[DSPGN_MAX_CLASSES];        // step plans of every decoder class (read by all warp roles)
@@ -220,37 +172,82 @@ struct TcSmemTail {
   int push_base, push_nF, push_nS;        // cooperative publication of an object's next-iteration tiles
   float ost[16]; int ost_rows;            // the tile's object: T_oc[12], dmin, dmax, dstep, dfar; rows of its term (counter)
 };
-constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcStages * kTcStageBytes + sizeof(TcSmemTail);
+constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail);
+static_assert(kTcSmemBytes <= 227 * 1024, "tensor-core engine shared memory exceeds the 227 KB per block of sm_90");
 
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      DSPGN_W8(v, 0), DSPGN_W8(v, 8)
-      : "memory");
-}
+// ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
+// 8-column block j = e >> 2 at row 16w + l/4 (+8 when e & 2), column 8j + 2(l%4) + (e & 1).
+__device__ __forceinline__ int frag_col(int e, int q) { return 8 * (e >> 2) + 2 * q + (e & 1); }
 
-// A-operand layout inside a 256-column TMEM region: 32-column units, unit u holds K elements [32u, 32u+32):
-// fp16 "hi" halves packed in columns [32u, 32u+16), "lo" halves in [32u+16, 32u+32).
-// K-step t (16 elements) -> hi at column 32*(t>>1) + 8*(t&1), lo 16 columns further.
-__device__ __forceinline__ uint32_t a_col_hi(int t) { return (uint32_t)(32 * (t >> 1) + 8 * (t & 1)); }
-
-__device__ __forceinline__ void store_a_unit(uint32_t taddr, const float (&t)[32]) {
-  uint32_t hi[16], lo[16];
+// accumulator-shaped values -> A operand of the next GEMM step: hi halves into `ah` (the register A fragment of
+// K-step t is columns [16t, 16t+16) of the accumulator fragment), lo halves into this warpgroup's swizzled image.
+// Ends with the proxy fence and the warpgroup barrier the wgmma reads need.
+__device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&ah)[64], unsigned char* alo, int rl, int q, int grp) {
 #pragma unroll
-  for (int p = 0; p < 16; ++p) split_pack(t[2 * p], t[2 * p + 1], hi[p], lo[p]);
-  tc_st16(taddr, hi);
-  tc_st16(taddr + 16, lo);
+  for (int t = 0; t < 16; ++t) {
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {       // h: (rows rl / rl+8) x (columns 16t+2q / 16t+8+2q)
+      uint32_t hi, lo;
+      split_pack(v[8 * t + 2 * h], v[8 * t + 2 * h + 1], hi, lo);
+      ah[4 * t + h] = hi;
+      const int row = rl + 8 * (h & 1), kk = 16 * t + 8 * (h >> 1) + 2 * q;
+      const int off = (kk >> 6) * 8192 + row * 128 + ((((kk & 63) >> 3) ^ (row & 7)) << 4) + (kk & 7) * 2;
+      *reinterpret_cast<uint32_t*>(alo + off) = lo;
+    }
+  }
+  fence_proxy_async();
+  wg_bar_sync(grp);
 }
 
-// signal "unit u of the next A operand is in TMEM" (or simply "done with this unit")
-// (one arrival per warp: 4 per unit instead of 128 -- the 128 individual arrivals on one mbarrier serialised for
-//  several hundred cycles on the path that decides when the next layer's first MMA can issue)
-__device__ __forceinline__ void unit_done(uint64_t* bar) {
-  tc_wait_st();
-  tc_fence_before();
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+// One GEMM step of a consumer warpgroup: acc = A * W^T over k_steps K-steps, W streamed through the ring (per K chunk of
+// 64: the hi image, then the lo image).  Every consumer warp releases a stage after its MMAs have completed.
+__device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[64], uint32_t alo, unsigned char* ring,
+                                        uint64_t* w_full, uint64_t* w_empty, uint32_t& stage, uint32_t& phase, int k_steps) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  wg_fence();
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    if (4 * c < k_steps) {
+      const uint32_t s_hi = stage;
+      mbar_wait(&w_full[stage], phase);
+      const uint32_t bh = smem_u32(ring + (size_t)stage * kTcStageBytes);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int t = 4 * c + k;
+        if (t < k_steps) {
+          const uint64_t bd = make_desc(bh + 32u * k);
+          wgmma_rs(acc, ah[4 * t], ah[4 * t + 1], ah[4 * t + 2], ah[4 * t + 3], bd);
+          wgmma_ss(acc, make_desc(alo + 8192u * c + 32u * k), bd);
+        }
+      }
+      if (++stage == kTcStages) { stage = 0; phase ^= 1; }
+      mbar_wait(&w_full[stage], phase);
+      const uint32_t bl = smem_u32(ring + (size_t)stage * kTcStageBytes);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int t = 4 * c + k;
+        if (t < k_steps) wgmma_rs(acc, ah[4 * t], ah[4 * t + 1], ah[4 * t + 2], ah[4 * t + 3], make_desc(bl + 32u * k));
+      }
+      wg_commit();
+      wg_wait0();
+      __syncwarp();
+      if ((threadIdx.x & 31) == 0) { mbar_arrive(&w_empty[s_hi]); mbar_arrive(&w_empty[stage]); }
+      if (++stage == kTcStages) { stage = 0; phase ^= 1; }
+    }
+  }
+}
+
+// producer side of the ring: the weight images of one GEMM step
+__device__ __forceinline__ void produce_step(const unsigned char* src, int k_steps, unsigned char* ring, uint64_t* w_full,
+                                             uint64_t* w_empty, uint32_t& stage, uint32_t& phase) {
+  const int nch = (k_steps + 3) >> 2;
+  for (int c = 0; c < 2 * nch; ++c) {           // hi image, lo image, hi, lo, ...
+    mbar_wait(&w_empty[stage], phase ^ 1);
+    mbar_expect_tx(&w_full[stage], (uint32_t)kTcStageBytes);
+    bulk_g2s(ring + (size_t)stage * kTcStageBytes, src + (size_t)c * kTcStageBytes, (uint32_t)kTcStageBytes, &w_full[stage]);
+    if (++stage == kTcStages) { stage = 0; phase ^= 1; }
+  }
 }
 
 struct TileRef { int o, row0, slot, mode, tile; };
@@ -348,7 +345,7 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
     if (M.n_rays > 0) vh = valid_sample_ranges<true>(M, sv.state[o], S.ctx_rays, S.ctx_D, q.vpre + vpre_base(M, o), tid, kTcEpiThreads, S.warp_tmp, q.vpre_exact != 0);
   }
   // ---- publish: finished, or the tiles of the next iteration.  All 256 threads write the queue slots (one thread
-  // pushing 176 ray tiles + their flags one by one took ~3 us on the single-object critical path).
+  // pushing every ray tile and its flag one by one is on the single-object critical path).
   if (tid == 0) {
     mega_event(q, EV_SOLVE_END, 0, o, it);
     int base = -1;
@@ -385,7 +382,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
   constexpr bool RENDER = SCHED == 2;
   extern __shared__ unsigned char tc_smem_raw[];
   unsigned char* ring = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);   // stays a shared-space pointer
-  TcSmemTail& S = *reinterpret_cast<TcSmemTail*>(ring + (size_t)kTcStages * kTcStageBytes);
+  TcSmemTail& S = *reinterpret_cast<TcSmemTail*>(ring + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   const int total_tiles = MEGA ? 0 : build_tile_prefix(a, kTcRows, S.prefix, S.warp_tmp);
@@ -397,21 +394,15 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
     }
   }
   if (tid == 0) {
-    for (int i = 0; i < kTcStages; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 1); }
-    mbar_init(&S.acc_full[0], 1);
-    for (int i = 0; i < 8; ++i) mbar_init(&S.a_ready[i], 4);
+    for (int i = 0; i < kTcStages; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
     S.cur_class = -1;
     S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
     if (MEGA) { S.ctx_q = q; S.ctx_sv = sv; S.ctx_D = a.D; S.ctx_rays = a.rays; }
     fence_barrier_init();
   }
-  if (warp == 8) tc_alloc(&S.tmem_base, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = S.tmem_base;
 
-  if (warp == 9) {
+  if (warp == 8) {
     // ===================== weight producer ======================================================
     if (lane == 0) {
       uint32_t stage = 0, phase = 0;
@@ -434,95 +425,23 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         const unsigned char* blob = a.decs[cls].tc_blob;
         const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD);
         const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
-        for (int s = 0; s < ns; ++s) {
-          const TcStep st = plan.step[s];
-          const uint32_t img = (uint32_t)st.n_mma * 128u;
-          const int nch = (st.k_steps + 3) >> 2;
-          const unsigned char* src = blob + st.w_off;
-          for (int c = 0; c < 2 * nch; ++c) {           // hi image, lo image, hi, lo, ...
-            mbar_wait(&S.w_empty[stage], phase ^ 1);
-            mbar_expect_tx(&S.w_full[stage], img);
-            bulk_g2s(ring + (size_t)stage * kTcStageBytes, src + (size_t)c * img, img, &S.w_full[stage]);
-            if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 8) {
-    // ===================== MMA issuer ===========================================================
-    // Full-width MMAs (N = the layer's padded output width): with the A operand in TMEM an MMA costs >= ~110
-    // cycles whatever its N (measured), so N is never split.  Overlap with the epilogue comes from the
-    // per-unit a_ready barriers: K chunk c of a step only needs operand units 2c and 2c+1.
-    uint32_t stage = 0, phase = 0, ar_phase = 0;
-    int clk_tile = -1;
-    for (int seq = 0;; ++seq) {
-      ++clk_tile;
-      TileRef tr;
-      if (!tile_at<SCHED>(a, S, seq, total_tiles, tr)) break;
-      const int o = tr.o;
-      const TcPlan& plan = S.plans[a.meta[o].class_id];
-      const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD);
-      const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
-      for (int s = 0; s < ns; ++s) {
-        const TcStep st = plan.step[s];
-        const uint32_t d_t = tmem + (uint32_t)st.d_reg * 256u;
-        const uint32_t a_t = tmem + (uint32_t)st.a_reg * 256u;
-        const int nch = (st.k_steps + 3) >> 2;
-        const uint32_t idesc = make_idesc(st.n_mma);
-        for (int c = 0; c < nch; ++c) {
-          const int nk = min(4, st.k_steps - 4 * c);
-          const bool last = (c == nch - 1);
-          // both 32-column units of this chunk must have been written by the epilogue warps; before the
-          // LAST chunk (whose commit releases the accumulator) every unit of the previous step must be
-          // finished, so no barrier phase can run ahead of a slow epilogue group
-          mbar_wait(&S.a_ready[2 * c], ar_phase);
-          mbar_wait(&S.a_ready[2 * c + 1], ar_phase);
-          if (last)
-            for (int u = 2 * c + 2; u < 8; ++u) mbar_wait(&S.a_ready[u], ar_phase);
-          if (MEGA && c == 0 && s == 0 && lane == 0) mega_event(q, EV_FIRST_MMA, tr.mode, tr.o, tr.tile);
-          if (c == 0 && lane == 0) {
-            DSPGN_CLK(4);
-            if (a.dbg_clk != nullptr && blockIdx.x == 0 && clk_tile < kClkTiles) {
-              unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-              a.dbg_clk[((size_t)clk_tile * kTcMaxSteps + s) * kClkSlots + 6] = (long long)gt;
-            }
-          }
-          // ---- W_hi image: A_hi*W_hi + A_lo*W_hi
-          mbar_wait(&S.w_full[stage], phase);
-          tc_fence_after();
-          {
-            const uint32_t b0 = smem_u32(ring + (size_t)stage * kTcStageBytes);
-            for (int k = 0; k < nk; ++k) {
-              const uint64_t bd = make_b_desc(b0 + 32u * k);
-              const uint32_t ah = a_t + 64u * c + a_col_hi(k);
-              tc_mma_ts_elect(d_t, ah, bd, idesc, (c | k) ? 1u : 0u);
-              tc_mma_ts_elect(d_t, ah + 16u, bd, idesc, 1u);
-            }
-            tc_commit_elect(&S.w_empty[stage]);
-          }
-          if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-          // ---- W_lo image: A_hi*W_lo
-          mbar_wait(&S.w_full[stage], phase);
-          tc_fence_after();
-          {
-            const uint32_t b0 = smem_u32(ring + (size_t)stage * kTcStageBytes);
-            for (int k = 0; k < nk; ++k) tc_mma_ts_elect(d_t, a_t + 64u * c + a_col_hi(k), make_b_desc(b0 + 32u * k), idesc, 1u);
-            tc_commit_elect(&S.w_empty[stage]);
-            if (last) { tc_commit_elect(&S.acc_full[0]); if (lane == 0) DSPGN_CLK(5); }
-          }
-          if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-        }
-        ar_phase ^= 1;
+        for (int s = 0; s < ns; ++s) produce_step(blob + plan.step[s].w_off, plan.step[s].k_steps, ring, S.w_full, S.w_empty, stage, phase);
       }
     }
   } else {
-    // ===================== epilogue groups ======================================================
-    // group g (warps 4g..4g+3) converts operand units g, g+2, g+4, g+6 (32 columns each), in that order, so
-    // that the two units of K chunk c are produced concurrently by the two groups; thread = tile row = TMEM lane.
+    // ===================== consumer warpgroups =================================================
+    // Warpgroup g issues the MMAs of tile rows [64g, 64g+64) and runs their epilogue on the accumulator fragment.  The
+    // per-row stages (prologue, pose columns, residual) use thread = tile row r (both groups hold the same row values).
     const int grp = warp >> 2;
     const int r = tid & 127;
-    const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;
-    uint32_t acc_phase = 0;
+    const int qd = lane & 3;                                   // fragment column pair
+    const int rl = 16 * (warp & 3) + (lane >> 2);              // fragment rows rl, rl + 8 of the warpgroup
+    const int rowA = 64 * grp + rl, rowB = rowA + 8;           // ... as tile rows
+    unsigned char* const alo = ring + (size_t)kTcStages * kTcStageBytes + (size_t)grp * kTcAloBytes;
+    const uint32_t alo_s = smem_u32(alo);
+    uint32_t stage = 0, phase = 0;
+    float acc[128];
+    uint32_t ah[64];
     int clk_tile = -1;
     for (int seq = 0;; ++seq) {
       ++clk_tile;
@@ -666,94 +585,85 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           sc = inside_unit_sphere(x0, x1, x2) ? 1.f : 0.f;            // loss.py:68
         }
       }
-      if (grp == 0) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; }
+      if (grp == 0) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; S.scr[r] = sc; }
       epi_bar_sync();                                // zs / xr / bias visible; previous tile fully drained
       if (tid == 0) S.cur_class = M.class_id;
 
-      // decoder input element i of this row: [z | x | 0...]
-      auto inp = [&](int i) -> float {
+      // decoder input element i of tile row `row`: [z | x | 0...]
+      auto inp = [&](int i, int row) -> float {
         const int j = i - L;
-        return (j < 0) ? S.zs[i] : ((unsigned)j < 3u ? S.xr[j * kTcRows + r] : 0.f);
+        return (j < 0) ? S.zs[i] : ((unsigned)j < 3u ? S.xr[j * kTcRows + row] : 0.f);
       };
+      uint32_t* const maskw = S.maskw + tid;           // word w of layer l: maskw[(4 * l + w) * kTcEpiThreads]
 
       // ---- A operand of the first GEMM step (= layer 1): layer 0 on the CUDA cores.  With W0[:, :L] z folded into
       // zb0, layer 0 is 3 FMAs per output:  h0[j] = relu(zb0[j] + W0[j][L..L+2] . x)  (deep_sdf_decoder.py:91,103).
-      // As a GEMM step (K = 80) it cost 4.8k cycles per tile, most of it the dependency bubble. --------------------
       {
-        const TcStep s0 = plan.step[0];
-        const uint32_t a_t = tmem + (uint32_t)s0.a_reg * 256u + lane_addr;
-        const int kk = s0.k_steps * 16;
+        const int kk = plan.step[0].k_steps * 16;
         const int n0out = dec.out_dim[0];
-        // (the three weight rows come from shared memory: as 768 uniform __ldg per thread and tile they were 6k L1
-        //  wavefronts per tile, most of the 8 us between a tile's begin and its first MMA)
         const float* w0x = S.w0x;
-        const float px = x0, py = x1, pz = x2;
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-          const int u = grp + 2 * j, n0 = 32 * u;
-          if (n0 < kk) {
-            float t[32];
-            uint32_t mw = 0;
+        const float xa0 = S.xr[rowA], xa1 = S.xr[kTcRows + rowA], xa2 = S.xr[2 * kTcRows + rowA];
+        const float xb0 = S.xr[rowB], xb1 = S.xr[kTcRows + rowB], xb2 = S.xr[2 * kTcRows + rowB];
+        uint32_t mw[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int c = n0 + i;
-              float w = S.bias[c];
-              w = fmaf(w0x[c], px, w);
-              w = fmaf(w0x[kHid + c], py, w);
-              w = fmaf(w0x[2 * kHid + c], pz, w);
-              const bool on = (c < n0out) && (w > 0.f);
-              mw |= (on ? 1u : 0u) << i;
-              t[i] = on ? w : 0.f;
-            }
-            S.maskw[(0 * 8 + u) * kTcRows + r] = mw;
-            store_a_unit(a_t + (uint32_t)n0, t);
-          } else {
-            S.maskw[(0 * 8 + u) * kTcRows + r] = 0u;
-          }
-          unit_done(&S.a_ready[u]);
+        for (int e = 0; e < 128; ++e) {
+          const int c = frag_col(e, qd);
+          const bool hb = (e & 2) != 0;
+          float w = S.bias[c];
+          w = fmaf(w0x[c], hb ? xb0 : xa0, w);
+          w = fmaf(w0x[kHid + c], hb ? xb1 : xa1, w);
+          w = fmaf(w0x[2 * kHid + c], hb ? xb2 : xa2, w);
+          const bool on = (c < kk) && (c < n0out) && (w > 0.f);
+          mw[e >> 5] |= (on ? 1u : 0u) << (e & 31);
+          acc[e] = on ? w : 0.f;
         }
+#pragma unroll
+        for (int w = 0; w < 4; ++w) maskw[w * kTcEpiThreads] = mw[w];
+        store_operand(acc, ah, alo, rl, qd, grp);
       }
 
       float yv = 0.f;
       for (int s = 0; s < ns; ++s) {
         const TcStep st = plan.step[s];
         const bool more = (s + 1 < ns);
-        const int a_next = more ? plan.step[s + 1].a_reg : 0;
         const int k_next = more ? plan.step[s + 1].k_steps * 16 : 0;
-        const uint32_t d_t = tmem + (uint32_t)st.d_reg * 256u + lane_addr;
-        const uint32_t an_t = tmem + (uint32_t)a_next * 256u + lane_addr;
-        mbar_wait(&S.acc_full[0], acc_phase);
-        tc_fence_after();
+        const int nm = st.n_mma;
+        if (tid == 0) {
+          DSPGN_CLK(4);
+          if (MEGA && s == 0) mega_event(q, EV_FIRST_MMA, tr.mode, tr.o, tr.tile);
+        }
+        wg_gemm(acc, ah, alo_s, ring, S.w_full, S.w_empty, stage, phase, st.k_steps);
+        wg_bar_sync(grp);                                // every MMA of the warpgroup has read the A lo image
         if (tid == 0) DSPGN_CLK(0);
 
         if (st.kind == TK_FWD_PENULT) {
           // ---- last hidden layer: bias + ReLU (mask saved), and the final Linear(width, 1) + tanh right here as a per-row
-          // dot product on the CUDA cores while the values are in registers.  As an MMA step it was the worst one: N = 16
-          // still costs the ~110-cycle floor per instruction (48 MMAs + the dependency bubble = 7.3k cycles for 256 MACs
-          // per row) and needed its own TMEM operand.  deep_sdf_decoder.py:91,103,107-108.
-          float part = 0.f;
-#pragma unroll 1
-          for (int j = 0; j < 4; ++j) {
-            const int u = grp + 2 * j, n0 = 32 * u;
-            uint32_t mw = 0;
-            if (n0 < st.n_mma) {
-              uint32_t v[32];
-              tc_ld32(d_t + (uint32_t)n0, v);
-              tc_wait_ld();
-              const float* bb = S.bias + st.layer * kHid + n0;
-              const float* wl = S.wlast + n0;
+          // dot product on the CUDA cores while the values are in registers (one GEMM step with N = 1 saved).
+          // deep_sdf_decoder.py:91,103,107-108.  The 4 lanes of a quad hold one row pair: combined in a fixed order.
+          const float* bb = S.bias + st.layer * kHid;
+          float pa = 0.f, pb = 0.f;
+          uint32_t mw[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                const float w = __uint_as_float(v[i]) + bb[i];
-                mw |= (w > 0.f ? 1u : 0u) << i;
-                part = fmaf(fmaxf(w, 0.f), wl[i], part);
-              }
+          for (int e = 0; e < 128; ++e) {
+            const int c = frag_col(e, qd);
+            if (c < nm) {
+              const float w = acc[e] + bb[c];
+              mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
+              if (e & 2) pb = fmaf(fmaxf(w, 0.f), S.wlast[c], pb);
+              else pa = fmaf(fmaxf(w, 0.f), S.wlast[c], pa);
             }
-            S.maskw[(st.layer * 8 + u) * kTcRows + r] = mw;
           }
-          (grp == 0 ? S.rr : S.rsc)[r] = part;             // the two column halves of the row, combined in a fixed order
-          epi_bar_sync();                                  // (also: every accumulator read of this step is finished)
-          yv = tanhf((S.rr[r] + S.rsc[r]) + S.bias[(st.layer + 1) * kHid]);      // deep_sdf_decoder.py:107-108
+#pragma unroll
+          for (int w = 0; w < 4; ++w) maskw[(4 * st.layer + w) * kTcEpiThreads] = mw[w];
+          pa += __shfl_xor_sync(0xffffffffu, pa, 1);
+          pb += __shfl_xor_sync(0xffffffffu, pb, 1);
+          pa += __shfl_xor_sync(0xffffffffu, pa, 2);
+          pb += __shfl_xor_sync(0xffffffffu, pb, 2);
+          const float blast = S.bias[(st.layer + 1) * kHid];
+          const float ya = tanhf(pa + blast), yb = tanhf(pb + blast);           // deep_sdf_decoder.py:107-108
+          if (qd == 0) { S.yrow[rowA] = ya; S.yrow[rowB] = yb; }
+          epi_bar_sync();
+          yv = S.yrow[r];
           if (fwd_only) {
             if (grp == 0 && r < nrows) {
               const size_t base = (mode == MODE_RAYFWD) ? (size_t)M.smp_off : (size_t)M.pts_off;
@@ -765,118 +675,68 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
             }
           }
           if (more) {
-            // seed of the backward chain: g = (1 - y^2) W_last, masked by this layer's ReLU, written into the (dead) A
-            // region of this step; the first backward GEMM accumulates into the region whose reads ended at the barrier
-            const float gy = 1.f - yv * yv;
-#pragma unroll 1
-            for (int j = 0; j < 4; ++j) {
-              const int u = grp + 2 * j, n0 = 32 * u;
-              if (n0 < k_next) {
-                const uint32_t mw = S.maskw[(st.layer * 8 + u) * kTcRows + r];
-                float t[32];
+            // seed of the backward chain: g = (1 - y^2) W_last, masked by this layer's ReLU
+            const float ga = 1.f - ya * ya, gb = 1.f - yb * yb;
 #pragma unroll
-                for (int i = 0; i < 32; ++i) t[i] = ((mw >> i) & 1u) ? gy * S.wlast[n0 + i] : 0.f;
-                store_a_unit(an_t + (uint32_t)n0, t);
-              }
-              unit_done(&S.a_ready[u]);
+            for (int e = 0; e < 128; ++e) {
+              const int c = frag_col(e, qd);
+              acc[e] = ((mw[e >> 5] >> (e & 31)) & 1u) ? ((e & 2) ? gb : ga) * S.wlast[c] : 0.f;
             }
+            store_operand(acc, ah, alo, rl, qd, grp);
           }
         } else if (st.kind == TK_FWD_HIDDEN) {
-#pragma unroll 1
-          for (int j = 0; j < 4; ++j) {
-            const int u = grp + 2 * j, n0 = 32 * u;
-            if (n0 < k_next) {
-              float t[32];
-              uint32_t mw = 0;
-              if (n0 < st.n_mma) {
-                uint32_t v[32];
-                tc_ld32(d_t + (uint32_t)n0, v);
-                tc_wait_ld();
-                const float* bb = S.bias + st.layer * kHid + n0;
+          const float* bb = S.bias + st.layer * kHid;
+          uint32_t mw[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                  const float w = __uint_as_float(v[i]) + bb[i];
-                  mw |= (w > 0.f ? 1u : 0u) << i;
-                  t[i] = fmaxf(w, 0.f);
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) t[i] = 0.f;
-              }
-              S.maskw[(st.layer * 8 + u) * kTcRows + r] = mw;
-              if (st.cat_off >= 0 && n0 + 32 > st.cat_off) {      // deep_sdf_decoder.py:87-88: cat[x, input]
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  if (n0 + i >= st.cat_off) t[i] = inp(n0 + i - st.cat_off);
-              }
-              store_a_unit(an_t + (uint32_t)n0, t);
+          for (int e = 0; e < 128; ++e) {
+            const int c = frag_col(e, qd);
+            float t = 0.f;
+            if (c < nm) {
+              const float w = acc[e] + bb[c];
+              mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
+              t = fmaxf(w, 0.f);
             }
-            unit_done(&S.a_ready[u]);
+            if (st.cat_off >= 0 && c >= st.cat_off) t = inp(c - st.cat_off, (e & 2) ? rowB : rowA);   // deep_sdf_decoder.py:87-88
+            acc[e] = (c < k_next) ? t : 0.f;
           }
+#pragma unroll
+          for (int w = 0; w < 4; ++w) maskw[(4 * st.layer + w) * kTcEpiThreads] = mw[w];
+          store_operand(acc, ah, alo, rl, qd, grp);
         } else if (st.kind == TK_BWD_MID) {
-#pragma unroll 1
-          for (int j = 0; j < 4; ++j) {
-            const int u = grp + 2 * j, n0 = 32 * u;
-            if (n0 < st.n_mma) {
-              uint32_t v[32];
-              tc_ld32(d_t + (uint32_t)n0, v);
-              tc_wait_ld();
-              const uint32_t mw = S.maskw[(st.mask_layer * 8 + u) * kTcRows + r];
-              float t[32];
+          uint32_t mw[4];
 #pragma unroll
-              for (int i = 0; i < 32; ++i) t[i] = ((mw >> i) & 1u) ? __uint_as_float(v[i]) : 0.f;
-              if (st.cat_off >= 0 && n0 + 32 > st.cat_off) {      // latent_in skip path -> d/d(input)
+          for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                  const int ii = n0 + i - st.cat_off;
-                  if (ii >= 0) {
-                    if (ii < in0) S.Jp[r * kJpStride + ((ii < L) ? ii : (kMaxCode + ii - L))] = __uint_as_float(v[i]);
-                    t[i] = 0.f;
-                  }
-                }
+          for (int e = 0; e < 128; ++e) {
+            const int c = frag_col(e, qd);
+            float t = 0.f;
+            if (c < nm) {
+              const float v = acc[e];
+              t = ((mw[e >> 5] >> (e & 31)) & 1u) ? v : 0.f;
+              if (st.cat_off >= 0 && c >= st.cat_off) {      // latent_in skip path -> d/d(input)
+                const int ii = c - st.cat_off;
+                if (ii < in0) S.Jp[((e & 2) ? rowB : rowA) * kJpStride + ((ii < L) ? ii : (kMaxCode + ii - L))] = v;
+                t = 0.f;
               }
-              if (n0 < k_next) store_a_unit(an_t + (uint32_t)n0, t);
             }
-            unit_done(&S.a_ready[u]);
+            acc[e] = (c < k_next) ? t : 0.f;
           }
+          if (more) store_operand(acc, ah, alo, rl, qd, grp);
         } else {
           // ---- TK_BWD_FIRST: d/d(input) complete -> Jacobian row (loss.py:34-41 / :143-150) -------------
-          float* jr = S.Jp + r * kJpStride;
-#pragma unroll 1
-          for (int j = 0; j < 4; ++j) {
-            const int n0 = 32 * (grp + 2 * j);
-            if (n0 < st.n_mma && n0 < in0) {
-              uint32_t v[32];
-              tc_ld32(d_t + (uint32_t)n0, v);         // columns beyond n_mma are never used below
-              tc_wait_ld();
-              if (L == kMaxCode && n0 + 32 <= kMaxCode) {
-                // thread-per-row accesses as float4: with the 76-float row stride a quarter-warp covers all 32 banks
-                // (the scalar form was a 4-way bank conflict)
 #pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                  float4* pj = reinterpret_cast<float4*>(jr + n0 + i);
-                  float4 g = make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-                  if (has_skip) { const float4 k = *pj; g.x += k.x; g.y += k.y; g.z += k.z; g.w += k.w; }
-                  g.x *= sc; g.y *= sc; g.z *= sc; g.w *= sc;      // loss.py:145 (de_ds) / inactive rows
-                  *pj = g;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                  const int ii = n0 + i;
-                  if (ii < in0) {
-                    const int jc = (ii < L) ? ii : (kMaxCode + ii - L);
-                    float g = __uint_as_float(v[i]);
-                    if (has_skip) g += jr[jc];
-                    jr[jc] = g * sc;                               // loss.py:145 (de_ds) / inactive rows
-                  }
-                }
-              }
+          for (int e = 0; e < 128; ++e) {
+            const int c = frag_col(e, qd);
+            if (c < nm && c < in0) {
+              const int row = (e & 2) ? rowB : rowA;
+              float* pj = S.Jp + row * kJpStride + ((c < L) ? c : (kMaxCode + c - L));
+              float g = acc[e];
+              if (has_skip) g += *pj;
+              *pj = g * S.scr[row];                                  // loss.py:145 (de_ds) / inactive rows
             }
           }
         }
         if (tid == 0) DSPGN_CLK(3);
-        acc_phase ^= 1;
       }
       if (!fwd_only) {
       // ---- pose columns, residual (thread = row; needs every d/d(input) column of the row) -----------
@@ -914,32 +774,22 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         int bi = 0, rem = tid;
         while (rem >= 18 - bi) { rem -= 18 - bi; ++bi; }
         const int bj = bi + rem;
-        // Packed fp32 FMAs (fma.rn.f32x2 -> FFMA2, two FMAs per lane and instruction: the plain FFMA pipe issues one
-        // warp instruction per two cycles, which made this loop 8k cycles on the two scheduler partitions that hold two of
-        // the six warps).  h2[u][w] = (h[u][2w], h[u][2w+1]); every FMA is the same operation as in the scalar form.
-        unsigned long long h2[4][2];
+        float h[4][4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) { h2[u][0] = 0ull; h2[u][1] = 0ull; }
+        for (int u = 0; u < 4; ++u)
+#pragma unroll
+          for (int v = 0; v < 4; ++v) h[u][v] = 0.f;
         const float* pa = S.Jp + 4 * bi;
         const float* pb = S.Jp + 4 * bj;
 #pragma unroll 4
         for (int p = 0; p < kTcRows; ++p) {
           const float4 A4 = *reinterpret_cast<const float4*>(pa + p * kJpStride);
-          const ulonglong2 B2 = *reinterpret_cast<const ulonglong2*>(pb + p * kJpStride);     // (b0, b1), (b2, b3)
-          const float av[4] = {A4.x, A4.y, A4.z, A4.w};
+          const float4 B4 = *reinterpret_cast<const float4*>(pb + p * kJpStride);
+          const float av[4] = {A4.x, A4.y, A4.z, A4.w}, bv[4] = {B4.x, B4.y, B4.z, B4.w};
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            unsigned long long aa;
-            asm("mov.b64 %0, {%1, %1};" : "=l"(aa) : "f"(av[u]));
-            asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(h2[u][0]) : "l"(aa), "l"(B2.x));
-            asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(h2[u][1]) : "l"(aa), "l"(B2.y));
-          }
-        }
-        float h[4][4];
+          for (int u = 0; u < 4; ++u)
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          asm("mov.b64 {%0, %1}, %2;" : "=f"(h[u][0]), "=f"(h[u][1]) : "l"(h2[u][0]));
-          asm("mov.b64 {%0, %1}, %2;" : "=f"(h[u][2]), "=f"(h[u][3]) : "l"(h2[u][1]));
+            for (int v = 0; v < 4; ++v) h[u][v] = fmaf(av[u], bv[v], h[u][v]);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u)
@@ -996,9 +846,6 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) tc_dealloc(tmem, 512);
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) k_decoder_tc(TermArgs a) {
@@ -1016,73 +863,45 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent_render(TermArgs
 
 // ------------------------------------------------------------------------------------------------
 // self-test kernel: D[128 x n_mma] = A[128 x 16*k_steps] * B^T through exactly the same operand paths
-// (TMEM A written by store_a_block, swizzled weight images, 3-pass split).  Used by tests only.
+// (register hi / swizzled shared-memory lo A operand, swizzled weight images through the ring, 3-pass split).
+// Used by tests only.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) k_tc_selftest(const float* __restrict__ A, int lda, const unsigned char* __restrict__ blob,
-                                                        int n_mma, int k_steps, float* __restrict__ D) {
+constexpr size_t kTcSelftestSmem = 1024 + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes + 64;
+__global__ void __launch_bounds__(kTcThreads, 1) k_tc_selftest(const float* __restrict__ A, int lda, const unsigned char* __restrict__ blob,
+                                                               int n_mma, int k_steps, float* __restrict__ D) {
   extern __shared__ unsigned char st_raw[];
   unsigned char* ring = st_raw + ((1024u - (smem_u32(st_raw) & 1023u)) & 1023u);
-  __shared__ uint64_t bar_w, bar_acc;
-  __shared__ uint32_t tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  if (tid == 0) { mbar_init(&bar_w, 1); mbar_init(&bar_acc, 1); fence_barrier_init(); }
-  if (warp == 0) tc_alloc(&tmem_base, 512);
-  tc_fence_before();
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes);
+  uint64_t* w_full = bars;
+  uint64_t* w_empty = bars + kTcStages;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int i = 0; i < kTcStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 8); }
+    fence_barrier_init();
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base;
-  const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-  const int nch = (k_steps + 3) >> 2;
-  // A operand -> TMEM region 0
-  for (int u = 0; u < 2 * nch; ++u) {
-    float t[32];
+  uint32_t stage = 0, phase = 0;
+  if (warp == 8) {
+    if (lane == 0) produce_step(blob, k_steps, ring, w_full, w_empty, stage, phase);
+    return;
+  }
+  const int grp = warp >> 2, qd = lane & 3, rl = 16 * (warp & 3) + (lane >> 2);
+  const int rowA = 64 * grp + rl, rowB = rowA + 8;
+  unsigned char* alo = ring + (size_t)kTcStages * kTcStageBytes + (size_t)grp * kTcAloBytes;
+  float acc[128];
+  uint32_t ah[64];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int kk = u * 32 + i;
-      t[i] = (kk < k_steps * 16) ? A[(size_t)tid * lda + kk] : 0.f;
-    }
-    store_a_unit(tmem + lane_addr + (uint32_t)u * 32u, t);
+  for (int e = 0; e < 128; ++e) {
+    const int c = frag_col(e, qd);
+    acc[e] = (c < k_steps * 16) ? A[(size_t)((e & 2) ? rowB : rowA) * lda + c] : 0.f;
   }
-  tc_wait_st();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t img = (uint32_t)n_mma * 128u;
-  const uint32_t idesc = make_idesc(n_mma);
-  uint32_t wph = 0;
-  for (int c = 0; c < nch; ++c) {
-    const int nq = min(4, k_steps - 4 * c);
-    if (tid == 0) {
-      mbar_expect_tx(&bar_w, 2 * img);
-      bulk_g2s(ring, blob + (size_t)(2 * c) * img, img, &bar_w);
-      bulk_g2s(ring + kTcStageBytes, blob + (size_t)(2 * c + 1) * img, img, &bar_w);
-    }
-    mbar_wait(&bar_w, wph);
-    wph ^= 1;
-    tc_fence_after();
-    if (tid == 0) {
-      const uint32_t bh = smem_u32(ring), bl = smem_u32(ring + kTcStageBytes);
-      const uint32_t a_blk = tmem + (uint32_t)c * 64u;
-      for (int q = 0; q < nq; ++q) {
-        tc_mma_ts(tmem + 256u, a_blk + a_col_hi(q), make_b_desc(bh + 32u * q), idesc, (c | q) ? 1u : 0u);
-        tc_mma_ts(tmem + 256u, a_blk + a_col_hi(q) + 16u, make_b_desc(bh + 32u * q), idesc, 1u);
-        tc_mma_ts(tmem + 256u, a_blk + a_col_hi(q), make_b_desc(bl + 32u * q), idesc, 1u);
-      }
-      tc_commit(&bar_acc);
-    }
-    mbar_wait(&bar_acc, (uint32_t)(c & 1));      // weights of this chunk consumed before the ring is reused
-    tc_fence_after();
-  }
-  for (int n0 = 0; n0 < n_mma; n0 += 16) {
-    uint32_t v[16];
-    tc_ld16(tmem + 256u + lane_addr + (uint32_t)n0, v);
-    tc_wait_ld();
+  store_operand(acc, ah, alo, rl, qd, grp);
+  wg_gemm(acc, ah, smem_u32(alo), ring, w_full, w_empty, stage, phase, k_steps);
 #pragma unroll
-    for (int i = 0; i < 16; ++i) D[(size_t)tid * n_mma + n0 + i] = __uint_as_float(v[i]);
+  for (int e = 0; e < 128; ++e) {
+    const int c = frag_col(e, qd);
+    if (c < n_mma) D[(size_t)((e & 2) ? rowB : rowA) * n_mma + c] = acc[e];
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc_dealloc(tmem, 512);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1094,11 +913,12 @@ struct TcDecoderHost {
   size_t blob_bytes = 0;
 };
 
-// image of B[n][kk] (n < n_mma, kk in [64c, 64c+64)) as fp16 hi / lo, K-major rows of 128 B, 128B swizzle
+// image of B[n][kk] (n < n_mma, kk in [64c, 64c+64)) as fp16 hi / lo, K-major rows of 128 B, 128B swizzle; rows
+// n_mma..255 are zero (every GEMM step is one N = 256 wgmma)
 template <class F>
 inline void tc_pack_images(std::vector<unsigned char>& out, int n_mma, int k_steps, F&& elem) {
   const int nch = (k_steps + 3) / 4;
-  const size_t img = (size_t)n_mma * 128;
+  const size_t img = (size_t)kTcStageBytes;
   const size_t base = out.size();
   out.resize(base + (size_t)nch * 2 * img, 0);
   for (int c = 0; c < nch; ++c) {
@@ -1195,7 +1015,7 @@ inline int tc_setup_kernels(std::string& err) {
     err = std::string("cudaFuncSetAttribute(k_gn_persistent): ") + cudaGetErrorString(cudaGetLastError());
     return DSPGN_E_CUDA;
   }
-  if (cudaFuncSetAttribute(k_tc_selftest, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kTcStageBytes + 1024) != cudaSuccess) {
+  if (cudaFuncSetAttribute(k_tc_selftest, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSelftestSmem) != cudaSuccess) {
     err = std::string("cudaFuncSetAttribute(k_tc_selftest): ") + cudaGetErrorString(cudaGetLastError());
     return DSPGN_E_CUDA;
   }

@@ -19,7 +19,7 @@ class DecoderWeights:
     deep_sdf_decoder.py concatenates at each layer's input -- cat_kind[k]: 0 nothing, 1 the decoder input
     (`latent_in`, :87-88), 2 xyz (`xyz_in_all`, :89-90) -- plus the optional LayerNorm (gamma, beta) after layer k
     (:58-63,96-102) and `use_tanh` (:93-94).  The plain shape (one latent_in layer, nothing else) runs on the
-    tcgen05 engine; every other variant on the fp32 SIMT engine."""
+    tensor-core engine; every other variant on the fp32 SIMT engine."""
 
     def __init__(self, W, b, latent_in, latent_size, xyz_in_all=False, use_tanh=False, ln=None):
         self.W = [np.ascontiguousarray(w, dtype=np.float32) for w in W]

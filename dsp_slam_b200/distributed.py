@@ -10,7 +10,7 @@ Two exchange mechanisms:
 
 * ``peer`` (default on GPUs): rank 0 owns a gather buffer in its HBM and exports it with CUDA IPC; the other
   ranks map it over NVLink/NVSwitch, and the solve step that finishes an object stores the record straight
-  into rank 0's buffer at the object's ORIGINAL index -- issued from the same kernel that runs the tcgen05
+  into rank 0's buffer at the object's ORIGINAL index -- issued from the same kernel that runs the tensor-core
   tiles.  No collective kernel, no reorder pass; a per-rank sequence flag publishes a finished step
   (include/dspgn.h "Multi-GPU result exchange").
 * ``nccl`` / gloo: one ``all_gather_into_tensor`` of the padded per-rank record blocks on the solver's stream

@@ -1,4 +1,4 @@
-"""Host-side mirror of DSP-SLAM's `reconstruct/optimizer.py` on top of libdspgn (CUDA, sm_100a).
+"""Host-side mirror of DSP-SLAM's `reconstruct/optimizer.py` on top of libdspgn (CUDA, sm_90a).
 
 Same names, positional orders and soft-failure behaviour as the reference so that the C++
 LocalMapping thread (src/LocalMapping.cc:38-40, src/LocalMapping_util.cc:109-110,179-196,390-428)

@@ -1,6 +1,6 @@
 /*
  * dspgn.h -- C ABI of libdspgn.so: DSP-SLAM's per-object shape-prior Gauss-Newton reconstruction
- * as hand-written CUDA for NVIDIA B200 (sm_100a).
+ * as hand-written CUDA for NVIDIA H100 (sm_90a).
  *
  * Drop-in boundary.  The reference has no native FFI for this path: its C++ LocalMapping thread
  * calls Python through pybind11 (src/LocalMapping.cc:38-40, src/LocalMapping_util.cc:109-110,
@@ -41,7 +41,7 @@ extern "C" {
 #define DSPGN_OK 0
 #define DSPGN_E_ARG (-1)      /* bad argument / unsupported decoder shape */
 #define DSPGN_E_CUDA (-2)     /* CUDA runtime error; see dspgn_last_error() */
-#define DSPGN_E_NOGPU (-3)    /* no usable sm_100 device */
+#define DSPGN_E_NOGPU (-3)    /* no usable sm_90 device */
 #define DSPGN_E_ALLOC (-4)
 #define DSPGN_E_PEER (-5)     /* multi-GPU exchange: a peer never published its results (timeout) */
 
@@ -61,7 +61,7 @@ extern "C" {
 /* decoder engines */
 #define DSPGN_ENGINE_AUTO 0
 #define DSPGN_ENGINE_SIMT 1    /* fp32 FFMA kernels: on-device ground truth */
-#define DSPGN_ENGINE_TC 2      /* tcgen05 tensor-core kernels, 3-pass split-fp16 (fp32-class accuracy) */
+#define DSPGN_ENGINE_TC 2      /* wgmma tensor-core kernels, 3-pass split-fp16 (fp32-class accuracy) */
 
 typedef struct DspgnDecoder DspgnDecoder;
 typedef struct DspgnSolver DspgnSolver;
@@ -84,7 +84,7 @@ typedef struct {
    *   layer_norm[k] 1: LayerNorm (eps 1e-5) between layer k and its ReLU (:58-63,96-102); gamma/beta through
    *                 dspgn_decoder_create_ex
    *   use_tanh      1: an extra tanh on the last layer before the final one (:93-94,107-108)
-   * Decoders that use any of them run on the fp32 SIMT engine (the tcgen05 engine covers the plain shape). */
+   * Decoders that use any of them run on the fp32 SIMT engine (the tensor-core engine covers the plain shape). */
   int32_t cat_kind[DSPGN_MAX_LINEAR];
   int32_t layer_norm[DSPGN_MAX_LINEAR];
   int32_t use_tanh;
@@ -199,7 +199,7 @@ int dspgn_enable_timing(DspgnSolver* s, int on);
  * One process per GPU.  There is no collective kernel: rank 0 owns a "gather buffer" in its HBM, exports it
  * with CUDA IPC, every other rank maps it over NVLink/NVSwitch, and the solve step that finishes an object
  * stores the object's 352-byte result record STRAIGHT INTO rank 0's buffer (peer st.global issued from the
- * same kernel that runs the tcgen05 tiles), at the object's slot = its index in the original batch.  A
+ * same kernel that runs the tensor-core tiles), at the object's slot = its index in the original batch.  A
  * per-rank sequence flag (release, system scope) publishes a finished step; rank 0 waits for all flags with
  * a one-warp kernel on its own stream.  Two slot sets alternate by step parity and rank 0 acknowledges
  * consumed steps, so ranks may run at most one step ahead of rank 0.  `seq` = 1, 2, 3, ... (caller-owned,
@@ -248,8 +248,8 @@ int dspgn_debug_inputs(DspgnSolver* s, int obj, float* t_cam_obj, float* pts, fl
  * env DSPGN_CLK at solver creation; returns the number of (timestamp, descriptor) pairs written, or a negative code. */
 int dspgn_debug_events(DspgnSolver* s, long long* out, int max_events);
 
-/* Test hook for the tcgen05 operand paths: D[128][n_mma] = A[128][16*k_steps] * B[n_mma][16*k_steps]^T
- * (A through the TMEM split-fp16 path, B through the pre-swizzled shared-memory images). Host buffers. */
+/* Test hook for the wgmma operand paths: D[128][n_mma] = A[128][16*k_steps] * B[n_mma][16*k_steps]^T
+ * (A through the register / shared-memory split-fp16 path, B through the pre-swizzled shared-memory images). Host buffers. */
 int dspgn_tc_selftest(int device, int n_mma, int k_steps, const float* A, const float* B, float* D);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-"""One-file replacement of DSP-SLAM's `reconstruct/optimizer.py` (222 lines of PyTorch) by the B200 path.
+"""One-file replacement of DSP-SLAM's `reconstruct/optimizer.py` (222 lines of PyTorch) by the H100 path.
 
 Copy this file over `reconstruct/optimizer.py` in a DSP-SLAM checkout and put `dsp_slam_b200/` (with the built
 `libdspgn.so`) on PYTHONPATH.  The C++ side is untouched: it keeps importing `reconstruct.optimizer`

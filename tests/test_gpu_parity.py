@@ -1,5 +1,5 @@
 """GPU parity: the CUDA path (through the C ABI / ctypes mirror) against the CPU oracle and the
-reference goldens.  Run on a B200: `python -m pytest tests -m gpu`.
+reference goldens.  Run on an H100: `python -m pytest tests -m gpu`.
 
 Tolerances (fp32; see tests/test_oracle_vs_golden.py for why whole runs are looser than single
 steps): single GN step at a fixed state  H,b rel 1e-4 (fp32 engine) / 3e-4 (tensor-core engine, 3-pass
@@ -234,7 +234,7 @@ def test_engines_agree_single_step(dec_path, cfg_kitti):
 
 @pytest.mark.parametrize("n_mma,k_steps", [(256, 16), (192, 16), (256, 5), (80, 16), (16, 16), (256, 12)])
 def test_tc_operand_paths_selftest(n_mma, k_steps):
-    """tcgen05 plumbing in isolation: D = A B^T with A through the TMEM split-fp16 path and B through the
+    """wgmma plumbing in isolation: D = A B^T with A through the register / shared-memory split-fp16 path and B through the
     pre-swizzled shared-memory images, vs float64 on the host.  3-pass split => ~1e-6 relative."""
     import ctypes as C
     from dsp_slam_b200 import _lib
@@ -672,7 +672,7 @@ def test_render_term_through_persistent_kernel(dec_path, cfg_kitti, oracle, orac
 def test_decoder_variants_layernorm_xyz_in_all_use_tanh(golden_dir, cfg_kitti, oracle):
     """Every optional feature of deep_sdf_decoder.py at once -- LayerNorm instead of weight-norm (:58-63,96-102),
     xyz_in_all (:41-47,89-90), use_tanh (:93-94), two latent_in layers (:87-88) -- through the fp32 SIMT engine
-    (selected automatically; the tcgen05 engine covers the plain shape and refuses this one loudly) against the
+    (selected automatically; the tensor-core engine covers the plain shape and refuses this one loudly) against the
     REFERENCE's own forward values, input Jacobian and SDF-term rows (tests/golden/variant.npz)."""
     from dsp_slam_b200.optimizer import Optimizer
     from dsp_slam_b200.decoder import DecoderWeights

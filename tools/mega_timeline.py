@@ -1,5 +1,5 @@
 """Event timeline of the persistent kernel (env DSPGN_CLK): where one GN iteration of one object spends its time.
-   python tools/mega_timeline.py [slam1|cfg3|cfg2_sdf|cfg2_full]   (on a B200)"""
+   python tools/mega_timeline.py [slam1|cfg3|cfg2_sdf|cfg2_full]   (on an H100)"""
 import os, sys, ctypes as C
 os.environ["DSPGN_CLK"] = "1"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,6 +1,6 @@
 // Micro-probe of the register-resident Gauss-Jordan pivot loop of dspgn_solve.cuh (test tooling, not product):
 // where do the cycles of one pivot go?  thread 0 accumulates clock64 deltas over the 71 pivots.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probes/solve_probe tools/probes/solve_probe.cu && ./solve_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probes/solve_probe tools/probes/solve_probe.cu && ./solve_probe
 #include <cstdio>
 #include <cuda_runtime.h>
 constexpr int N = 71, NP = 72, STRIDE = 73;

@@ -1,11 +1,10 @@
 """Per-kernel SASS opcode histogram of dsp_slam_b200/libdspgn.so -> profiles/sass_summary.txt
-(evidence that the tcgen05 / TMEM / bulk-copy path is what the library ships; B200_PROFILING.md "What proves a
-Blackwell-native kernel").   python tools/sass_summary.py"""
+(evidence that the wgmma / bulk-copy / mbarrier path is what the library ships).   python tools/sass_summary.py"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = os.path.join(ROOT, "dsp_slam_b200", "libdspgn.so")
 out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-KEY = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTCBAR", "UTCCP", "UBLKCP", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "HGMMA",
+KEY = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTCBAR", "UTCCP", "UBLKCP", "UTMALDG", "UTMASTG", "SYNCS", "WARPGROUP", "HMMA", "HGMMA",
        "FFMA", "DFMA", "LDS", "STS", "LDG", "STG", "LDGSTS", "ATOMG", "RED", "BAR", "SHFL", "MUFU", "LDL", "STL", "NANOSLEEP", "ELECT"]
 kern, hist, arch = None, collections.OrderedDict(), set()
 for line in out.splitlines():
@@ -27,11 +26,12 @@ for line in out.splitlines():
                 break
 demangle = subprocess.run(["c++filt"], input="\n".join(hist), capture_output=True, text=True).stdout.splitlines()
 lines = [f"libdspgn.so SASS summary (cuobjdump -sass; arch: {', '.join(sorted(arch))})",
-         "tcgen05.mma -> UTCHMMA, tcgen05.ld/st -> LDTM/STTM, tcgen05.commit -> UTCBAR, cp.async.bulk -> UBLKCP, cp.async -> LDGSTS", ""]
+         "wgmma.mma_async -> HGMMA, wgmma.fence/commit/wait -> WARPGROUP, cp.async.bulk -> UBLKCP, mbarrier -> SYNCS, cp.async -> LDGSTS", ""]
 for (k, h), d in zip(hist.items(), demangle):
     name = re.sub(r"\(.*", "", d)
     lines.append(f"{name}: {h['_total']} instructions")
     lines.append("    " + "  ".join(f"{op} {h[op]}" for op in KEY if h[op]))
 txt = "\n".join(lines) + "\n"
+os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
 open(os.path.join(ROOT, "profiles", "sass_summary.txt"), "w").write(txt)
 print(txt)
