@@ -12,6 +12,7 @@ RESULT_FLOATS = 88
 
 ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC = 0, 1, 2
 SCHED_AUTO, SCHED_LAUNCHES, SCHED_PERSISTENT = 0, 1, 2
+MODE_JOINT, MODE_POSE = 0, 1
 ST_OK, ST_SDF_NAN, ST_RENDER_FEW, ST_RENDER_NAN, ST_SOLVE, ST_BAD_INPUT = 0, 1, 2, 3, 4, 5
 E_ARG, E_CUDA, E_NOGPU, E_ALLOC, E_PEER = -1, -2, -3, -4, -5
 IPC_HANDLE_BYTES = 64
@@ -88,6 +89,8 @@ SYMBOLS = [
     ("dspgn_run_batch", C.c_int, [_VP, C.c_int]),
     ("dspgn_results", C.c_int, [_VP, C.POINTER(ObjectOut)]),
     ("dspgn_results_device", _VP, [_VP]),
+    ("dspgn_run_batch_modes", C.c_int, [_VP, C.POINTER(C.c_int32)]),
+    ("dspgn_keyframe_batch", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(ObjectOut)]),
     ("dspgn_decode_sdf", C.c_int, [_VP, C.c_int, _FP, _FP, C.c_int, C.c_int, C.c_int, _FP]),
     ("dspgn_counters", C.c_int, [_VP, C.POINTER(Counters)]),
     ("dspgn_enable_timing", C.c_int, [_VP, C.c_int]),

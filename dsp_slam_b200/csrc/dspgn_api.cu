@@ -98,7 +98,12 @@ struct DspgnSolver {
   DevBuf d_q_flag, d_q_ctr, d_tiles_left, d_obj_iter;   // persistent-kernel work queue
   int* d_tbase_static = nullptr;   // [n_obj] first 128-row SDF tile of each object (inside the staging block)
   int* d_tbase_r_static = nullptr; // [n_obj] first band-tile partial slot of each object (capacity: its ray-sample tiles + 1)
-  int* d_q0_render = nullptr;      // [n_obj] first iteration-0 queue slot of each object in a run with the render term
+  // per-run object table: mode [n_obj] | first iteration-0 queue slot of the persistent kernel [n_obj]
+  DevBuf d_run;
+  HostBuf h_run;                   // pinned staging of the table; rewritten only after ev_run_upload
+  cudaEvent_t ev_run_upload = nullptr;
+  bool run_upload_pending = false;
+  bool run_table_valid = false;    // d_run holds h_run for the resident batch (a repeated run skips the copy)
   int total_tiles128 = 0;          // SDF tiles of the batch
   long long total_ray_tiles128 = 0;// ray-sample tiles of the batch
   int max_tiles128 = 0;            // largest tile count of one term of one object (queue items hold 19 bits)
@@ -331,6 +336,7 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
     s->clk_on = true;
   }
   CU(cudaEventCreateWithFlags(&s->ev_upload, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&s->ev_run_upload, cudaEventDisableTiming));
   CU(cudaStreamCreateWithFlags(&s->stream2, cudaStreamNonBlocking));
   CU(cudaEventCreateWithFlags(&s->ev_fork, cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(&s->ev_join, cudaEventDisableTiming));
@@ -354,12 +360,14 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   dspgn_gather_close(s);
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_clk, &s->d_q_flag, &s->d_q_ctr,
-                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre}) b->release();
+                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_run}) b->release();
   s->h_stage.release();
   s->h_results.release();
+  s->h_run.release();
   for (auto e : s->ev) cudaEventDestroy(e);
   for (auto e : s->ev_solve) cudaEventDestroy(e);
   if (s->ev_upload) cudaEventDestroy(s->ev_upload);
+  if (s->ev_run_upload) cudaEventDestroy(s->ev_run_upload);
   if (s->ev_fork) cudaEventDestroy(s->ev_fork);
   if (s->ev_join) cudaEventDestroy(s->ev_join);
   if (s->stream2) cudaStreamDestroy(s->stream2);
@@ -436,7 +444,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
   const size_t o_meta = 0, o_T = al(o_meta + sizeof(ObjMeta) * n_obj), o_code = al(o_T + 64 * n_obj),
                o_pts = al(o_code + 4 * kMaxCode * (size_t)n_obj), o_rays = al(o_pts + 12 * (size_t)tp),
                o_depth = al(o_rays + 12 * (size_t)tr), o_tb = al(o_depth + 4 * (size_t)tf),
-               o_aux = al(o_tb + 3 * 4 * (size_t)n_obj),
+               o_aux = al(o_tb + 2 * 4 * (size_t)n_obj),
                total = al(o_aux + (any_build ? 4 * (size_t)kAuxFloats * n_obj : 0));
   if (s->upload_pending) { CU(cudaEventSynchronize(s->ev_upload)); s->upload_pending = false; }
   if (s->d_stage.cap < total) CU(cudaStreamSynchronize(s->stream));      // kernels of an earlier batch may still read the old block
@@ -451,14 +459,13 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
   int* hTB = reinterpret_cast<int*>(hb + o_tb);
   {
     int acc = 0, mx = 0;
-    long long accr = 0, accq = 0;
+    long long accr = 0;
     int* hTBr = hTB + n_obj;
-    int* hQ0 = hTB + 2 * n_obj;
     for (int o = 0; o < n_obj; ++o) {
       const int nt = (s->h_meta[o].n_pts + kTcRows - 1) / kTcRows;
       const int ntf = (int)(((long long)s->h_meta[o].n_rays * D + kTcRows - 1) / kTcRows);
-      hTB[o] = acc; hTBr[o] = (int)(accr + o); hQ0[o] = (int)accq;
-      acc += nt; accr += ntf; accq += nt + ntf;
+      hTB[o] = acc; hTBr[o] = (int)(accr + o);
+      acc += nt; accr += ntf;
       if (nt > mx) mx = nt;
       if (ntf > mx) mx = ntf;
     }
@@ -511,7 +518,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
   s->d_depth = reinterpret_cast<float*>(db + o_depth);
   s->d_tbase_static = reinterpret_cast<int*>(db + o_tb);
   s->d_tbase_r_static = s->d_tbase_static + n_obj;
-  s->d_q0_render = s->d_tbase_static + 2 * n_obj;
+  s->run_table_valid = false;
   s->n_obj = n_obj; s->tot_pts = (int)tp; s->tot_rays = (int)tr; s->tot_fg = (int)tf; s->tot_smp = ts; s->max_rays = max_rays;
   s->gather.bound_n = -1;
   int bad = 0;
@@ -578,7 +585,7 @@ TermArgs base_term(DspgnSolver* s, int mode) {
   TermArgs a{};
   a.meta = s->d_meta; a.state = s->d_state.as<ObjState>(); a.decs = s->d_decs.as<DecoderDev>();
   a.n_obj = s->n_obj; a.n_classes = (int)s->classes.size(); a.mode = mode;
-  a.pts = s->d_pts; a.pt_active = nullptr; a.pt_active_out = nullptr; a.cut_iter = -1; a.rays = s->d_rays;
+  a.pts = s->d_pts; a.pt_active = nullptr; a.cut_iter = -1; a.iter = 0; a.rays = s->d_rays;
   a.band_x = s->d_bx.as<float>(); a.band_s = s->d_bs.as<float>(); a.band_r = s->d_br.as<float>();
   a.band_m = s->d_m.as<int>(); a.sdf_out = s->d_sdf.as<float>(); a.V_count = s->d_V.as<int>();
   a.part = (mode == MODE_BAND) ? s->d_part_r.as<float>() : (mode == MODE_SDF ? s->d_part_s.as<float>() : nullptr);
@@ -590,24 +597,81 @@ TermArgs base_term(DspgnSolver* s, int mode) {
   return a;
 }
 
-int launch_init(DspgnSolver* s, int pose_only, bool mega = false, bool render = false) {
+// What a run does with the resident batch, given one mode per object: iteration counts and row counters per mode, and
+// the work queue of the persistent kernel (capacity, iteration-0 slots).  A uniform mode array is dspgn_run_batch(s, m).
+struct RunPlan {
+  int iters[2];            // GN iterations of a joint / pose-only object
+  bool any[2];             // the run has objects of this mode
+  bool render;             // the joint objects run the render term
+  long long pts[2];        // surface points of the objects of each mode
+  long long smp_joint;     // ray samples (n_rays x D) of the joint objects
+  long long q_cap;         // persistent kernel: work items that can ever be pushed
+  int total0;              // persistent kernel: iteration-0 queue slots (k_init seeds them)
+};
+
+// Checks the modes, fills the plan and stages the per-run object table (modes | first iteration-0 queue slot of each
+// object) into d_run, async on the stream; `unlimited`: objects never finish (the debug hooks advance the batch freely).
+int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = false) {
+  const DspgnConfig& c = s->cfg;
+  const int n = s->n_obj, D = c.num_depth_samples;
+  p = RunPlan{};
+  for (int o = 0; o < n; ++o) {
+    if (modes[o] != DSPGN_MODE_JOINT && modes[o] != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
+    p.any[modes[o]] = true;
+  }
+  if (p.any[DSPGN_MODE_POSE] && c.pose_only_iterations < 1) return fail(DSPGN_E_ARG, "pose_only_iterations must be >= 1");
+  p.iters[DSPGN_MODE_JOINT] = unlimited ? (1 << 30) : c.num_iterations;
+  p.iters[DSPGN_MODE_POSE] = unlimited ? (1 << 30) : c.pose_only_iterations;
+  p.render = p.any[DSPGN_MODE_JOINT] && !c.sdf_only;
+  if (s->run_upload_pending) { CU(cudaEventSynchronize(s->ev_run_upload)); s->run_upload_pending = false; }
+  const size_t bytes = 8 * (size_t)n;
+  const bool same = s->run_table_valid && memcmp(s->h_run.p, modes, 4 * (size_t)n) == 0;
+  if (!same) {
+    if (s->d_run.cap < bytes) CU(cudaStreamSynchronize(s->stream));      // kernels of an earlier run may still read it
+    if (s->h_run.reserve(bytes) || s->d_run.reserve(bytes)) return fail(DSPGN_E_ALLOC, "run table allocation failed");
+  }
+  int* h = s->h_run.as<int>();
+  for (int o = 0; o < n; ++o) {
+    const ObjMeta& M = s->h_meta[o];
+    const int m = modes[o];
+    const bool r = p.render && m == DSPGN_MODE_JOINT;
+    const long long ntS = (M.n_pts + kTcRows - 1) / kTcRows, ntF = ((long long)M.n_rays * D + kTcRows - 1) / kTcRows;
+    p.pts[m] += M.n_pts;
+    if (m == DSPGN_MODE_JOINT) p.smp_joint += (long long)M.n_rays * D;
+    // per iteration: every SDF tile, every ray-sample tile, one scan item per 64 rays and at most as many band tiles
+    // as ray-sample tiles (iteration 0 reserves every ray-sample tile of the object)
+    p.q_cap += (long long)p.iters[m] * (ntS + (r ? 2 * ntF + (M.n_rays + kScanChunkRays - 1) / kScanChunkRays : 0));
+    if (!same) { h[o] = m; h[n + o] = p.total0; }
+    p.total0 += (int)(ntS + (r ? ntF : 0));
+  }
+  if (!same) {
+    CU(cudaMemcpyAsync(s->d_run.p, h, bytes, cudaMemcpyHostToDevice, s->stream));
+    CU(cudaEventRecord(s->ev_run_upload, s->stream));
+    s->run_upload_pending = true;
+    s->run_table_valid = true;
+  }
+  return 0;
+}
+
+int launch_init(DspgnSolver* s, const RunPlan& p, bool mega = false) {
   InitArgs ia{};
   ia.meta = s->d_meta; ia.state = s->d_state.as<ObjState>(); ia.T_init = s->d_Tinit; ia.code_init = s->d_code;
   ia.V_count = s->d_V.as<int>(); ia.band_m = s->d_m.as<int>();
-  ia.pt_active = nullptr; ia.n_obj = s->n_obj; ia.code_len = s->cfg.code_len; ia.D = s->cfg.num_depth_samples;
-  ia.pose_only = pose_only;
+  ia.n_obj = s->n_obj; ia.code_len = s->cfg.code_len; ia.D = s->cfg.num_depth_samples;
+  ia.modes = s->d_run.as<int>(); ia.n_iter_joint = p.iters[DSPGN_MODE_JOINT]; ia.n_iter_pose = p.iters[DSPGN_MODE_POSE];
   ia.gather = s->gdev; ia.results = s->d_results.as<float>(); ia.n_bad = s->n_bad;
   ia.decs = s->d_decs.as<DecoderDev>();
   ia.mega = mega ? 1 : 0;
   if (mega) {
+    const bool render = p.render;
     ia.render = render ? 1 : 0;
-    ia.q0_off = render ? s->d_q0_render : s->d_tbase_static; ia.tile_rows = kTcRows;
+    ia.q0_off = s->d_run.as<int>() + s->n_obj; ia.tile_rows = kTcRows;
     ia.q_flag = s->d_q_flag.as<int>();
     ia.q_head = s->d_q_ctr.as<int>(); ia.q_tail = s->d_q_ctr.as<int>() + 32; ia.done_objects = s->d_q_ctr.as<int>() + 64;
     ia.band_rows_total = s->d_q_ctr.as<int>() + 80; ia.abort_flag = s->d_q_ctr.as<int>() + 96;
     ia.pending = s->d_tiles_left.as<int>(); ia.ray_left = s->d_tiles_left.as<int>() + s->n_obj;
     ia.obj_iter = s->d_obj_iter.as<int>();
-    ia.total_tiles0 = s->total_tiles128 + (render ? (int)s->total_ray_tiles128 : 0);
+    ia.total_tiles0 = p.total0;
     ia.vpre_exact = s->vpre_exact ? 1 : 0;
     ia.rays = s->d_rays; ia.vpre = (render && s->compact_rays) ? s->d_vpre.as<int>() : nullptr;
     ia.valid_rows_total = reinterpret_cast<unsigned long long*>(s->d_q_ctr.as<int>() + 88);
@@ -629,16 +693,19 @@ ScanArgs base_scan(DspgnSolver* s) {
   return sa;
 }
 
-// one GN iteration's residual-term kernels (everything before the solve)
-int launch_terms(DspgnSolver* s, int pose_only, float* dbg_J, float* dbg_res, int dbg_obj, int iter_index = 0) {
+// one GN iteration's residual-term kernels (everything before the solve); objects past their own last iteration
+// contribute no rows
+int launch_terms(DspgnSolver* s, const RunPlan& p, int iter, float* dbg_J = nullptr, float* dbg_res = nullptr, int dbg_obj = -1,
+                 int dbg_P = 0) {
   const DspgnConfig& c = s->cfg;
-  const bool render = !pose_only && !c.sdf_only;
+  const bool render = p.render && iter < p.iters[DSPGN_MODE_JOINT];
   // The SDF-row pass and the forward-only pass over the ray samples are independent: fork the latter onto a
   // second stream (matters for small batches, where each pass is a single wave of tiles) unless per-launch
   // timing is on.
   const bool fork = render && !s->timing;
   if (render) {
     TermArgs f = base_term(s, MODE_RAYFWD);
+    f.iter = iter;
     if (fork) {
       CU(cudaEventRecord(s->ev_fork, s->stream));
       CU(cudaStreamWaitEvent(s->stream2, s->ev_fork, 0));
@@ -647,19 +714,17 @@ int launch_terms(DspgnSolver* s, int pose_only, float* dbg_J, float* dbg_res, in
     } else {
       if (int rc = launch_term(s, f, s->tot_smp)) return rc;
     }
-    s->ctr.rows_fwd_only += s->tot_smp;
+    s->ctr.rows_fwd_only += p.smp_joint;
   }
   {
     TermArgs a = base_term(s, MODE_SDF);
-    a.huber_b = pose_only ? INFINITY : c.b2;       // optimizer.py:71 uses raw residuals
-    a.pose_only = pose_only;
-    if (pose_only) {                                   // optimizer.py:76-78: inlier cut taken after iteration index 4
-      if (iter_index == 4) a.pt_active_out = s->d_active.as<uint8_t>();
-      if (iter_index > 4) a.pt_active = s->d_active.as<uint8_t>();
-    }
-    a.dbg_J = dbg_J; a.dbg_res = dbg_res; a.dbg_obj = dbg_obj; a.dbg_P = pose_only ? 6 : 7 + c.code_len;
+    a.huber_b = c.b2;                                  // pose-only objects: raw residuals (optimizer.py:71, term_huber)
+    a.iter = iter;
+    a.pt_active = s->d_active.as<uint8_t>(); a.cut_iter = 4;   // optimizer.py:76-78: inlier cut taken after iteration index 4
+    a.dbg_J = dbg_J; a.dbg_res = dbg_res; a.dbg_obj = dbg_obj; a.dbg_P = dbg_P;
     if (int rc = launch_term(s, a, s->tot_pts)) return rc;
-    s->ctr.rows_fwd_bwd += s->tot_pts;
+    for (int m = 0; m < 2; ++m)
+      if (iter < p.iters[m]) s->ctr.rows_fwd_bwd += p.pts[m];
   }
   if (render) {
     if (fork) CU(cudaStreamWaitEvent(s->stream, s->ev_join, 0));
@@ -669,12 +734,13 @@ int launch_terms(DspgnSolver* s, int pose_only, float* dbg_J, float* dbg_res, in
     CU(cudaGetLastError());
     TermArgs b = base_term(s, MODE_BAND);
     b.huber_b = c.b1;
+    b.iter = iter;
     if (int rc = launch_term(s, b, s->tot_smp)) return rc;
   }
   return 0;
 }
 
-SolveArgs base_solve(DspgnSolver* s, int pose_only) {
+SolveArgs base_solve(DspgnSolver* s) {
   const DspgnConfig& c = s->cfg;
   SolveArgs v{};
   v.meta = s->d_meta; v.state = s->d_state.as<ObjState>();
@@ -683,7 +749,7 @@ SolveArgs base_solve(DspgnSolver* s, int pose_only) {
   v.tile_rows = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
   v.V_count = s->d_V.as<int>(); v.band_m = s->d_m.as<int>();
   v.prm = SolverParams{c.k1, c.k2, c.k3, c.k4, c.b1, c.b2, c.lr, c.s_damp, c.code_len, c.num_depth_samples, c.cut_off, c.sdf_only};
-  v.n_obj = s->n_obj; v.pose_only = pose_only; v.results = s->d_results.as<float>();
+  v.n_obj = s->n_obj; v.results = s->d_results.as<float>();
   v.gather = s->gdev;
   v.decs = s->d_decs.as<DecoderDev>();
   v.dbg_obj = -1; v.dbg_H = nullptr; v.dbg_b = nullptr; v.dbg_dx = nullptr; v.dbg_loss = nullptr;
@@ -694,27 +760,25 @@ SolveArgs base_solve(DspgnSolver* s, int pose_only) {
 }  // namespace
 
 namespace {
-int run_batch_impl(DspgnSolver* s, int mode) {
-  if (!s) return fail(DSPGN_E_ARG, "null solver");
-  if (s->n_obj < 1) return fail(DSPGN_E_ARG, "no batch uploaded");
-  if (mode != 0 && mode != 1) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
+// One run of the resident batch, modes[o] = DSPGN_MODE_* of object o.  Every object runs its own mode's iterations,
+// terms and update and finishes after its own last iteration; dspgn_run_batch(s, m) is the uniform case.
+int run_batch_impl(DspgnSolver* s, const int32_t* modes) {
   CU(cudaSetDevice(s->device));
-  const int pose_only = mode;
-  const int iters = pose_only ? s->cfg.pose_only_iterations : s->cfg.num_iterations;
+  RunPlan p;
+  if (int rc = plan_run(s, modes, p)) return rc;
+  const int max_iters = std::max(p.any[DSPGN_MODE_JOINT] ? p.iters[DSPGN_MODE_JOINT] : 0,
+                                 p.any[DSPGN_MODE_POSE] ? p.iters[DSPGN_MODE_POSE] : 0);
   s->ctr = DspgnCounters{};
   s->band_rows_pending = false;
   s->ev_used = 0;
   s->evs_used = 0;
   CU(cudaEventRecord(s->ev_run0, s->stream));
-  const bool render = !pose_only && !s->cfg.sdf_only;
-  // queue capacity: per iteration every SDF tile, every ray-sample tile and at most as many band tiles again
-  const long long items_per_iter = (long long)s->total_tiles128 +
-                                   (render ? 2 * s->total_ray_tiles128 + s->tot_rays / kScanChunkRays + s->n_obj : 0);
+  const bool render = p.render;
   const bool mega = s->mega_enabled && s->engine == DSPGN_ENGINE_TC && s->total_tiles128 > 0 &&
-                    s->max_tiles128 <= kItemTileMask && s->n_obj <= kItemObjMask + 1 && items_per_iter * iters < (1LL << 27);
+                    s->max_tiles128 <= kItemTileMask && s->n_obj <= kItemObjMask + 1 && p.q_cap < (1LL << 27);
   if (mega) {
     // ---- persistent object-pipelined kernel: every GN iteration of every object in ONE launch --------------
-    const int cap = (int)(items_per_iter * iters);
+    const int cap = (int)p.q_cap;
     int bad = 0;
     bad |= s->d_q_flag.reserve(4 * (size_t)cap);
     bad |= s->d_q_ctr.reserve(4 * 128);
@@ -725,17 +789,16 @@ int run_batch_impl(DspgnSolver* s, int mode) {
     bad |= s->d_obj_iter.reserve(4 * (size_t)s->n_obj);
     if (bad) return fail(DSPGN_E_ALLOC, "queue allocation failed");
     CU(cudaMemsetAsync(s->d_q_flag.p, 0, 4 * (size_t)cap, s->stream));
-    if (int rc = launch_init(s, pose_only, true, render)) return rc;
+    if (int rc = launch_init(s, p, true)) return rc;
     TermArgs a = base_term(s, MODE_SDF);
-    a.huber_b = pose_only ? INFINITY : s->cfg.b2;
+    a.huber_b = s->cfg.b2;                   // pose-only objects: raw residuals (term_huber)
     a.huber_b1 = s->cfg.b1;
-    a.pose_only = pose_only;
     a.tile_base = s->d_tbase_static;
     a.part_r = s->d_part_r.as<float>(); a.tile_base_r = s->d_tbase_r_static;
     a.dbg_clk = nullptr;
-    if (pose_only && iters > 5) { a.pt_active_out = s->d_active.as<uint8_t>(); a.cut_iter = 4; }
+    if (p.any[DSPGN_MODE_POSE] && p.iters[DSPGN_MODE_POSE] > 5) { a.pt_active = s->d_active.as<uint8_t>(); a.cut_iter = 4; }
     MegaArgs q{};
-    q.n_iters = iters; q.q_cap = cap; q.render = render ? 1 : 0;
+    q.q_cap = cap; q.render = render ? 1 : 0;
     q.q_flag = s->d_q_flag.as<int>();
     q.q_head = s->d_q_ctr.as<int>(); q.q_tail = s->d_q_ctr.as<int>() + 32; q.done_objects = s->d_q_ctr.as<int>() + 64;
     q.band_rows_total = s->d_q_ctr.as<int>() + 80;
@@ -751,9 +814,9 @@ int run_batch_impl(DspgnSolver* s, int mode) {
       CU(cudaMemsetAsync(s->d_ev.p, 0, 8, s->stream));
       q.ev = s->d_ev.as<long long>(); q.ev_cap = kEvCap;
     }
-    SolveArgs v = base_solve(s, pose_only);
+    SolveArgs v = base_solve(s);
     v.ev = q.ev; v.ev_cap = q.ev_cap;
-    v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.last_iter = 0; v.iter_index = 0; v.dbg_clk = nullptr;
+    v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0; v.dbg_clk = nullptr;
     ScanArgs sa = base_scan(s);
     sa.vpre = q.vpre;
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
@@ -761,18 +824,18 @@ int run_batch_impl(DspgnSolver* s, int mode) {
     else k_gn_persistent<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(a, q, v);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
     s->ctr.kernel_launches += 1;
-    s->ctr.rows_fwd_bwd += (long long)s->tot_pts * iters;
+    for (int m = 0; m < 2; ++m) s->ctr.rows_fwd_bwd += p.pts[m] * p.iters[m];
     s->band_rows_pending = render;           // band rows and valid ray samples are counted by the kernel (dspgn_results)
     s->mega_ran = true;
     CU(cudaGetLastError());
     CU(cudaEventRecord(s->ev_run1, s->stream));
     return 0;
   }
-  if (int rc = launch_init(s, pose_only)) return rc;
-  for (int e = 0; e < iters; ++e) {
-    if (int rc = launch_terms(s, pose_only, nullptr, nullptr, -1, e)) return rc;
-    SolveArgs v = base_solve(s, pose_only);
-    v.last_iter = (e == iters - 1); v.iter_index = e;
+  if (int rc = launch_init(s, p)) return rc;
+  for (int e = 0; e < max_iters; ++e) {
+    if (int rc = launch_terms(s, p, e)) return rc;
+    SolveArgs v = base_solve(s);
+    v.iter_index = e;
     if (s->timing) {
       if (s->evs_used + 2 > s->ev_solve.size()) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); s->ev_solve.push_back(e0); s->ev_solve.push_back(e1); }
       cudaEventRecord(s->ev_solve[s->evs_used], s->stream);
@@ -783,6 +846,29 @@ int run_batch_impl(DspgnSolver* s, int mode) {
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(s->ev_run1, s->stream));
+  return 0;
+}
+
+// dspgn_run_batch / dspgn_run_batch_gather: every object in `mode`
+int run_uniform(DspgnSolver* s, int mode) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  if (s->n_obj < 1) return fail(DSPGN_E_ARG, "no batch uploaded");
+  if (mode != DSPGN_MODE_JOINT && mode != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
+  const std::vector<int32_t> modes(s->n_obj, mode);
+  return run_batch_impl(s, modes.data());
+}
+
+// call-level misuse of the per-object entry points: modes outside {0, 1}; a pose-only object without a code or with
+// scale <= 0 (estimate_pose_cam_obj's arguments, checked like dspgn_estimate_pose_batch does).  The objects are the
+// caller's `in` or, when it is null, the resident batch.
+int check_modes(const DspgnSolver* s, const int32_t* modes, int n, const DspgnObjectIn* in) {
+  for (int o = 0; o < n; ++o) {
+    if (modes[o] != DSPGN_MODE_JOINT && modes[o] != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
+    const bool code = in ? in[o].code != nullptr : s->h_meta[o].has_code != 0;
+    const float scale = in ? in[o].scale : s->h_meta[o].scale;
+    if (modes[o] == DSPGN_MODE_POSE && (!code || !(scale > 0.f)))
+      return fail(DSPGN_E_ARG, "a pose-only object needs a code and a positive scale");
+  }
   return 0;
 }
 
@@ -813,7 +899,15 @@ int gather_layout(DspgnSolver* s, int n_slots, int world, int rank) {
 
 int dspgn_run_batch(DspgnSolver* s, int mode) {
   if (s) s->gdev = GatherDev{};
-  return run_batch_impl(s, mode);
+  return run_uniform(s, mode);
+}
+
+int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes) {
+  if (!s || !modes) return fail(DSPGN_E_ARG, "null argument");
+  if (s->n_obj < 1) return fail(DSPGN_E_ARG, "no batch uploaded");
+  if (int rc = check_modes(s, modes, s->n_obj, nullptr)) return rc;
+  s->gdev = GatherDev{};
+  return run_batch_impl(s, modes);
 }
 
 // ---- multi-GPU result exchange ----------------------------------------------------------------------------------
@@ -893,7 +987,7 @@ int dspgn_run_batch_gather(DspgnSolver* s, int mode, int seq) {
   const GatherDev g = gather_dev(s, seq);
   if (G.bound_n > 0) {
     s->gdev = g;
-    const int rc = run_batch_impl(s, mode);
+    const int rc = run_uniform(s, mode);
     s->gdev = GatherDev{};
     if (rc) return rc;
   }
@@ -1015,6 +1109,19 @@ int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in
   return 0;
 }
 
+int dspgn_keyframe_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, DspgnObjectOut* out) {
+  if (!s || !in || !modes || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
+  if (int rc = check_modes(s, modes, n_obj, in)) return rc;
+  for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
+    const int n = std::min(kMaxObjScan, n_obj - o0);
+    if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
+    s->gdev = GatherDev{};
+    if (int rc = run_batch_impl(s, modes + o0)) return rc;
+    if (int rc = dspgn_results(s, out + o0)) return rc;
+  }
+  return 0;
+}
+
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n, int x_rs, int x_cs,
                      float* sdf_out) {
   if (!s || !code || !x || !sdf_out || n < 1) return fail(DSPGN_E_ARG, "bad argument");
@@ -1029,7 +1136,10 @@ int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const floa
   s->ctr = DspgnCounters{};
   s->ev_used = 0;
   s->gdev = GatherDev{};
-  if (int rc = launch_init(s, 0)) return rc;
+  const int32_t joint = DSPGN_MODE_JOINT;
+  RunPlan p;
+  if (int rc = plan_run(s, &joint, p)) return rc;
+  if (int rc = launch_init(s, p)) return rc;
   TermArgs a = base_term(s, MODE_PTSFWD);
   if (int rc = launch_term(s, a, n)) return rc;
   s->ctr.rows_fwd_only += n;
@@ -1048,9 +1158,12 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
   if (!s || !H || !b || !dx) return fail(DSPGN_E_ARG, "null argument");
   if (obj < 0 || obj >= s->n_obj) return fail(DSPGN_E_ARG, "bad object index");
   if (iter < 0 || iter > 1000) return fail(DSPGN_E_ARG, "bad iteration index");
+  if (mode != DSPGN_MODE_JOINT && mode != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
   CU(cudaSetDevice(s->device));
-  const int pose_only = mode;
-  const int P = pose_only ? 6 : 7 + s->cfg.code_len;
+  const std::vector<int32_t> modes(s->n_obj, mode);
+  RunPlan p;
+  if (int rc = plan_run(s, modes.data(), p, true)) return rc;
+  const int P = (mode == DSPGN_MODE_POSE) ? 6 : 7 + s->cfg.code_len;
   const int npts = s->h_meta[obj].n_pts;
   DevBuf dJ;
   if (dJ.reserve(4 * ((size_t)npts * P + npts))) return fail(DSPGN_E_ALLOC, "cudaMalloc");
@@ -1059,21 +1172,21 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
   s->ctr = DspgnCounters{};
   s->ev_used = 0;
   s->gdev = GatherDev{};
-  int rc = launch_init(s, pose_only);
+  int rc = launch_init(s, p);
   for (int e = 0; e < iter && !rc; ++e) {            // advance the whole batch `iter` GN iterations (per-iteration schedule)
-    rc = launch_terms(s, pose_only, nullptr, nullptr, -1, e);
+    rc = launch_terms(s, p, e);
     if (rc) break;
-    SolveArgs v = base_solve(s, pose_only);
-    v.last_iter = 0; v.iter_index = e;
+    SolveArgs v = base_solve(s);
+    v.iter_index = e;
     k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
     if (cudaGetLastError() != cudaSuccess) rc = fail(DSPGN_E_CUDA, "k_solve launch failed");
   }
-  if (!rc) rc = launch_terms(s, pose_only, dJp, dres, obj, iter);
+  if (!rc) rc = launch_terms(s, p, iter, dJp, dres, obj, P);
   if (!rc) {
-    SolveArgs v = base_solve(s, pose_only);
+    SolveArgs v = base_solve(s);
     float* d = s->d_dbg.as<float>();
     v.dbg_obj = obj; v.dbg_H = d; v.dbg_b = d + kPMax * kPMax; v.dbg_dx = v.dbg_b + kPMax; v.dbg_loss = v.dbg_dx + kPMax;
-    v.last_iter = 0; v.iter_index = iter;
+    v.iter_index = iter;
     cudaMemsetAsync(d, 0, 4 * ((size_t)kPMax * kPMax + 2 * kPMax + 8), s->stream);
     k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
     if (cudaGetLastError() != cudaSuccess) rc = fail(DSPGN_E_CUDA, "k_solve launch failed");

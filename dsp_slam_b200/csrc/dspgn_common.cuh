@@ -43,6 +43,8 @@ struct ObjState {
   int iters;
   int V, m;                    // last render counters
   int n_active;                // pose-only inlier count (optimizer.py:76-78)
+  int mode;                    // DSPGN_MODE_JOINT / DSPGN_MODE_POSE, set by k_init for the whole run
+  int n_iter;                  // GN iterations this object runs (num_iterations or pose_only_iterations)
   // layer 0 with the latent part folded: zb0[j] = b0[j] + sum_i W0[j][i] z[i]  (i < latent size), refreshed whenever z
   // changes (k_init, end of the solve step).  The tensor-core engine then needs only the 3 xyz columns of layer 0 per
   // point, which it evaluates on the CUDA cores while building the first GEMM operand.

@@ -43,9 +43,10 @@ struct TermArgs {
   int mode;
   // sources
   const float* pts;          // MODE_SDF: camera-frame points (xyz interleaved)
-  const uint8_t* pt_active;  // optional inlier mask (pose-only, optimizer.py:76-78), may be null
-  uint8_t* pt_active_out;    // when non-null: write |res| <= 0.05 per point (the cut taken after iteration index 4)
-  int cut_iter;              // persistent mode: object iteration at which the cut is recorded (4), -1 = never
+  uint8_t* pt_active;        // inlier mask of the pose-only objects (optimizer.py:76-78), may be null: |res| <= 0.05 per
+                             // point, written while the object runs iteration cut_iter and applied after it
+  int cut_iter;              // object iteration at which the cut is recorded (4), -1 = never
+  int iter;                  // per-iteration schedule: the iteration being evaluated (objects with n_iter <= iter are done)
   const float* rays;         // MODE_RAYFWD
   const float* band_x;       // MODE_BAND: object-frame points xyz interleaved, per-sample capacity
   const float* band_s;       // de_ds per band row
@@ -60,7 +61,6 @@ struct TermArgs {
   float* part_r; const int* tile_base_r; float huber_b1;
   float* ln_scratch;         // SIMT engine, LayerNorm decoders: per-CTA [layer][256][kTP] normalised activations
   int D;
-  int pose_only;             // 1: 6-D se3 Jacobian (no scale column)
   // debug dump of Jacobian rows (external order [pose | code]) for one object
   float* dbg_J; float* dbg_res; int dbg_obj; int dbg_P;
   long long* dbg_clk;         // optional phase timeline of CTA 0 (tensor-core engine)
@@ -78,9 +78,8 @@ __host__ __device__ __forceinline__ int make_item(int kind, int o, int tile) {
 // from host-side upper bounds): consumers skip it.  Never a real item (a scan item's tile index is < 128); + 1 fits an int.
 constexpr int kItemNop = 0x7ffffffe;
 struct MegaArgs {
-  int n_iters;               // GN iterations per object
   int q_cap;                 // total items that can ever be pushed
-  int render;                // 1: joint run with the render term (ray-sample tiles -> per-ray scan -> band tiles)
+  int render;                // 1: the joint objects run the render term (ray-sample tiles -> per-ray scan -> band tiles)
   int* q_flag;               // one word per slot (no wrap-around): 0 = empty, item + 1 = published
   int* q_head; int* q_tail;  // consumer ticket counter / producer reservation counter
   int* pending;              // [n_obj] SDF + band tiles of the object's current iteration still running (+1 while the
@@ -115,10 +114,24 @@ __device__ __forceinline__ void mega_event(const MegaArgs& q, int kind, int mode
 // ---------------------------------------------------------------------------------------------
 // tile scheduling shared by all decoder kernels: rows per object -> tiles, scanned per CTA
 __device__ __forceinline__ int term_rows(const TermArgs& a, int o) {
-  if (a.state[o].status != 0) return 0;
+  const ObjState& st = a.state[o];
+  if (st.status != 0 || a.iter >= st.n_iter) return 0;
   if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) return a.meta[o].n_pts;
+  if (st.mode != DSPGN_MODE_JOINT) return 0;          // pose-only objects have no render term
   if (a.mode == MODE_BAND) return a.band_m[o];
   return a.meta[o].n_rays * a.D;
+}
+
+// SDF rows of a pose-only object: raw residuals (optimizer.py:71), otherwise the term's Huber threshold
+__device__ __forceinline__ float term_huber(const TermArgs& a, int term, int obj_mode, float b) {
+  return (term == MODE_SDF && obj_mode == DSPGN_MODE_POSE) ? INFINITY : b;
+}
+
+// inlier cut of a pose-only object at object iteration `it` (optimizer.py:76-78): the mask it reads / writes, or null
+__device__ __forceinline__ void cut_masks(const TermArgs& a, int obj_mode, int it, const uint8_t*& in, uint8_t*& out) {
+  const bool on = a.pt_active != nullptr && a.cut_iter >= 0 && obj_mode == DSPGN_MODE_POSE;
+  in = (on && it > a.cut_iter) ? a.pt_active : nullptr;
+  out = (on && it == a.cut_iter) ? a.pt_active : nullptr;
 }
 
 // exclusive scan of tiles per object into s_prefix[0..n_obj]; returns total (all threads)
@@ -263,6 +276,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
     const DecoderDev& dec = a.decs[M.class_id];
     const int L = dec.L, in0 = dec.in0, nl = dec.n_lin;
     const int nrows = min(kTP, term_rows(a, o) - row0);
+    const int omode = st.mode;
+    const uint8_t* mask_in; uint8_t* mask_out;
+    cut_masks(a, omode, a.iter, mask_in, mask_out);
 
     // ---- phase 0: points in the object frame, decoder input rows -----------------------------
     if (tid < kTP) {
@@ -272,7 +288,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
         if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) {
           const float* q = a.pts + 3 * (size_t)(M.pts_off + r);
           xform_point(st.T_oc, q[0], q[1], q[2], x, y, z);
-          sc = (a.pt_active == nullptr || a.pt_active[M.pts_off + r]) ? 1.f : 0.f;
+          sc = (mask_in == nullptr || mask_in[M.pts_off + r]) ? 1.f : 0.f;
         } else if (a.mode == MODE_BAND) {
           const size_t s = (size_t)M.smp_off + r;
           x = a.band_x[3 * s]; y = a.band_x[3 * s + 1]; z = a.band_x[3 * s + 2];
@@ -489,19 +505,19 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
       S.act[(kMaxCode + 3) * kTP + p] = y * gz - z * gy;
       S.act[(kMaxCode + 4) * kTP + p] = z * gx - x * gz;
       S.act[(kMaxCode + 5) * kTP + p] = x * gy - y * gx;
-      S.act[(kMaxCode + 6) * kTP + p] = a.pose_only ? 0.f : (gx * x + gy * y + gz * z);
+      S.act[(kMaxCode + 6) * kTP + p] = (omode == DSPGN_MODE_POSE) ? 0.f : (gx * x + gy * y + gz * z);
       S.act[(kMaxCode + 7) * kTP + p] = 0.f;
       float res = (a.mode == MODE_SDF) ? S.yv[p] : S.rr[p];
       const float sc = S.rscale[p];
       if (sc == 0.f && (a.mode == MODE_SDF || p >= nrows)) res = 0.f;
-      if (a.pt_active_out != nullptr && a.mode == MODE_SDF && p < nrows)
-        a.pt_active_out[M.pts_off + row0 + p] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;   // optimizer.py:76-78
+      if (mask_out != nullptr && a.mode == MODE_SDF && p < nrows)
+        mask_out[M.pts_off + row0 + p] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;   // optimizer.py:76-78
       S.yv[p] = res;                                        // raw residual (debug dump)
-      S.rr[p] = huber_weight(fabsf(res), a.huber_b) * res;  // loss_utils.py:250-265
+      S.rr[p] = huber_weight(fabsf(res), term_huber(a, a.mode, omode, a.huber_b)) * res;  // loss_utils.py:250-265
     }
     __syncthreads();
     if (a.dbg_J != nullptr && o == a.dbg_obj && a.mode == MODE_SDF) {
-      const int P = a.dbg_P, npose = a.pose_only ? 6 : 7;
+      const int P = a.dbg_P, npose = (omode == DSPGN_MODE_POSE) ? 6 : 7;
       for (int idx = tid; idx < nrows * P; idx += kThreads) {
         const int p = idx / P, c = idx - p * P;
         const int ci = (c < npose) ? (kMaxCode + c) : (c - npose);

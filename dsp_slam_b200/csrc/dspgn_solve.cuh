@@ -79,12 +79,12 @@ __global__ void k_gather_wait(GatherDev g) {
 
 // Result record of one object (DspgnObjectOut layout): pose back in camera<-object form (optimizer.py:200 / :83-84),
 // code, loss, status, counters; mirrored into rank 0's gather buffer when the exchange is on.
-__device__ inline void write_record(float* results, const GatherDev& g, int o, const ObjState& st, int pose_only, float scale) {
+__device__ inline void write_record(float* results, const GatherDev& g, int o, const ObjState& st, float scale) {
   float* r = results + (size_t)o * DSPGN_RESULT_FLOATS;
   float Toc[12], Tco[12];
   for (int i = 0; i < 12; ++i) Toc[i] = ldv(&st.T_oc[i]);
   inv_affine(Toc, Tco, nullptr);                         // optimizer.py:200 / :83
-  if (pose_only) {                                       // optimizer.py:84: t_cam_obj[:3,:3] /= scale
+  if (st.mode == DSPGN_MODE_POSE) {                      // optimizer.py:84: t_cam_obj[:3,:3] /= scale
     for (int i = 0; i < 3; ++i)
       for (int c = 0; c < 3; ++c) Tco[i * 4 + c] /= scale;
   }
@@ -252,8 +252,9 @@ struct InitArgs {
   const float* code_init;  // [n_obj][64]
   int* V_count;
   int* band_m;
-  uint8_t* pt_active;      // [total_pts] reset to 1 (pose-only mode)
-  int n_obj, code_len, D, pose_only;
+  int n_obj, code_len, D;
+  const int* modes;        // [n_obj] DSPGN_MODE_* of each object for this run
+  int n_iter_joint, n_iter_pose;   // GN iterations of a joint / pose-only object
   // persistent-kernel mode: also seed the work queue with every object's iteration-0 tiles (ray-sample tiles first)
   int mega; int render; const int* q0_off; int tile_rows; int* q_flag; int* q_head; int* q_tail;
   int* pending; int* ray_left; int* obj_iter; int* done_objects; int* band_rows_total; int* abort_flag; int total_tiles0;
@@ -282,19 +283,19 @@ __global__ void k_init(InitArgs a) {
   if (o == 0 && tid == 0) gather_step_begin(a.gather);
   ObjState& st = a.state[o];
   const ObjMeta M = a.meta[o];
-  if (a.pt_active != nullptr)
-    for (int i = tid; i < M.n_pts; i += blockDim.x) a.pt_active[M.pts_off + i] = 1;
+  const int mode = a.modes[o];
   if (tid < kMaxCode) st.z[tid] = (M.has_code && tid < a.code_len) ? a.code_init[o * kMaxCode + tid] : 0.f;
   if (tid == 0) {
     float Tco[12];
     for (int r = 0; r < 3; ++r)
       for (int c = 0; c < 4; ++c) Tco[r * 4 + c] = a.T_init[o * 16 + r * 4 + c];
-    if (a.pose_only)                       // optimizer.py:54: t_cam_obj[:3,:3] *= scale
+    if (mode == DSPGN_MODE_POSE)           // optimizer.py:54: t_cam_obj[:3,:3] *= scale
       for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 3; ++c) Tco[r * 4 + c] *= M.scale;
     inv_affine(Tco, st.T_oc, nullptr);     // optimizer.py:55 / :104
     derive_depth_range(st, a.D);
     st.loss = 0.f; st.status = M.bad ? DSPGN_ST_BAD_INPUT : 0; st.iters = 0; st.V = 0; st.m = 0; st.n_active = M.n_pts;
+    st.mode = mode; st.n_iter = (mode == DSPGN_MODE_POSE) ? a.n_iter_pose : a.n_iter_joint;
     a.V_count[o] = 0;
     a.band_m[o] = 0;
   }
@@ -302,12 +303,13 @@ __global__ void k_init(InitArgs a) {
   refresh_zb0(st, a.decs[M.class_id], tid, blockDim.x);
   if (M.bad) {                               // rejected at upload: no tile, no solve -- its record is final now
     __syncthreads();
-    if (tid == 0) write_record(a.results, a.gather, o, st, a.pose_only, M.scale);
+    if (tid == 0) write_record(a.results, a.gather, o, st, M.scale);
   }
   if (a.mega) {
     const int ntS = (M.n_pts + a.tile_rows - 1) / a.tile_rows;
-    // slots reserved by the host for this object's iteration 0: every ray sample + every SDF tile
-    const int ntF_cap = (a.render && !M.bad) ? (M.n_rays * a.D + a.tile_rows - 1) / a.tile_rows : 0;
+    // slots reserved by the host for this object's iteration 0: every ray sample (joint objects of a run with the render
+    // term) + every SDF tile
+    const int ntF_cap = (a.render && !M.bad && mode == DSPGN_MODE_JOINT) ? (M.n_rays * a.D + a.tile_rows - 1) / a.tile_rows : 0;
     int ntF = ntF_cap;
     if (a.vpre != nullptr && ntF_cap > 0) {
       __shared__ int s_wsum[32];
@@ -337,9 +339,7 @@ struct SolveArgs {
   int* band_m;
   SolverParams prm;
   int n_obj;
-  int pose_only;          // estimate_pose_cam_obj variant
-  int last_iter;          // write the result record
-  int iter_index;
+  int iter_index;         // per-iteration schedule: the iteration being solved (an object's last one writes its record)
   float* results;         // [n_obj][DSPGN_RESULT_FLOATS]
   const DecoderDev* decs; // layer-0 fold (ObjState.zb0) is refreshed when the code changes
   GatherDev gather;       // optional: the record also goes straight into rank 0's HBM (peer store over NVLink)
@@ -370,7 +370,7 @@ __device__ __forceinline__ int ext_to_int(int e, int npose, int L) {
 }
 
 __device__ __forceinline__ void write_result(const SolveArgs& a, int o, const ObjState& st) {
-  write_record(a.results, a.gather, o, st, a.pose_only, a.meta[o].scale);
+  write_record(a.results, a.gather, o, st, a.meta[o].scale);
 }
 
 constexpr int kElimThreads = 96;      // rows 0..70 live in the first three warps
@@ -439,12 +439,13 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   ObjState& st = a.state[o];
   const SolverParams& prm = a.prm;
   const int L = prm.code_len;
-  const int npose = a.pose_only ? 6 : 7;
-  const int P = a.pose_only ? 6 : (7 + L);
+  const bool pose_only = st.mode == DSPGN_MODE_POSE;      // estimate_pose_cam_obj variant
+  const int npose = pose_only ? 6 : 7;
+  const int P = pose_only ? 6 : (7 + L);
 #define SOLVE_CLK(k) do { if (!MEGA && a.dbg_clk != nullptr && o == 0 && tid == 0) a.dbg_clk[k] = clock64(); if (MEGA && tid == 0) solve_event(a, o, k); } while (0)
   SOLVE_CLK(0);
   const bool dbg = (a.dbg_H != nullptr);
-  const bool use_render = !a.pose_only && !prm.sdf_only;
+  const bool use_render = !pose_only && !prm.sdf_only;
   // tile partials of this object, summed in tile order (deterministic), fp64
   const int V = ldv(a.V_count + o), m = use_render ? ldv(a.band_m + o) : 0;
   const int ntS = (a.meta[o].n_pts + a.tile_rows - 1) / a.tile_rows;
@@ -494,7 +495,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   if (tid == 0) {
     s_flag = 0;
     s_rot[0] = s_rot[1] = s_rot[2] = s_rot[3] = 0.f;
-    if (!a.pose_only) {
+    if (!pose_only) {
       // rotation prior (loss.py:155-178): r = 1 - (R_co e_y).n_g, n_g = (0,-1,0)
       float Toc[12], Tco[12];
       double det_oc;
@@ -520,7 +521,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
 
   SOLVE_CLK(2);
   // ---- assemble the lower triangle of H and the b row (optimizer.py:161-184; pose-only: :68-71) ----
-  const double wS = a.pose_only ? 1.0 / nS : (double)prm.k2 / nS;
+  const double wS = pose_only ? 1.0 / nS : (double)prm.k2 / nS;
   const double wR = use_render ? (double)prm.k1 / (double)m : 0.0;
   // Entry e = tid + q*256 of a tile partial: e < kTriInt -> packed upper-triangle element (r, c) of the internal matrix,
   // then the 72 b entries.  Consecutive threads read consecutive floats.  (i, j) = position in the EXTERNAL system
@@ -528,7 +529,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   // (padding column 71, code rows >= code_len, every code row in a pose-only run).
   auto int_to_ext = [&](int r) -> int {
     if (r >= kMaxCode) { const int p = r - kMaxCode; return (p < npose) ? p : -1; }
-    return (!a.pose_only && r < L) ? npose + r : -1;
+    return (!pose_only && r < L) ? npose + r : -1;
   };
   int ei[kMaxEnt], ej[kMaxEnt], eidx[kMaxEnt];
   double accv[kMaxEnt], accr[kMaxEnt];
@@ -588,7 +589,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
     double v;
     if (i < P) {
       v = wS * accv[q] + wR * accr[q];
-      if (a.pose_only) {
+      if (pose_only) {
         if (i == j) v += 1e-2;                                           // optimizer.py:70
       } else {
         if (i == j && i >= 7) v += (double)prm.k3;                       // optimizer.py:170
@@ -603,7 +604,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
       if (dbg && o == a.dbg_obj) { a.dbg_H[i * P + j] = (float)v; a.dbg_H[j * P + i] = (float)v; }
     } else {
       v = -(wS * accv[q] + wR * accr[q]);
-      if (!a.pose_only) {
+      if (!pose_only) {
         if (j >= 7) v -= (double)prm.k3 * (double)ldv(&st.z[j - 7]);     // optimizer.py:172
         if (s_rot[3] != 0.f && (j == 3 || j == 5))                       // optimizer.py:177-179 sign
           v += (double)prm.k4 * (double)(j == 3 ? s_rot[0] : s_rot[1]) * (double)s_rot[2];
@@ -656,9 +657,9 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   }
   // ---- update (optimizer.py:186-192 / :72-74), clear accumulators, next depth range -----------
   const bool fail = (s_flag != 0);
-  if (!a.pose_only && tid < L && !fail) st.z[tid] = ldv(&st.z[tid]) + prm.lr * xs[tid + 7];
+  if (!pose_only && tid < L && !fail) st.z[tid] = ldv(&st.z[tid]) + prm.lr * xs[tid + 7];
   solve_sync<MEGA>();                        // the result record below reads every z entry
-  if (!a.pose_only && !fail && !last_iter) refresh_zb0(st, a.decs[a.meta[o].class_id], tid, kSolveThreads);
+  if (!pose_only && !fail && !last_iter) refresh_zb0(st, a.decs[a.meta[o].class_id], tid, kSolveThreads);
   if (tid == 0) {
     st.loss = loss; st.V = V; st.m = m;
     a.V_count[o] = 0;
@@ -666,10 +667,10 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
       st.status = DSPGN_ST_SOLVE;
     } else {
       float dp[7];
-      for (int i = 0; i < npose; ++i) dp[i] = (a.pose_only ? 1.0f : prm.lr) * xs[i];
+      for (int i = 0; i < npose; ++i) dp[i] = (pose_only ? 1.0f : prm.lr) * xs[i];
       float dT[12], Tn[12], Toc[12];
       for (int i = 0; i < 12; ++i) Toc[i] = ldv(&st.T_oc[i]);
-      exp_sim3_dev(dp, !a.pose_only, dT);
+      exp_sim3_dev(dp, !pose_only, dT);
       mul_affine(dT, Toc, Tn);
       for (int i = 0; i < 12; ++i) st.T_oc[i] = Tn[i];
       derive_depth_range(st, prm.D);
@@ -683,7 +684,9 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
 
 __global__ void __launch_bounds__(kSolveThreads) k_solve(SolveArgs a) {
   __shared__ SolveSmem SM;
-  solve_object<false>(a, blockIdx.x, threadIdx.x, SM, a.last_iter != 0);
+  const int o = blockIdx.x, n_iter = a.state[o].n_iter;
+  if (a.iter_index >= n_iter) return;               // finished after its own last iteration
+  solve_object<false>(a, o, threadIdx.x, SM, a.iter_index + 1 == n_iter);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -942,7 +945,7 @@ __global__ void __launch_bounds__(kScanThreads) k_ray_scan(ScanArgs a) {
   __shared__ int s_cnt[kScanMaxRays];
   __shared__ int s_wsum[32];
   const int o = blockIdx.x;
-  if (a.state[o].status != 0) return;
+  if (a.state[o].status != 0 || a.state[o].mode != DSPGN_MODE_JOINT) return;   // pose-only objects: no render term
   scan_object<false>(a, o, threadIdx.x, kScanThreads, s_cnt, s_wsum);
 }
 

@@ -334,13 +334,14 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
   __threadfence();
   SolveSmem& SM = *reinterpret_cast<SolveSmem*>(S.Jp);
   const int it = ldv(q.obj_iter + o);
+  const bool render = q.render && sv.state[o].mode == DSPGN_MODE_JOINT;     // pose-only objects: SDF tiles only
   if (tid == 0) mega_event(q, EV_SOLVE_BEGIN, 0, o, it);
-  const int fin = solve_object<true>(sv, o, tid, SM, it + 1 >= q.n_iters);
+  const int fin = solve_object<true>(sv, o, tid, SM, it + 1 >= sv.state[o].n_iter);
   epi_bar_sync();
   // ---- the next iteration's ray samples: only the run of samples inside the unit sphere of every ray (new pose and
   // depth range, written by the solve above).  `fin` is the same in every thread (shared-memory flags).
   int vh = -1;
-  if (!fin && q.render && q.vpre != nullptr) {
+  if (!fin && render && q.vpre != nullptr) {
     const ObjMeta M = sv.meta[o];
     if (M.n_rays > 0) vh = valid_sample_ranges<true>(M, sv.state[o], S.ctx_rays, S.ctx_D, q.vpre + vpre_base(M, o), tid, kTcEpiThreads, S.warp_tmp, q.vpre_exact != 0);
   }
@@ -356,7 +357,7 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
       // (no fence in this branch: q_tail only reserves slots; state and counters are fenced below, before any slot is published)
       const ObjMeta M = sv.meta[o];
       const int ntS = (M.n_pts + kTcRows - 1) / kTcRows;
-      const int ntF = q.render ? ((vh >= 0 ? vh : M.n_rays * S.ctx_D) + kTcRows - 1) / kTcRows : 0;
+      const int ntF = render ? ((vh >= 0 ? vh : M.n_rays * S.ctx_D) + kTcRows - 1) / kTcRows : 0;
       *reinterpret_cast<volatile int*>(q.obj_iter + o) = it + 1;
       *reinterpret_cast<volatile int*>(q.pending + o) = ntS + (ntF > 0 ? 1 : 0);
       *reinterpret_cast<volatile int*>(q.ray_left + o) = ntF;
@@ -491,7 +492,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       const bool has_skip = dec.latent_in >= 0;
       const bool fwd_only = (mode == MODE_RAYFWD || mode == MODE_PTSFWD);
       const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
-      const float huber_b = (RENDER && mode == MODE_BAND) ? a.huber_b1 : a.huber_b;
+      const float huber_b = term_huber(a, mode, ost.mode, (RENDER && mode == MODE_BAND) ? a.huber_b1 : a.huber_b);
       float* const part = (RENDER && mode == MODE_BAND) ? a.part_r : a.part;
       // ---- prologue, phase A: everything that comes from global memory, then ONE barrier ------------------------------
       // The pose / depth range of this object may have been rewritten by another CTA's solve: read (cache-bypassing) once
@@ -514,13 +515,8 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       // written after the per-class reload above, read after the barriers below
       S.bias[tid] = ldv(&ost.zb0[tid]);
       // pose-only inlier cut (optimizer.py:76-78): recorded while iteration `cut_iter` runs, applied afterwards
-      const uint8_t* mask_in = a.pt_active;
-      uint8_t* mask_out = a.pt_active_out;
-      if (MEGA && a.cut_iter >= 0) {
-        const int it_now = ldv(q.obj_iter + o);
-        mask_in = (it_now > a.cut_iter) ? a.pt_active_out : nullptr;
-        mask_out = (it_now == a.cut_iter) ? a.pt_active_out : nullptr;
-      }
+      const uint8_t* mask_in; uint8_t* mask_out;
+      cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
       const int* segp = nullptr;
       int nseg = 0;
       const bool compact = RENDER && mode == MODE_RAYFWD && q.vpre != nullptr;
@@ -749,7 +745,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         jr[kMaxCode + 3] = x1 * g2 - x2 * g1;
         jr[kMaxCode + 4] = x2 * g0 - x0 * g2;
         jr[kMaxCode + 5] = x0 * g1 - x1 * g0;
-        jr[kMaxCode + 6] = a.pose_only ? 0.f : (g0 * x0 + g1 * x1 + g2 * x2);
+        jr[kMaxCode + 6] = (ost.mode == DSPGN_MODE_POSE) ? 0.f : (g0 * x0 + g1 * x1 + g2 * x2);
         jr[kMaxCode + 7] = 0.f;
         float res = (mode == MODE_SDF) ? yv : res_in;
         if (sc == 0.f && (mode == MODE_SDF || r >= nrows)) res = 0.f;
@@ -761,7 +757,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       }
       epi_bar_sync();
       if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF) {
-        const int P = a.dbg_P, npose = a.pose_only ? 6 : 7;
+        const int P = a.dbg_P, npose = (ost.mode == DSPGN_MODE_POSE) ? 6 : 7;
         for (int idx = tid; idx < nrows * P; idx += kTcEpiThreads) {
           const int p = idx / P, c = idx - p * P;
           const int ci = (c < npose) ? (kMaxCode + c) : (c - npose);

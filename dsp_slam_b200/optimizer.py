@@ -216,6 +216,13 @@ class BatchSolver:
     def run(self, mode=0):
         _lib.check(_lib.load().dspgn_run_batch(self.handle, mode))
 
+    def run_modes(self, modes):
+        """Run the resident batch with one mode per object (_lib.MODE_JOINT / MODE_POSE)."""
+        m = _modes_array(modes)
+        if len(m) != self.n_obj:
+            raise ValueError(f"{len(m)} modes for {self.n_obj} resident objects")
+        _lib.check(_lib.load().dspgn_run_batch_modes(self.handle, m))
+
     def synchronize(self):
         _lib.check(_lib.load().dspgn_solver_sync(self.handle))
 
@@ -246,6 +253,17 @@ class BatchSolver:
         arr, keep = self._pack(objs)
         out = (_lib.ObjectOut * len(objs))()
         _lib.check(_lib.load().dspgn_estimate_pose_batch(self.handle, len(objs), arr, out))
+        self.n_obj = len(objs)
+        return out
+
+    def keyframe(self, objs, modes):
+        """Joint and pose-only objects in one call: modes[i] = _lib.MODE_JOINT (reconstruct) or MODE_POSE (estimate_pose)."""
+        m = _modes_array(modes)
+        if len(m) != len(objs):
+            raise ValueError(f"{len(m)} modes for {len(objs)} objects")
+        arr, keep = self._pack(objs)
+        out = (_lib.ObjectOut * len(objs))()
+        _lib.check(_lib.load().dspgn_keyframe_batch(self.handle, len(objs), arr, m, out))
         self.n_obj = len(objs)
         return out
 
@@ -282,6 +300,10 @@ class BatchSolver:
             self.close()
         except Exception:
             pass
+
+
+def _modes_array(modes):
+    return (C.c_int32 * len(modes))(*[int(m) for m in modes])
 
 
 def _records(out, n):
@@ -404,6 +426,25 @@ class Optimizer(object):
             Ts.append(np.array(out[i].t_cam_obj[:], dtype=np.float32).reshape(4, 4) if s == _lib.ST_OK
                       else np.array(o["t_cam_obj"], dtype=np.float32).reshape(4, 4))
         return (Ts, st) if return_status else Ts
+
+    def keyframe_batch(self, new_objects, tracked_objects, return_status=False):
+        """The stereo keyframe's two passes (src/LocalMapping.cc:88-95) as ONE library call: reconstruct_batch(new_objects)
+        (CreateNewMapObjects) and estimate_pose_batch(tracked_objects) (GetNewObservations; dicts with t_cam_obj, pts,
+        code, scale).  Returns (results, poses) or (results, poses, status) with exactly the values of those two calls:
+        a failed pose comes back as the input pose."""
+        objs = list(new_objects) + list(tracked_objects)
+        n_new = len(new_objects)
+        if not objs:
+            return ([], [], []) if return_status else ([], [])
+        out = self.solver.keyframe(objs, [_lib.MODE_JOINT] * n_new + [_lib.MODE_POSE] * (len(objs) - n_new))
+        results = _unpack_all(out, n_new, self.code_len) if n_new else []
+        Ts, st = [], []
+        for i, o in enumerate(tracked_objects):
+            s = int(out[n_new + i].status)
+            st.append(s)
+            Ts.append(np.array(out[n_new + i].t_cam_obj[:], dtype=np.float32).reshape(4, 4) if s == _lib.ST_OK
+                      else np.array(o["t_cam_obj"], dtype=np.float32).reshape(4, 4))
+        return (results, Ts, st) if return_status else (results, Ts)
 
 
 def create_voxel_grid(vol_dim=128):

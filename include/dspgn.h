@@ -174,6 +174,19 @@ int dspgn_run_batch(DspgnSolver* s, int mode);
 int dspgn_results(DspgnSolver* s, DspgnObjectOut* out);
 const float* dspgn_results_device(DspgnSolver* s);
 
+/* Per-object run modes: one keyframe's tracked objects (estimate_pose_cam_obj, src/LocalMapping_util.cc:109) and new
+ * objects (reconstruct_object, :179) in ONE run.  Every object gets exactly the record the single-mode entry point for
+ * its mode writes (pose-only objects: no render term, their rays are ignored; pose_only_iterations iterations).
+ * dspgn_run_batch(s, m) is the same run with every mode = m.  A mode outside {0, 1}, or a pose-only object without a
+ * code or with scale <= 0, returns DSPGN_E_ARG before anything is enqueued; unusable detections stay per-object
+ * DSPGN_ST_BAD_INPUT.  The multi-GPU exchange (dspgn_run_batch_gather) stays single-mode. */
+#define DSPGN_MODE_JOINT 0   /* reconstruct_object */
+#define DSPGN_MODE_POSE 1    /* estimate_pose_cam_obj */
+/* resident batch: modes[i] for uploaded object i (host array of n_obj entries) */
+int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes);
+/* whole call: upload + run + results, walked in resident chunks of 1024 like dspgn_reconstruct_batch */
+int dspgn_keyframe_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, DspgnObjectOut* out);
+
 /* Forward-only decode (loss_utils.decode_sdf): x (n,3) host, strides in elements -> sdf (n,) host. */
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n,
                      int x_rs, int x_cs, float* sdf_out);

@@ -1,5 +1,5 @@
 """Event timeline of the persistent kernel (env DSPGN_CLK): where one GN iteration of one object spends its time.
-   python tools/mega_timeline.py [slam1|cfg3|cfg2_sdf|cfg2_full]   (on an H100)"""
+   python tools/mega_timeline.py [slam1|cfg3|cfg2_sdf|cfg2_full|keyframe]   (on an H100)"""
 import os, sys, ctypes as C
 os.environ["DSPGN_CLK"] = "1"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -10,12 +10,19 @@ from dsp_slam_b200 import _lib
 from dsp_slam_b200.optimizer import Optimizer
 
 wl = sys.argv[1] if len(sys.argv) > 1 else "slam1"
-B, M, nfg, nbg, cls, cfgname, sdf_only, desc = bench.WORKLOADS[wl]
-cfg, ins, clss, sdf_only = bench.make_inputs(wl, 1)
+if wl == "keyframe":                # tracked objects pose-only + new objects joint, one run (tools/keyframe_bench.py)
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    import keyframe_bench
+    cfg, ins, modes = keyframe_bench.keyframe_inputs()
+    cls, sdf_only = "cars", False
+else:
+    B, M, nfg, nbg, cls, cfgname, sdf_only, desc = bench.WORKLOADS[wl]
+    cfg, ins, clss, sdf_only = bench.make_inputs(wl, 1)
+    modes = [0] * len(ins)
 opt = Optimizer(os.path.join(ROOT, "tests", "golden", f"decoder_{cls}.npz"), cfg, sdf_only=sdf_only, engine="tc")
 opt.solver.upload(ins)
 for _ in range(3):
-    opt.solver.run(0); opt.solver.results_raw()
+    opt.solver.run_modes(modes); opt.solver.results_raw()
 cap = 1 << 18
 buf = (C.c_longlong * (2 * cap))()
 n = _lib.load().dspgn_debug_events(opt.solver.handle, buf, cap)
@@ -26,6 +33,11 @@ kind, mode, sm, o, tile = d >> 56, (d >> 52) & 15, (d >> 40) & 4095, (d >> 24) &
 K = ["tile_begin", "tile_end", "scan_begin", "scan_end", "solve_begin", "solve_end", "popped", "first_mma"]
 MODE = {0: "SDF", 1: "BAND", 2: "RAY", 3: "SCAN"}
 print(f"{wl}: {n} events, kernel span {t.max() / 1e3:.1f} us")
+for m_, name in ((1, "pose-only"), (0, "joint")):
+    objs_m = [i for i, x in enumerate(modes) if x == m_]
+    if objs_m:
+        fin = t[(kind == 5) & np.isin(o, objs_m)]
+        print(f"{name} objects ({len(objs_m)}): last solve ends at {fin.max() / 1e3:.1f} us")
 obj = 0
 sel = o == obj
 sb, se = np.sort(t[sel & (kind == 4)]), np.sort(t[sel & (kind == 5)])
