@@ -10,6 +10,11 @@ CUDA path.  Run in the authoring container only:
 
 Writes stages.npz (single-stage inputs/outputs at a fixed state) and recon_*.npz (whole GN runs,
 with the 71x71 system of every iteration captured by wrapping torch.mv).
+
+    python tests/golden/make_golden.py --states
+
+re-runs every whole-run golden from its stored inputs, asserts that the reference reproduces it bit for bit, and writes
+states_*.npz (the reference's state at every iteration) and pose_only_cut.npz for the teacher-forced tests.
 """
 import os
 import sys
@@ -103,17 +108,64 @@ class RenderRecorder:
         ns.optimizer.compute_render_loss = self._crl
 
 
+class StateRecorder:
+    """The state the reference's loop starts each iteration from, captured without touching the reference: the
+    t_obj_cam and latent_vector handed to compute_sdf_loss (optimizer.py:62-65,129; cloned, because the code is
+    updated in place), the number of surface points, the SDF residuals, and the loss of every get_robust_res call
+    (sdf then render in reconstruct_object, sdf only in estimate_pose_cam_obj)."""
+
+    def __enter__(self):
+        self.Toc, self.z, self.n_pts, self.res, self.losses = [], [], [], [], []
+        self._csl = ns.optimizer.compute_sdf_loss
+        self._grr = ns.optimizer.get_robust_res
+        rec = self
+
+        def csl(decoder, pts, t_obj_cam, latent, *a, **k):
+            rec.Toc.append(t_obj_cam.detach().clone().numpy())
+            rec.z.append(latent.detach().clone().numpy())
+            rec.n_pts.append(int(pts.shape[0]))
+            r = rec._csl(decoder, pts, t_obj_cam, latent, *a, **k)
+            rec.res.append(None if r is None else r[2].detach().reshape(-1).clone().numpy())
+            return r
+
+        def grr(res, b, *a, **k):
+            r = rec._grr(res, b, *a, **k)
+            rec.losses.append(np.float32(r[1].item()))
+            return r
+
+        ns.optimizer.compute_sdf_loss = csl
+        ns.optimizer.get_robust_res = grr
+        return self
+
+    def __exit__(self, *a):
+        ns.optimizer.compute_sdf_loss = self._csl
+        ns.optimizer.get_robust_res = self._grr
+
+
 def np_f(x):
     return np.asfortranarray(np.array(x, dtype=np.float32))
 
 
-def run_reconstruct(dec, cfg, obj, with_code=False):
+def run_reconstruct(dec, cfg, obj, with_code=False, states=None):
+    """One reference reconstruct_object run with its per-iteration systems.  With states={} the per-iteration
+    state is also captured into that dict (StateRecorder), plus the final state after the last update."""
     opt = ns.optimizer.Optimizer(dec, cfg)
     code = None if not with_code else np.array(obj["code_init"], dtype=np.float32)
-    with SolveRecorder() as rec, RenderRecorder() as rr:
+    with SolveRecorder() as rec, RenderRecorder() as rr, StateRecorder() as sr:
         out = opt.reconstruct_object(np_f(obj["t_cam_obj_init"]), np_f(obj["pts"]),
                                      np_f(obj["rays"]), np.array(obj["depth"], dtype=np.float32),
                                      code)
+    if states is not None:
+        n = len(rec.dx)
+        assert out.is_good and len(sr.Toc) == n and len(sr.losses) == 2 * n
+        # the update the reference applies after its last solve (optimizer.py:187-192), with its own functions
+        dx = torch.from_numpy(rec.dx[-1])
+        Toc_end = torch.mm(ns.loss_utils.exp_sim3(opt.lr * dx[:7]), torch.from_numpy(sr.Toc[-1]))
+        assert np.array_equal(torch.inverse(Toc_end).numpy(), out.t_cam_obj)
+        states.update(Toc_iters=np.stack(sr.Toc + [Toc_end.numpy()]),
+                      z_iters=np.stack(sr.z + [np.asarray(out.code)]),
+                      sdf_loss_iters=np.array(sr.losses[0::2], np.float32),
+                      render_loss_iters=np.array(sr.losses[1::2], np.float32))
     res = dict(is_good=np.array(bool(out.is_good)), loss=np.array(float(out.loss), dtype=np.float32))
     if out.is_good:
         res["t_cam_obj"] = np.ascontiguousarray(out.t_cam_obj)
@@ -135,9 +187,10 @@ def pack_inputs(obj, with_code=False):
     return d
 
 
-def sdf_only_composed(dec, cfg, obj):
+def sdf_only_composed(dec, cfg, obj, states=None):
     """optimizer.py:118-192 with the render block removed, built from the reference's own
-    functions (BASELINE config 2 'surface-SDF loss' mode; SURVEY.md 8d)."""
+    functions (BASELINE config 2 'surface-SDF loss' mode; SURVEY.md 8d).  states={} also captures
+    the state of every iteration, as run_reconstruct does."""
     lu, lo = ns.loss_utils, ns.loss
     o = cfg.optimizer
     j = o.joint_optim
@@ -146,10 +199,13 @@ def sdf_only_composed(dec, cfg, obj):
     t_obj_cam = torch.inverse(torch.from_numpy(np.array(obj["t_cam_obj_init"])))
     pts = torch.from_numpy(np.ascontiguousarray(obj["pts"]))
     Hs, bs, dxs = [], [], []
+    Tocs, zs, sdf_losses = [], [], []
     loss = 0.0
     for _ in range(j.num_iterations):
+        Tocs.append(t_obj_cam.clone().numpy()); zs.append(z.clone().numpy())
         jt, jc, res = lo.compute_sdf_loss(dec, pts, t_obj_cam, z)
         rr, sdf_loss, _ = lu.get_robust_res(res, j.b2)
+        sdf_losses.append(np.float32(sdf_loss.item()))
         drot, res_rot = lo.compute_rotation_loss_sim3(t_obj_cam)
         loss = j.k2 * sdf_loss
         J = torch.cat([jt, jc], dim=-1)
@@ -167,6 +223,10 @@ def sdf_only_composed(dec, cfg, obj):
         Hs.append(H.clone().numpy()); bs.append(b.clone().numpy()); dxs.append(dx.clone().numpy())
         t_obj_cam = torch.mm(lu.exp_sim3(j.learning_rate * dx[:7]), t_obj_cam)
         z = z + j.learning_rate * dx[7:7 + L]
+    if states is not None:
+        states.update(Toc_iters=np.stack(Tocs + [t_obj_cam.numpy()]), z_iters=np.stack(zs + [z.numpy()]),
+                      sdf_loss_iters=np.array(sdf_losses, np.float32),
+                      render_loss_iters=np.zeros(len(sdf_losses), np.float32))
     return dict(t_cam_obj=torch.inverse(t_obj_cam).numpy(), code=z.numpy(),
                 loss=np.array(float(loss), dtype=np.float32), is_good=np.array(True),
                 H_iters=np.stack(Hs), b_iters=np.stack(bs), dx_iters=np.stack(dxs))
@@ -353,15 +413,93 @@ HYPER = dict(num_depth_samples=24, cut_off_threshold=0.02,
                               num_iterations=6))
 
 
-def hyper_golden():
-    """A whole run with EVERY hyper-parameter of the `optimizer` block moved off the shipped configs' values (D = 24
-    depth samples instead of 50, band half-width, all weights, both Huber thresholds, learning rate, scale damping,
-    iteration count): pins that the restatement reads each of them where the reference does."""
+def hyper_cfg():
     cfg = ref_harness.load_config("config_kitti.json")
     cfg.optimizer.num_depth_samples = HYPER["num_depth_samples"]
     cfg.optimizer.cut_off_threshold = HYPER["cut_off_threshold"]
     for k, v in HYPER["joint_optim"].items():
         cfg.optimizer.joint_optim[k] = v
+    return cfg
+
+
+def pose_only_cut_golden(cars):
+    """estimate_pose_cam_obj (optimizer.py:45-86) for 8 iterations on a 300-point car with 10 % gross outliers, so that
+    the inlier cut after iteration index 4 (:76-78) removes points: the 6x6 system and the state of every iteration,
+    the inlier mask the reference applies and the final pose."""
+    cfg = cfg_with("config_kitti.json")
+    cfg.optimizer.pose_only_optim.num_iterations = 8
+    o = synth.make_object(41, 300)
+    pts = np.array(o["pts"], dtype=np.float32)
+    rng = np.random.default_rng(41)
+    bad = rng.choice(300, 30, replace=False)
+    pts[bad] += rng.normal(0, 0.6, size=(30, 3)).astype(np.float32)
+    T = np.array(o["t_cam_obj_init"], dtype=np.float32)
+    s = np.float32(np.cbrt(np.linalg.det(T[:3, :3].astype(np.float64))))
+    se3 = T.copy(); se3[:3, :3] /= s
+    code = (0.8 * o["code_gt"]).astype(np.float32)
+    opt = ns.optimizer.Optimizer(cars, cfg)
+    with SolveRecorder() as rec, StateRecorder() as sr:
+        Tout = opt.estimate_pose_cam_obj(se3.copy(), float(s), np_f(pts), code.copy()).numpy()
+    assert len(rec.dx) == len(sr.Toc) == 8 and sr.n_pts[:5] == [300] * 5
+    mask = np.abs(sr.res[4]) <= 0.05
+    assert sr.n_pts[5:] == [int(mask.sum())] * 3 and mask.sum() < 300
+    Toc_end = torch.mm(ns.loss_utils.exp_se3(torch.from_numpy(rec.dx[-1])), torch.from_numpy(sr.Toc[-1]))
+    T_end = torch.inverse(Toc_end)
+    T_end[:3, :3] /= float(s)
+    assert np.array_equal(T_end.numpy(), Tout)
+    np.savez_compressed(os.path.join(HERE, "pose_only_cut.npz"), in_t_co_se3=se3, in_scale=s, in_pts=pts, in_code=code,
+                        H_iters=np.stack(rec.H), b_iters=np.stack(rec.b), dx_iters=np.stack(rec.dx),
+                        Toc_iters=np.stack(sr.Toc + [Toc_end.numpy()]), sdf_loss_iters=np.array(sr.losses, np.float32),
+                        inlier_mask=mask, t_cam_obj=Tout)
+    print("pose_only_cut.npz written:", int(mask.sum()), "inliers")
+
+
+def states_golden():
+    """Re-runs every whole-run golden from its stored inputs, asserts that the reference reproduces the committed
+    arrays bit for bit, and writes states_<name>.npz with the reference's state at every iteration:
+    Toc_iters (iters+1, 4, 4) = t_obj_cam before each update and after the last one, z_iters (iters+1, L),
+    sdf_loss_iters and render_loss_iters (iters,).  Teacher-forced tests start one step from each of these states."""
+    cars, chairs = load_ref_decoder("cars"), load_ref_decoder("chairs")
+    cfgk = cfg_with("config_kitti.json")
+    cfg3 = cfg_with("config_redwood_01053.json", num_iterations=10)
+    runs = [("recon_cfg1", cars, cfg_with("config_kitti.json", num_iterations=5), False),
+            ("recon_kitti250", cars, cfgk, False), ("recon_cfg2full", cars, cfgk, False),
+            ("recon_cfg3", chairs, cfg3, True), ("recon_cfg3_b8", chairs, cfg3, True),
+            ("recon_hyper", cars, hyper_cfg(), False), ("recon_sdf_only", cars, cfgk, False)]
+    for name, dec, cfg, with_code in runs:
+        d = np.load(os.path.join(HERE, name + ".npz"))
+        if name == "recon_hyper":
+            assert json.loads(bytes(d["hyper_json"]).decode()) == HYPER
+        stacked = d["in_pts"].ndim == 3
+        n = d["in_pts"].shape[0] if stacked else 1
+        per_res, per_st = [], []
+        for i in range(n):
+            g = (lambda k: d[k][i]) if stacked else (lambda k: d[k])
+            o = dict(t_cam_obj_init=g("in_t_cam_obj"), pts=g("in_pts"))
+            st = {}
+            if name == "recon_sdf_only":
+                per_res.append(sdf_only_composed(dec, cfg, o, states=st))
+            else:
+                o.update(rays=g("in_rays"), depth=g("in_depth"))
+                if with_code:
+                    o["code_init"] = g("in_code")
+                per_res.append(run_reconstruct(dec, cfg, o, with_code, states=st))
+            per_st.append(st)
+        for k in ("H_iters", "b_iters", "dx_iters", "V_iters", "m_iters", "t_cam_obj", "code", "is_good", "loss"):
+            if k in d.files:
+                got = np.stack([r[k] for r in per_res]) if stacked else per_res[0][k]
+                assert got.dtype == d[k].dtype and np.array_equal(got, d[k]), (name, k)
+        out = {k: np.stack([s[k] for s in per_st]) if stacked else per_st[0][k] for k in per_st[0]}
+        np.savez_compressed(os.path.join(HERE, "states_" + name[len("recon_"):] + ".npz"), **out)
+        print(f"states_{name[len('recon_'):]}.npz: bit-identical re-run, {out['Toc_iters'].shape}")
+    pose_only_cut_golden(cars)
+
+
+def hyper_golden():
+    """A whole run with EVERY hyper-parameter of the `optimizer` block moved off the shipped configs' values (D = 24
+    depth samples instead of 50, band half-width, all weights, both Huber thresholds, learning rate, scale damping,
+    iteration count): pins that the restatement reads each of them where the reference does."""
+    cfg = hyper_cfg()
     cars = load_ref_decoder("cars")
     o = synth.make_object(11, 400, 300, 100)
     a = np.deg2rad(3.0)                              # tilted 3 degrees about the object's own x axis: the rotation prior is active
@@ -379,6 +517,8 @@ if __name__ == "__main__":
         variant_golden()
     elif "--hyper-only" in sys.argv:
         hyper_golden()
+    elif "--states" in sys.argv:
+        states_golden()
     else:
         main()
         voxel_golden()

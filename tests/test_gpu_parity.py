@@ -7,9 +7,13 @@ split-fp16), dx abs 2e-4;  whole runs: |dT| 3e-2, |dcode| 1.5e-2 with the render
 band flips), |dT| 3e-3 / |dcode| 1e-3 for SDF-only runs; identical is_good everywhere.
 """
 import os
+import sys
 
 import numpy as np
 import pytest
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import teacher_states as TS  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -90,6 +94,7 @@ RUNS = [  # file, decoder, config, iters, with_code, sdf_only, tol_T, tol_code
     ("recon_kitti250", "cars", "kitti", 10, False, False, 3e-2, 1.5e-2),
     ("recon_cfg3", "chairs", "redwood", 10, True, False, 3e-2, 1e-2),
     ("recon_sdf_only", "cars", "kitti", 10, False, True, 3e-3, 1e-3),
+    ("recon_hyper", "cars", "hyper", 6, False, False, 3e-2, 1.5e-2),
 ]
 
 
@@ -97,10 +102,8 @@ RUNS = [  # file, decoder, config, iters, with_code, sdf_only, tol_T, tol_code
 @pytest.mark.parametrize("name,dec,cfgname,iters,with_code,sdf_only,tol_T,tol_code", RUNS)
 def test_whole_runs_vs_reference_goldens(engine, golden_dir, dec_path, cfg_kitti, cfg_redwood, name, dec, cfgname,
                                          iters, with_code, sdf_only, tol_T, tol_code):
-    import copy
     d = np.load(os.path.join(golden_dir, name + ".npz"))
-    cfg = copy.deepcopy(cfg_kitti if cfgname == "kitti" else cfg_redwood)
-    cfg["optimizer"]["joint_optim"]["num_iterations"] = iters
+    cfg = TS.run_cfg(cfgname, iters, cfg_kitti, cfg_redwood, d)
     opt = _engine_or_skip(engine, dec_path[dec], cfg, sdf_only=sdf_only)
     code = d["in_code"] if with_code else None
     if sdf_only:
@@ -409,6 +412,7 @@ ITER_RUNS = [  # file, decoder, config, iters, with_code, object index (stacked 
     ("recon_cfg3", "chairs", "redwood", 10, True, None),
     ("recon_cfg3_b8", "chairs", "redwood", 10, True, 0),
     ("recon_cfg3_b8", "chairs", "redwood", 10, True, 5),
+    ("recon_hyper", "cars", "hyper", 6, False, None),
 ]
 
 
@@ -433,11 +437,9 @@ def test_iteration_by_iteration_vs_reference(engine, golden_dir, dec_path, cfg_k
     the reference up to that iteration (measured live), because two correct fp32 trajectories of this iteration
     separate exponentially.  The first iteration whose render row sets (V, m) differ from the reference's by more than
     a few boundary flips is reported and must not come early."""
-    import copy
     d = np.load(os.path.join(golden_dir, name + ".npz"))
     g = (lambda k: d[k][oi]) if oi is not None else (lambda k: d[k])
-    cfg = copy.deepcopy(cfg_kitti if cfgname == "kitti" else cfg_redwood)
-    cfg["optimizer"]["joint_optim"]["num_iterations"] = iters
+    cfg = TS.run_cfg(cfgname, iters, cfg_kitti, cfg_redwood, d)
     opt = _engine_or_skip(engine, dec_path[dec], cfg)
     o = dict(t_cam_obj=g("in_t_cam_obj"), pts=g("in_pts"), rays=g("in_rays"), depth=g("in_depth"))
     if with_code:
