@@ -1250,7 +1250,8 @@ int dspgn_tc_selftest(int device, int n_mma, int k_steps, const float* A, const 
   if (int rc = tc_setup_kernels(g_err)) return rc;
   const int K = 16 * k_steps;
   std::vector<unsigned char> blob;
-  tc_pack_images(blob, n_mma, k_steps, [&](int n, int kk) { return B[(size_t)n * K + kk]; });
+  tc_pack_images(blob, tc_mma_n(n_mma), tc_pad_k_steps(k_steps),
+                 [&](int n, int kk) { return (n < n_mma && kk < K) ? B[(size_t)n * K + kk] : 0.f; });
   DevBuf dA, dB, dD;
   if (dA.reserve(4 * (size_t)128 * K) || dB.reserve(blob.size()) || dD.reserve(4 * (size_t)128 * n_mma)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
   CU(cudaMemcpy(dA.p, A, 4 * (size_t)128 * K, cudaMemcpyHostToDevice));

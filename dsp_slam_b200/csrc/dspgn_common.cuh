@@ -56,8 +56,9 @@ constexpr int kTcMaxSteps = 18;
 enum { TK_FWD_HIDDEN = 0, TK_FWD_PENULT = 1, TK_BWD_MID = 2, TK_BWD_FIRST = 3 };   // PENULT: last hidden layer + the final Linear(.,1) on the CUDA cores
 struct TcStep {
   int kind;
-  int n_mma;         // real output width rounded up to 16 (<= 256; the wgmma itself always runs N = 256)
-  int k_steps;       // K=16 steps of the reduction
+  int n_mma;         // wgmma N of the step: the real output width rounded up to 80, 192 or 256 (tc_mma_n); the
+                     // step's weight images hold n_mma rows
+  int k_steps;       // K=16 steps of the reduction, a multiple of 4 (whole 64-wide chunks, zero padded)
   int a_reg, d_reg;  // operand / accumulator ping-pong slot of the step (plan bookkeeping)
   unsigned w_off;    // byte offset of this step's first weight image in the blob
   int layer;         // decoder layer (bias / ReLU-mask slot)

@@ -8,9 +8,9 @@
 //     every fp32 value is split into fp16 hi + fp16 lo.  The wgmma accumulator fragment of columns [16t, 16t+16) is
 //     exactly the register A fragment of K-step t, so the hi halves stay in registers as the next GEMM's A operand and
 //     the lo halves go to a 128B-swizzled shared-memory image (A from a descriptor);
-//   * weights are pre-split (hi/lo fp16), pre-swizzled (128B swizzle, K-major, padded to 256 rows) on the host into
-//     exactly the shared-memory image the wgmma descriptor expects, and streamed from L2 through a 2 x 32 KB ring with
-//     1-D bulk copies (cp.async.bulk) signalling mbarriers;
+//   * weights are pre-split (hi/lo fp16), pre-swizzled (64B swizzle, K-major, 32-wide K halves, padded to the step's
+//     wgmma N of 80, 192 or 256 rows) on the host into exactly the shared-memory images the wgmma descriptor expects,
+//     and streamed from L2 through a 4 x 16 KB ring with 1-D bulk copies (cp.async.bulk) signalling mbarriers;
 //   * every product is formed as  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo  (3 fp16 MMAs, fp32 accumulate):
 //     ~2^-21 relative error per product, which keeps the Gauss-Newton iteration inside the fp32 noise
 //     floor of the reference (SURVEY.md B.3: >= 15 mantissa bits needed; bf16/tf32 single pass is not);
@@ -19,8 +19,9 @@
 //     final Linear(width, 1) + tanh is a per-row dot product in the epilogue of the last hidden layer;
 //   * J^T J / J^T r of the tile on the CUDA cores, written as per-tile partials.
 //
-// Warp roles (288 threads): warps 0-3 / 4-7 = consumer warpgroups (MMA issue + epilogue, rows [64g, 64g+64)), warp 8 =
-// weight producer and, in the persistent kernels, the CTA's scheduler (pops the device work queue).
+// Warp roles (384 threads): warps 0-3 / 4-7 = consumer warpgroups (MMA issue + epilogue, rows [64g, 64g+64)), warps
+// 8-11 = producer warpgroup: warp 8 lane 0 is the weight producer and, in the persistent kernels, the CTA's scheduler
+// (pops the device work queue); warps 9-11 exit after giving their registers to the consumers (setmaxnreg).
 //
 // Three schedules share this body (template SCHED): 0 = one launch per term and iteration (k_decoder_tc), 1 = persistent
 // kernel with SDF tiles only (k_gn_persistent), 2 = persistent kernel with the render term: ray-sample tiles (only the run
@@ -40,12 +41,22 @@
 namespace dspgn {
 
 constexpr int kTcRows = 128;
-constexpr int kTcThreads = 288;
+constexpr int kTcThreads = 384;           // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int kTcEpiThreads = 256;
-constexpr int kTcStages = 2;
-constexpr int kTcStageBytes = 32768;      // one weight image: 256 rows x 64 K x fp16
-constexpr int kTcN = 256;                 // wgmma N of every GEMM step (weight images are zero padded to 256 rows)
+constexpr int kTcStages = 4;              // one 64-wide K chunk: hi[k 0..31], hi[k 32..63], lo[k 0..31], lo[k 32..63]
+constexpr int kTcStageBytes = 16384;      // one ring stage: up to 256 rows x 32 K x fp16 (64 B rows, SWIZZLE_64B)
 constexpr int kTcAloBytes = 32768;        // lo halves of one warpgroup's A operand: 4 x (64 rows x 128 B)
+// Registers are allocated per warpgroup: the producer warpgroup hands most of its share to the two consumer
+// warpgroups (setmaxnreg), which hold the fp32 accumulator (128) and the register A fragment (64).  The pair must fit
+// the 384 x 168 registers the launch bound gives the CTA.
+constexpr int kTcProducerRegs = 40, kTcConsumerRegs = 232;
+static_assert(128 * kTcProducerRegs + 256 * kTcConsumerRegs <= 384 * 168, "setmaxnreg budget exceeds the CTA's registers");
+
+// wgmma N of a GEMM step with `n` output columns: the narrowest instantiated N (80, 192, 256) that holds them.  The
+// weight images of the step hold exactly that many rows.
+__host__ __device__ constexpr int tc_mma_n(int n) { return n <= 80 ? 80 : (n <= 192 ? 192 : 256); }
+// K of every GEMM step is padded to whole 64-wide chunks (zero weight columns): each chunk is one fixed MMA sequence
+__host__ __device__ constexpr int tc_pad_k_steps(int k_steps) { return (k_steps + 3) / 4 * 4; }
 
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -55,13 +66,13 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
@@ -70,8 +81,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "@p bra DONE;\n\t"
       "bra WAIT_LOOP;\n\t"
       "DONE:\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+      "}" ::"r"(bar), "r"(parity) : "memory");
 }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
@@ -84,6 +96,9 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+template <int REGS> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
 // the 128 threads of consumer warpgroup g (ids 1 / 2 are taken by the epilogue and the solve step)
 __device__ __forceinline__ void wg_bar_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(3 + g) : "memory"); }
 
@@ -91,28 +106,43 @@ __device__ __forceinline__ void wg_bar_sync(int g) { asm volatile("bar.sync %0, 
 #define DSPGN_D128                                                                                                    \
   DSPGN_D8(0), DSPGN_D8(8), DSPGN_D8(16), DSPGN_D8(24), DSPGN_D8(32), DSPGN_D8(40), DSPGN_D8(48), DSPGN_D8(56),         \
       DSPGN_D8(64), DSPGN_D8(72), DSPGN_D8(80), DSPGN_D8(88), DSPGN_D8(96), DSPGN_D8(104), DSPGN_D8(112), DSPGN_D8(120)
-#define DSPGN_ACC_OPS "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+#define DSPGN_D96                                                                                                     \
+  DSPGN_D8(0), DSPGN_D8(8), DSPGN_D8(16), DSPGN_D8(24), DSPGN_D8(32), DSPGN_D8(40), DSPGN_D8(48), DSPGN_D8(56),         \
+      DSPGN_D8(64), DSPGN_D8(72), DSPGN_D8(80), DSPGN_D8(88)
+#define DSPGN_D40 DSPGN_D8(0), DSPGN_D8(8), DSPGN_D8(16), DSPGN_D8(24), DSPGN_D8(32)
+#define DSPGN_ACC_OPS128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+#define DSPGN_ACC_OPS96 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+#define DSPGN_ACC_OPS40 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, "
 
-// D[64 x 256] += A[64 x 16] * B[256 x 16]^T, kind f16 (fp32 accumulate); A from registers (fragment of K-step t)
-__device__ __forceinline__ void wgmma_rs(float (&d)[128], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " DSPGN_ACC_OPS
-      "{%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
-      : DSPGN_D128
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(1)
-      : "memory");
-}
-// same with A from a shared-memory descriptor
-__device__ __forceinline__ void wgmma_ss(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " DSPGN_ACC_OPS
-      "%128, %129, p, 1, 1, 0, 0;\n\t}"
-      : DSPGN_D128
-      : "l"(a_desc), "l"(b_desc), "r"(1)
-      : "memory");
-}
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, kind f16 (fp32 accumulate), for the instantiated N (tc_mma_n).  rs: A from
+// registers (fragment of K-step t); ss: A from a shared-memory descriptor.  Both use accumulator registers d[0, N/2):
+// element e of the fragment covers columns 8(e >> 2) .. +7 whatever N is, so the columns >= N keep their value.
+// R0..R5 / S0..S2: asm operand numbers of the inputs (after the N/2 accumulator operands).
+template <int N> struct Wgmma;
+#define DSPGN_WGMMA(N, DREGS, OPS, R0, R1, R2, R3, R4, R5, S0, S1, S2)                                          \
+  template <> struct Wgmma<N> {                                                                                 \
+    static __device__ __forceinline__ void rs(float (&d)[128], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, \
+                                              uint64_t b_desc) {                                                \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #R5 ", 0;\n\t"                                       \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 " OPS                                 \
+                   "{%" #R0 ", %" #R1 ", %" #R2 ", %" #R3 "}, %" #R4 ", p, 1, 1, 0;\n\t}"                         \
+                   : DREGS                                                                                      \
+                   : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(1)                                    \
+                   : "memory");                                                                                 \
+    }                                                                                                           \
+    static __device__ __forceinline__ void ss(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {              \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #S2 ", 0;\n\t"                                       \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 " OPS                                 \
+                   "%" #S0 ", %" #S1 ", p, 1, 1, 0, 0;\n\t}"                                                     \
+                   : DREGS                                                                                      \
+                   : "l"(a_desc), "l"(b_desc), "r"(1)                                                           \
+                   : "memory");                                                                                 \
+    }                                                                                                           \
+  };
+DSPGN_WGMMA(256, DSPGN_D128, DSPGN_ACC_OPS128, 128, 129, 130, 131, 132, 133, 128, 129, 130)
+DSPGN_WGMMA(192, DSPGN_D96, DSPGN_ACC_OPS96, 96, 97, 98, 99, 100, 101, 96, 97, 98)
+DSPGN_WGMMA(80, DSPGN_D40, DSPGN_ACC_OPS40, 40, 41, 42, 43, 44, 45, 40, 41, 42)
+#undef DSPGN_WGMMA
 
 // debug timeline (CTA 0 only, when TermArgs.dbg_clk != nullptr): [tile][step][slot] = clock64
 constexpr int kClkSlots = 8, kClkTiles = 4;
@@ -133,6 +163,16 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)64 << 32;
   d |= (uint64_t)1 << 62;
+  return d;
+}
+// same for a weight ring stage: K-major rows of 64 B (32 K), 64B-swizzled: SBO>>4 = 32 (8 rows x 64 B), layout 2
+// (SWIZZLE_64B); 512 B aligned atoms
+__device__ __forceinline__ uint64_t make_desc_w(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)32 << 32;
+  d |= (uint64_t)2 << 62;
   return d;
 }
 
@@ -161,7 +201,7 @@ struct TcSmemTail {
   float yrow[kTcRows], scr[kTcRows];      // decoder output and row weight (0 = inactive row) of every row
   int prefix[kMaxObjScan + 1];
   int warp_tmp[32];
-  uint64_t w_full[kTcStages], w_empty[kTcStages];
+  uint64_t w_full[kTcStages], w_empty[kTcStages];   // adjacent: wg_gemm addresses both from w_full
   int cur_class;
   int fifo[4]; int fifo_pub; int epi_seq; int last_flag;   // persistent mode: CTA-local tile FIFO (scheduler = producer warp)
   TcPlan plans[DSPGN_MAX_CLASSES];        // step plans of every decoder class (read by all warp roles)
@@ -178,6 +218,13 @@ static_assert(kTcSmemBytes <= 227 * 1024, "tensor-core engine shared memory exce
 // ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
 // 8-column block j = e >> 2 at row 16w + l/4 (+8 when e & 2), column 8j + 2(l%4) + (e & 1).
 __device__ __forceinline__ int frag_col(int e, int q) { return 8 * (e >> 2) + 2 * q + (e & 1); }
+// The epilogues take the fragment column pair q through an opaque move made inside the tile loop.  With the plain value
+// the compiler hoists the 64 distinct frag_col() results out of the loop, and they end up in local memory.
+__device__ __forceinline__ int opaque_int(int v) {
+  int r;
+  asm volatile("mov.b32 %0, %1;" : "=r"(r) : "r"(v));
+  return r;
+}
 
 // accumulator-shaped values -> A operand of the next GEMM step: hi halves into `ah` (the register A fragment of
 // K-step t is columns [16t, 16t+16) of the accumulator fragment), lo halves into this warpgroup's swizzled image.
@@ -199,54 +246,71 @@ __device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&
   wg_bar_sync(grp);
 }
 
-// One GEMM step of a consumer warpgroup: acc = A * W^T over k_steps K-steps, W streamed through the ring (per K chunk of
-// 64: the hi image, then the lo image).  Every consumer warp releases a stage after its MMAs have completed.
-__device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[64], uint32_t alo, unsigned char* ring,
-                                        uint64_t* w_full, uint64_t* w_empty, uint32_t& stage, uint32_t& phase, int k_steps) {
-#pragma unroll
-  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-  wg_fence();
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    if (4 * c < k_steps) {
-      const uint32_t s_hi = stage;
-      mbar_wait(&w_full[stage], phase);
-      const uint32_t bh = smem_u32(ring + (size_t)stage * kTcStageBytes);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int t = 4 * c + k;
-        if (t < k_steps) {
-          const uint64_t bd = make_desc(bh + 32u * k);
-          wgmma_rs(acc, ah[4 * t], ah[4 * t + 1], ah[4 * t + 2], ah[4 * t + 3], bd);
-          wgmma_ss(acc, make_desc(alo + 8192u * c + 32u * k), bd);
-        }
-      }
-      if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-      mbar_wait(&w_full[stage], phase);
-      const uint32_t bl = smem_u32(ring + (size_t)stage * kTcStageBytes);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int t = 4 * c + k;
-        if (t < k_steps) wgmma_rs(acc, ah[4 * t], ah[4 * t + 1], ah[4 * t + 2], ah[4 * t + 3], make_desc(bl + 32u * k));
-      }
-      wg_commit();
-      wg_wait0();
-      __syncwarp();
-      if ((threadIdx.x & 31) == 0) { mbar_arrive(&w_empty[s_hi]); mbar_arrive(&w_empty[stage]); }
-      if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-    }
-  }
+// every consumer warp has finished reading ring stage s (its wgmma groups have completed)
+__device__ __forceinline__ void release_stage(uint32_t w_empty, int s) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(w_empty + 8u * s);
 }
 
-// producer side of the ring: the weight images of one GEMM step
-__device__ __forceinline__ void produce_step(const unsigned char* src, int k_steps, unsigned char* ring, uint64_t* w_full,
-                                             uint64_t* w_empty, uint32_t& stage, uint32_t& phase) {
-  const int nch = (k_steps + 3) >> 2;
-  for (int c = 0; c < 2 * nch; ++c) {           // hi image, lo image, hi, lo, ...
-    mbar_wait(&w_empty[stage], phase ^ 1);
-    mbar_expect_tx(&w_full[stage], (uint32_t)kTcStageBytes);
-    bulk_g2s(ring + (size_t)stage * kTcStageBytes, src + (size_t)c * kTcStageBytes, (uint32_t)kTcStageBytes, &w_full[stage]);
-    if (++stage == kTcStages) { stage = 0; phase ^= 1; }
+// One GEMM step of a consumer warpgroup: acc = A * W^T over nch K chunks of 64, W streamed through the 4-stage ring.  The
+// stages of a chunk arrive as hi[k 0..31], hi[k 32..63], lo[k 0..31], lo[k 32..63], so every output element accumulates in
+// the order  A_hi W_hi, A_lo W_hi  per K-step, then  A_hi W_lo  per K-step,  as when the chunk was one image pair.  Each
+// chunk is a fixed, unrolled MMA sequence (only the chunk count varies), one commit group per stage.  Behind every
+// second stage `wgmma.wait_group 1` retires all but the newest group and their stages go back to the producer, which
+// refills them while the newest group runs.  Every step consumes whole chunks, so the ring is at stage 0 on entry.
+// alo, ring, bars: shared-space addresses (32-bit: the MMA sequence runs with few registers to spare); bars holds the
+// kTcStages full barriers followed by the kTcStages empty barriers.
+template <int N>
+__device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[64], uint32_t alo, uint32_t ring,
+                                        uint32_t bars, uint32_t& phase, int nch) {
+  static_assert(kTcStages == 4, "one ring lap per K chunk");
+  const uint32_t w_full = bars, w_empty = bars + 8u * kTcStages;
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    if (c < nch) {
+      const uint32_t ph = phase ^ (uint32_t)(c & 1);
+#pragma unroll
+      for (int s = 0; s < kTcStages; ++s) {
+        mbar_wait(w_full + 8u * s, ph);
+        wg_fence();
+        const uint32_t bw = ring + (uint32_t)s * kTcStageBytes;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int t = 4 * c + 2 * (s & 1) + k;             // K-step of the step
+          const uint64_t bd = make_desc_w(bw + 32u * k);
+          Wgmma<N>::rs(acc, ah[4 * t], ah[4 * t + 1], ah[4 * t + 2], ah[4 * t + 3], bd);
+          if (s < 2) Wgmma<N>::ss(acc, make_desc(alo + 8192u * c + 32u * (t & 3)), bd);
+        }
+        wg_commit();
+        if (s == 1) {
+          wg_wait1();
+          release_stage(w_empty, 0);
+          if (c > 0) release_stage(w_empty, 3);
+        } else if (s == 3) {
+          wg_wait1();
+          release_stage(w_empty, 1);
+          release_stage(w_empty, 2);
+        }
+      }
+    }
+  }
+  wg_wait0();
+  release_stage(w_empty, 3);
+  phase ^= (uint32_t)(nch & 1);
+}
+
+// producer side of the ring: the weight images of one GEMM step, nch chunks of 4 stages of img_bytes each
+__device__ __forceinline__ void produce_step(const unsigned char* src, int nch, uint32_t img_bytes, unsigned char* ring,
+                                             uint64_t* w_full, uint64_t* w_empty, uint32_t& phase) {
+  for (int c = 0; c < nch; ++c) {
+    for (int s = 0; s < kTcStages; ++s) {
+      mbar_wait(&w_empty[s], phase ^ 1);
+      mbar_expect_tx(&w_full[s], img_bytes);
+      bulk_g2s(ring + (size_t)s * kTcStageBytes, src + (size_t)(kTcStages * c + s) * img_bytes, img_bytes, &w_full[s]);
+    }
+    phase ^= 1;
   }
 }
 
@@ -403,10 +467,12 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
   }
   __syncthreads();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // ===================== weight producer ======================================================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
+    // The producer warpgroup gives its registers to the consumers; only warp 8 lane 0 has work.
+    setmaxnreg_dec<kTcProducerRegs>();
+    if (warp == 8 && lane == 0) {
+      uint32_t phase = 0;
       for (int seq = 0;; ++seq) {
         if (MEGA) {
           // scheduler: fetch this CTA's next tile into the local FIFO (at most 3 entries ahead of the epilogue)
@@ -426,11 +492,14 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         const unsigned char* blob = a.decs[cls].tc_blob;
         const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD);
         const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
-        for (int s = 0; s < ns; ++s) produce_step(blob + plan.step[s].w_off, plan.step[s].k_steps, ring, S.w_full, S.w_empty, stage, phase);
+        for (int s = 0; s < ns; ++s)
+          produce_step(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full,
+                       S.w_empty, phase);
       }
     }
   } else {
     // ===================== consumer warpgroups =================================================
+    setmaxnreg_inc<kTcConsumerRegs>();
     // Warpgroup g issues the MMAs of tile rows [64g, 64g+64) and runs their epilogue on the accumulator fragment.  The
     // per-row stages (prologue, pose columns, residual) use thread = tile row r (both groups hold the same row values).
     const int grp = warp >> 2;
@@ -439,8 +508,8 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
     const int rl = 16 * (warp & 3) + (lane >> 2);              // fragment rows rl, rl + 8 of the warpgroup
     const int rowA = 64 * grp + rl, rowB = rowA + 8;           // ... as tile rows
     unsigned char* const alo = ring + (size_t)kTcStages * kTcStageBytes + (size_t)grp * kTcAloBytes;
-    const uint32_t alo_s = smem_u32(alo);
-    uint32_t stage = 0, phase = 0;
+    const uint32_t alo_s = smem_u32(alo), ring_s = smem_u32(ring);
+    uint32_t phase = 0;
     float acc[128];
     uint32_t ah[64];
     int clk_tile = -1;
@@ -600,10 +669,11 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         const float* w0x = S.w0x;
         const float xa0 = S.xr[rowA], xa1 = S.xr[kTcRows + rowA], xa2 = S.xr[2 * kTcRows + rowA];
         const float xb0 = S.xr[rowB], xb1 = S.xr[kTcRows + rowB], xb2 = S.xr[2 * kTcRows + rowB];
+        const int qs = opaque_int(qd);
         uint32_t mw[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
         for (int e = 0; e < 128; ++e) {
-          const int c = frag_col(e, qd);
+          const int c = frag_col(e, qs);
           const bool hb = (e & 2) != 0;
           float w = S.bias[c];
           w = fmaf(w0x[c], hb ? xb0 : xa0, w);
@@ -628,9 +698,13 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           DSPGN_CLK(4);
           if (MEGA && s == 0) mega_event(q, EV_FIRST_MMA, tr.mode, tr.o, tr.tile);
         }
-        wg_gemm(acc, ah, alo_s, ring, S.w_full, S.w_empty, stage, phase, st.k_steps);
+        const int nch = st.k_steps / 4;
+        if (nm == 80) wg_gemm<80>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
+        else if (nm == 192) wg_gemm<192>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
+        else wg_gemm<256>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
         wg_bar_sync(grp);                                // every MMA of the warpgroup has read the A lo image
         if (tid == 0) DSPGN_CLK(0);
+        const int qs = opaque_int(qd);
 
         if (st.kind == TK_FWD_PENULT) {
           // ---- last hidden layer: bias + ReLU (mask saved), and the final Linear(width, 1) + tanh right here as a per-row
@@ -641,7 +715,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           uint32_t mw[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
           for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qd);
+            const int c = frag_col(e, qs);
             if (c < nm) {
               const float w = acc[e] + bb[c];
               mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
@@ -675,7 +749,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
             const float ga = 1.f - ya * ya, gb = 1.f - yb * yb;
 #pragma unroll
             for (int e = 0; e < 128; ++e) {
-              const int c = frag_col(e, qd);
+              const int c = frag_col(e, qs);
               acc[e] = ((mw[e >> 5] >> (e & 31)) & 1u) ? ((e & 2) ? gb : ga) * S.wlast[c] : 0.f;
             }
             store_operand(acc, ah, alo, rl, qd, grp);
@@ -685,7 +759,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           uint32_t mw[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
           for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qd);
+            const int c = frag_col(e, qs);
             float t = 0.f;
             if (c < nm) {
               const float w = acc[e] + bb[c];
@@ -704,7 +778,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
 #pragma unroll
           for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qd);
+            const int c = frag_col(e, qs);
             float t = 0.f;
             if (c < nm) {
               const float v = acc[e];
@@ -722,7 +796,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           // ---- TK_BWD_FIRST: d/d(input) complete -> Jacobian row (loss.py:34-41 / :143-150) -------------
 #pragma unroll
           for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qd);
+            const int c = frag_col(e, qs);
             if (c < nm && c < in0) {
               const int row = (e & 2) ? rowB : rowA;
               float* pj = S.Jp + row * kJpStride + ((c < L) ? c : (kMaxCode + c - L));
@@ -731,6 +805,12 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
               *pj = g * S.scr[row];                                  // loss.py:145 (de_ds) / inactive rows
             }
           }
+        }
+        if (!more || st.kind == TK_BWD_FIRST) {
+          // no next operand: overwriting the register A fragment ends its live range at the GEMM above.  Otherwise it
+          // would stay live through this epilogue (for the loop's next wg_gemm) and push the epilogue into local memory.
+#pragma unroll
+          for (int i = 0; i < 64; ++i) ah[i] = 0u;
         }
         if (tid == 0) DSPGN_CLK(3);
       }
@@ -876,11 +956,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_tc_selftest(const float* __re
     fence_barrier_init();
   }
   __syncthreads();
-  uint32_t stage = 0, phase = 0;
-  if (warp == 8) {
-    if (lane == 0) produce_step(blob, k_steps, ring, w_full, w_empty, stage, phase);
+  const int n_img = tc_mma_n(n_mma), nch = tc_pad_k_steps(k_steps) / 4;
+  uint32_t phase = 0;
+  if (warp >= 8) {
+    setmaxnreg_dec<kTcProducerRegs>();
+    if (warp == 8 && lane == 0) produce_step(blob, nch, 64u * (uint32_t)n_img, ring, w_full, w_empty, phase);
     return;
   }
+  setmaxnreg_inc<kTcConsumerRegs>();
   const int grp = warp >> 2, qd = lane & 3, rl = 16 * (warp & 3) + (lane >> 2);
   const int rowA = 64 * grp + rl, rowB = rowA + 8;
   unsigned char* alo = ring + (size_t)kTcStages * kTcStageBytes + (size_t)grp * kTcAloBytes;
@@ -892,7 +975,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_tc_selftest(const float* __re
     acc[e] = (c < k_steps * 16) ? A[(size_t)((e & 2) ? rowB : rowA) * lda + c] : 0.f;
   }
   store_operand(acc, ah, alo, rl, qd, grp);
-  wg_gemm(acc, ah, smem_u32(alo), ring, w_full, w_empty, stage, phase, k_steps);
+  if (n_img == 80) wg_gemm<80>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), phase, nch);
+  else if (n_img == 192) wg_gemm<192>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), phase, nch);
+  else wg_gemm<256>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), phase, nch);
 #pragma unroll
   for (int e = 0; e < 128; ++e) {
     const int c = frag_col(e, qd);
@@ -909,28 +994,30 @@ struct TcDecoderHost {
   size_t blob_bytes = 0;
 };
 
-// image of B[n][kk] (n < n_mma, kk in [64c, 64c+64)) as fp16 hi / lo, K-major rows of 128 B, 128B swizzle; rows
-// n_mma..255 are zero (every GEMM step is one N = 256 wgmma)
+// images of B[n][kk] (n < n_img, kk < 16 k_steps) as fp16 hi / lo for the ring (wg_gemm / produce_step): per 64-wide K
+// chunk c the four stages hi[64c, 64c+32), hi[64c+32, 64c+64), lo[...), lo[...), each n_img K-major rows of 64 B with
+// 64B swizzle.  n_img is the step's wgmma N (tc_mma_n), k_steps a multiple of 4 (tc_pad_k_steps); elem returns 0 for the
+// padding rows and columns.
 template <class F>
-inline void tc_pack_images(std::vector<unsigned char>& out, int n_mma, int k_steps, F&& elem) {
-  const int nch = (k_steps + 3) / 4;
-  const size_t img = (size_t)kTcStageBytes;
+inline void tc_pack_images(std::vector<unsigned char>& out, int n_img, int k_steps, F&& elem) {
+  const int nch = k_steps / 4;
+  const size_t img = (size_t)n_img * 64;
   const size_t base = out.size();
-  out.resize(base + (size_t)nch * 2 * img, 0);
-  for (int c = 0; c < nch; ++c) {
-    unsigned char* hi = out.data() + base + (size_t)(2 * c) * img;
-    unsigned char* lo = hi + img;
-    for (int n = 0; n < n_mma; ++n)
-      for (int e = 0; e < 64; ++e) {
-        const int kk = c * 64 + e;
-        const float w = (kk < k_steps * 16) ? elem(n, kk) : 0.f;
-        const __half h = __float2half_rn(w);
-        const __half l = __float2half_rn(w - __half2float(h));
-        const size_t off = (size_t)n * 128 + (size_t)(((e >> 3) ^ (n & 7)) << 4) + (size_t)(e & 7) * 2;
-        memcpy(hi + off, &h, 2);
-        memcpy(lo + off, &l, 2);
-      }
-  }
+  out.resize(base + (size_t)nch * kTcStages * img, 0);
+  for (int c = 0; c < nch; ++c)
+    for (int half = 0; half < 2; ++half) {
+      unsigned char* hi = out.data() + base + (size_t)(kTcStages * c + half) * img;
+      unsigned char* lo = hi + 2 * img;
+      for (int n = 0; n < n_img; ++n)
+        for (int e = 0; e < 32; ++e) {
+          const float w = elem(n, c * 64 + half * 32 + e);
+          const __half h = __float2half_rn(w);
+          const __half l = __float2half_rn(w - __half2float(h));
+          const size_t off = (size_t)n * 64 + (size_t)(((e >> 3) ^ ((n >> 1) & 3)) << 4) + (size_t)(e & 7) * 2;
+          memcpy(hi + off, &h, 2);
+          memcpy(lo + off, &l, 2);
+        }
+    }
 }
 
 inline int round16(int x) { return (x + 15) / 16 * 16; }
@@ -956,8 +1043,8 @@ inline int tc_pack_decoder(const DspgnDecoderSpec& spec, const float* const* W, 
     TcStep& s = P.step[ns];
     const int nin = spec.in_dim[k], nout = spec.out_dim[k];
     s.kind = (k == nl - 2) ? TK_FWD_PENULT : TK_FWD_HIDDEN;
-    s.n_mma = round16(nout);
-    s.k_steps = round16(nin) / 16;
+    s.n_mma = tc_mma_n(nout);
+    s.k_steps = tc_pad_k_steps(round16(nin) / 16);
     s.a_reg = ns & 1; s.d_reg = (ns & 1) ^ 1;
     s.layer = k; s.n_real = nout;
     s.cat_off = (k + 1 == li) ? nout : -1;
@@ -974,8 +1061,8 @@ inline int tc_pack_decoder(const DspgnDecoderSpec& spec, const float* const* W, 
     TcStep& s = P.step[ns];
     const int nin = spec.in_dim[k], nout = spec.out_dim[k];
     s.kind = (k == 0) ? TK_BWD_FIRST : TK_BWD_MID;
-    s.n_mma = round16(nin);
-    s.k_steps = round16(nout) / 16;
+    s.n_mma = tc_mma_n(nin);
+    s.k_steps = tc_pad_k_steps(round16(nout) / 16);
     s.a_reg = a_reg; s.d_reg = a_reg ^ 1;
     a_reg ^= 1;
     s.layer = k; s.n_real = nin;
