@@ -13,6 +13,7 @@ RESULT_FLOATS = 88
 ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC = 0, 1, 2
 SCHED_AUTO, SCHED_LAUNCHES, SCHED_PERSISTENT = 0, 1, 2
 MODE_JOINT, MODE_POSE = 0, 1
+GATE_OFF, GATE_KEPT, GATE_REJECTED = 0, 1, 2
 ST_OK, ST_SDF_NAN, ST_RENDER_FEW, ST_RENDER_NAN, ST_SOLVE, ST_BAD_INPUT = 0, 1, 2, 3, 4, 5
 E_ARG, E_CUDA, E_NOGPU, E_ALLOC, E_PEER = -1, -2, -3, -4, -5
 IPC_HANDLE_BYTES = 64
@@ -54,7 +55,13 @@ class ObjectIn(C.Structure):
 class ObjectOut(C.Structure):
     _fields_ = [("t_cam_obj", C.c_float * 16), ("code", C.c_float * MAX_CODE), ("loss", C.c_float),
                 ("status", C.c_int32), ("n_valid", C.c_int32), ("n_band", C.c_int32),
-                ("iters_done", C.c_int32), ("pad_", C.c_int32 * 3)]
+                ("iters_done", C.c_int32), ("gate", C.c_int32), ("pad_", C.c_int32 * 2)]
+
+
+class GateIn(C.Structure):
+    _fields_ = [("t_cam_obj_map", _FP), ("map_rs", C.c_int32), ("map_cs", C.c_int32),
+                ("t_cam_obj_sim3", _FP), ("sim3_rs", C.c_int32), ("sim3_cs", C.c_int32),
+                ("gate", C.c_int32)]
 
 
 class Counters(C.Structure):
@@ -91,6 +98,8 @@ SYMBOLS = [
     ("dspgn_results_device", _VP, [_VP]),
     ("dspgn_run_batch_modes", C.c_int, [_VP, C.POINTER(C.c_int32)]),
     ("dspgn_keyframe_batch", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(ObjectOut)]),
+    ("dspgn_keyframe_batch_gated", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(GateIn),
+                                             C.POINTER(ObjectOut)]),
     ("dspgn_decode_sdf", C.c_int, [_VP, C.c_int, _FP, _FP, C.c_int, C.c_int, C.c_int, _FP]),
     ("dspgn_counters", C.c_int, [_VP, C.POINTER(Counters)]),
     ("dspgn_enable_timing", C.c_int, [_VP, C.c_int]),

@@ -104,6 +104,7 @@ struct DspgnSolver {
   cudaEvent_t ev_run_upload = nullptr;
   bool run_upload_pending = false;
   bool run_table_valid = false;    // d_run holds h_run for the resident batch (a repeated run skips the copy)
+  bool run_table_gated = false;    // ... and it is the table of a gated run (link | t_map after the two int arrays)
   int total_tiles128 = 0;          // SDF tiles of the batch
   long long total_ray_tiles128 = 0;// ray-sample tiles of the batch
   int max_tiles128 = 0;            // largest tile count of one term of one object (queue items hold 19 bits)
@@ -607,25 +608,32 @@ struct RunPlan {
   long long smp_joint;     // ray samples (n_rays x D) of the joint objects
   long long q_cap;         // persistent kernel: work items that can ever be pushed
   int total0;              // persistent kernel: iteration-0 queue slots (k_init seeds them)
+  bool gated;              // the run table carries link | t_map (a gated keyframe run)
+  bool any_dormant;        // ... and has joint slots that only run when their pose-only object is rejected
 };
 
 // Checks the modes, fills the plan and stages the per-run object table (modes | first iteration-0 queue slot of each
-// object) into d_run, async on the stream; `unlimited`: objects never finish (the debug hooks advance the batch freely).
-int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = false) {
+// object [| link | t_map of a gated run]) into d_run, async on the stream; `unlimited`: objects never finish (the debug
+// hooks advance the batch freely).  link[o] >= 0 on a joint object marks the dormant joint slot of pose-only object
+// link[o]: it counts towards the queue capacity and the render term but reserves no iteration-0 slot and no row counter.
+int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = false, const int32_t* link = nullptr,
+             const float* t_map = nullptr) {
   const DspgnConfig& c = s->cfg;
   const int n = s->n_obj, D = c.num_depth_samples;
   p = RunPlan{};
+  p.gated = link != nullptr;
   for (int o = 0; o < n; ++o) {
     if (modes[o] != DSPGN_MODE_JOINT && modes[o] != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
-    p.any[modes[o]] = true;
+    if (link && link[o] >= 0 && modes[o] == DSPGN_MODE_JOINT) p.any_dormant = true;
+    else p.any[modes[o]] = true;
   }
   if (p.any[DSPGN_MODE_POSE] && c.pose_only_iterations < 1) return fail(DSPGN_E_ARG, "pose_only_iterations must be >= 1");
   p.iters[DSPGN_MODE_JOINT] = unlimited ? (1 << 30) : c.num_iterations;
   p.iters[DSPGN_MODE_POSE] = unlimited ? (1 << 30) : c.pose_only_iterations;
-  p.render = p.any[DSPGN_MODE_JOINT] && !c.sdf_only;
+  p.render = (p.any[DSPGN_MODE_JOINT] || p.any_dormant) && !c.sdf_only;
   if (s->run_upload_pending) { CU(cudaEventSynchronize(s->ev_run_upload)); s->run_upload_pending = false; }
-  const size_t bytes = 8 * (size_t)n;
-  const bool same = s->run_table_valid && memcmp(s->h_run.p, modes, 4 * (size_t)n) == 0;
+  const size_t bytes = (p.gated ? 12 + 64 : 8) * (size_t)n;
+  const bool same = s->run_table_valid && !p.gated && !s->run_table_gated && memcmp(s->h_run.p, modes, 4 * (size_t)n) == 0;
   if (!same) {
     if (s->d_run.cap < bytes) CU(cudaStreamSynchronize(s->stream));      // kernels of an earlier run may still read it
     if (s->h_run.reserve(bytes) || s->d_run.reserve(bytes)) return fail(DSPGN_E_ALLOC, "run table allocation failed");
@@ -634,16 +642,24 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
   for (int o = 0; o < n; ++o) {
     const ObjMeta& M = s->h_meta[o];
     const int m = modes[o];
+    const bool dormant = link && link[o] >= 0 && m == DSPGN_MODE_JOINT;
     const bool r = p.render && m == DSPGN_MODE_JOINT;
     const long long ntS = (M.n_pts + kTcRows - 1) / kTcRows, ntF = ((long long)M.n_rays * D + kTcRows - 1) / kTcRows;
-    p.pts[m] += M.n_pts;
-    if (m == DSPGN_MODE_JOINT) p.smp_joint += (long long)M.n_rays * D;
+    if (!dormant) {
+      p.pts[m] += M.n_pts;
+      if (m == DSPGN_MODE_JOINT) p.smp_joint += (long long)M.n_rays * D;
+    }
     // per iteration: every SDF tile, every ray-sample tile, one scan item per 64 rays and at most as many band tiles
     // as ray-sample tiles (iteration 0 reserves every ray-sample tile of the object)
     p.q_cap += (long long)p.iters[m] * (ntS + (r ? 2 * ntF + (M.n_rays + kScanChunkRays - 1) / kScanChunkRays : 0));
     if (!same) { h[o] = m; h[n + o] = p.total0; }
-    p.total0 += (int)(ntS + (r ? ntF : 0));
+    if (!dormant) p.total0 += (int)(ntS + (r ? ntF : 0));
   }
+  if (p.gated) {
+    memcpy(h + 2 * n, link, 4 * (size_t)n);
+    memcpy(h + 3 * n, t_map, 64 * (size_t)n);
+  }
+  s->run_table_gated = p.gated;
   if (!same) {
     CU(cudaMemcpyAsync(s->d_run.p, h, bytes, cudaMemcpyHostToDevice, s->stream));
     CU(cudaEventRecord(s->ev_run_upload, s->stream));
@@ -661,6 +677,7 @@ int launch_init(DspgnSolver* s, const RunPlan& p, bool mega = false) {
   ia.modes = s->d_run.as<int>(); ia.n_iter_joint = p.iters[DSPGN_MODE_JOINT]; ia.n_iter_pose = p.iters[DSPGN_MODE_POSE];
   ia.gather = s->gdev; ia.results = s->d_results.as<float>(); ia.n_bad = s->n_bad;
   ia.decs = s->d_decs.as<DecoderDev>();
+  if (p.gated) { ia.link = s->d_run.as<int>() + 2 * s->n_obj; ia.t_map = reinterpret_cast<const float*>(s->d_run.as<int>() + 3 * s->n_obj); }
   ia.mega = mega ? 1 : 0;
   if (mega) {
     const bool render = p.render;
@@ -698,7 +715,7 @@ ScanArgs base_scan(DspgnSolver* s) {
 int launch_terms(DspgnSolver* s, const RunPlan& p, int iter, float* dbg_J = nullptr, float* dbg_res = nullptr, int dbg_obj = -1,
                  int dbg_P = 0) {
   const DspgnConfig& c = s->cfg;
-  const bool render = p.render && iter < p.iters[DSPGN_MODE_JOINT];
+  const bool render = p.render && p.any[DSPGN_MODE_JOINT] && iter < p.iters[DSPGN_MODE_JOINT];
   // The SDF-row pass and the forward-only pass over the ray samples are independent: fork the latter onto a
   // second stream (matters for small batches, where each pass is a single wave of tiles) unless per-launch
   // timing is on.
@@ -762,10 +779,19 @@ SolveArgs base_solve(DspgnSolver* s) {
 namespace {
 // One run of the resident batch, modes[o] = DSPGN_MODE_* of object o.  Every object runs its own mode's iterations,
 // terms and update and finishes after its own last iteration; dspgn_run_batch(s, m) is the uniform case.
-int run_batch_impl(DspgnSolver* s, const int32_t* modes) {
+// A gated run (link != nullptr, see plan_run) also checks every gated pose-only object at its last solve and runs the joint
+// slots of the rejected ones: woken on the device by the persistent kernel; in the per-iteration schedule as a second
+// phase after a readback of the verdicts.
+int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = nullptr, const float* t_map = nullptr) {
   CU(cudaSetDevice(s->device));
   RunPlan p;
-  if (int rc = plan_run(s, modes, p)) return rc;
+  if (int rc = plan_run(s, modes, p, false, link, t_map)) return rc;
+  auto gate_args = [&](SolveArgs& v) {
+    if (!p.gated) return;
+    v.link = s->d_run.as<int>() + 2 * s->n_obj;
+    v.t_map = reinterpret_cast<const float*>(s->d_run.as<int>() + 3 * s->n_obj);
+    v.T_init = s->d_Tinit;
+  };
   const int max_iters = std::max(p.any[DSPGN_MODE_JOINT] ? p.iters[DSPGN_MODE_JOINT] : 0,
                                  p.any[DSPGN_MODE_POSE] ? p.iters[DSPGN_MODE_POSE] : 0);
   s->ctr = DspgnCounters{};
@@ -815,6 +841,7 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes) {
       q.ev = s->d_ev.as<long long>(); q.ev_cap = kEvCap;
     }
     SolveArgs v = base_solve(s);
+    gate_args(v);
     v.ev = q.ev; v.ev_cap = q.ev_cap;
     v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0; v.dbg_clk = nullptr;
     ScanArgs sa = base_scan(s);
@@ -832,18 +859,47 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes) {
     return 0;
   }
   if (int rc = launch_init(s, p)) return rc;
-  for (int e = 0; e < max_iters; ++e) {
-    if (int rc = launch_terms(s, p, e)) return rc;
-    SolveArgs v = base_solve(s);
-    v.iter_index = e;
-    if (s->timing) {
-      if (s->evs_used + 2 > s->ev_solve.size()) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); s->ev_solve.push_back(e0); s->ev_solve.push_back(e1); }
-      cudaEventRecord(s->ev_solve[s->evs_used], s->stream);
+  auto iterate = [&](const RunPlan& pl, int n_iters) -> int {
+    for (int e = 0; e < n_iters; ++e) {
+      if (int rc = launch_terms(s, pl, e)) return rc;
+      SolveArgs v = base_solve(s);
+      gate_args(v);
+      v.iter_index = e;
+      if (s->timing) {
+        if (s->evs_used + 2 > s->ev_solve.size()) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); s->ev_solve.push_back(e0); s->ev_solve.push_back(e1); }
+        cudaEventRecord(s->ev_solve[s->evs_used], s->stream);
+      }
+      k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
+      if (s->timing) { cudaEventRecord(s->ev_solve[s->evs_used + 1], s->stream); s->evs_used += 2; }
+      s->ctr.kernel_launches++;
+      CU(cudaGetLastError());
     }
-    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
-    if (s->timing) { cudaEventRecord(s->ev_solve[s->evs_used + 1], s->stream); s->evs_used += 2; }
-    s->ctr.kernel_launches++;
-    CU(cudaGetLastError());
+    return 0;
+  };
+  if (int rc = iterate(p, max_iters)) return rc;
+  if (p.any_dormant) {
+    // second phase: the verdicts of the first (record gate words) decide which joint slots run
+    const int n = s->n_obj;
+    if (s->h_results.reserve(4 * DSPGN_RESULT_FLOATS * (size_t)n + 512)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
+    CU(cudaMemcpyAsync(s->h_results.p, s->d_results.p, 4 * DSPGN_RESULT_FLOATS * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
+    CU(cudaStreamSynchronize(s->stream));
+    const int* rec = s->h_results.as<int>();
+    RunPlan pb = p;
+    pb.any[DSPGN_MODE_POSE] = false; pb.any[DSPGN_MODE_JOINT] = false;
+    pb.pts[DSPGN_MODE_POSE] = 0; pb.pts[DSPGN_MODE_JOINT] = 0; pb.smp_joint = 0;
+    for (int o = 0; o < n; ++o)
+      if (link[o] >= 0 && modes[o] == DSPGN_MODE_JOINT && rec[(size_t)link[o] * DSPGN_RESULT_FLOATS + 85] == DSPGN_GATE_REJECTED) {
+        pb.any[DSPGN_MODE_JOINT] = true;
+        pb.pts[DSPGN_MODE_JOINT] += s->h_meta[o].n_pts;
+        pb.smp_joint += (long long)s->h_meta[o].n_rays * s->cfg.num_depth_samples;
+      }
+    if (pb.any[DSPGN_MODE_JOINT]) {
+      k_gate_wake<<<(n + 127) / 128, 128, 0, s->stream>>>(s->d_state.as<ObjState>(), s->d_run.as<int>(), s->d_run.as<int>() + 2 * n,
+                                                          s->d_results.as<float>(), n, p.iters[DSPGN_MODE_JOINT]);
+      s->ctr.kernel_launches++;
+      CU(cudaGetLastError());
+      if (int rc = iterate(pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
+    }
   }
   CU(cudaEventRecord(s->ev_run1, s->stream));
   return 0;
@@ -1110,14 +1166,72 @@ int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in
 }
 
 int dspgn_keyframe_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, DspgnObjectOut* out) {
+  return dspgn_keyframe_batch_gated(s, n_obj, in, modes, nullptr, out);
+}
+
+int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
+                               const DspgnGateIn* gates, DspgnObjectOut* out) {
   if (!s || !in || !modes || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
   if (int rc = check_modes(s, modes, n_obj, in)) return rc;
-  for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
-    const int n = std::min(kMaxObjScan, n_obj - o0);
-    if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
+  auto gated = [&](int o) { return gates != nullptr && gates[o].gate != 0; };
+  for (int o = 0; gates && o < n_obj; ++o) {
+    const DspgnGateIn& g = gates[o];
+    if (g.gate != 0 && g.gate != 1) return fail(DSPGN_E_ARG, "gate must be 0 or 1");
+    if (!gated(o)) continue;
+    if (modes[o] != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "a gate needs a pose-only object");
+    if (!g.t_cam_obj_map || !g.t_cam_obj_sim3) return fail(DSPGN_E_ARG, "a gate needs t_cam_obj_map and t_cam_obj_sim3");
+    if (in[o].t_cam_world) return fail(DSPGN_E_ARG, "a gated object takes camera-frame inputs (no t_cam_world)");
+  }
+  // resident chunks of at most kMaxObjScan slots; a gated object and its joint slot (appended after the chunk's
+  // objects) always share a chunk
+  std::vector<DspgnObjectIn> ins;
+  std::vector<int32_t> cm, link;
+  std::vector<float> t_map;
+  std::vector<DspgnObjectOut> res;
+  for (int o0 = 0; o0 < n_obj;) {
+    int o1 = o0, slots = 0;
+    while (o1 < n_obj && slots + 1 + (gated(o1) ? 1 : 0) <= kMaxObjScan) slots += 1 + (gated(o1++) ? 1 : 0);
+    const int n = o1 - o0;
     s->gdev = GatherDev{};
-    if (int rc = run_batch_impl(s, modes + o0)) return rc;
-    if (int rc = dspgn_results(s, out + o0)) return rc;
+    if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
+      if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
+      if (int rc = run_batch_impl(s, modes + o0)) return rc;
+      if (int rc = dspgn_results(s, out + o0)) return rc;
+      o0 = o1;
+      continue;
+    }
+    ins.assign(in + o0, in + o1);
+    cm.assign(modes + o0, modes + o1);
+    link.assign(n, -1);
+    t_map.assign(16 * (size_t)slots, 0.f);
+    for (int k = 0; k < n; ++k) {
+      if (!gated(o0 + k)) continue;
+      const DspgnGateIn& g = gates[o0 + k];
+      DspgnObjectIn J = in[o0 + k];                    // the detection as reconstruct_object(Sim3Tco, pts, rays, depth) sees it
+      J.t_cam_obj = g.t_cam_obj_sim3; J.t_rs = g.sim3_rs; J.t_cs = g.sim3_cs;
+      J.code = nullptr;
+      link[k] = (int)ins.size();
+      link.push_back(k);
+      ins.push_back(J);
+      cm.push_back(DSPGN_MODE_JOINT);
+      for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) t_map[16 * (size_t)k + 4 * r + c] = g.t_cam_obj_map[(size_t)r * g.map_rs + (size_t)c * g.map_cs];
+    }
+    if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
+    if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data())) return rc;
+    const bool mega = s->mega_ran;
+    res.resize(slots);
+    if (int rc = dspgn_results(s, res.data())) return rc;
+    for (int k = 0; k < n; ++k) {
+      DspgnObjectOut& r = out[o0 + k];
+      r = res[k];
+      if (link[k] >= 0 && res[k].gate == DSPGN_GATE_REJECTED) {
+        r = res[link[k]];
+        r.gate = DSPGN_GATE_REJECTED;
+        if (mega) s->ctr.rows_fwd_bwd += (long long)s->h_meta[link[k]].n_pts * s->cfg.num_iterations;   // the woken slot's SDF rows
+      }
+    }
+    o0 = o1;
   }
   return 0;
 }

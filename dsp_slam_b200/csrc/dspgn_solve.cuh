@@ -109,6 +109,114 @@ __device__ inline void write_record(float* results, const GatherDev& g, int o, c
   }
 }
 
+// ---- the map-consistency check of a tracked detection (dspgn_keyframe_batch_gated) -----------------------------------
+// GetNewObservations (src/LocalMapping_util.cc:104-147) compares the pose-only estimate Zco with the pose the map
+// predicts, Tco = Tcw Two: dist2D, the x/z translation difference in fp32 (Eigen::Vector2f::norm), and e = log(Tco^-1 Zco)
+// with both poses as g2o SE3Quat (unit quaternion + translation, fp64).  Restated here:
+//   quaternion of a rotation matrix: the trace form when tr > 0, else the form pivoted on the largest diagonal entry;
+//   then the sign is chosen so that w >= 0 and the quaternion is normalised (SE3Quat(R, t));
+//   inverse (q*, -q* t), product (t1 + q1 t2, q1 q2, renormalised);
+//   log: R of the quaternion, d = (tr R - 1) / 2, dR = (R21 - R12, R02 - R20, R10 - R01);
+//        d > 0.99999:  w = dR / 2,                                V^-1 = I - W/2 + W^2/12
+//        otherwise:    w = acos(d) / (2 sqrt(1 - d^2)) dR,      V^-1 = I - W/2 + (1 - th / (2 tan(th/2))) / th^2 W^2
+//        u = V^-1 t,  e = (w, u).
+// Kept: dist2D < 1 and |e| < 1.5 (a NaN fails).  oracle/gate_check.py is the same check in numpy.
+struct GateQuat { double w, x, y, z; };
+__device__ inline GateQuat gate_normalise(GateQuat q) {
+  if (q.w < 0.0) { q.w = -q.w; q.x = -q.x; q.y = -q.y; q.z = -q.z; }
+  const double n = sqrt(q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z);
+  q.w /= n; q.x /= n; q.y /= n; q.z /= n;
+  return q;
+}
+// rotation part of a row-major 4x4 float matrix (fp64), normalised quaternion
+__device__ inline GateQuat gate_quat(const float* T) {
+  double m[3][3];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) m[r][c] = (double)T[r * 4 + c];
+  double v[4];                                       // x, y, z, w
+  const double tr = m[0][0] + m[1][1] + m[2][2];
+  if (tr > 0.0) {
+    const double s = sqrt(tr + 1.0), h = 0.5 / s;
+    v[3] = 0.5 * s;
+    v[0] = (m[2][1] - m[1][2]) * h; v[1] = (m[0][2] - m[2][0]) * h; v[2] = (m[1][0] - m[0][1]) * h;
+  } else {
+    int i = 0;
+    if (m[1][1] > m[0][0]) i = 1;
+    if (m[2][2] > m[i][i]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    const double s = sqrt(m[i][i] - m[j][j] - m[k][k] + 1.0), h = 0.5 / s;
+    v[i] = 0.5 * s;
+    v[3] = (m[k][j] - m[j][k]) * h;
+    v[j] = (m[j][i] + m[i][j]) * h;
+    v[k] = (m[k][i] + m[i][k]) * h;
+  }
+  return gate_normalise(GateQuat{v[3], v[0], v[1], v[2]});
+}
+__device__ inline GateQuat gate_qmul(const GateQuat& a, const GateQuat& b) {
+  return GateQuat{a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
+                  a.w * b.y - a.x * b.z + a.y * b.w + a.z * b.x, a.w * b.z + a.x * b.y - a.y * b.x + a.z * b.w};
+}
+// R of a unit quaternion, row-major
+__device__ inline void gate_rot(const GateQuat& q, double R[9]) {
+  const double tx = 2.0 * q.x, ty = 2.0 * q.y, tz = 2.0 * q.z;
+  const double twx = tx * q.w, twy = ty * q.w, twz = tz * q.w, txx = tx * q.x, txy = ty * q.x, txz = tz * q.x;
+  const double tyy = ty * q.y, tyz = tz * q.y, tzz = tz * q.z;
+  R[0] = 1.0 - (tyy + tzz); R[1] = txy - twz;         R[2] = txz + twy;
+  R[3] = txy + twz;         R[4] = 1.0 - (txx + tzz); R[5] = tyz - twx;
+  R[6] = txz - twy;         R[7] = tyz + twx;         R[8] = 1.0 - (txx + tyy);
+}
+__device__ inline void gate_qrot(const GateQuat& q, const double v[3], double out[3]) {
+  double R[9];
+  gate_rot(q, R);
+  for (int r = 0; r < 3; ++r) out[r] = R[3 * r] * v[0] + R[3 * r + 1] * v[1] + R[3 * r + 2] * v[2];
+}
+// DSPGN_GATE_KEPT or DSPGN_GATE_REJECTED for the estimate Z against the map's prediction M (row-major 4x4 floats)
+__device__ __noinline__ int gate_decide(const float* Z, const float* M) {
+  const float dx = __fsub_rn(Z[3], M[3]), dz = __fsub_rn(Z[11], M[11]);
+  const float dist2d = sqrtf(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dz, dz)));
+  const GateQuat qm = gate_quat(M), qz = gate_quat(Z);
+  // Tco^-1 = (q*, -(q* t)),  Tco^-1 Zco = (q* tz + t_inv, q* qz)
+  const GateQuat qi{qm.w, -qm.x, -qm.y, -qm.z};
+  const double tm[3] = {-(double)M[3], -(double)M[7], -(double)M[11]}, tz[3] = {(double)Z[3], (double)Z[7], (double)Z[11]};
+  double ti[3], tr[3];
+  gate_qrot(qi, tm, ti);
+  gate_qrot(qi, tz, tr);
+  for (int i = 0; i < 3; ++i) tr[i] += ti[i];
+  const GateQuat q = gate_normalise(gate_qmul(qi, qz));
+  double R[9];
+  gate_rot(q, R);
+  const double d = 0.5 * (R[0] + R[4] + R[8] - 1.0);
+  const double dR[3] = {R[7] - R[5], R[2] - R[6], R[3] - R[1]};
+  double w[3], c2;
+  if (d > 0.99999) {
+    for (int i = 0; i < 3; ++i) w[i] = 0.5 * dR[i];
+    c2 = 1.0 / 12.0;
+  } else {
+    const double th = acos(d), f = th / (2.0 * sqrt(1.0 - d * d));
+    for (int i = 0; i < 3; ++i) w[i] = f * dR[i];
+    c2 = (1.0 - th / (2.0 * tan(th / 2.0))) / (th * th);
+  }
+  // V^-1 t = t - W t / 2 + c2 W (W t),  W t = w x t
+  const double wt[3] = {w[1] * tr[2] - w[2] * tr[1], w[2] * tr[0] - w[0] * tr[2], w[0] * tr[1] - w[1] * tr[0]};
+  const double wwt[3] = {w[1] * wt[2] - w[2] * wt[1], w[2] * wt[0] - w[0] * wt[2], w[0] * wt[1] - w[1] * wt[0]};
+  double e2 = 0.0;
+  for (int i = 0; i < 3; ++i) {
+    const double u = tr[i] - 0.5 * wt[i] + c2 * wwt[i];
+    e2 += w[i] * w[i] + u * u;
+  }
+  return (dist2d < 1.0f && sqrt(e2) < 1.5) ? DSPGN_GATE_KEPT : DSPGN_GATE_REJECTED;
+}
+
+// Gate of a finished gated pose-only object o (one thread, after its record was written): the record's pose, or after a
+// soft failure the input pose, against the map's prediction; the verdict goes into the record's gate word.
+__device__ inline int gate_record(float* results, int o, const float* T_init, const float* t_map) {
+  float* r = results + (size_t)o * DSPGN_RESULT_FLOATS;
+  const float* Z = (reinterpret_cast<const int*>(r)[81] == DSPGN_ST_OK) ? r : T_init + 16 * (size_t)o;
+  const int g = gate_decide(Z, t_map + 16 * (size_t)o);
+  reinterpret_cast<int*>(r)[85] = g;
+  return g;
+}
+
 // ---- device-side input construction (SURVEY 8 row f4) --------------------------------------------------------------
 // Runs once per upload, in place on the uploaded staging block: ray slots hold (u, v, 1) and become inv_k [u, v, 1]
 // (loss_utils.py:23-37 / LocalMapping_util.cc:378-386); world map points become camera points x_c = R x_w + t
@@ -265,6 +373,9 @@ struct InitArgs {
   unsigned long long* valid_rows_total;
   int vpre_exact;
   const float* rays; int* vpre;   // render runs of the persistent kernel: valid-sample ranges (nullptr = off)
+  // gated keyframe runs (nullptr = none): link[o] = the joint slot of gated pose-only object o / the pose-only object of
+  // joint slot o, -1 otherwise; t_map [n_obj][16] the map's prediction of each gated object
+  const int* link; const float* t_map;
 };
 
 // zb0 = b0 + W0[:, :L] z   (fp32 FMA chain in i order; all threads of the calling CTA / epilogue)
@@ -284,6 +395,10 @@ __global__ void k_init(InitArgs a) {
   ObjState& st = a.state[o];
   const ObjMeta M = a.meta[o];
   const int mode = a.modes[o];
+  const int link = (a.link != nullptr) ? a.link[o] : -1;
+  // the joint slot of a gated object starts dormant: fully initialised here, no tiles queued; the solve step that finishes
+  // its pose-only object wakes it (persistent kernel) or k_gate_wake does (per-iteration schedule, n_iter 0 until then)
+  const bool dormant = link >= 0 && mode == DSPGN_MODE_JOINT;
   if (tid < kMaxCode) st.z[tid] = (M.has_code && tid < a.code_len) ? a.code_init[o * kMaxCode + tid] : 0.f;
   if (tid == 0) {
     float Tco[12];
@@ -295,7 +410,7 @@ __global__ void k_init(InitArgs a) {
     inv_affine(Tco, st.T_oc, nullptr);     // optimizer.py:55 / :104
     derive_depth_range(st, a.D);
     st.loss = 0.f; st.status = M.bad ? DSPGN_ST_BAD_INPUT : 0; st.iters = 0; st.V = 0; st.m = 0; st.n_active = M.n_pts;
-    st.mode = mode; st.n_iter = (mode == DSPGN_MODE_POSE) ? a.n_iter_pose : a.n_iter_joint;
+    st.mode = mode; st.n_iter = (mode == DSPGN_MODE_POSE) ? a.n_iter_pose : ((dormant && !a.mega) ? 0 : a.n_iter_joint);
     a.V_count[o] = 0;
     a.band_m[o] = 0;
   }
@@ -304,6 +419,9 @@ __global__ void k_init(InitArgs a) {
   if (M.bad) {                               // rejected at upload: no tile, no solve -- its record is final now
     __syncthreads();
     if (tid == 0) write_record(a.results, a.gather, o, st, M.scale);
+    // a gated object rejected at upload is checked with its input pose; its joint slot has the same points, rays and
+    // depths, so it is rejected at upload too and its record is already final
+    if (tid == 0 && link >= 0 && mode == DSPGN_MODE_POSE) gate_record(a.results, o, a.T_init, a.t_map);
   }
   if (a.mega) {
     const int ntS = (M.n_pts + a.tile_rows - 1) / a.tile_rows;
@@ -318,9 +436,11 @@ __global__ void k_init(InitArgs a) {
       ntF = (vh + a.tile_rows - 1) / a.tile_rows;
     }
     const int base = a.q0_off[o];
-    for (int j = tid; j < ntF; j += blockDim.x) a.q_flag[base + j] = make_item(MODE_RAYFWD, o, j) + 1;
-    for (int j = tid; j < ntS; j += blockDim.x) a.q_flag[base + ntF + j] = make_item(MODE_SDF, o, j) + 1;
-    for (int j = ntF + ntS + tid; j < ntF_cap + ntS; j += blockDim.x) a.q_flag[base + j] = kItemNop + 1;
+    if (!dormant) {                          // a dormant slot has no reserved slots: its wake pushes these items
+      for (int j = tid; j < ntF; j += blockDim.x) a.q_flag[base + j] = make_item(MODE_RAYFWD, o, j) + 1;
+      for (int j = tid; j < ntS; j += blockDim.x) a.q_flag[base + ntF + j] = make_item(MODE_SDF, o, j) + 1;
+      for (int j = ntF + ntS + tid; j < ntF_cap + ntS; j += blockDim.x) a.q_flag[base + j] = kItemNop + 1;
+    }
     if (tid == 0) { a.pending[o] = ntS + (ntF > 0 ? 1 : 0); a.ray_left[o] = ntF; a.obj_iter[o] = 0; }
     if (o == 0 && tid == 0) { *a.q_head = 0; *a.q_tail = a.total_tiles0; *a.done_objects = a.n_bad; *a.band_rows_total = 0; *a.valid_rows_total = 0ull; *a.abort_flag = 0; }
   }
@@ -347,6 +467,7 @@ struct SolveArgs {
   int dbg_obj; float* dbg_H; float* dbg_b; float* dbg_dx; float* dbg_loss;
   long long* dbg_clk;      // optional: 16 clock64 stamps of object 0's CTA
   long long* ev; int ev_cap;   // optional event log of the persistent kernel (phase stamps of the solve step)
+  const int* link; const float* t_map; const float* T_init;   // gated keyframe runs (InitArgs); link = nullptr: none
 };
 __device__ __forceinline__ void solve_event(const SolveArgs& a, int o, int phase) {
   if (a.ev == nullptr) return;
@@ -686,7 +807,22 @@ __global__ void __launch_bounds__(kSolveThreads) k_solve(SolveArgs a) {
   __shared__ SolveSmem SM;
   const int o = blockIdx.x, n_iter = a.state[o].n_iter;
   if (a.iter_index >= n_iter) return;               // finished after its own last iteration
-  solve_object<false>(a, o, threadIdx.x, SM, a.iter_index + 1 == n_iter);
+  const bool last = a.iter_index + 1 == n_iter;
+  solve_object<false>(a, o, threadIdx.x, SM, last);
+  // gated pose-only object: the map-consistency check on the record thread 0 has just written
+  if (last && a.link != nullptr && a.dbg_H == nullptr && threadIdx.x == 0 && a.link[o] >= 0 && a.state[o].mode == DSPGN_MODE_POSE)
+    gate_record(a.results, o, a.T_init, a.t_map);
+}
+
+// Per-iteration schedule of a gated run, between its two phases: the joint slots whose pose-only object was rejected
+// run num_iterations from their k_init state, every other object is finished (its record is final).
+__global__ void k_gate_wake(ObjState* state, const int* modes, const int* link, const float* results, int n_obj, int n_iter_joint) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= n_obj) return;
+  const int lk = link[o];
+  const bool wake = lk >= 0 && modes[o] == DSPGN_MODE_JOINT &&
+                    reinterpret_cast<const int*>(results + (size_t)lk * DSPGN_RESULT_FLOATS)[85] == DSPGN_GATE_REJECTED;
+  state[o].n_iter = wake ? n_iter_joint : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -946,6 +1082,7 @@ __global__ void __launch_bounds__(kScanThreads) k_ray_scan(ScanArgs a) {
   __shared__ int s_wsum[32];
   const int o = blockIdx.x;
   if (a.state[o].status != 0 || a.state[o].mode != DSPGN_MODE_JOINT) return;   // pose-only objects: no render term
+  if (a.state[o].n_iter == 0) return;                // a dormant joint slot of a gated run
   scan_object<false>(a, o, threadIdx.x, kScanThreads, s_cnt, s_wsum);
 }
 

@@ -209,7 +209,7 @@ struct TcSmemTail {
   // parameters themselves would make them address-taken: the compiler then parks all of them in local memory and the tile
   // loop reads its pointers with LDL instead of from the constant bank.
   MegaArgs ctx_q; SolveArgs ctx_sv; int ctx_D; const float* ctx_rays;
-  int push_base, push_nF, push_nS;        // cooperative publication of an object's next-iteration tiles
+  int push_base, push_nF, push_nS, push_o;   // cooperative publication of an object's next-iteration tiles
   float ost[16]; int ost_rows;            // the tile's object: T_oc[12], dmin, dmax, dstep, dfar; rows of its term (counter)
 };
 constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail);
@@ -415,8 +415,18 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
     mega_event(q, EV_SOLVE_END, 0, o, it);
     int base = -1;
     if (fin) {
+      // a gated pose-only object: the map-consistency check on its record; rejected, it wakes its joint slot (k_init
+      // left the slot initialised, its iteration-0 counters set and no item queued), kept, the slot is done unrun
+      // (a slot rejected at upload never gets here: its pose-only object was rejected at upload too)
+      const int slot = (sv.link != nullptr && sv.state[o].mode == DSPGN_MODE_POSE) ? sv.link[o] : -1;
+      const bool wake = slot >= 0 && gate_record(sv.results, o, sv.T_init, sv.t_map) == DSPGN_GATE_REJECTED;
       __threadfence();                       // the result record before the object counts as done
-      atomicAdd(q.done_objects, 1);
+      atomicAdd(q.done_objects, (slot >= 0 && !wake) ? 2 : 1);
+      if (wake) {
+        const int ntF = ldv(q.ray_left + slot), ntS = (sv.meta[slot].n_pts + kTcRows - 1) / kTcRows;
+        base = atomicAdd(q.q_tail, ntF + ntS);
+        S.push_nF = ntF; S.push_nS = ntS; S.push_o = slot;
+      }
     } else {
       // (no fence in this branch: q_tail only reserves slots; state and counters are fenced below, before any slot is published)
       const ObjMeta M = sv.meta[o];
@@ -426,7 +436,7 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
       *reinterpret_cast<volatile int*>(q.pending + o) = ntS + (ntF > 0 ? 1 : 0);
       *reinterpret_cast<volatile int*>(q.ray_left + o) = ntF;
       base = atomicAdd(q.q_tail, ntF + ntS);  // the long chain (rays -> scan -> band -> solve) first, then the SDF tiles
-      S.push_nF = ntF; S.push_nS = ntS;
+      S.push_nF = ntF; S.push_nS = ntS; S.push_o = o;
     }
     S.push_base = base;
   }
@@ -434,10 +444,11 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
   const int base = S.push_base;
   if (base >= 0) {
     const int nF = S.push_nF, n = nF + S.push_nS;
+    const int po = S.push_o;                  // o, or the joint slot it woke
     __threadfence();                          // this thread's share of the ray range words (thread 0: state, counters)
     epi_bar_sync();                           // ... of every thread, before the first slot is published
     for (int j = tid; j < n; j += kTcEpiThreads)
-      *reinterpret_cast<volatile int*>(q.q_flag + base + j) = ((j < nF) ? make_item(MODE_RAYFWD, o, j) : make_item(MODE_SDF, o, j - nF)) + 1;
+      *reinterpret_cast<volatile int*>(q.q_flag + base + j) = ((j < nF) ? make_item(MODE_RAYFWD, po, j) : make_item(MODE_SDF, po, j - nF)) + 1;
   }
 }
 

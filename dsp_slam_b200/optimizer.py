@@ -256,14 +256,32 @@ class BatchSolver:
         self.n_obj = len(objs)
         return out
 
-    def keyframe(self, objs, modes):
-        """Joint and pose-only objects in one call: modes[i] = _lib.MODE_JOINT (reconstruct) or MODE_POSE (estimate_pose)."""
+    def keyframe(self, objs, modes, gates=None):
+        """Joint and pose-only objects in one call: modes[i] = _lib.MODE_JOINT (reconstruct) or MODE_POSE (estimate_pose).
+        gates: None, or one entry per object: None (not gated) or dict(t_cam_obj_map, t_cam_obj_sim3) for a pose-only
+        object checked against the map's prediction (dspgn_keyframe_batch_gated); the record's `gate` word tells
+        _lib.GATE_KEPT (pose-only record) from _lib.GATE_REJECTED (the joint record of the detection from t_cam_obj_sim3)."""
         m = _modes_array(modes)
         if len(m) != len(objs):
             raise ValueError(f"{len(m)} modes for {len(objs)} objects")
         arr, keep = self._pack(objs)
         out = (_lib.ObjectOut * len(objs))()
-        _lib.check(_lib.load().dspgn_keyframe_batch(self.handle, len(objs), arr, m, out))
+        if gates is None:
+            _lib.check(_lib.load().dspgn_keyframe_batch(self.handle, len(objs), arr, m, out))
+        else:
+            if len(gates) != len(objs):
+                raise ValueError(f"{len(gates)} gates for {len(objs)} objects")
+            g = (_lib.GateIn * len(objs))()
+            for i, d in enumerate(gates):
+                if d is None:
+                    continue
+                Tm = np.ascontiguousarray(d["t_cam_obj_map"], dtype=np.float32).reshape(4, 4)
+                Ts = np.ascontiguousarray(d["t_cam_obj_sim3"], dtype=np.float32).reshape(4, 4)
+                keep.append((Tm, Ts))
+                g[i].t_cam_obj_map = Tm.ctypes.data_as(_FP); g[i].map_rs = 4; g[i].map_cs = 1
+                g[i].t_cam_obj_sim3 = Ts.ctypes.data_as(_FP); g[i].sim3_rs = 4; g[i].sim3_cs = 1
+                g[i].gate = 1
+            _lib.check(_lib.load().dspgn_keyframe_batch_gated(self.handle, len(objs), arr, m, g, out))
         self.n_obj = len(objs)
         return out
 
@@ -431,20 +449,42 @@ class Optimizer(object):
         """The stereo keyframe's two passes (src/LocalMapping.cc:88-95) as ONE library call: reconstruct_batch(new_objects)
         (CreateNewMapObjects) and estimate_pose_batch(tracked_objects) (GetNewObservations; dicts with t_cam_obj, pts,
         code, scale).  Returns (results, poses) or (results, poses, status) with exactly the values of those two calls:
-        a failed pose comes back as the input pose."""
+        a failed pose comes back as the input pose.
+
+        A tracked dict that also carries t_cam_obj_map (Tcw * Two, the pose the map predicts), t_cam_obj_sim3
+        (det->Sim3Tco), rays and depth is gated: GetNewObservations' check of a static map object with more than two
+        observations (src/LocalMapping_util.cc:104-147) runs on the device, and a detection that fails it is
+        reconstructed in the same call like CreateNewMapObjects does (:179).  Then the call returns one more list,
+        `rejected`: per tracked object None, or the reconstruct_object-shaped result of the rejected detection (whose
+        pose and status entries are None)."""
         objs = list(new_objects) + list(tracked_objects)
         n_new = len(new_objects)
+        gate_keys = ("t_cam_obj_map", "t_cam_obj_sim3", "rays", "depth")
+        gates = [dict(t_cam_obj_map=o["t_cam_obj_map"], t_cam_obj_sim3=o["t_cam_obj_sim3"])
+                 if all(o.get(k) is not None for k in gate_keys) else None for o in tracked_objects]
+        gated = any(g is not None for g in gates)
         if not objs:
             return ([], [], []) if return_status else ([], [])
-        out = self.solver.keyframe(objs, [_lib.MODE_JOINT] * n_new + [_lib.MODE_POSE] * (len(objs) - n_new))
+        out = self.solver.keyframe(objs, [_lib.MODE_JOINT] * n_new + [_lib.MODE_POSE] * (len(objs) - n_new),
+                                   [None] * n_new + gates if gated else None)
         results = _unpack_all(out, n_new, self.code_len) if n_new else []
-        Ts, st = [], []
+        Ts, st, rejected = [], [], []
         for i, o in enumerate(tracked_objects):
-            s = int(out[n_new + i].status)
+            rec = out[n_new + i]
+            if rec.gate == _lib.GATE_REJECTED:
+                from .distributed import records_to_results
+                raw = np.frombuffer(rec, dtype=np.float32, count=_lib.RESULT_FLOATS).reshape(1, -1)
+                rejected.append(records_to_results(raw, self.code_len)[0])
+                Ts.append(None)
+                st.append(None)
+                continue
+            rejected.append(None)
+            s = int(rec.status)
             st.append(s)
-            Ts.append(np.array(out[n_new + i].t_cam_obj[:], dtype=np.float32).reshape(4, 4) if s == _lib.ST_OK
+            Ts.append(np.array(rec.t_cam_obj[:], dtype=np.float32).reshape(4, 4) if s == _lib.ST_OK
                       else np.array(o["t_cam_obj"], dtype=np.float32).reshape(4, 4))
-        return (results, Ts, st) if return_status else (results, Ts)
+        ret = (results, Ts, st) if return_status else (results, Ts)
+        return ret + (rejected,) if gated else ret
 
 
 def create_voxel_grid(vol_dim=128):

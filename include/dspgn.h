@@ -14,6 +14,9 @@
  *   Optimizer.__init__           (reconstruct/optimizer.py:27)  dspgn_solver_create
  *   Optimizer.reconstruct_object (reconstruct/optimizer.py:88)  dspgn_reconstruct_batch
  *   Optimizer.estimate_pose_cam_obj (optimizer.py:45)           dspgn_estimate_pose_batch
+ *   one stereo keyframe's two passes (LocalMapping.cc:88-95)     dspgn_keyframe_batch
+ *   ... with GetNewObservations' map check (LocalMapping_util.cc:104-147) and the demoted detections'
+ *       reconstruction in CreateNewMapObjects (:179)             dspgn_keyframe_batch_gated
  *   loss_utils.decode_sdf        (reconstruct/loss_utils.py:51) dspgn_decode_sdf
  *   loss.compute_sdf_loss / compute_render_loss (loss.py:22,46) dspgn_debug_system (test hook)
  *
@@ -135,7 +138,8 @@ typedef struct {
   int32_t n_valid;                /* V: ray samples inside the unit sphere, last iteration */
   int32_t n_band;                 /* m: band rows kept, last iteration */
   int32_t iters_done;
-  int32_t pad_[3];
+  int32_t gate;                   /* dspgn_keyframe_batch_gated: DSPGN_GATE_*; 0 everywhere else */
+  int32_t pad_[2];
 } DspgnObjectOut;                 /* 88 floats */
 
 /* device-side result record (same layout), for callers that keep results on the GPU */
@@ -186,6 +190,29 @@ const float* dspgn_results_device(DspgnSolver* s);
 int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes);
 /* whole call: upload + run + results, walked in resident chunks of 1024 like dspgn_reconstruct_batch */
 int dspgn_keyframe_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, DspgnObjectOut* out);
+
+/* The keyframe call with the consistency check of GetNewObservations (src/LocalMapping_util.cc:104-147) on the device,
+ * and the joint reconstruction of CreateNewMapObjects (:179) for every tracked detection that fails it, in the same run.
+ * For a gated object (gate = 1, mode DSPGN_MODE_POSE) the pose-only estimate Zco -- the record's pose, or the input
+ * t_cam_obj after a pose-only soft failure -- is compared with the pose the map predicts, Tco = t_cam_obj_map:
+ *   dist2D = |(Zco - Tco) translation x, z| (fp32)  and  e = |log(Tco^-1 Zco)| (SE3Quat, fp64).
+ * dist2D < 1 && e < 1.5: out.gate = DSPGN_GATE_KEPT and the record is the pose-only record.  Otherwise the detection is
+ * new again: out.gate = DSPGN_GATE_REJECTED and the record is exactly what dspgn_reconstruct_batch returns for the
+ * object's DspgnObjectIn with t_cam_obj = t_cam_obj_sim3 and code = NULL (so a gated object carries its rays / depths).
+ * The static-object and Observations() > 2 conditions stay with the caller (gate = 0 for the others).  gates = NULL is
+ * dspgn_keyframe_batch.  A gate on a joint object, a gate without both matrices, a gate value outside {0, 1} or a gated
+ * object with t_cam_world returns DSPGN_E_ARG before anything is enqueued.  A gated object and its joint run occupy two
+ * slots of a resident batch of 1024. */
+#define DSPGN_GATE_OFF 0        /* not gated */
+#define DSPGN_GATE_KEPT 1       /* consistent with the map: the pose-only record */
+#define DSPGN_GATE_REJECTED 2   /* inconsistent: the joint record of the detection */
+typedef struct {
+  const float* t_cam_obj_map;  int32_t map_rs, map_cs;   /* iniSE3Tco = Tcw * Two (SE3), LocalMapping_util.cc:106 */
+  const float* t_cam_obj_sim3; int32_t sim3_rs, sim3_cs; /* det->Sim3Tco: the joint run's initial pose */
+  int32_t gate;   /* 1: static map object with Observations() > 2 -> apply the check; 0: plain pose-only */
+} DspgnGateIn;
+int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
+                               const DspgnGateIn* gates /* n_obj entries, or NULL */, DspgnObjectOut* out);
 
 /* Forward-only decode (loss_utils.decode_sdf): x (n,3) host, strides in elements -> sdf (n,) host. */
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n,
