@@ -114,7 +114,6 @@ SYMBOLS = [
     ("dspgn_debug_exp", C.c_int, [C.c_int, C.c_int, _FP, C.c_int, _FP]),
     ("dspgn_debug_system", C.c_int, [_VP, C.c_int, C.c_int, _FP, _FP, _FP, _FP, _FP, _FP]),
     ("dspgn_debug_system_iter", C.c_int, [_VP, C.c_int, C.c_int, C.c_int, _FP, _FP, _FP, _FP, _FP, _FP]),
-    ("dspgn_debug_clocks", C.c_int, [_VP, C.POINTER(C.c_longlong), C.c_int]),
     ("dspgn_debug_inputs", C.c_int, [_VP, C.c_int, _FP, _FP, _FP]),
     ("dspgn_debug_events", C.c_int, [_VP, C.POINTER(C.c_longlong), C.c_int]),
     ("dspgn_tc_selftest", C.c_int, [C.c_int, C.c_int, C.c_int, _FP, _FP, _FP]),

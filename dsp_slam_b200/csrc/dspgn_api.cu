@@ -98,21 +98,20 @@ struct DspgnSolver {
   DevBuf d_q_flag, d_q_ctr, d_tiles_left, d_obj_iter;   // persistent-kernel work queue
   int* d_tbase_static = nullptr;   // [n_obj] first 128-row SDF tile of each object (inside the staging block)
   int* d_tbase_r_static = nullptr; // [n_obj] first band-tile partial slot of each object (capacity: its ray-sample tiles + 1)
-  // per-run object table: mode [n_obj] | first iteration-0 queue slot of the persistent kernel [n_obj]
+  // per-run object table (layout: run_table)
   DevBuf d_run;
   HostBuf h_run;                   // pinned staging of the table; rewritten only after ev_run_upload
   cudaEvent_t ev_run_upload = nullptr;
   bool run_upload_pending = false;
   bool run_table_valid = false;    // d_run holds h_run for the resident batch (a repeated run skips the copy)
-  bool run_table_gated = false;    // ... and it is the table of a gated run (link | t_map after the two int arrays)
+  bool run_table_gated = false;    // ... and it is the table of a gated run (it has link and t_map)
   int total_tiles128 = 0;          // SDF tiles of the batch
   long long total_ray_tiles128 = 0;// ray-sample tiles of the batch
   int max_tiles128 = 0;            // largest tile count of one term of one object (queue items hold 19 bits)
   bool mega_enabled = true;
   bool compact_rays = true;        // persistent kernel, render term: forward-only tiles over the valid-sample hulls only (env DSPGN_COMPACT_RAYS=0: all n_rays x D samples)
-  bool vpre_exact = false;         // env DSPGN_VPRE_EXACT=1: exhaustive valid-range pre-pass (A/B switch)
-  DevBuf d_clk, d_ev, d_seg, d_ln, d_vpre;
-  bool clk_on = false;
+  DevBuf d_ev, d_seg, d_ln, d_vpre;
+  bool events_on = false;          // env DSPGN_CLK: the persistent kernel writes its event log (dspgn_debug_events)
   HostBuf h_results;
   // counters
   DspgnCounters ctr{};
@@ -300,7 +299,6 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, device));
   s->num_sms = prop.multiProcessorCount;
-  if (const char* g = getenv("DSPGN_GRID")) { int v = atoi(g); if (v >= 1 && v <= s->num_sms) s->num_sms = v; }   // experiments only
   for (int c = 0; c < n_classes; ++c) s->classes.push_back(classes[c]);
   std::vector<DecoderDev> decs;
   for (auto* d : s->classes) decs.push_back(d->dev);
@@ -326,16 +324,10 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
   if (int rc = tc_setup_kernels(g_err)) { dspgn_solver_destroy(s); return rc; }
   if (const char* m = getenv("DSPGN_MEGA")) s->mega_enabled = (m[0] != '0');
   if (const char* m = getenv("DSPGN_COMPACT_RAYS")) s->compact_rays = (m[0] != '0');   // A/B switch of the valid-sample hulls
-  if (const char* m = getenv("DSPGN_VPRE_EXACT")) s->vpre_exact = (m[0] != '0');
   if (cfg->schedule == DSPGN_SCHED_LAUNCHES) s->mega_enabled = false;
   else if (cfg->schedule == DSPGN_SCHED_PERSISTENT) s->mega_enabled = true;
   else if (cfg->schedule != DSPGN_SCHED_AUTO) { dspgn_solver_destroy(s); return fail(DSPGN_E_ARG, "bad schedule"); }
-  if (getenv("DSPGN_CLK")) {
-    const size_t nb = sizeof(long long) * (kClkTiles * kTcMaxSteps * kClkSlots + 16);
-    if (s->d_clk.reserve(nb)) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
-    CU(cudaMemset(s->d_clk.p, 0, nb));
-    s->clk_on = true;
-  }
+  s->events_on = getenv("DSPGN_CLK") != nullptr;
   CU(cudaEventCreateWithFlags(&s->ev_upload, cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(&s->ev_run_upload, cudaEventDisableTiming));
   CU(cudaStreamCreateWithFlags(&s->stream2, cudaStreamNonBlocking));
@@ -360,7 +352,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   cudaDeviceSynchronize();
   dspgn_gather_close(s);
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
-                    &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_clk, &s->d_q_flag, &s->d_q_ctr,
+                    &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
                     &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_run}) b->release();
   s->h_stage.release();
   s->h_results.release();
@@ -563,18 +555,19 @@ cudaEvent_t next_event(DspgnSolver* s) {
   return s->ev[s->ev_used++];
 }
 
-int launch_term(DspgnSolver* s, TermArgs& a, long long rows_upper, cudaStream_t stream = nullptr, bool use_given = false) {
+int launch_term(DspgnSolver* s, const BatchDev& b, const TermArgs& a, long long rows_upper, cudaStream_t stream = nullptr,
+                bool use_given = false) {
   cudaStream_t st = use_given ? stream : s->stream;
   const bool timed = s->timing && !use_given;
   if (timed) cudaEventRecord(next_event(s), st);
   const long long tile_rows = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
   long long tiles = (rows_upper + tile_rows - 1) / tile_rows + s->n_obj;
   if (s->engine == DSPGN_ENGINE_TC) {
-    if (int rc = tc_launch_term(a, s->num_sms, tiles, st, g_err)) return rc;
+    if (int rc = tc_launch_term(b, a, s->num_sms, tiles, st, g_err)) return rc;
   } else {
     int grid = (int)std::min<long long>(tiles, s->num_sms);
     if (grid < 1) grid = 1;
-    k_decoder_simt<<<grid, kThreads, sizeof(SimtSmem), st>>>(a);
+    k_decoder_simt<<<grid, kThreads, sizeof(SimtSmem), st>>>(b, a);
   }
   if (timed) cudaEventRecord(next_event(s), st);
   s->ctr.kernel_launches++;
@@ -584,18 +577,38 @@ int launch_term(DspgnSolver* s, TermArgs& a, long long rows_upper, cudaStream_t 
 
 TermArgs base_term(DspgnSolver* s, int mode) {
   TermArgs a{};
-  a.meta = s->d_meta; a.state = s->d_state.as<ObjState>(); a.decs = s->d_decs.as<DecoderDev>();
-  a.n_obj = s->n_obj; a.n_classes = (int)s->classes.size(); a.mode = mode;
-  a.pts = s->d_pts; a.pt_active = nullptr; a.cut_iter = -1; a.iter = 0; a.rays = s->d_rays;
-  a.band_x = s->d_bx.as<float>(); a.band_s = s->d_bs.as<float>(); a.band_r = s->d_br.as<float>();
-  a.band_m = s->d_m.as<int>(); a.sdf_out = s->d_sdf.as<float>(); a.V_count = s->d_V.as<int>();
+  a.mode = mode;
+  a.pt_active = nullptr; a.cut_iter = -1; a.iter = 0;
   a.part = (mode == MODE_BAND) ? s->d_part_r.as<float>() : (mode == MODE_SDF ? s->d_part_s.as<float>() : nullptr);
   a.tile_base = (mode == MODE_BAND) ? s->d_tbase.as<int>() + s->n_obj : (mode == MODE_SDF ? s->d_tbase.as<int>() : nullptr);
-  a.D = s->cfg.num_depth_samples;
   a.ln_scratch = s->d_ln.as<float>();
   a.dbg_J = nullptr; a.dbg_res = nullptr; a.dbg_obj = -1; a.dbg_P = 0;
-  a.dbg_clk = (s->clk_on && mode == MODE_SDF) ? s->d_clk.as<long long>() : nullptr;
   return a;
+}
+
+// The per-run object table, staged in h_run and copied to d_run: modes [n] | first iteration-0 queue slot of the
+// persistent kernel [n] | link [n] | t_map [n][16] (the last two in a gated run only).
+struct RunTable { int* modes; int* q0_off; int* link; float* t_map; };
+size_t run_table_bytes(int n, bool gated) { return (gated ? 12 + 64 : 8) * (size_t)n; }
+RunTable run_table(void* base, int n, bool gated) {
+  int* p = static_cast<int*>(base);
+  return RunTable{p, p + n, gated ? p + 2 * n : nullptr, gated ? reinterpret_cast<float*>(p + 3 * n) : nullptr};
+}
+
+// The resident batch and its run table as the kernels see them.  Call after plan_run (it may move d_run) and after
+// every buffer reservation of the run.
+BatchDev batch_dev(DspgnSolver* s) {
+  BatchDev b{};
+  b.meta = s->d_meta; b.state = s->d_state.as<ObjState>(); b.decs = s->d_decs.as<DecoderDev>();
+  b.n_obj = s->n_obj; b.n_classes = (int)s->classes.size(); b.D = s->cfg.num_depth_samples;
+  b.pts = s->d_pts; b.rays = s->d_rays; b.depth_fg = s->d_depth; b.T_init = s->d_Tinit; b.code_init = s->d_code;
+  b.sdf = s->d_sdf.as<float>(); b.band_x = s->d_bx.as<float>(); b.band_s = s->d_bs.as<float>(); b.band_r = s->d_br.as<float>();
+  b.band_m = s->d_m.as<int>(); b.V_count = s->d_V.as<int>();
+  b.results = s->d_results.as<float>();
+  b.gather = s->gdev;
+  const RunTable t = run_table(s->d_run.p, s->n_obj, s->run_table_gated);
+  b.modes = t.modes; b.q0_off = t.q0_off; b.link = t.link; b.t_map = t.t_map;
+  return b;
 }
 
 // What a run does with the resident batch, given one mode per object: iteration counts and row counters per mode, and
@@ -612,8 +625,8 @@ struct RunPlan {
   bool any_dormant;        // ... and has joint slots that only run when their pose-only object is rejected
 };
 
-// Checks the modes, fills the plan and stages the per-run object table (modes | first iteration-0 queue slot of each
-// object [| link | t_map of a gated run]) into d_run, async on the stream; `unlimited`: objects never finish (the debug
+// Checks the modes, fills the plan and stages the per-run object table (run_table) into d_run, async on the stream;
+// `unlimited`: objects never finish (the debug
 // hooks advance the batch freely).  link[o] >= 0 on a joint object marks the dormant joint slot of pose-only object
 // link[o]: it counts towards the queue capacity and the render term but reserves no iteration-0 slot and no row counter.
 int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = false, const int32_t* link = nullptr,
@@ -632,13 +645,14 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
   p.iters[DSPGN_MODE_POSE] = unlimited ? (1 << 30) : c.pose_only_iterations;
   p.render = (p.any[DSPGN_MODE_JOINT] || p.any_dormant) && !c.sdf_only;
   if (s->run_upload_pending) { CU(cudaEventSynchronize(s->ev_run_upload)); s->run_upload_pending = false; }
-  const size_t bytes = (p.gated ? 12 + 64 : 8) * (size_t)n;
-  const bool same = s->run_table_valid && !p.gated && !s->run_table_gated && memcmp(s->h_run.p, modes, 4 * (size_t)n) == 0;
+  const size_t bytes = run_table_bytes(n, p.gated);
+  const bool same = s->run_table_valid && !p.gated && !s->run_table_gated &&
+                    memcmp(run_table(s->h_run.p, n, false).modes, modes, 4 * (size_t)n) == 0;
   if (!same) {
     if (s->d_run.cap < bytes) CU(cudaStreamSynchronize(s->stream));      // kernels of an earlier run may still read it
     if (s->h_run.reserve(bytes) || s->d_run.reserve(bytes)) return fail(DSPGN_E_ALLOC, "run table allocation failed");
   }
-  int* h = s->h_run.as<int>();
+  const RunTable h = run_table(s->h_run.p, n, p.gated);
   for (int o = 0; o < n; ++o) {
     const ObjMeta& M = s->h_meta[o];
     const int m = modes[o];
@@ -652,16 +666,16 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
     // per iteration: every SDF tile, every ray-sample tile, one scan item per 64 rays and at most as many band tiles
     // as ray-sample tiles (iteration 0 reserves every ray-sample tile of the object)
     p.q_cap += (long long)p.iters[m] * (ntS + (r ? 2 * ntF + (M.n_rays + kScanChunkRays - 1) / kScanChunkRays : 0));
-    if (!same) { h[o] = m; h[n + o] = p.total0; }
+    if (!same) { h.modes[o] = m; h.q0_off[o] = p.total0; }
     if (!dormant) p.total0 += (int)(ntS + (r ? ntF : 0));
   }
   if (p.gated) {
-    memcpy(h + 2 * n, link, 4 * (size_t)n);
-    memcpy(h + 3 * n, t_map, 64 * (size_t)n);
+    memcpy(h.link, link, 4 * (size_t)n);
+    memcpy(h.t_map, t_map, 64 * (size_t)n);
   }
   s->run_table_gated = p.gated;
   if (!same) {
-    CU(cudaMemcpyAsync(s->d_run.p, h, bytes, cudaMemcpyHostToDevice, s->stream));
+    CU(cudaMemcpyAsync(s->d_run.p, s->h_run.p, bytes, cudaMemcpyHostToDevice, s->stream));
     CU(cudaEventRecord(s->ev_run_upload, s->stream));
     s->run_upload_pending = true;
     s->run_table_valid = true;
@@ -669,51 +683,22 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
   return 0;
 }
 
-int launch_init(DspgnSolver* s, const RunPlan& p, bool mega = false) {
+// q: the persistent kernel's queue (mega_args) when it runs next, else empty
+int launch_init(DspgnSolver* s, const BatchDev& b, const RunPlan& p, const MegaArgs& q = MegaArgs{}) {
   InitArgs ia{};
-  ia.meta = s->d_meta; ia.state = s->d_state.as<ObjState>(); ia.T_init = s->d_Tinit; ia.code_init = s->d_code;
-  ia.V_count = s->d_V.as<int>(); ia.band_m = s->d_m.as<int>();
-  ia.n_obj = s->n_obj; ia.code_len = s->cfg.code_len; ia.D = s->cfg.num_depth_samples;
-  ia.modes = s->d_run.as<int>(); ia.n_iter_joint = p.iters[DSPGN_MODE_JOINT]; ia.n_iter_pose = p.iters[DSPGN_MODE_POSE];
-  ia.gather = s->gdev; ia.results = s->d_results.as<float>(); ia.n_bad = s->n_bad;
-  ia.decs = s->d_decs.as<DecoderDev>();
-  if (p.gated) { ia.link = s->d_run.as<int>() + 2 * s->n_obj; ia.t_map = reinterpret_cast<const float*>(s->d_run.as<int>() + 3 * s->n_obj); }
-  ia.mega = mega ? 1 : 0;
-  if (mega) {
-    const bool render = p.render;
-    ia.render = render ? 1 : 0;
-    ia.q0_off = s->d_run.as<int>() + s->n_obj; ia.tile_rows = kTcRows;
-    ia.q_flag = s->d_q_flag.as<int>();
-    ia.q_head = s->d_q_ctr.as<int>(); ia.q_tail = s->d_q_ctr.as<int>() + 32; ia.done_objects = s->d_q_ctr.as<int>() + 64;
-    ia.band_rows_total = s->d_q_ctr.as<int>() + 80; ia.abort_flag = s->d_q_ctr.as<int>() + 96;
-    ia.pending = s->d_tiles_left.as<int>(); ia.ray_left = s->d_tiles_left.as<int>() + s->n_obj;
-    ia.obj_iter = s->d_obj_iter.as<int>();
-    ia.total_tiles0 = p.total0;
-    ia.vpre_exact = s->vpre_exact ? 1 : 0;
-    ia.rays = s->d_rays; ia.vpre = (render && s->compact_rays) ? s->d_vpre.as<int>() : nullptr;
-    ia.valid_rows_total = reinterpret_cast<unsigned long long*>(s->d_q_ctr.as<int>() + 88);
-  }
-  k_init<<<s->n_obj, 128, 0, s->stream>>>(ia);
+  ia.code_len = s->cfg.code_len;
+  ia.n_iter_joint = p.iters[DSPGN_MODE_JOINT]; ia.n_iter_pose = p.iters[DSPGN_MODE_POSE];
+  ia.n_bad = s->n_bad;
+  k_init<<<s->n_obj, 128, 0, s->stream>>>(b, ia, q);
   s->ctr.kernel_launches++;
   CU(cudaGetLastError());
   return 0;
 }
 
-ScanArgs base_scan(DspgnSolver* s) {
-  const DspgnConfig& c = s->cfg;
-  ScanArgs sa{};
-  sa.meta = s->d_meta; sa.state = s->d_state.as<ObjState>(); sa.rays = s->d_rays; sa.depth_fg = s->d_depth;
-  sa.sdf = s->d_sdf.as<float>(); sa.band_x = s->d_bx.as<float>(); sa.band_s = s->d_bs.as<float>();
-  sa.band_r = s->d_br.as<float>(); sa.band_m = s->d_m.as<int>(); sa.th = c.cut_off; sa.D = c.num_depth_samples;
-  sa.n_obj = s->n_obj;
-  sa.V_count = s->d_V.as<int>();
-  return sa;
-}
-
 // one GN iteration's residual-term kernels (everything before the solve); objects past their own last iteration
 // contribute no rows
-int launch_terms(DspgnSolver* s, const RunPlan& p, int iter, float* dbg_J = nullptr, float* dbg_res = nullptr, int dbg_obj = -1,
-                 int dbg_P = 0) {
+int launch_terms(DspgnSolver* s, const BatchDev& b, const RunPlan& p, int iter, float* dbg_J = nullptr, float* dbg_res = nullptr,
+                 int dbg_obj = -1, int dbg_P = 0) {
   const DspgnConfig& c = s->cfg;
   const bool render = p.render && p.any[DSPGN_MODE_JOINT] && iter < p.iters[DSPGN_MODE_JOINT];
   // The SDF-row pass and the forward-only pass over the ray samples are independent: fork the latter onto a
@@ -726,10 +711,10 @@ int launch_terms(DspgnSolver* s, const RunPlan& p, int iter, float* dbg_J = null
     if (fork) {
       CU(cudaEventRecord(s->ev_fork, s->stream));
       CU(cudaStreamWaitEvent(s->stream2, s->ev_fork, 0));
-      if (int rc = launch_term(s, f, s->tot_smp, s->stream2, true)) return rc;
+      if (int rc = launch_term(s, b, f, s->tot_smp, s->stream2, true)) return rc;
       CU(cudaEventRecord(s->ev_join, s->stream2));
     } else {
-      if (int rc = launch_term(s, f, s->tot_smp)) return rc;
+      if (int rc = launch_term(s, b, f, s->tot_smp)) return rc;
     }
     s->ctr.rows_fwd_only += p.smp_joint;
   }
@@ -739,20 +724,19 @@ int launch_terms(DspgnSolver* s, const RunPlan& p, int iter, float* dbg_J = null
     a.iter = iter;
     a.pt_active = s->d_active.as<uint8_t>(); a.cut_iter = 4;   // optimizer.py:76-78: inlier cut taken after iteration index 4
     a.dbg_J = dbg_J; a.dbg_res = dbg_res; a.dbg_obj = dbg_obj; a.dbg_P = dbg_P;
-    if (int rc = launch_term(s, a, s->tot_pts)) return rc;
+    if (int rc = launch_term(s, b, a, s->tot_pts)) return rc;
     for (int m = 0; m < 2; ++m)
       if (iter < p.iters[m]) s->ctr.rows_fwd_bwd += p.pts[m];
   }
   if (render) {
     if (fork) CU(cudaStreamWaitEvent(s->stream, s->ev_join, 0));
-    ScanArgs sa = base_scan(s);
-    k_ray_scan<<<s->n_obj, kScanThreads, 0, s->stream>>>(sa);
+    k_ray_scan<<<s->n_obj, kScanThreads, 0, s->stream>>>(b, c.cut_off);
     s->ctr.kernel_launches++;
     CU(cudaGetLastError());
-    TermArgs b = base_term(s, MODE_BAND);
-    b.huber_b = c.b1;
-    b.iter = iter;
-    if (int rc = launch_term(s, b, s->tot_smp)) return rc;
+    TermArgs band = base_term(s, MODE_BAND);
+    band.huber_b = c.b1;
+    band.iter = iter;
+    if (int rc = launch_term(s, b, band, s->tot_smp)) return rc;
   }
   return 0;
 }
@@ -760,18 +744,40 @@ int launch_terms(DspgnSolver* s, const RunPlan& p, int iter, float* dbg_J = null
 SolveArgs base_solve(DspgnSolver* s) {
   const DspgnConfig& c = s->cfg;
   SolveArgs v{};
-  v.meta = s->d_meta; v.state = s->d_state.as<ObjState>();
   v.part_s = s->d_part_s.as<float>(); v.part_r = s->d_part_r.as<float>();
   v.base_s = s->d_tbase.as<int>(); v.base_r = s->d_tbase.as<int>() + s->n_obj;
   v.tile_rows = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
-  v.V_count = s->d_V.as<int>(); v.band_m = s->d_m.as<int>();
   v.prm = SolverParams{c.k1, c.k2, c.k3, c.k4, c.b1, c.b2, c.lr, c.s_damp, c.code_len, c.num_depth_samples, c.cut_off, c.sdf_only};
-  v.n_obj = s->n_obj; v.results = s->d_results.as<float>();
-  v.gather = s->gdev;
-  v.decs = s->d_decs.as<DecoderDev>();
   v.dbg_obj = -1; v.dbg_H = nullptr; v.dbg_b = nullptr; v.dbg_dx = nullptr; v.dbg_loss = nullptr;
-  v.dbg_clk = s->clk_on ? s->d_clk.as<long long>() + kClkTiles * kTcMaxSteps * kClkSlots : nullptr;
   return v;
+}
+
+// The persistent kernel's work queue for the run: reserves its buffers and builds its MegaArgs (k_init seeds it, the
+// kernel runs on it).
+int mega_args(DspgnSolver* s, const RunPlan& p, MegaArgs& q) {
+  const bool render = p.render;
+  const int cap = (int)p.q_cap;
+  const int n = s->n_obj;
+  const size_t nseg_cap = (size_t)s->tot_rays / kSegRays + 2 * (size_t)n + 4;
+  int bad = 0;
+  bad |= s->d_q_flag.reserve(4 * (size_t)cap);
+  bad |= s->d_q_ctr.reserve(sizeof(QueueCounters));
+  bad |= s->d_tiles_left.reserve(4 * 3 * (size_t)n);
+  if (render) bad |= s->d_seg.reserve(4 * 2 * nseg_cap);
+  if (render && s->compact_rays) bad |= s->d_vpre.reserve(4 * ((size_t)s->tot_rays + (size_t)n + 4));
+  bad |= s->d_obj_iter.reserve(4 * (size_t)n);
+  if (s->events_on) bad |= s->d_ev.reserve(8 * (1 + 2 * (size_t)kEvCap));
+  if (bad) return fail(DSPGN_E_ALLOC, "queue allocation failed");
+  q = MegaArgs{};
+  q.q_cap = cap; q.render = render ? 1 : 0; q.total0 = p.total0;
+  q.q_flag = s->d_q_flag.as<int>();
+  q.ctr = s->d_q_ctr.as<QueueCounters>();
+  q.pending = s->d_tiles_left.as<int>(); q.ray_left = s->d_tiles_left.as<int>() + n; q.scan_left = s->d_tiles_left.as<int>() + 2 * n;
+  q.seg_cnt = s->d_seg.as<int>(); q.seg_prefix = s->d_seg.as<int>() + nseg_cap;
+  q.obj_iter = s->d_obj_iter.as<int>();
+  q.vpre = (render && s->compact_rays) ? s->d_vpre.as<int>() : nullptr;
+  if (s->events_on) q.log = EventLog{s->d_ev.as<long long>(), kEvCap};
+  return 0;
 }
 
 }  // namespace
@@ -786,12 +792,7 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
   CU(cudaSetDevice(s->device));
   RunPlan p;
   if (int rc = plan_run(s, modes, p, false, link, t_map)) return rc;
-  auto gate_args = [&](SolveArgs& v) {
-    if (!p.gated) return;
-    v.link = s->d_run.as<int>() + 2 * s->n_obj;
-    v.t_map = reinterpret_cast<const float*>(s->d_run.as<int>() + 3 * s->n_obj);
-    v.T_init = s->d_Tinit;
-  };
+  const BatchDev b = batch_dev(s);
   const int max_iters = std::max(p.any[DSPGN_MODE_JOINT] ? p.iters[DSPGN_MODE_JOINT] : 0,
                                  p.any[DSPGN_MODE_POSE] ? p.iters[DSPGN_MODE_POSE] : 0);
   s->ctr = DspgnCounters{};
@@ -804,51 +805,22 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
                     s->max_tiles128 <= kItemTileMask && s->n_obj <= kItemObjMask + 1 && p.q_cap < (1LL << 27);
   if (mega) {
     // ---- persistent object-pipelined kernel: every GN iteration of every object in ONE launch --------------
-    const int cap = (int)p.q_cap;
-    int bad = 0;
-    bad |= s->d_q_flag.reserve(4 * (size_t)cap);
-    bad |= s->d_q_ctr.reserve(4 * 128);
-    bad |= s->d_tiles_left.reserve(4 * 3 * (size_t)s->n_obj);
-    const size_t nseg_cap = (size_t)s->tot_rays / kSegRays + 2 * (size_t)s->n_obj + 4;
-    if (render) bad |= s->d_seg.reserve(4 * 2 * nseg_cap);
-    if (render && s->compact_rays) bad |= s->d_vpre.reserve(4 * ((size_t)s->tot_rays + (size_t)s->n_obj + 4));
-    bad |= s->d_obj_iter.reserve(4 * (size_t)s->n_obj);
-    if (bad) return fail(DSPGN_E_ALLOC, "queue allocation failed");
-    CU(cudaMemsetAsync(s->d_q_flag.p, 0, 4 * (size_t)cap, s->stream));
-    if (int rc = launch_init(s, p, true)) return rc;
+    MegaArgs q;
+    if (int rc = mega_args(s, p, q)) return rc;
+    CU(cudaMemsetAsync(q.q_flag, 0, 4 * (size_t)q.q_cap, s->stream));
+    if (int rc = launch_init(s, b, p, q)) return rc;
     TermArgs a = base_term(s, MODE_SDF);
     a.huber_b = s->cfg.b2;                   // pose-only objects: raw residuals (term_huber)
     a.huber_b1 = s->cfg.b1;
     a.tile_base = s->d_tbase_static;
     a.part_r = s->d_part_r.as<float>(); a.tile_base_r = s->d_tbase_r_static;
-    a.dbg_clk = nullptr;
     if (p.any[DSPGN_MODE_POSE] && p.iters[DSPGN_MODE_POSE] > 5) { a.pt_active = s->d_active.as<uint8_t>(); a.cut_iter = 4; }
-    MegaArgs q{};
-    q.q_cap = cap; q.render = render ? 1 : 0;
-    q.q_flag = s->d_q_flag.as<int>();
-    q.q_head = s->d_q_ctr.as<int>(); q.q_tail = s->d_q_ctr.as<int>() + 32; q.done_objects = s->d_q_ctr.as<int>() + 64;
-    q.band_rows_total = s->d_q_ctr.as<int>() + 80;
-    q.abort_flag = s->d_q_ctr.as<int>() + 96;
-    q.pending = s->d_tiles_left.as<int>(); q.ray_left = s->d_tiles_left.as<int>() + s->n_obj; q.obj_iter = s->d_obj_iter.as<int>();
-    q.scan_left = s->d_tiles_left.as<int>() + 2 * s->n_obj;
-    q.seg_cnt = s->d_seg.as<int>(); q.seg_prefix = s->d_seg.as<int>() + nseg_cap;
-    q.valid_rows_total = reinterpret_cast<unsigned long long*>(s->d_q_ctr.as<int>() + 88);
-    q.vpre = (render && s->compact_rays) ? s->d_vpre.as<int>() : nullptr;
-    q.vpre_exact = s->vpre_exact ? 1 : 0;
-    if (s->clk_on) {
-      if (s->d_ev.reserve(8 * (1 + 2 * (size_t)kEvCap))) return fail(DSPGN_E_ALLOC, "cudaMalloc");
-      CU(cudaMemsetAsync(s->d_ev.p, 0, 8, s->stream));
-      q.ev = s->d_ev.as<long long>(); q.ev_cap = kEvCap;
-    }
+    if (q.log.ev) CU(cudaMemsetAsync(q.log.ev, 0, 8, s->stream));
     SolveArgs v = base_solve(s);
-    gate_args(v);
-    v.ev = q.ev; v.ev_cap = q.ev_cap;
-    v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0; v.dbg_clk = nullptr;
-    ScanArgs sa = base_scan(s);
-    sa.vpre = q.vpre;
+    v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0;
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
-    if (render) k_gn_persistent_render<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(a, q, v, sa);
-    else k_gn_persistent<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(a, q, v);
+    if (render) k_gn_persistent_render<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
+    else k_gn_persistent<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
     s->ctr.kernel_launches += 1;
     for (int m = 0; m < 2; ++m) s->ctr.rows_fwd_bwd += p.pts[m] * p.iters[m];
@@ -858,18 +830,17 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     CU(cudaEventRecord(s->ev_run1, s->stream));
     return 0;
   }
-  if (int rc = launch_init(s, p)) return rc;
+  if (int rc = launch_init(s, b, p)) return rc;
   auto iterate = [&](const RunPlan& pl, int n_iters) -> int {
     for (int e = 0; e < n_iters; ++e) {
-      if (int rc = launch_terms(s, pl, e)) return rc;
+      if (int rc = launch_terms(s, b, pl, e)) return rc;
       SolveArgs v = base_solve(s);
-      gate_args(v);
       v.iter_index = e;
       if (s->timing) {
         if (s->evs_used + 2 > s->ev_solve.size()) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); s->ev_solve.push_back(e0); s->ev_solve.push_back(e1); }
         cudaEventRecord(s->ev_solve[s->evs_used], s->stream);
       }
-      k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
+      k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(b, v);
       if (s->timing) { cudaEventRecord(s->ev_solve[s->evs_used + 1], s->stream); s->evs_used += 2; }
       s->ctr.kernel_launches++;
       CU(cudaGetLastError());
@@ -894,8 +865,7 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
         pb.smp_joint += (long long)s->h_meta[o].n_rays * s->cfg.num_depth_samples;
       }
     if (pb.any[DSPGN_MODE_JOINT]) {
-      k_gate_wake<<<(n + 127) / 128, 128, 0, s->stream>>>(s->d_state.as<ObjState>(), s->d_run.as<int>(), s->d_run.as<int>() + 2 * n,
-                                                          s->d_results.as<float>(), n, p.iters[DSPGN_MODE_JOINT]);
+      k_gate_wake<<<(n + 127) / 128, 128, 0, s->stream>>>(b, p.iters[DSPGN_MODE_JOINT]);
       s->ctr.kernel_launches++;
       CU(cudaGetLastError());
       if (int rc = iterate(pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
@@ -1112,20 +1082,21 @@ int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
   static_assert(sizeof(DspgnObjectOut) == 4 * DSPGN_RESULT_FLOATS, "result record layout");
   const size_t bytes = sizeof(DspgnObjectOut) * (size_t)s->n_obj;
   const bool mega = s->mega_ran;           // the queue counters (abort flag, band-row total) ride on the same copy + sync
-  if (s->h_results.reserve(bytes + 512)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
-  int* hq = reinterpret_cast<int*>(s->h_results.as<unsigned char>() + ((bytes + 63) / 64) * 64);
+  const size_t ctr_off = (bytes + 63) / 64 * 64;
+  if (s->h_results.reserve(ctr_off + sizeof(QueueCounters))) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
+  const QueueCounters& hq = *reinterpret_cast<const QueueCounters*>(s->h_results.as<unsigned char>() + ctr_off);
   CU(cudaMemcpyAsync(s->h_results.p, s->d_results.p, bytes, cudaMemcpyDeviceToHost, s->stream));
-  if (mega) CU(cudaMemcpyAsync(hq, s->d_q_ctr.as<int>() + 64, 4 * 40, cudaMemcpyDeviceToHost, s->stream));
+  if (mega) CU(cudaMemcpyAsync(s->h_results.as<unsigned char>() + ctr_off, s->d_q_ctr.p, sizeof(QueueCounters), cudaMemcpyDeviceToHost, s->stream));
   CU(cudaStreamSynchronize(s->stream));
   memcpy(out, s->h_results.p, bytes);
   if (mega) {
     s->mega_ran = false;
     if (s->band_rows_pending) {              // roofline accounting: what the reference decodes (loss.py:77-78, :143-144)
-      s->ctr.rows_fwd_bwd += hq[80 - 64];    // band rows of all iterations
-      { long long v; memcpy(&v, hq + (88 - 64), 8); s->ctr.rows_fwd_only += v; }   // V: ray samples inside the unit sphere, all iterations
+      s->ctr.rows_fwd_bwd += hq.band_rows_total;                  // band rows of all iterations
+      s->ctr.rows_fwd_only += (long long)hq.valid_rows_total;     // V: ray samples inside the unit sphere, all iterations
     }
     s->band_rows_pending = false;
-    if (hq[96 - 64]) return fail(DSPGN_E_CUDA, "persistent kernel: a work-queue wait timed out (aborted softly; results incomplete)");
+    if (hq.abort_flag) return fail(DSPGN_E_CUDA, "persistent kernel: a work-queue wait timed out (aborted softly; results incomplete)");
   }
   if (s->timing) {
     float dec = 0.f;
@@ -1253,9 +1224,9 @@ int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const floa
   const int32_t joint = DSPGN_MODE_JOINT;
   RunPlan p;
   if (int rc = plan_run(s, &joint, p)) return rc;
-  if (int rc = launch_init(s, p)) return rc;
-  TermArgs a = base_term(s, MODE_PTSFWD);
-  if (int rc = launch_term(s, a, n)) return rc;
+  const BatchDev b = batch_dev(s);
+  if (int rc = launch_init(s, b, p)) return rc;
+  if (int rc = launch_term(s, b, base_term(s, MODE_PTSFWD), n)) return rc;
   s->ctr.rows_fwd_only += n;
   CU(cudaMemcpyAsync(sdf_out, s->d_sdf.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
   CU(cudaStreamSynchronize(s->stream));
@@ -1286,23 +1257,24 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
   s->ctr = DspgnCounters{};
   s->ev_used = 0;
   s->gdev = GatherDev{};
-  int rc = launch_init(s, p);
+  const BatchDev bd = batch_dev(s);
+  int rc = launch_init(s, bd, p);
   for (int e = 0; e < iter && !rc; ++e) {            // advance the whole batch `iter` GN iterations (per-iteration schedule)
-    rc = launch_terms(s, p, e);
+    rc = launch_terms(s, bd, p, e);
     if (rc) break;
     SolveArgs v = base_solve(s);
     v.iter_index = e;
-    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
+    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(bd, v);
     if (cudaGetLastError() != cudaSuccess) rc = fail(DSPGN_E_CUDA, "k_solve launch failed");
   }
-  if (!rc) rc = launch_terms(s, p, iter, dJp, dres, obj, P);
+  if (!rc) rc = launch_terms(s, bd, p, iter, dJp, dres, obj, P);
   if (!rc) {
     SolveArgs v = base_solve(s);
     float* d = s->d_dbg.as<float>();
     v.dbg_obj = obj; v.dbg_H = d; v.dbg_b = d + kPMax * kPMax; v.dbg_dx = v.dbg_b + kPMax; v.dbg_loss = v.dbg_dx + kPMax;
     v.iter_index = iter;
     cudaMemsetAsync(d, 0, 4 * ((size_t)kPMax * kPMax + 2 * kPMax + 8), s->stream);
-    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(v);
+    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(bd, v);
     if (cudaGetLastError() != cudaSuccess) rc = fail(DSPGN_E_CUDA, "k_solve launch failed");
     if (!rc) {
       cudaMemcpyAsync(H, v.dbg_H, 4 * (size_t)P * P, cudaMemcpyDeviceToHost, s->stream);
@@ -1317,17 +1289,6 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
   dJ.release();
   if (rc) return rc;
   if (e != cudaSuccess) return fail(DSPGN_E_CUDA, std::string("debug_system: ") + cudaGetErrorString(e));
-  return 0;
-}
-
-int dspgn_debug_clocks(DspgnSolver* s, long long* out, int n) {
-  // phase timeline of CTA 0's first tiles of the last SDF-term launch (enabled by env DSPGN_CLK=1 at solver creation)
-  if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
-  if (!s->clk_on) return fail(DSPGN_E_ARG, "timeline not enabled (DSPGN_CLK)");
-  const int have = kClkTiles * kTcMaxSteps * kClkSlots + 16;
-  CU(cudaSetDevice(s->device));
-  CU(cudaStreamSynchronize(s->stream));
-  CU(cudaMemcpy(out, s->d_clk.p, sizeof(long long) * (size_t)std::min(n, have), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1346,7 +1307,7 @@ int dspgn_debug_events(DspgnSolver* s, long long* out, int max_events) {
   // event log of the last persistent-kernel run (env DSPGN_CLK=1 at solver creation): returns the number of events,
   // out[2*i] = %globaltimer (ns), out[2*i+1] = kind<<56 | mode<<52 | sm<<40 | object<<24 | tile (or iteration)
   if (!s || !out || max_events < 1) return fail(DSPGN_E_ARG, "bad argument");
-  if (!s->clk_on || !s->d_ev.p) return fail(DSPGN_E_ARG, "event log not enabled (DSPGN_CLK)");
+  if (!s->events_on || !s->d_ev.p) return fail(DSPGN_E_ARG, "event log not enabled (DSPGN_CLK)");
   CU(cudaSetDevice(s->device));
   CU(cudaStreamSynchronize(s->stream));
   long long n = 0;

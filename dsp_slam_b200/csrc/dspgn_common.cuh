@@ -79,6 +79,19 @@ struct SolverParams {
   int sdf_only;
 };
 
+// ---- multi-GPU result exchange (include/dspgn.h "Multi-GPU result exchange") ------------------------------
+// All pointers but slot_of point into rank 0's HBM: local memory on rank 0, CUDA-IPC peer mappings (NVLink)
+// on every other rank.
+struct GatherDev {
+  float* slots;          // slot set of this step [n_slots][DSPGN_RESULT_FLOATS]; nullptr = exchange off
+  const int* slot_of;    // [n_obj] slot of each resident object (local memory)
+  int* flags;            // [world] last step each rank has published
+  int* ack;              // last step rank 0 has consumed
+  int* err;              // LOCAL error word: 1 = a wait timed out
+  long long* wait_ns;    // LOCAL: duration of the last wait (rank 0), for the bench's exchange_ms
+  int rank, world, seq;
+};
+
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float huber_weight(float a_abs, float b) {
   // loss_utils.py:236-247: w = sqrt(rho)/a; rho = a^2 (a<=b) else 2ba-b^2; a==0 -> 0

@@ -5,11 +5,13 @@
 // Restates: loss.py:22-43 (SDF term), loss.py:143-150 (band rows of the render term),
 // loss_utils.py:51-103 (decode / input Jacobian), deep_sdf_decoder.py:75-110, optimizer.py:161-167.
 #pragma once
+#include <stddef.h>
 #include "dspgn_common.cuh"
 
 namespace dspgn {
 
 constexpr int kTP = 64;          // rows (points) per tile
+constexpr int kTcRows = 128;     // rows per tile of the tensor-core engine (dspgn_tc.cuh)
 constexpr int kThreads = 256;
 constexpr int kHid = 256;        // max layer width
 constexpr int kKC = 16;          // reduction chunk staged in smem
@@ -34,36 +36,51 @@ struct DecoderDev {
 
 enum { MODE_SDF = 0, MODE_BAND = 1, MODE_RAYFWD = 2, MODE_PTSFWD = 3 };
 
-struct TermArgs {
+// The resident batch and its run, as every kernel of the run sees it (one by-value kernel parameter; the persistent
+// kernel keeps a copy in shared memory for its out-of-line solve step).
+struct BatchDev {
   const ObjMeta* meta;
   ObjState* state;
   const DecoderDev* decs;
-  int n_obj;
-  int n_classes;
+  int n_obj, n_classes;
+  int D;                     // depth samples per ray
+  const float* pts;          // camera-frame surface points (xyz interleaved)
+  const float* rays;         // camera-frame ray directions (xyz interleaved)
+  const float* depth_fg;     // observed depth of the foreground rays
+  const float* T_init;       // [n_obj][16] row-major object->camera input pose
+  const float* code_init;    // [n_obj][64]
+  // render buffers
+  float* sdf;                // per ray sample (MODE_PTSFWD: per point): sdf, +inf when outside the unit sphere
+  float* band_x;             // band rows: object-frame points xyz interleaved, per-sample capacity
+  float* band_s;             // de_ds per band row
+  float* band_r;             // residual per band row
+  int* band_m;               // band rows per object
+  int* V_count;              // ray samples inside the unit sphere per object
+  float* results;            // [n_obj][DSPGN_RESULT_FLOATS]
+  GatherDev gather;          // optional: the record also goes straight into rank 0's HBM (peer store over NVLink)
+  // per-run object table
+  const int* modes;          // [n_obj] DSPGN_MODE_* of each object
+  const int* q0_off;         // [n_obj] first iteration-0 slot of each object in the persistent kernel's queue
+  // gated keyframe runs (nullptr = none): link[o] = the joint slot of gated pose-only object o / the pose-only object of
+  // joint slot o, -1 otherwise; t_map [n_obj][16] the map's prediction of each gated object
+  const int* link;
+  const float* t_map;
+};
+
+struct TermArgs {
   int mode;
-  // sources
-  const float* pts;          // MODE_SDF: camera-frame points (xyz interleaved)
+  int iter;                  // per-iteration schedule: the iteration being evaluated (objects with n_iter <= iter are done)
   uint8_t* pt_active;        // inlier mask of the pose-only objects (optimizer.py:76-78), may be null: |res| <= 0.05 per
                              // point, written while the object runs iteration cut_iter and applied after it
   int cut_iter;              // object iteration at which the cut is recorded (4), -1 = never
-  int iter;                  // per-iteration schedule: the iteration being evaluated (objects with n_iter <= iter are done)
-  const float* rays;         // MODE_RAYFWD
-  const float* band_x;       // MODE_BAND: object-frame points xyz interleaved, per-sample capacity
-  const float* band_s;       // de_ds per band row
-  const float* band_r;       // residual per band row
-  const int* band_m;         // rows per object
-  float* sdf_out;            // MODE_RAYFWD: per sample sdf (+inf when outside the unit sphere)
-  int* V_count;              // MODE_RAYFWD: valid samples per object
   float* part;               // per-tile partial sums of this term: [tile][kAccStride] (H upper | b | loss, rows)
   int* tile_base;            // [n_obj] first tile of each object in this launch (written by CTA 0)
   float huber_b;
   // persistent kernel with the render term: the band rows' partials / tile bases / Huber threshold (SDF ones above)
   float* part_r; const int* tile_base_r; float huber_b1;
   float* ln_scratch;         // SIMT engine, LayerNorm decoders: per-CTA [layer][256][kTP] normalised activations
-  int D;
   // debug dump of Jacobian rows (external order [pose | code]) for one object
   float* dbg_J; float* dbg_res; int dbg_obj; int dbg_P;
-  long long* dbg_clk;         // optional phase timeline of CTA 0 (tensor-core engine)
 };
 
 // Device work queue of the persistent object-pipelined kernel (dspgn_tc.cuh).
@@ -77,49 +94,69 @@ __host__ __device__ __forceinline__ int make_item(int kind, int o, int tile) {
 // filler for reserved queue slots that turned out not to be needed (k_init reserves every object's iteration-0 slots
 // from host-side upper bounds): consumers skip it.  Never a real item (a scan item's tile index is < 128); + 1 fits an int.
 constexpr int kItemNop = 0x7ffffffe;
+
+// Counters of the work queue: one device block, read back whole by dspgn_results.  The contended atomics (head, tail,
+// done_objects, abort_flag) sit 128 bytes apart.
+struct QueueCounters {
+  int head; int pad0_[31];          // consumer ticket counter
+  int tail; int pad1_[31];          // producer reservation counter
+  int done_objects; int pad2_[15];  // objects finished (last iteration or frozen)
+  int band_rows_total; int pad3_[7];          // sum of band rows over all objects and iterations (roofline accounting)
+  unsigned long long valid_rows_total; int pad4_[6];   // sum of V (ray samples inside the unit sphere), same
+  int abort_flag; int pad5_[31];    // set when a queue wait timed out: every CTA drains and exits (soft failure, never a trap)
+};
+static_assert(offsetof(QueueCounters, head) == 4 * 0 && offsetof(QueueCounters, tail) == 4 * 32 &&
+              offsetof(QueueCounters, done_objects) == 4 * 64 && offsetof(QueueCounters, band_rows_total) == 4 * 80 &&
+              offsetof(QueueCounters, valid_rows_total) == 4 * 88 && offsetof(QueueCounters, abort_flag) == 4 * 96 &&
+              sizeof(QueueCounters) == 4 * 128, "queue counter layout");
+
+// Optional event log of the persistent kernel (env DSPGN_CLK): ev[0] = count, then per event {%globaltimer ns,
+// descriptor kind<<56 | mode<<52 | sm<<40 | object<<24 | tile (or iteration / solve phase)}.
+struct EventLog { long long* ev; int cap; };
+enum { EV_TILE_BEGIN = 0, EV_TILE_END = 1, EV_SCAN_BEGIN = 2, EV_SCAN_END = 3, EV_SOLVE_BEGIN = 4, EV_SOLVE_END = 5, EV_POPPED = 6,
+       EV_FIRST_MMA = 7, EV_SOLVE_PHASE = 8 };
+__device__ __forceinline__ long long ev_desc(int kind, int mode, int o, int tile) {
+  return ((long long)kind << 56) | ((long long)mode << 52) | ((long long)o << 24) | (long long)tile;
+}
+// the writer adds the SM to the descriptor
+__device__ __forceinline__ void log_event(const EventLog& log, long long desc) {
+  if (log.ev == nullptr) return;
+  const unsigned long long slot = atomicAdd(reinterpret_cast<unsigned long long*>(log.ev), 1ull);
+  if ((long long)slot >= log.cap) return;
+  unsigned long long t; unsigned sm;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+  log.ev[1 + 2 * slot] = (long long)t;
+  log.ev[2 + 2 * slot] = desc | ((long long)sm << 40);
+}
+
 struct MegaArgs {
   int q_cap;                 // total items that can ever be pushed
   int render;                // 1: the joint objects run the render term (ray-sample tiles -> per-ray scan -> band tiles)
+  int total0;                // iteration-0 slots, seeded by k_init (the initial tail)
   int* q_flag;               // one word per slot (no wrap-around): 0 = empty, item + 1 = published
-  int* q_head; int* q_tail;  // consumer ticket counter / producer reservation counter
+  QueueCounters* ctr;
   int* pending;              // [n_obj] SDF + band tiles of the object's current iteration still running (+1 while the
                              //         render term has not been expanded into band tiles yet)
   int* ray_left;             // [n_obj] ray-sample tiles of the current iteration still running
   int* scan_left;            // [n_obj] scan items (64-ray chunks) of the current iteration still running
   int* seg_cnt; int* seg_prefix;   // band rows kept per 8-ray segment / their exclusive prefix per object (dspgn_solve.cuh)
   int* obj_iter;             // [n_obj] current iteration of each object
-  int* done_objects;         // objects finished (last iteration or frozen)
-  int* band_rows_total;      // sum of band rows over all objects and iterations (roofline accounting)
-  unsigned long long* valid_rows_total;   // sum of V (ray samples inside the unit sphere) over all objects and iterations
-  int vpre_exact;            // 1: the range pre-pass tests all D samples of every ray (debug / A-B switch)
   int* vpre;                 // per ray: (exclusive prefix of the valid-sample hulls << 7) | first valid sample, n_rays + 1
                              // entries per object at ray_off + o (dspgn_solve.cuh: valid_sample_ranges); nullptr = the
                              // forward-only tiles enumerate all n_rays * D samples
-  int* abort_flag;           // set when a queue wait timed out: every CTA drains and exits (soft failure, never a trap)
-  long long* ev; int ev_cap; // optional event log (env DSPGN_CLK): ev[0] = count, then {globaltimer ns, kind<<48|sm<<32|o<<20|tile}
+  EventLog log;
 };
-// event kinds of the persistent kernel's debug log
-enum { EV_TILE_BEGIN = 0, EV_TILE_END = 1, EV_SCAN_BEGIN = 2, EV_SCAN_END = 3, EV_SOLVE_BEGIN = 4, EV_SOLVE_END = 5, EV_POPPED = 6, EV_FIRST_MMA = 7 };
-__device__ __forceinline__ void mega_event(const MegaArgs& q, int kind, int mode, int o, int tile) {
-  if (q.ev == nullptr) return;
-  const unsigned long long slot = atomicAdd(reinterpret_cast<unsigned long long*>(q.ev), 1ull);
-  if ((long long)slot >= q.ev_cap) return;
-  unsigned long long t; unsigned sm;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
-  q.ev[1 + 2 * slot] = (long long)t;
-  q.ev[2 + 2 * slot] = ((long long)kind << 56) | ((long long)mode << 52) | ((long long)sm << 40) | ((long long)o << 24) | (long long)tile;
-}
 
 // ---------------------------------------------------------------------------------------------
 // tile scheduling shared by all decoder kernels: rows per object -> tiles, scanned per CTA
-__device__ __forceinline__ int term_rows(const TermArgs& a, int o) {
-  const ObjState& st = a.state[o];
+__device__ __forceinline__ int term_rows(const BatchDev& b, const TermArgs& a, int o) {
+  const ObjState& st = b.state[o];
   if (st.status != 0 || a.iter >= st.n_iter) return 0;
-  if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) return a.meta[o].n_pts;
+  if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) return b.meta[o].n_pts;
   if (st.mode != DSPGN_MODE_JOINT) return 0;          // pose-only objects have no render term
-  if (a.mode == MODE_BAND) return a.band_m[o];
-  return a.meta[o].n_rays * a.D;
+  if (a.mode == MODE_BAND) return b.band_m[o];
+  return b.meta[o].n_rays * b.D;
 }
 
 // SDF rows of a pose-only object: raw residuals (optimizer.py:71), otherwise the term's Huber threshold
@@ -135,12 +172,12 @@ __device__ __forceinline__ void cut_masks(const TermArgs& a, int obj_mode, int i
 }
 
 // exclusive scan of tiles per object into s_prefix[0..n_obj]; returns total (all threads)
-__device__ inline int build_tile_prefix(const TermArgs& a, int tile_rows, int* s_prefix, int* s_warp) {
+__device__ inline int build_tile_prefix(const BatchDev& b, const TermArgs& a, int tile_rows, int* s_prefix, int* s_warp) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   int carry = 0;
-  for (int base = 0; base < a.n_obj; base += blockDim.x) {
+  for (int base = 0; base < b.n_obj; base += blockDim.x) {
     int o = base + tid;
-    int v = (o < a.n_obj) ? (term_rows(a, o) + tile_rows - 1) / tile_rows : 0;
+    int v = (o < b.n_obj) ? (term_rows(b, a, o) + tile_rows - 1) / tile_rows : 0;
     int x = v;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) { int y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += y; }
@@ -150,14 +187,14 @@ __device__ inline int build_tile_prefix(const TermArgs& a, int tile_rows, int* s
     for (int w = 0; w < warp; ++w) woff += s_warp[w];
     int tot = 0;
     for (int w = 0; w < nw; ++w) tot += s_warp[w];
-    if (o < a.n_obj) s_prefix[o] = carry + woff + x - v;
+    if (o < b.n_obj) s_prefix[o] = carry + woff + x - v;
     carry += tot;
     __syncthreads();
   }
-  if (tid == 0) s_prefix[a.n_obj] = carry;
+  if (tid == 0) s_prefix[b.n_obj] = carry;
   __syncthreads();
   if (blockIdx.x == 0 && a.tile_base != nullptr)
-    for (int o = tid; o < a.n_obj; o += blockDim.x) a.tile_base[o] = s_prefix[o];
+    for (int o = tid; o < b.n_obj; o += blockDim.x) a.tile_base[o] = s_prefix[o];
   return carry;
 }
 
@@ -262,20 +299,20 @@ __device__ inline void simt_ln_backward(float* act, float* red, const float* rst
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
+__global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SimtSmem& S = *reinterpret_cast<SimtSmem*>(smem_raw);
   const int tid = threadIdx.x, jg = tid >> 3, pg = tid & 7;
-  const int total_tiles = build_tile_prefix(a, kTP, S.prefix, S.warp_tmp);
+  const int total_tiles = build_tile_prefix(b, a, kTP, S.prefix, S.warp_tmp);
 
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int o = find_object(S.prefix, a.n_obj, tile);
+    const int o = find_object(S.prefix, b.n_obj, tile);
     const int row0 = (tile - S.prefix[o]) * kTP;
-    const ObjMeta M = a.meta[o];
-    const ObjState& st = a.state[o];
-    const DecoderDev& dec = a.decs[M.class_id];
+    const ObjMeta M = b.meta[o];
+    const ObjState& st = b.state[o];
+    const DecoderDev& dec = b.decs[M.class_id];
     const int L = dec.L, in0 = dec.in0, nl = dec.n_lin;
-    const int nrows = min(kTP, term_rows(a, o) - row0);
+    const int nrows = min(kTP, term_rows(b, a, o) - row0);
     const int omode = st.mode;
     const uint8_t* mask_in; uint8_t* mask_out;
     cut_masks(a, omode, a.iter, mask_in, mask_out);
@@ -286,17 +323,17 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
       float x = 0.f, y = 0.f, z = 0.f, sc = 0.f, res = 0.f;
       if (p < nrows) {
         if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) {
-          const float* q = a.pts + 3 * (size_t)(M.pts_off + r);
+          const float* q = b.pts + 3 * (size_t)(M.pts_off + r);
           xform_point(st.T_oc, q[0], q[1], q[2], x, y, z);
           sc = (mask_in == nullptr || mask_in[M.pts_off + r]) ? 1.f : 0.f;
         } else if (a.mode == MODE_BAND) {
           const size_t s = (size_t)M.smp_off + r;
-          x = a.band_x[3 * s]; y = a.band_x[3 * s + 1]; z = a.band_x[3 * s + 2];
-          sc = a.band_s[s]; res = a.band_r[s];
+          x = b.band_x[3 * s]; y = b.band_x[3 * s + 1]; z = b.band_x[3 * s + 2];
+          sc = b.band_s[s]; res = b.band_r[s];
         } else {
-          const int ray = r / a.D, j = r - ray * a.D;
-          const float* q = a.rays + 3 * (size_t)(M.ray_off + ray);
-          const float d = lin_depth(st.dmin, st.dmax, st.dstep, j, a.D);
+          const int ray = r / b.D, j = r - ray * b.D;
+          const float* q = b.rays + 3 * (size_t)(M.ray_off + ray);
+          const float d = lin_depth(st.dmin, st.dmax, st.dstep, j, b.D);
           xform_point(st.T_oc, __fmul_rn(q[0], d), __fmul_rn(q[1], d), __fmul_rn(q[2], d), x, y, z);
           sc = inside_unit_sphere(x, y, z) ? 1.f : 0.f;                // loss.py:68
         }
@@ -313,7 +350,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
       // whole tile outside the unit sphere: nothing to decode
       int any = __syncthreads_or(tid < kTP && S.rscale[tid] != 0.f);
       if (!any) {
-        if (tid < nrows) a.sdf_out[(size_t)M.smp_off + row0 + tid] = INFINITY;
+        if (tid < nrows) b.sdf[(size_t)M.smp_off + row0 + tid] = INFINITY;
         __syncthreads();
         continue;
       }
@@ -429,11 +466,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(TermArgs a) {
       if (tid < nrows) {
         const bool valid = S.rscale[tid] != 0.f;
         const size_t base = (a.mode == MODE_RAYFWD) ? (size_t)M.smp_off : (size_t)M.pts_off;
-        a.sdf_out[base + row0 + tid] = valid ? S.yv[tid] : INFINITY;
+        b.sdf[base + row0 + tid] = valid ? S.yv[tid] : INFINITY;
         cnt = valid ? 1 : 0;
       }
       cnt = __syncthreads_count(cnt);
-      if (tid == 0 && cnt && a.mode == MODE_RAYFWD) atomicAdd(a.V_count + o, cnt);
+      if (tid == 0 && cnt && a.mode == MODE_RAYFWD) atomicAdd(b.V_count + o, cnt);
       continue;
     }
 

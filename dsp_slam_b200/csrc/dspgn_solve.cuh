@@ -11,19 +11,7 @@ namespace dspgn {
 template <class T>
 __device__ __forceinline__ T ldv(const T* p) { return *reinterpret_cast<const volatile T*>(p); }
 
-// ---- multi-GPU result exchange (include/dspgn.h "Multi-GPU result exchange") ------------------------------
-// All pointers but slot_of point into rank 0's HBM: local memory on rank 0, CUDA-IPC peer mappings (NVLink)
-// on every other rank.
-struct GatherDev {
-  float* slots;          // slot set of this step [n_slots][DSPGN_RESULT_FLOATS]; nullptr = exchange off
-  const int* slot_of;    // [n_obj] slot of each resident object (local memory)
-  int* flags;            // [world] last step each rank has published
-  int* ack;              // last step rank 0 has consumed
-  int* err;              // LOCAL error word: 1 = a wait timed out
-  long long* wait_ns;    // LOCAL: duration of the last wait (rank 0), for the bench's exchange_ms
-  int rank, world, seq;
-};
-
+// ---- multi-GPU result exchange (GatherDev: dspgn_common.cuh) ------------------------------------------------
 __device__ __forceinline__ int ld_acquire_sys(const int* p) {
   int v;
   asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -272,8 +260,7 @@ __global__ void k_build_inputs(BuildArgs a) {
 // (|u d + t| < 1 with u = R_oc q) brackets the hull to within a fraction of a sample, the search window is that bracket
 // +- 2 samples, found ends are extended outwards while the neighbour is valid, and a ray with an empty window is scanned
 // completely unless its line misses the ball by more than 1 % of the radius -- so the result is the hull of the exhaustive
-// test (`exact` = 1, env DSPGN_VPRE_EXACT: no bracket, the whole sample range is searched from both ends, which tests all D
-// samples of every ray).
+// test of all D samples (tests/valid_ranges_model.py checks the window against it).
 // Called by all `nthreads` (multiple of 32, <= 1024) threads; s_wsum: 32 ints of shared memory.  Returns the total.
 __device__ __forceinline__ int vpre_base(const ObjMeta& M, int o) { return M.ray_off + o; }
 template <bool NAMED_BAR>
@@ -283,7 +270,7 @@ __device__ __forceinline__ void vpre_sync() {
 }
 template <bool NAMED_BAR>
 __device__ inline int valid_sample_ranges(const ObjMeta& M, const ObjState& st, const float* __restrict__ rays, const int D,
-                                          int* vp, const int tid, const int nthreads, int* s_wsum, const bool exact) {
+                                          int* vp, const int tid, const int nthreads, int* s_wsum) {
   const int lane = tid & 31, warp = tid >> 5, nw = nthreads >> 5;
   float T[12];
 #pragma unroll
@@ -307,7 +294,7 @@ __device__ inline int valid_sample_ranges(const ObjMeta& M, const ObjState& st, 
       const float ux = T[0] * q0 + T[1] * q1 + T[2] * q2, uy = T[4] * q0 + T[5] * q1 + T[6] * q2, uz = T[8] * q0 + T[9] * q1 + T[10] * q2;
       const float aa = ux * ux + uy * uy + uz * uz, bb = ux * T[3] + uy * T[7] + uz * T[11];
       const float cc = T[3] * T[3] + T[7] * T[7] + T[11] * T[11] - 1.0f;
-      if (!exact && aa > 1e-20f && aa < 1e20f && dstep > 1e-12f && fabsf(dmin) < 1e4f && fabsf(dmax) < 1e4f && fabsf(bb) < 1e20f && fabsf(cc) < 1e20f) {
+      if (aa > 1e-20f && aa < 1e20f && dstep > 1e-12f && fabsf(dmin) < 1e4f && fabsf(dmax) < 1e4f && fabsf(bb) < 1e20f && fabsf(cc) < 1e20f) {
         const float inv = 1.0f / aa;
         if (cc - bb * bb * inv > 0.02f) none = true;          // closest approach > 1.01: no sample can test inside
         else {
@@ -354,28 +341,9 @@ __device__ inline int valid_sample_ranges(const ObjMeta& M, const ObjState& st, 
 }
 
 struct InitArgs {
-  const ObjMeta* meta;
-  ObjState* state;
-  const float* T_init;     // [n_obj][16] row-major object->camera
-  const float* code_init;  // [n_obj][64]
-  int* V_count;
-  int* band_m;
-  int n_obj, code_len, D;
-  const int* modes;        // [n_obj] DSPGN_MODE_* of each object for this run
+  int code_len;
   int n_iter_joint, n_iter_pose;   // GN iterations of a joint / pose-only object
-  // persistent-kernel mode: also seed the work queue with every object's iteration-0 tiles (ray-sample tiles first)
-  int mega; int render; const int* q0_off; int tile_rows; int* q_flag; int* q_head; int* q_tail;
-  int* pending; int* ray_left; int* obj_iter; int* done_objects; int* band_rows_total; int* abort_flag; int total_tiles0;
-  GatherDev gather;
-  float* results;          // records of objects rejected at upload are written here
-  int n_bad;
-  const DecoderDev* decs;  // layer-0 fold (ObjState.zb0)
-  unsigned long long* valid_rows_total;
-  int vpre_exact;
-  const float* rays; int* vpre;   // render runs of the persistent kernel: valid-sample ranges (nullptr = off)
-  // gated keyframe runs (nullptr = none): link[o] = the joint slot of gated pose-only object o / the pose-only object of
-  // joint slot o, -1 otherwise; t_map [n_obj][16] the map's prediction of each gated object
-  const int* link; const float* t_map;
+  int n_bad;                       // objects rejected at upload (they count as done from the start)
 };
 
 // zb0 = b0 + W0[:, :L] z   (fp32 FMA chain in i order; all threads of the calling CTA / epilogue)
@@ -389,96 +357,81 @@ __device__ __forceinline__ void refresh_zb0(ObjState& st, const DecoderDev& dec,
   }
 }
 
-__global__ void k_init(InitArgs a) {
+// q.q_flag != nullptr: the persistent kernel runs next, so also seed its work queue with every object's iteration-0
+// tiles (ray-sample tiles first)
+__global__ void k_init(BatchDev b, InitArgs a, MegaArgs q) {
   const int o = blockIdx.x, tid = threadIdx.x;
-  if (o == 0 && tid == 0) gather_step_begin(a.gather);
-  ObjState& st = a.state[o];
-  const ObjMeta M = a.meta[o];
-  const int mode = a.modes[o];
-  const int link = (a.link != nullptr) ? a.link[o] : -1;
+  const bool mega = q.q_flag != nullptr;
+  if (o == 0 && tid == 0) gather_step_begin(b.gather);
+  ObjState& st = b.state[o];
+  const ObjMeta M = b.meta[o];
+  const int mode = b.modes[o];
+  const int link = (b.link != nullptr) ? b.link[o] : -1;
   // the joint slot of a gated object starts dormant: fully initialised here, no tiles queued; the solve step that finishes
   // its pose-only object wakes it (persistent kernel) or k_gate_wake does (per-iteration schedule, n_iter 0 until then)
   const bool dormant = link >= 0 && mode == DSPGN_MODE_JOINT;
-  if (tid < kMaxCode) st.z[tid] = (M.has_code && tid < a.code_len) ? a.code_init[o * kMaxCode + tid] : 0.f;
+  if (tid < kMaxCode) st.z[tid] = (M.has_code && tid < a.code_len) ? b.code_init[o * kMaxCode + tid] : 0.f;
   if (tid == 0) {
     float Tco[12];
     for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 4; ++c) Tco[r * 4 + c] = a.T_init[o * 16 + r * 4 + c];
+      for (int c = 0; c < 4; ++c) Tco[r * 4 + c] = b.T_init[o * 16 + r * 4 + c];
     if (mode == DSPGN_MODE_POSE)           // optimizer.py:54: t_cam_obj[:3,:3] *= scale
       for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 3; ++c) Tco[r * 4 + c] *= M.scale;
     inv_affine(Tco, st.T_oc, nullptr);     // optimizer.py:55 / :104
-    derive_depth_range(st, a.D);
+    derive_depth_range(st, b.D);
     st.loss = 0.f; st.status = M.bad ? DSPGN_ST_BAD_INPUT : 0; st.iters = 0; st.V = 0; st.m = 0; st.n_active = M.n_pts;
-    st.mode = mode; st.n_iter = (mode == DSPGN_MODE_POSE) ? a.n_iter_pose : ((dormant && !a.mega) ? 0 : a.n_iter_joint);
-    a.V_count[o] = 0;
-    a.band_m[o] = 0;
+    st.mode = mode; st.n_iter = (mode == DSPGN_MODE_POSE) ? a.n_iter_pose : ((dormant && !mega) ? 0 : a.n_iter_joint);
+    b.V_count[o] = 0;
+    b.band_m[o] = 0;
   }
   __syncthreads();
-  refresh_zb0(st, a.decs[M.class_id], tid, blockDim.x);
+  refresh_zb0(st, b.decs[M.class_id], tid, blockDim.x);
   if (M.bad) {                               // rejected at upload: no tile, no solve -- its record is final now
     __syncthreads();
-    if (tid == 0) write_record(a.results, a.gather, o, st, M.scale);
+    if (tid == 0) write_record(b.results, b.gather, o, st, M.scale);
     // a gated object rejected at upload is checked with its input pose; its joint slot has the same points, rays and
     // depths, so it is rejected at upload too and its record is already final
-    if (tid == 0 && link >= 0 && mode == DSPGN_MODE_POSE) gate_record(a.results, o, a.T_init, a.t_map);
+    if (tid == 0 && link >= 0 && mode == DSPGN_MODE_POSE) gate_record(b.results, o, b.T_init, b.t_map);
   }
-  if (a.mega) {
-    const int ntS = (M.n_pts + a.tile_rows - 1) / a.tile_rows;
+  if (mega) {
+    const int ntS = (M.n_pts + kTcRows - 1) / kTcRows;
     // slots reserved by the host for this object's iteration 0: every ray sample (joint objects of a run with the render
     // term) + every SDF tile
-    const int ntF_cap = (a.render && !M.bad && mode == DSPGN_MODE_JOINT) ? (M.n_rays * a.D + a.tile_rows - 1) / a.tile_rows : 0;
+    const int ntF_cap = (q.render && !M.bad && mode == DSPGN_MODE_JOINT) ? (M.n_rays * b.D + kTcRows - 1) / kTcRows : 0;
     int ntF = ntF_cap;
-    if (a.vpre != nullptr && ntF_cap > 0) {
+    if (q.vpre != nullptr && ntF_cap > 0) {
       __shared__ int s_wsum[32];
       __syncthreads();                         // T_oc / depth range written by thread 0 above
-      const int vh = valid_sample_ranges<false>(M, st, a.rays, a.D, a.vpre + vpre_base(M, o), tid, blockDim.x, s_wsum, a.vpre_exact != 0);
-      ntF = (vh + a.tile_rows - 1) / a.tile_rows;
+      const int vh = valid_sample_ranges<false>(M, st, b.rays, b.D, q.vpre + vpre_base(M, o), tid, blockDim.x, s_wsum);
+      ntF = (vh + kTcRows - 1) / kTcRows;
     }
-    const int base = a.q0_off[o];
+    const int base = b.q0_off[o];
     if (!dormant) {                          // a dormant slot has no reserved slots: its wake pushes these items
-      for (int j = tid; j < ntF; j += blockDim.x) a.q_flag[base + j] = make_item(MODE_RAYFWD, o, j) + 1;
-      for (int j = tid; j < ntS; j += blockDim.x) a.q_flag[base + ntF + j] = make_item(MODE_SDF, o, j) + 1;
-      for (int j = ntF + ntS + tid; j < ntF_cap + ntS; j += blockDim.x) a.q_flag[base + j] = kItemNop + 1;
+      for (int j = tid; j < ntF; j += blockDim.x) q.q_flag[base + j] = make_item(MODE_RAYFWD, o, j) + 1;
+      for (int j = tid; j < ntS; j += blockDim.x) q.q_flag[base + ntF + j] = make_item(MODE_SDF, o, j) + 1;
+      for (int j = ntF + ntS + tid; j < ntF_cap + ntS; j += blockDim.x) q.q_flag[base + j] = kItemNop + 1;
     }
-    if (tid == 0) { a.pending[o] = ntS + (ntF > 0 ? 1 : 0); a.ray_left[o] = ntF; a.obj_iter[o] = 0; }
-    if (o == 0 && tid == 0) { *a.q_head = 0; *a.q_tail = a.total_tiles0; *a.done_objects = a.n_bad; *a.band_rows_total = 0; *a.valid_rows_total = 0ull; *a.abort_flag = 0; }
+    if (tid == 0) { q.pending[o] = ntS + (ntF > 0 ? 1 : 0); q.ray_left[o] = ntF; q.obj_iter[o] = 0; }
+    if (o == 0 && tid == 0) {
+      QueueCounters& c = *q.ctr;
+      c.head = 0; c.tail = q.total0; c.done_objects = a.n_bad; c.band_rows_total = 0; c.valid_rows_total = 0ull; c.abort_flag = 0;
+    }
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 struct SolveArgs {
-  const ObjMeta* meta;
-  ObjState* state;
   const float* part_s;     // SDF-term tile partials [tile][kAccStride]
   const float* part_r;     // render-term (band rows) tile partials
   const int* base_s;       // [n_obj] first tile of each object in the SDF / band launches
   const int* base_r;
   int tile_rows;           // rows per tile of the decoder engine
-  int* V_count;
-  int* band_m;
   SolverParams prm;
-  int n_obj;
   int iter_index;         // per-iteration schedule: the iteration being solved (an object's last one writes its record)
-  float* results;         // [n_obj][DSPGN_RESULT_FLOATS]
-  const DecoderDev* decs; // layer-0 fold (ObjState.zb0) is refreshed when the code changes
-  GatherDev gather;       // optional: the record also goes straight into rank 0's HBM (peer store over NVLink)
   // debug: dump the system of object dbg_obj and do not update any state
   int dbg_obj; float* dbg_H; float* dbg_b; float* dbg_dx; float* dbg_loss;
-  long long* dbg_clk;      // optional: 16 clock64 stamps of object 0's CTA
-  long long* ev; int ev_cap;   // optional event log of the persistent kernel (phase stamps of the solve step)
-  const int* link; const float* t_map; const float* T_init;   // gated keyframe runs (InitArgs); link = nullptr: none
 };
-__device__ __forceinline__ void solve_event(const SolveArgs& a, int o, int phase) {
-  if (a.ev == nullptr) return;
-  const unsigned long long slot = atomicAdd(reinterpret_cast<unsigned long long*>(a.ev), 1ull);
-  if ((long long)slot >= a.ev_cap) return;
-  unsigned long long t; unsigned sm;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
-  a.ev[1 + 2 * slot] = (long long)t;
-  a.ev[2 + 2 * slot] = (8ll << 56) | ((long long)sm << 40) | ((long long)o << 24) | (long long)phase;
-}
 
 constexpr int kSolveThreads = 256;
 constexpr int kPMax = 7 + kMaxCode;   // 71
@@ -490,8 +443,8 @@ __device__ __forceinline__ int ext_to_int(int e, int npose, int L) {
   return (e < npose) ? (kMaxCode + e) : (e - npose);
 }
 
-__device__ __forceinline__ void write_result(const SolveArgs& a, int o, const ObjState& st) {
-  write_record(a.results, a.gather, o, st, a.meta[o].scale);
+__device__ __forceinline__ void write_result(const BatchDev& b, int o, const ObjState& st) {
+  write_record(b.results, b.gather, o, st, b.meta[o].scale);
 }
 
 constexpr int kElimThreads = 96;      // rows 0..70 live in the first three warps
@@ -548,34 +501,36 @@ __device__ __forceinline__ void gj_pivots(const int k0, const int k1, const int 
 }
 
 // One CTA (or the epilogue half of one) per object: fixed-order reduction of the tile partials (fp64), priors
-// and damping (optimizer.py:161-184), Gaussian elimination of the SPD 71x71 system with thread = row in
-// registers, back-substitution, Sim(3)/SE(3) update, next depth range, soft failures (optimizer.py:130-150).
+// and damping (optimizer.py:161-184), Gauss-Jordan elimination of the SPD 71x71 system with thread = row in
+// registers (the system ends diagonal: no back-substitution), Sim(3)/SE(3) update, next depth range, soft failures
+// (optimizer.py:130-150).  `log`: the persistent kernel's event log (solve phases).
 // Returns 1 when the object is finished (last iteration, frozen or soft-failed), else 0.
 template <bool MEGA>
-__device__ int solve_object(const SolveArgs& a, const int o, const int tid, SolveSmem& SM, const bool last_iter) {
+__device__ int solve_object(const BatchDev& b, const SolveArgs& a, const EventLog& log, const int o, const int tid, SolveSmem& SM,
+                            const bool last_iter) {
   float (&As)[kPMax * kAsStride] = SM.As;
   float4 (&bcast)[2][(kPMax + 1) / 4 + 1] = SM.bcast;
   float (&xs)[kPMax] = SM.xs;
   float (&s_rot)[4] = SM.s_rot; double (&s_sum)[4] = SM.s_sum; int& s_flag = SM.s_flag;
-  ObjState& st = a.state[o];
+  ObjState& st = b.state[o];
   const SolverParams& prm = a.prm;
   const int L = prm.code_len;
   const bool pose_only = st.mode == DSPGN_MODE_POSE;      // estimate_pose_cam_obj variant
   const int npose = pose_only ? 6 : 7;
   const int P = pose_only ? 6 : (7 + L);
-#define SOLVE_CLK(k) do { if (!MEGA && a.dbg_clk != nullptr && o == 0 && tid == 0) a.dbg_clk[k] = clock64(); if (MEGA && tid == 0) solve_event(a, o, k); } while (0)
-  SOLVE_CLK(0);
+#define SOLVE_EV(k) do { if (MEGA && tid == 0) log_event(log, ev_desc(EV_SOLVE_PHASE, 0, o, k)); } while (0)
+  SOLVE_EV(0);
   const bool dbg = (a.dbg_H != nullptr);
   const bool use_render = !pose_only && !prm.sdf_only;
   // tile partials of this object, summed in tile order (deterministic), fp64
-  const int V = ldv(a.V_count + o), m = use_render ? ldv(a.band_m + o) : 0;
-  const int ntS = (a.meta[o].n_pts + a.tile_rows - 1) / a.tile_rows;
+  const int V = ldv(b.V_count + o), m = use_render ? ldv(b.band_m + o) : 0;
+  const int ntS = (b.meta[o].n_pts + a.tile_rows - 1) / a.tile_rows;
   const int ntR = use_render ? (m + a.tile_rows - 1) / a.tile_rows : 0;
   const float* pS = a.part_s + (size_t)a.base_s[o] * kAccStride;
   const float* pR = use_render ? a.part_r + (size_t)a.base_r[o] * kAccStride : nullptr;
   // ---- losses and the reference's soft-failure exits (optimizer.py:130-150) -----------------
   if (ldv(&st.status) != 0) {                    // frozen object: keep its record
-    if (last_iter && tid == 0 && !dbg) write_result(a, o, st);
+    if (last_iter && tid == 0 && !dbg) write_result(b, o, st);
     return 1;
   }
   if (tid < 96) {
@@ -591,7 +546,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
     if (ln == 0) s_sum[w] = v;
   }
   solve_sync<MEGA>();
-  SOLVE_CLK(1);
+  SOLVE_EV(1);
   const double nS = s_sum[1];
   const float sdf_loss = (float)(s_sum[0] / nS);
   float render_loss = 0.f;
@@ -608,10 +563,12 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
     a.dbg_loss[0] = sdf_loss; a.dbg_loss[1] = render_loss; a.dbg_loss[2] = (float)V; a.dbg_loss[3] = (float)m;
   }
   if (status != 0) {
-    if (!dbg && tid == 0) { st.status = status; st.V = V; st.m = m; if (last_iter || MEGA) write_result(a, o, st); }
+    if (!dbg && tid == 0) { st.status = status; st.V = V; st.m = m; if (last_iter || MEGA) write_result(b, o, st); }
     return 1;
   }
-  const float loss = prm.k1 * render_loss + prm.k2 * sdf_loss;     // optimizer.py:155
+  // optimizer.py:155.  The contraction is spelled out: left to the compiler, which product it fuses depends on the
+  // surrounding code, and both schedules (k_solve, the persistent kernel) must round alike.
+  const float loss = __fmaf_rn(prm.k1, render_loss, __fmul_rn(prm.k2, sdf_loss));
 
   if (tid == 0) {
     s_flag = 0;
@@ -640,7 +597,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   }
   solve_sync<MEGA>();
 
-  SOLVE_CLK(2);
+  SOLVE_EV(2);
   // ---- assemble the lower triangle of H and the b row (optimizer.py:161-184; pose-only: :68-71) ----
   const double wS = pose_only ? 1.0 / nS : (double)prm.k2 / nS;
   const double wR = use_render ? (double)prm.k1 / (double)m : 0.0;
@@ -702,7 +659,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   };
   sum_tiles(pS, ntS, accv);
   if (ntR > 0) sum_tiles(pR, ntR, accr);
-  SOLVE_CLK(3);
+  SOLVE_EV(3);
 #pragma unroll
   for (int q = 0; q < kMaxEnt; ++q) {
     const int i = ei[q], j = ej[q];
@@ -743,7 +700,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
     if (i >= P || (j >= P && j < kPMax)) As[i * kAsStride + j] = (i == j) ? 1.f : 0.f;
   }
   solve_sync<MEGA>();
-  SOLVE_CLK(4);
+  SOLVE_EV(4);
   // ---- Gauss-Jordan elimination of the SPD system, thread i = row i in registers; one barrier per pivot ----------
   if (tid < kElimThreads) {
     // Thread i keeps row i of [H | b] in registers, rotated so that the current pivot column is always index 0: after
@@ -769,7 +726,7 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
     if (bad_pivot && tid == 0) s_flag = 1;
   }
   solve_sync<MEGA>();
-  SOLVE_CLK(5);
+  SOLVE_EV(5);
   if (tid < P && !isfinite(xs[tid])) s_flag = 1;
   solve_sync<MEGA>();
   if (dbg) {
@@ -780,10 +737,10 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
   const bool fail = (s_flag != 0);
   if (!pose_only && tid < L && !fail) st.z[tid] = ldv(&st.z[tid]) + prm.lr * xs[tid + 7];
   solve_sync<MEGA>();                        // the result record below reads every z entry
-  if (!pose_only && !fail && !last_iter) refresh_zb0(st, a.decs[a.meta[o].class_id], tid, kSolveThreads);
+  if (!pose_only && !fail && !last_iter) refresh_zb0(st, b.decs[b.meta[o].class_id], tid, kSolveThreads);
   if (tid == 0) {
     st.loss = loss; st.V = V; st.m = m;
-    a.V_count[o] = 0;
+    b.V_count[o] = 0;
     if (fail) {
       st.status = DSPGN_ST_SOLVE;
     } else {
@@ -797,54 +754,39 @@ __device__ int solve_object(const SolveArgs& a, const int o, const int tid, Solv
       derive_depth_range(st, prm.D);
       st.iters = ldv(&st.iters) + 1;
     }
-    if (last_iter || (MEGA && fail)) write_result(a, o, st);
+    if (last_iter || (MEGA && fail)) write_result(b, o, st);
   }
-  SOLVE_CLK(6);
+  SOLVE_EV(6);
   return (last_iter || fail) ? 1 : 0;
 }
 
-__global__ void __launch_bounds__(kSolveThreads) k_solve(SolveArgs a) {
+__global__ void __launch_bounds__(kSolveThreads) k_solve(BatchDev b, SolveArgs a) {
   __shared__ SolveSmem SM;
-  const int o = blockIdx.x, n_iter = a.state[o].n_iter;
+  const int o = blockIdx.x, n_iter = b.state[o].n_iter;
   if (a.iter_index >= n_iter) return;               // finished after its own last iteration
   const bool last = a.iter_index + 1 == n_iter;
-  solve_object<false>(a, o, threadIdx.x, SM, last);
+  solve_object<false>(b, a, EventLog{}, o, threadIdx.x, SM, last);
   // gated pose-only object: the map-consistency check on the record thread 0 has just written
-  if (last && a.link != nullptr && a.dbg_H == nullptr && threadIdx.x == 0 && a.link[o] >= 0 && a.state[o].mode == DSPGN_MODE_POSE)
-    gate_record(a.results, o, a.T_init, a.t_map);
+  if (last && b.link != nullptr && a.dbg_H == nullptr && threadIdx.x == 0 && b.link[o] >= 0 && b.state[o].mode == DSPGN_MODE_POSE)
+    gate_record(b.results, o, b.T_init, b.t_map);
 }
 
 // Per-iteration schedule of a gated run, between its two phases: the joint slots whose pose-only object was rejected
 // run num_iterations from their k_init state, every other object is finished (its record is final).
-__global__ void k_gate_wake(ObjState* state, const int* modes, const int* link, const float* results, int n_obj, int n_iter_joint) {
+__global__ void k_gate_wake(BatchDev b, int n_iter_joint) {
   const int o = blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= n_obj) return;
-  const int lk = link[o];
-  const bool wake = lk >= 0 && modes[o] == DSPGN_MODE_JOINT &&
-                    reinterpret_cast<const int*>(results + (size_t)lk * DSPGN_RESULT_FLOATS)[85] == DSPGN_GATE_REJECTED;
-  state[o].n_iter = wake ? n_iter_joint : 0;
+  if (o >= b.n_obj) return;
+  const int lk = b.link[o];
+  const bool wake = lk >= 0 && b.modes[o] == DSPGN_MODE_JOINT &&
+                    reinterpret_cast<const int*>(b.results + (size_t)lk * DSPGN_RESULT_FLOATS)[85] == DSPGN_GATE_REJECTED;
+  b.state[o].n_iter = wake ? n_iter_joint : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
 // Render term, per-ray part (loss.py:84-141).  One CTA per object, one warp per ray, two passes:
 // pass 1 counts the band samples each ray keeps, a block scan turns counts into row offsets, pass 2
 // recomputes and writes rows (x_o, de/ds, clamped depth residual) in (ray, sample) order -- the same
-// order torch.where yields, and deterministic.
-struct ScanArgs {
-  const ObjMeta* meta;
-  const ObjState* state;
-  const float* rays;
-  const float* depth_fg;
-  const float* sdf;       // per sample, +inf outside the unit sphere
-  float* band_x; float* band_s; float* band_r;
-  int* band_m;
-  float th;
-  int D;
-  int n_obj;
-  const int* vpre;        // persistent kernel: sdf values are stored compactly per ray (valid_sample_ranges); nullptr = n_rays x D
-  int* V_count;           // persistent kernel: the scan items count V (samples with a finite sdf value) per object
-};
-
+// order torch.where yields, and deterministic.  th: the occupancy cut-off (SolverParams::th).
 constexpr int kScanThreads = 1024;
 constexpr int kScanMaxRays = 8192;
 
@@ -858,18 +800,18 @@ __device__ __forceinline__ void load_scan_state(const ObjState& st, ScanState& c
 }
 
 // sdf values of one ray (lane = sample slot, two slots per lane); +inf beyond D / outside the unit sphere
-__device__ __forceinline__ void ray_load(const ScanArgs& a, const ObjMeta& M, int ray, int lane, float s[2]) {
-  const float* srow = a.sdf + (size_t)M.smp_off + (size_t)ray * a.D;
+__device__ __forceinline__ void ray_load(const BatchDev& b, const ObjMeta& M, int ray, int lane, float s[2]) {
+  const float* srow = b.sdf + (size_t)M.smp_off + (size_t)ray * b.D;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int j = lane + 32 * h;
-    s[h] = (j < a.D) ? __ldcg(srow + j) : INFINITY;  // written by other CTAs (L2 is the point of coherence)
+    s[h] = (j < b.D) ? __ldcg(srow + j) : INFINITY;  // written by other CTAs (L2 is the point of coherence)
   }
 }
 
 // same for the compact layout: the ray's hull [j0, j0 + cnt) starts at sample slot `p` of the object
-__device__ __forceinline__ void ray_load_compact(const ScanArgs& a, const ObjMeta& M, int p, int j0, int cnt, int lane, float s[2]) {
-  const float* srow = a.sdf + (size_t)M.smp_off + (size_t)p;
+__device__ __forceinline__ void ray_load_compact(const BatchDev& b, const ObjMeta& M, int p, int j0, int cnt, int lane, float s[2]) {
+  const float* srow = b.sdf + (size_t)M.smp_off + (size_t)p;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int k = lane + 32 * h - j0;
@@ -877,10 +819,9 @@ __device__ __forceinline__ void ray_load_compact(const ScanArgs& a, const ObjMet
   }
 }
 
-__device__ __forceinline__ void ray_scan_vals(const ScanArgs& a, const ObjMeta& M, const ScanState& st, int ray, int lane,
-                                              const float s[2], bool keep[2], float de_ds[2], float& res) {
-  const int D = a.D;
-  const float th = a.th;
+__device__ __forceinline__ void ray_scan_vals(const BatchDev& b, const float th, const ObjMeta& M, const ScanState& st, int ray,
+                                              int lane, const float s[2], bool keep[2], float de_ds[2], float& res) {
+  const int D = b.D;
   float o[2], q[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -929,34 +870,34 @@ __device__ __forceinline__ void ray_scan_vals(const ScanArgs& a, const ObjMeta& 
     keep[h] = band && (de_do > 1e-2f);                  // loss.py:125
     de_ds[h] = de_do * delta_d * do_ds;                 // loss.py:128-130
   }
-  const float dobs = (ray < M.n_fg) ? a.depth_fg[M.fg_off + ray] : st.dfar;   // optimizer.py:126
+  const float dobs = (ray < M.n_fg) ? b.depth_fg[M.fg_off + ray] : st.dfar;   // optimizer.py:126
   res = fminf(fmaxf(dobs - du, -0.3f), 0.3f);           // loss.py:136-141
 }
 
-__device__ __forceinline__ void ray_scan(const ScanArgs& a, const ObjMeta& M, const ScanState& st, int ray, int lane,
+__device__ __forceinline__ void ray_scan(const BatchDev& b, const float th, const ObjMeta& M, const ScanState& st, int ray, int lane,
                                          bool keep[2], float de_ds[2], float& res) {
   float s[2];
-  ray_load(a, M, ray, lane, s);
-  ray_scan_vals(a, M, st, ray, lane, s, keep, de_ds, res);
+  ray_load(b, M, ray, lane, s);
+  ray_scan_vals(b, th, M, st, ray, lane, s, keep, de_ds, res);
 }
 
 // write the kept samples of one ray as band rows (x_o, de/ds, residual) starting at row `base` (ray, sample order)
-__device__ __forceinline__ int ray_emit(const ScanArgs& a, const ObjMeta& M, const ScanState& st, int ray, int lane,
+__device__ __forceinline__ int ray_emit(const BatchDev& b, const ObjMeta& M, const ScanState& st, int ray, int lane,
                                         const bool keep[2], const float de_ds[2], float res, size_t base) {
   const unsigned b0 = __ballot_sync(0xffffffffu, keep[0]), b1 = __ballot_sync(0xffffffffu, keep[1]);
-  const float* q = a.rays + 3 * (size_t)(M.ray_off + ray);
+  const float* q = b.rays + 3 * (size_t)(M.ray_off + ray);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     if (!keep[h]) continue;
     const int j = lane + 32 * h;
     const int pos = (h == 0 ? __popc(b0 & ((1u << lane) - 1u)) : __popc(b0) + __popc(b1 & ((1u << lane) - 1u)));
-    const float d = lin_depth(st.dmin, st.dmax, st.dstep, j, a.D);
+    const float d = lin_depth(st.dmin, st.dmax, st.dstep, j, b.D);
     float x, y, z;
     xform_point(st.T, __fmul_rn(q[0], d), __fmul_rn(q[1], d), __fmul_rn(q[2], d), x, y, z);
     const size_t row = base + pos;
-    a.band_x[3 * row] = x; a.band_x[3 * row + 1] = y; a.band_x[3 * row + 2] = z;
-    a.band_s[row] = de_ds[h];
-    a.band_r[row] = res;
+    b.band_x[3 * row] = x; b.band_x[3 * row + 1] = y; b.band_x[3 * row + 2] = z;
+    b.band_s[row] = de_ds[h];
+    b.band_r[row] = res;
   }
   return __popc(b0) + __popc(b1);
 }
@@ -970,24 +911,26 @@ constexpr int kSegRays = 8, kScanChunkRays = 64;
 // first segment slot of object o: its nseg counts / nseg + 1 prefix entries never overlap the next object's
 __device__ __forceinline__ int seg_base(const ObjMeta& M, int o) { return M.ray_off / kSegRays + 2 * o; }
 
-__device__ inline void scan_chunk(const ScanArgs& a, int* seg_cnt, const int o, const int chunk, const int tid) {
+// vpre: the compact sdf layout of valid_sample_ranges, nullptr = n_rays x D
+__device__ inline void scan_chunk(const BatchDev& b, const float th, const int* vpre, int* seg_cnt, const int o, const int chunk,
+                                  const int tid) {
   const int lane = tid & 31, warp = tid >> 5;
-  const ObjMeta M = a.meta[o];
+  const ObjMeta M = b.meta[o];
   const int seg = chunk * (kScanChunkRays / kSegRays) + warp;
   const int ray0 = seg * kSegRays;
   if (ray0 >= M.n_rays) return;
   ScanState st;
-  load_scan_state(a.state[o], st);
+  load_scan_state(b.state[o], st);
   float sv[kSegRays][2];
   // compact sdf layout: lanes 0..8 fetch the segment's 9 range words once
   int vw = 0;
-  if (a.vpre != nullptr && lane <= kSegRays && ray0 + lane <= M.n_rays) vw = __ldcg(a.vpre + vpre_base(M, o) + ray0 + lane);
+  if (vpre != nullptr && lane <= kSegRays && ray0 + lane <= M.n_rays) vw = __ldcg(vpre + vpre_base(M, o) + ray0 + lane);
 #pragma unroll
   for (int i = 0; i < kSegRays; ++i) {
     const int v0 = __shfl_sync(0xffffffffu, vw, i), v1 = __shfl_sync(0xffffffffu, vw, i + 1);
     if (ray0 + i < M.n_rays) {
-      if (a.vpre != nullptr) ray_load_compact(a, M, v0 >> 7, v0 & 127, (v1 >> 7) - (v0 >> 7), lane, sv[i]);
-      else ray_load(a, M, ray0 + i, lane, sv[i]);
+      if (vpre != nullptr) ray_load_compact(b, M, v0 >> 7, v0 & 127, (v1 >> 7) - (v0 >> 7), lane, sv[i]);
+      else ray_load(b, M, ray0 + i, lane, sv[i]);
     } else { sv[i][0] = INFINITY; sv[i][1] = INFINITY; }
   }
   // V (loss.py:68,73): samples inside the unit sphere = the finite sdf values.  Counted here, one atomic per segment,
@@ -996,23 +939,23 @@ __device__ inline void scan_chunk(const ScanArgs& a, int* seg_cnt, const int o, 
 #pragma unroll
   for (int i = 0; i < kSegRays; ++i)
     nvalid += __popc(__ballot_sync(0xffffffffu, sv[i][0] != INFINITY)) + __popc(__ballot_sync(0xffffffffu, sv[i][1] != INFINITY));
-  if (lane == 0 && nvalid != 0) atomicAdd(a.V_count + o, nvalid);
+  if (lane == 0 && nvalid != 0) atomicAdd(b.V_count + o, nvalid);
   int count = 0;
-  const size_t base = (size_t)M.smp_off + (size_t)ray0 * a.D;
+  const size_t base = (size_t)M.smp_off + (size_t)ray0 * b.D;
 #pragma unroll
   for (int i = 0; i < kSegRays; ++i) {
     if (ray0 + i >= M.n_rays) break;                       // warp-uniform
     bool keep[2]; float de_ds[2]; float res;
-    ray_scan_vals(a, M, st, ray0 + i, lane, sv[i], keep, de_ds, res);
-    count += ray_emit(a, M, st, ray0 + i, lane, keep, de_ds, res, base + count);
+    ray_scan_vals(b, th, M, st, ray0 + i, lane, sv[i], keep, de_ds, res);
+    count += ray_emit(b, M, st, ray0 + i, lane, keep, de_ds, res, base + count);
   }
   if (lane == 0) seg_cnt[seg_base(M, o) + seg] = count;
 }
 
 // exclusive prefix over the object's segment counts -> seg_prefix[0..nseg], band_m[o] = total.  256 threads, named barrier 1.
-__device__ inline void scan_prefix(const ScanArgs& a, const int* seg_cnt, int* seg_prefix, const int o, const int tid, int* s_wsum) {
+__device__ inline void scan_prefix(const BatchDev& b, const int* seg_cnt, int* seg_prefix, const int o, const int tid, int* s_wsum) {
   const int lane = tid & 31, warp = tid >> 5;
-  const ObjMeta M = a.meta[o];
+  const ObjMeta M = b.meta[o];
   const int nseg = (M.n_rays + kSegRays - 1) / kSegRays, sb = seg_base(M, o);
   int carry = 0;
   for (int b0 = 0; b0 < nseg; b0 += 256) {
@@ -1029,31 +972,25 @@ __device__ inline void scan_prefix(const ScanArgs& a, const int* seg_cnt, int* s
     carry += tot;
     asm volatile("bar.sync 1, 256;" ::: "memory");
   }
-  if (tid == 0) { seg_prefix[sb + nseg] = carry; a.band_m[o] = carry; }
+  if (tid == 0) { seg_prefix[sb + nseg] = carry; b.band_m[o] = carry; }
 }
 
-// The per-object scan: called by all `nthreads` threads of k_ray_scan's CTA (MEGA = false) or by the 256 epilogue
-// threads of the persistent kernel's CTA that finished the object's last ray-sample tile (MEGA = true).
+// The per-object scan of the per-iteration schedule: all `nthreads` threads of k_ray_scan's CTA.
 // s_cnt: kScanMaxRays ints, s_wsum: 32 ints of shared memory.
-template <bool MEGA>
-__device__ __forceinline__ void scan_sync() {
-  if (MEGA) asm volatile("bar.sync 1, 256;" ::: "memory");
-  else __syncthreads();
-}
-template <bool MEGA>
-__device__ inline void scan_object(const ScanArgs& a, const int o, const int tid, const int nthreads, int* s_cnt, int* s_wsum) {
+__device__ inline void scan_object(const BatchDev& b, const float th, const int o, const int tid, const int nthreads, int* s_cnt,
+                                   int* s_wsum) {
   const int lane = tid & 31, warp = tid >> 5, nw = nthreads >> 5;
-  const ObjMeta M = a.meta[o];
+  const ObjMeta M = b.meta[o];
   ScanState st;
-  load_scan_state(a.state[o], st);
+  load_scan_state(b.state[o], st);
   const int N = M.n_rays;
   bool keep[2]; float de_ds[2]; float res;
   for (int ray = warp; ray < N; ray += nw) {
-    ray_scan(a, M, st, ray, lane, keep, de_ds, res);
+    ray_scan(b, th, M, st, ray, lane, keep, de_ds, res);
     const int c = __popc(__ballot_sync(0xffffffffu, keep[0])) + __popc(__ballot_sync(0xffffffffu, keep[1]));
     if (lane == 0) s_cnt[ray] = c;
   }
-  scan_sync<MEGA>();
+  __syncthreads();
   // block exclusive scan of s_cnt[0..N)
   int carry = 0;
   for (int base = 0; base < N; base += nthreads) {
@@ -1063,27 +1000,27 @@ __device__ inline void scan_object(const ScanArgs& a, const int o, const int tid
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) { int y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += y; }
     if (lane == 31) s_wsum[warp] = x;
-    scan_sync<MEGA>();
+    __syncthreads();
     int woff = 0, tot = 0;
     for (int w = 0; w < nw; ++w) { if (w < warp) woff += s_wsum[w]; tot += s_wsum[w]; }
     if (i < N) s_cnt[i] = carry + woff + x - v;
     carry += tot;
-    scan_sync<MEGA>();
+    __syncthreads();
   }
-  if (tid == 0) a.band_m[o] = carry;
+  if (tid == 0) b.band_m[o] = carry;
   for (int ray = warp; ray < N; ray += nw) {
-    ray_scan(a, M, st, ray, lane, keep, de_ds, res);
-    ray_emit(a, M, st, ray, lane, keep, de_ds, res, (size_t)M.smp_off + s_cnt[ray]);
+    ray_scan(b, th, M, st, ray, lane, keep, de_ds, res);
+    ray_emit(b, M, st, ray, lane, keep, de_ds, res, (size_t)M.smp_off + s_cnt[ray]);
   }
 }
 
-__global__ void __launch_bounds__(kScanThreads) k_ray_scan(ScanArgs a) {
+__global__ void __launch_bounds__(kScanThreads) k_ray_scan(BatchDev b, float th) {
   __shared__ int s_cnt[kScanMaxRays];
   __shared__ int s_wsum[32];
   const int o = blockIdx.x;
-  if (a.state[o].status != 0 || a.state[o].mode != DSPGN_MODE_JOINT) return;   // pose-only objects: no render term
-  if (a.state[o].n_iter == 0) return;                // a dormant joint slot of a gated run
-  scan_object<false>(a, o, threadIdx.x, kScanThreads, s_cnt, s_wsum);
+  if (b.state[o].status != 0 || b.state[o].mode != DSPGN_MODE_JOINT) return;   // pose-only objects: no render term
+  if (b.state[o].n_iter == 0) return;                // a dormant joint slot of a gated run
+  scan_object(b, th, o, threadIdx.x, kScanThreads, s_cnt, s_wsum);
 }
 
 }  // namespace dspgn

@@ -40,8 +40,7 @@
 
 namespace dspgn {
 
-constexpr int kTcRows = 128;
-constexpr int kTcThreads = 384;           // 2 consumer warpgroups + 1 producer warpgroup
+constexpr int kTcThreads = 384;          // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int kTcEpiThreads = 256;
 constexpr int kTcStages = 4;              // one 64-wide K chunk: hi[k 0..31], hi[k 32..63], lo[k 0..31], lo[k 32..63]
 constexpr int kTcStageBytes = 16384;      // one ring stage: up to 256 rows x 32 K x fp16 (64 B rows, SWIZZLE_64B)
@@ -144,14 +143,6 @@ DSPGN_WGMMA(192, DSPGN_D96, DSPGN_ACC_OPS96, 96, 97, 98, 99, 100, 101, 96, 97, 9
 DSPGN_WGMMA(80, DSPGN_D40, DSPGN_ACC_OPS40, 40, 41, 42, 43, 44, 45, 40, 41, 42)
 #undef DSPGN_WGMMA
 
-// debug timeline (CTA 0 only, when TermArgs.dbg_clk != nullptr): [tile][step][slot] = clock64
-constexpr int kClkSlots = 8, kClkTiles = 4;
-#define DSPGN_CLK(slot)                                                                                   \
-  do {                                                                                                    \
-    if (a.dbg_clk != nullptr && blockIdx.x == 0 && clk_tile < kClkTiles)                                  \
-      a.dbg_clk[((size_t)clk_tile * kTcMaxSteps + s) * kClkSlots + (slot)] = clock64();                   \
-  } while (0)
-
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // K-major, 128B-swizzled shared-memory matrix descriptor (sm90 GMMA descriptor):
@@ -208,7 +199,7 @@ struct TcSmemTail {
   // persistent mode: copies of the kernel arguments for the out-of-line solve step.  Passing references to the kernel
   // parameters themselves would make them address-taken: the compiler then parks all of them in local memory and the tile
   // loop reads its pointers with LDL instead of from the constant bank.
-  MegaArgs ctx_q; SolveArgs ctx_sv; int ctx_D; const float* ctx_rays;
+  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
   int push_base, push_nF, push_nS, push_o;   // cooperative publication of an object's next-iteration tiles
   float ost[16]; int ost_rows;            // the tile's object: T_oc[12], dmin, dmax, dstep, dfar; rows of its term (counter)
 };
@@ -323,19 +314,19 @@ struct TileRef { int o, row0, slot, mode, tile; };
 constexpr unsigned long long kMegaTimeoutNs = 30ull * 1000ull * 1000ull * 1000ull;
 __device__ inline int mega_pop(const MegaArgs& q, int n_obj) {
   for (;;) {
-    const int t = atomicAdd(q.q_head, 1);
+    const int t = atomicAdd(&q.ctr->head, 1);
     if (t >= q.q_cap) return -1;
     unsigned long long t0 = 0;
     int item = kItemNop;
     for (unsigned spins = 0;; ++spins) {
       const int v = ldv(q.q_flag + t);
       if (v != 0) { __threadfence(); item = v - 1; break; }
-      if (ldv(q.done_objects) >= n_obj || ldv(q.abort_flag) != 0) return -1;
+      if (ldv(&q.ctr->done_objects) >= n_obj || ldv(&q.ctr->abort_flag) != 0) return -1;
       __nanosleep(256);
       if ((spins & 1023u) == 1023u) {
         const unsigned long long now = globaltimer_ns();
         if (t0 == 0) t0 = now;
-        else if (now - t0 > kMegaTimeoutNs) { atomicExch(q.abort_flag, 1); return -1; }
+        else if (now - t0 > kMegaTimeoutNs) { atomicExch(&q.ctr->abort_flag, 1); return -1; }
       }
     }
     if (item != kItemNop) return item;       // filler of a reserved slot that was not needed: take the next ticket
@@ -346,12 +337,12 @@ __device__ inline int mega_pop(const MegaArgs& q, int n_obj) {
 // SCHED: 0 = one launch per term (static tiles), 1 = persistent kernel, SDF tiles only (SDF-only joint runs, pose-only
 // runs: the tile kind is a compile-time constant), 2 = persistent kernel with the render term (all item kinds)
 template <int SCHED>
-__device__ __forceinline__ bool tile_at(const TermArgs& a, TcSmemTail& S, int seq, int total_tiles, TileRef& t) {
+__device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, TcSmemTail& S, int seq, int total_tiles, TileRef& t) {
   constexpr bool MEGA = SCHED != 0;
   if (!MEGA) {
     const int tile = blockIdx.x + seq * gridDim.x;
     if (tile >= total_tiles) return false;
-    t.o = find_object(S.prefix, a.n_obj, tile);
+    t.o = find_object(S.prefix, b.n_obj, tile);
     t.tile = tile - S.prefix[t.o];
     t.row0 = t.tile * kTcRows;
     t.slot = tile;
@@ -373,69 +364,69 @@ __device__ __forceinline__ bool tile_at(const TermArgs& a, TcSmemTail& S, int se
 }
 
 // rows of the term a tile belongs to (persistent kernel: the tile's own kind, counters written by other CTAs)
-__device__ __forceinline__ int mega_rows(const TermArgs& a, const MegaArgs& q, const ObjMeta& M, int o, int mode) {
+__device__ __forceinline__ int mega_rows(const BatchDev& b, const MegaArgs& q, const ObjMeta& M, int o, int mode) {
   if (mode == MODE_SDF) return M.n_pts;
-  if (mode == MODE_BAND) return ldv(a.band_m + o);
+  if (mode == MODE_BAND) return ldv(b.band_m + o);
   if (q.vpre != nullptr) return ldv(q.vpre + vpre_base(M, o) + M.n_rays) >> 7;   // valid-sample hulls only
-  return M.n_rays * a.D;
+  return M.n_rays * b.D;
 }
 
 // publish `n` queue items (kind, object, tile 0..n-1): reserve slots, fence (everything the items depend on, incl. the
 // counters updated just before the call), one word per slot.  One thread.
 __device__ inline void mega_push(const MegaArgs& q, int kind, int o, int n) {
   if (n <= 0) return;
-  const int base = atomicAdd(q.q_tail, n);
+  const int base = atomicAdd(&q.ctr->tail, n);
   __threadfence();
   for (int j = 0; j < n; ++j) *reinterpret_cast<volatile int*>(q.q_flag + base + j) = make_item(kind, o, j) + 1;
 }
 
 // all terms of the object's current iteration are in: solve, update, queue the next iteration (or finish).  Called by
 // the 256 epilogue threads of the CTA that completed the object's last outstanding tile.
-template <bool MEGA>
 __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int tid) {
+  const BatchDev& b = S.ctx_b;
   const MegaArgs& q = S.ctx_q;
   const SolveArgs& sv = S.ctx_sv;
   __threadfence();
   SolveSmem& SM = *reinterpret_cast<SolveSmem*>(S.Jp);
   const int it = ldv(q.obj_iter + o);
-  const bool render = q.render && sv.state[o].mode == DSPGN_MODE_JOINT;     // pose-only objects: SDF tiles only
-  if (tid == 0) mega_event(q, EV_SOLVE_BEGIN, 0, o, it);
-  const int fin = solve_object<true>(sv, o, tid, SM, it + 1 >= sv.state[o].n_iter);
+  const bool render = q.render && b.state[o].mode == DSPGN_MODE_JOINT;     // pose-only objects: SDF tiles only
+  if (tid == 0) log_event(q.log, ev_desc(EV_SOLVE_BEGIN, 0, o, it));
+  const int fin = solve_object<true>(b, sv, q.log, o, tid, SM, it + 1 >= b.state[o].n_iter);
   epi_bar_sync();
   // ---- the next iteration's ray samples: only the run of samples inside the unit sphere of every ray (new pose and
   // depth range, written by the solve above).  `fin` is the same in every thread (shared-memory flags).
   int vh = -1;
   if (!fin && render && q.vpre != nullptr) {
-    const ObjMeta M = sv.meta[o];
-    if (M.n_rays > 0) vh = valid_sample_ranges<true>(M, sv.state[o], S.ctx_rays, S.ctx_D, q.vpre + vpre_base(M, o), tid, kTcEpiThreads, S.warp_tmp, q.vpre_exact != 0);
+    const ObjMeta M = b.meta[o];
+    if (M.n_rays > 0) vh = valid_sample_ranges<true>(M, b.state[o], b.rays, b.D, q.vpre + vpre_base(M, o), tid, kTcEpiThreads, S.warp_tmp);
   }
   // ---- publish: finished, or the tiles of the next iteration.  All 256 threads write the queue slots (one thread
   // pushing every ray tile and its flag one by one is on the single-object critical path).
   if (tid == 0) {
-    mega_event(q, EV_SOLVE_END, 0, o, it);
+    log_event(q.log, ev_desc(EV_SOLVE_END, 0, o, it));
     int base = -1;
     if (fin) {
       // a gated pose-only object: the map-consistency check on its record; rejected, it wakes its joint slot (k_init
       // left the slot initialised, its iteration-0 counters set and no item queued), kept, the slot is done unrun
       // (a slot rejected at upload never gets here: its pose-only object was rejected at upload too)
-      const int slot = (sv.link != nullptr && sv.state[o].mode == DSPGN_MODE_POSE) ? sv.link[o] : -1;
-      const bool wake = slot >= 0 && gate_record(sv.results, o, sv.T_init, sv.t_map) == DSPGN_GATE_REJECTED;
+      const int slot = (b.link != nullptr && b.state[o].mode == DSPGN_MODE_POSE) ? b.link[o] : -1;
+      const bool wake = slot >= 0 && gate_record(b.results, o, b.T_init, b.t_map) == DSPGN_GATE_REJECTED;
       __threadfence();                       // the result record before the object counts as done
-      atomicAdd(q.done_objects, (slot >= 0 && !wake) ? 2 : 1);
+      atomicAdd(&q.ctr->done_objects, (slot >= 0 && !wake) ? 2 : 1);
       if (wake) {
-        const int ntF = ldv(q.ray_left + slot), ntS = (sv.meta[slot].n_pts + kTcRows - 1) / kTcRows;
-        base = atomicAdd(q.q_tail, ntF + ntS);
+        const int ntF = ldv(q.ray_left + slot), ntS = (b.meta[slot].n_pts + kTcRows - 1) / kTcRows;
+        base = atomicAdd(&q.ctr->tail, ntF + ntS);
         S.push_nF = ntF; S.push_nS = ntS; S.push_o = slot;
       }
     } else {
-      // (no fence in this branch: q_tail only reserves slots; state and counters are fenced below, before any slot is published)
-      const ObjMeta M = sv.meta[o];
+      // (no fence in this branch: the tail only reserves slots; state and counters are fenced below, before any slot is published)
+      const ObjMeta M = b.meta[o];
       const int ntS = (M.n_pts + kTcRows - 1) / kTcRows;
-      const int ntF = render ? ((vh >= 0 ? vh : M.n_rays * S.ctx_D) + kTcRows - 1) / kTcRows : 0;
+      const int ntF = render ? ((vh >= 0 ? vh : M.n_rays * b.D) + kTcRows - 1) / kTcRows : 0;
       *reinterpret_cast<volatile int*>(q.obj_iter + o) = it + 1;
       *reinterpret_cast<volatile int*>(q.pending + o) = ntS + (ntF > 0 ? 1 : 0);
       *reinterpret_cast<volatile int*>(q.ray_left + o) = ntF;
-      base = atomicAdd(q.q_tail, ntF + ntS);  // the long chain (rays -> scan -> band -> solve) first, then the SDF tiles
+      base = atomicAdd(&q.ctr->tail, ntF + ntS);  // the long chain (rays -> scan -> band -> solve) first, then the SDF tiles
       S.push_nF = ntF; S.push_nS = ntS; S.push_o = o;
     }
     S.push_base = base;
@@ -453,7 +444,7 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
 }
 
 template <int SCHED>
-__device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, const SolveArgs& sv, const ScanArgs& sc_args) {
+__device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, const MegaArgs& q, const SolveArgs& sv) {
   constexpr bool MEGA = SCHED != 0;
   constexpr bool RENDER = SCHED == 2;
   extern __shared__ unsigned char tc_smem_raw[];
@@ -461,19 +452,19 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
   TcSmemTail& S = *reinterpret_cast<TcSmemTail*>(ring + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  const int total_tiles = MEGA ? 0 : build_tile_prefix(a, kTcRows, S.prefix, S.warp_tmp);
+  const int total_tiles = MEGA ? 0 : build_tile_prefix(b, a, kTcRows, S.prefix, S.warp_tmp);
   {
-    const int nwords = a.n_classes * (int)(sizeof(TcPlan) / 4);
+    const int nwords = b.n_classes * (int)(sizeof(TcPlan) / 4);
     for (int i = tid; i < nwords; i += kTcThreads) {
       const int c = i / (int)(sizeof(TcPlan) / 4), w = i % (int)(sizeof(TcPlan) / 4);
-      reinterpret_cast<int*>(&S.plans[c])[w] = reinterpret_cast<const int*>(&a.decs[c].tc_plan)[w];
+      reinterpret_cast<int*>(&S.plans[c])[w] = reinterpret_cast<const int*>(&b.decs[c].tc_plan)[w];
     }
   }
   if (tid == 0) {
     for (int i = 0; i < kTcStages; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
     S.cur_class = -1;
     S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
-    if (MEGA) { S.ctx_q = q; S.ctx_sv = sv; S.ctx_D = a.D; S.ctx_rays = a.rays; }
+    if (MEGA) { S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv; }
     fence_barrier_init();
   }
   __syncthreads();
@@ -489,18 +480,18 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           // scheduler: fetch this CTA's next tile into the local FIFO (at most 3 entries ahead of the epilogue)
           volatile int* es = &S.epi_seq;
           while (seq - *es >= 3) __nanosleep(64);   // the epilogue warps always make progress (bounded tile work)
-          const int item = mega_pop(q, a.n_obj);
-          if (item >= 0) mega_event(q, EV_POPPED, item >> kItemKindShift, (item >> kItemObjShift) & kItemObjMask, item & kItemTileMask);
+          const int item = mega_pop(q, b.n_obj);
+          if (item >= 0) log_event(q.log, ev_desc(EV_POPPED, item >> kItemKindShift, (item >> kItemObjShift) & kItemObjMask, item & kItemTileMask));
           reinterpret_cast<volatile int*>(S.fifo)[seq & 3] = item;
           __threadfence_block();
           *reinterpret_cast<volatile int*>(&S.fifo_pub) = seq + 1;
         }
         TileRef tr;
-        if (!tile_at<SCHED>(a, S, seq, total_tiles, tr)) break;
+        if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
         const int o = tr.o;
-        const int cls = a.meta[o].class_id;
+        const int cls = b.meta[o].class_id;
         const TcPlan& plan = S.plans[cls];
-        const unsigned char* blob = a.decs[cls].tc_blob;
+        const unsigned char* blob = b.decs[cls].tc_blob;
         const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD);
         const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
         for (int s = 0; s < ns; ++s)
@@ -523,20 +514,18 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
     uint32_t phase = 0;
     float acc[128];
     uint32_t ah[64];
-    int clk_tile = -1;
     for (int seq = 0;; ++seq) {
-      ++clk_tile;
       TileRef tr;
-      if (!tile_at<SCHED>(a, S, seq, total_tiles, tr)) break;
-      if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = seq + 1; mega_event(q, EV_TILE_BEGIN, tr.mode, tr.o, tr.tile); }
+      if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
+      if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = seq + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
       if (RENDER && tr.mode == kKindScan) {
         // ---- scan item: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141); no GEMM steps ----------
         const int o = tr.o;
-        scan_chunk(sc_args, q.seg_cnt, o, tr.tile, tid);
+        scan_chunk(b, sv.prm.th, q.vpre, q.seg_cnt, o, tr.tile, tid);
         __threadfence();
         epi_bar_sync();
         if (tid == 0) {
-          mega_event(q, EV_TILE_END, tr.mode, o, tr.tile);
+          log_event(q.log, ev_desc(EV_TILE_END, tr.mode, o, tr.tile));
           *reinterpret_cast<volatile int*>(&S.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
         }
         epi_bar_sync();
@@ -544,14 +533,14 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         if (act == 1) {
           // last chunk of the object: segment prefix -> band row count -> band tiles
           __threadfence();
-          scan_prefix(sc_args, q.seg_cnt, q.seg_prefix, o, tid, S.warp_tmp);
+          scan_prefix(b, q.seg_cnt, q.seg_prefix, o, tid, S.warp_tmp);
           epi_bar_sync();
           if (tid == 0) {
             __threadfence();                         // prefix / band_m / band rows before the band tiles are published
-            atomicAdd(q.valid_rows_total, (unsigned long long)ldv(sc_args.V_count + o));   // V of this iteration is complete (roofline accounting)
-            const int m = ldv(sc_args.band_m + o);
+            atomicAdd(&q.ctr->valid_rows_total, (unsigned long long)ldv(b.V_count + o));   // V of this iteration is complete (roofline accounting)
+            const int m = ldv(b.band_m + o);
             const int ntB = (m + kTcRows - 1) / kTcRows;
-            atomicAdd(q.band_rows_total, m);
+            atomicAdd(&q.ctr->band_rows_total, m);
             // the render term's placeholder in `pending` becomes its ntB band tiles BEFORE they can be popped
             const int left = atomicAdd(q.pending + o, ntB - 1) + ntB - 1;
             mega_push(q, MODE_BAND, o, ntB);
@@ -560,13 +549,13 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           epi_bar_sync();
           act = *reinterpret_cast<volatile int*>(&S.last_flag);
         } else act = 0;
-        if (act == 2) mega_solve_and_advance<MEGA>(S, o, tid);
+        if (act == 2) mega_solve_and_advance(S, o, tid);
         continue;
       }
       const int o = tr.o, row0 = tr.row0, tile = tr.slot, mode = tr.mode;
-      const ObjMeta M = a.meta[o];
-      const ObjState& ost = a.state[o];
-      const DecoderDev& dec = a.decs[M.class_id];
+      const ObjMeta M = b.meta[o];
+      const ObjState& ost = b.state[o];
+      const DecoderDev& dec = b.decs[M.class_id];
       const TcPlan& plan = S.plans[M.class_id];
       const int L = dec.L, in0 = dec.in0, n_lin = dec.n_lin;
       const bool has_skip = dec.latent_in >= 0;
@@ -581,7 +570,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       if (tid < 12) S.ost[tid] = ldv(&ost.T_oc[tid]);
       else if (tid < 16) S.ost[tid] = ldv(&ost.dmin + (tid - 12));          // dmin, dmax, dstep, dfar
       const bool pts_mode = (mode == MODE_SDF || mode == MODE_PTSFWD);
-      if (MEGA && !pts_mode && tid == 16) S.ost_rows = mega_rows(a, q, M, o, mode);   // band / ray-sample rows: a counter
+      if (MEGA && !pts_mode && tid == 16) S.ost_rows = mega_rows(b, q, M, o, mode);   // band / ray-sample rows: a counter
 
       // per-class constants in smem (bias, last row, xyz rows of layer 0), the tile's latent code
       if (S.cur_class != M.class_id) {
@@ -619,9 +608,9 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       int nrows = 0;
       float p0 = 0.f, p1 = 0.f, p2 = 0.f, sc = 0.f;
       if (pts_mode) {
-        nrows = min(kTcRows, (MEGA ? M.n_pts : term_rows(a, o)) - row0);
+        nrows = min(kTcRows, (MEGA ? M.n_pts : term_rows(b, a, o)) - row0);
         if (r < nrows) {
-          const float* pq = a.pts + 3 * (size_t)(M.pts_off + row0 + r);
+          const float* pq = b.pts + 3 * (size_t)(M.pts_off + row0 + r);
           p0 = pq[0]; p1 = pq[1]; p2 = pq[2];
           sc = (mask_in == nullptr || ldv(mask_in + M.pts_off + row0 + r)) ? 1.f : 0.f;
         }
@@ -632,7 +621,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
       float Toc[12];
 #pragma unroll
       for (int i = 0; i < 12; ++i) Toc[i] = S.ost[i];
-      if (!pts_mode) nrows = min(kTcRows, (MEGA ? S.ost_rows : term_rows(a, o)) - row0);
+      if (!pts_mode) nrows = min(kTcRows, (MEGA ? S.ost_rows : term_rows(b, a, o)) - row0);
       float x0 = 0.f, x1 = 0.f, x2 = 0.f, res_in = 0.f;
       if (r < nrows) {
         const int rr_ = row0 + r;
@@ -644,19 +633,19 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           if (RENDER) {
             int lo = 0, hi = nseg;                     // largest segment with prefix <= row
             while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (segp[mid] <= rr_) lo = mid; else hi = mid; }
-            sidx = (size_t)M.smp_off + (size_t)lo * kSegRays * a.D + (size_t)(rr_ - segp[lo]);
+            sidx = (size_t)M.smp_off + (size_t)lo * kSegRays * b.D + (size_t)(rr_ - segp[lo]);
           }
-          x0 = __ldcg(a.band_x + 3 * sidx); x1 = __ldcg(a.band_x + 3 * sidx + 1); x2 = __ldcg(a.band_x + 3 * sidx + 2);
-          sc = __ldcg(a.band_s + sidx); res_in = __ldcg(a.band_r + sidx);
+          x0 = __ldcg(b.band_x + 3 * sidx); x1 = __ldcg(b.band_x + 3 * sidx + 1); x2 = __ldcg(b.band_x + 3 * sidx + 2);
+          sc = __ldcg(b.band_s + sidx); res_in = __ldcg(b.band_r + sidx);
         } else {
-          int ray = rr_ / a.D, j = rr_ - ray * a.D;
+          int ray = rr_ / b.D, j = rr_ - ray * b.D;
           if (compact) {
             int lo = 0, hi = M.n_rays;                 // largest ray whose hull starts at or before this row
             while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((segp[mid] >> 7) <= rr_) lo = mid; else hi = mid; }
             ray = lo; j = (segp[lo] & 127) + (rr_ - (segp[lo] >> 7));
           }
-          const float* rq = a.rays + 3 * (size_t)(M.ray_off + ray);
-          const float d = lin_depth(S.ost[12], S.ost[13], S.ost[14], j, a.D);
+          const float* rq = b.rays + 3 * (size_t)(M.ray_off + ray);
+          const float d = lin_depth(S.ost[12], S.ost[13], S.ost[14], j, b.D);
           xform_point(Toc, __fmul_rn(rq[0], d), __fmul_rn(rq[1], d), __fmul_rn(rq[2], d), x0, x1, x2);
           sc = inside_unit_sphere(x0, x1, x2) ? 1.f : 0.f;            // loss.py:68
         }
@@ -705,16 +694,12 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         const bool more = (s + 1 < ns);
         const int k_next = more ? plan.step[s + 1].k_steps * 16 : 0;
         const int nm = st.n_mma;
-        if (tid == 0) {
-          DSPGN_CLK(4);
-          if (MEGA && s == 0) mega_event(q, EV_FIRST_MMA, tr.mode, tr.o, tr.tile);
-        }
+        if (MEGA && tid == 0 && s == 0) log_event(q.log, ev_desc(EV_FIRST_MMA, tr.mode, tr.o, tr.tile));
         const int nch = st.k_steps / 4;
         if (nm == 80) wg_gemm<80>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
         else if (nm == 192) wg_gemm<192>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
         else wg_gemm<256>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
         wg_bar_sync(grp);                                // every MMA of the warpgroup has read the A lo image
-        if (tid == 0) DSPGN_CLK(0);
         const int qs = opaque_int(qd);
 
         if (st.kind == TK_FWD_PENULT) {
@@ -748,11 +733,11 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
           if (fwd_only) {
             if (grp == 0 && r < nrows) {
               const size_t base = (mode == MODE_RAYFWD) ? (size_t)M.smp_off : (size_t)M.pts_off;
-              a.sdf_out[base + row0 + r] = (sc != 0.f) ? yv : INFINITY;
+              b.sdf[base + row0 + r] = (sc != 0.f) ? yv : INFINITY;
             }
             if (!RENDER && mode == MODE_RAYFWD) {        // (persistent kernel: counted by the scan items, dspgn_solve.cuh)
-              const unsigned b = __ballot_sync(0xffffffffu, grp == 0 && r < nrows && sc != 0.f);
-              if (lane == 0 && b) atomicAdd(a.V_count + o, __popc(b));
+              const unsigned bal = __ballot_sync(0xffffffffu, grp == 0 && r < nrows && sc != 0.f);
+              if (lane == 0 && bal) atomicAdd(b.V_count + o, __popc(bal));
             }
           }
           if (more) {
@@ -823,7 +808,6 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
 #pragma unroll
           for (int i = 0; i < 64; ++i) ah[i] = 0u;
         }
-        if (tid == 0) DSPGN_CLK(3);
       }
       if (!fwd_only) {
       // ---- pose columns, residual (thread = row; needs every d/d(input) column of the row) -----------
@@ -911,7 +895,7 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
         __threadfence();                             // this tile's partial sums / sdf values are visible device-wide
         epi_bar_sync();
         if (tid == 0) {
-          mega_event(q, EV_TILE_END, mode, o, tr.tile);
+          log_event(q.log, ev_desc(EV_TILE_END, mode, o, tr.tile));
           int act = 0;
           if (RENDER && mode == MODE_RAYFWD) { if (atomicSub(q.ray_left + o, 1) == 1) act = 1; }
           else if (atomicSub(q.pending + o, 1) == 1) act = 2;
@@ -928,24 +912,24 @@ __device__ __forceinline__ void tc_body(const TermArgs& a, const MegaArgs& q, co
             mega_push(q, kKindScan, o, nch);
           }
         }
-        if (act == 2) mega_solve_and_advance<MEGA>(S, o, tid);
+        if (act == 2) mega_solve_and_advance(S, o, tid);
       }
       // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
     }
   }
 }
 
-__global__ void __launch_bounds__(kTcThreads, 1) k_decoder_tc(TermArgs a) {
-  tc_body<0>(a, MegaArgs{}, SolveArgs{}, ScanArgs{});
+__global__ void __launch_bounds__(kTcThreads, 1) k_decoder_tc(BatchDev b, TermArgs a) {
+  tc_body<0>(b, a, MegaArgs{}, SolveArgs{});
 }
 // persistent object-pipelined variants: all GN iterations of all objects in ONE launch.
 // k_gn_persistent: SDF tiles only (SDF-only joint runs, pose-only runs); k_gn_persistent_render: joint runs with the
 // render term (ray-sample tiles, scan items, band tiles, SDF tiles)
-__global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent(TermArgs a, MegaArgs q, SolveArgs sv) {
-  tc_body<1>(a, q, sv, ScanArgs{});
+__global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv) {
+  tc_body<1>(b, a, q, sv);
 }
-__global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent_render(TermArgs a, MegaArgs q, SolveArgs sv, ScanArgs sc) {
-  tc_body<2>(a, q, sv, sc);
+__global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent_render(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv) {
+  tc_body<2>(b, a, q, sv);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1118,10 +1102,11 @@ inline int tc_setup_kernels(std::string& err) {
 
 inline bool tc_engine_default() { return true; }
 
-inline int tc_launch_term(TermArgs& a, int num_sms, long long tiles_upper, cudaStream_t stream, std::string& err) {
+inline int tc_launch_term(const BatchDev& b, const TermArgs& a, int num_sms, long long tiles_upper, cudaStream_t stream,
+                          std::string& err) {
   int grid = (int)std::min<long long>(tiles_upper, num_sms);
   if (grid < 1) grid = 1;
-  k_decoder_tc<<<grid, kTcThreads, kTcSmemBytes, stream>>>(a);
+  k_decoder_tc<<<grid, kTcThreads, kTcSmemBytes, stream>>>(b, a);
   (void)err;
   return 0;
 }

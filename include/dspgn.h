@@ -276,16 +276,14 @@ int dspgn_debug_system(DspgnSolver* s, int obj, int mode, float* H, float* b, fl
 int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* H, float* b, float* dx,
                             float* J_rows, float* res_rows, float* losses);
 
-/* Debug: clock64 timeline of CTA 0 of the tensor-core decoder kernel, [4 tiles][18 steps][8 slots]
- * (only when the solver was created with env DSPGN_CLK set). */
-int dspgn_debug_clocks(DspgnSolver* s, long long* out, int n);
-
 /* Test hook for the device-side input construction: the resident batch's object `obj` as the kernels see it --
  * t_cam_obj (16, row-major), pts (n_pts*3, xyz interleaved), rays (n_rays*3).  Any pointer may be NULL. */
 int dspgn_debug_inputs(DspgnSolver* s, int obj, float* t_cam_obj, float* pts, float* rays);
 
 /* Debug: event log of the last persistent-kernel run (tile begin/end per kind, scan, solve, queue pops), enabled by
- * env DSPGN_CLK at solver creation; returns the number of (timestamp, descriptor) pairs written, or a negative code. */
+ * env DSPGN_CLK at solver creation; returns the number of (timestamp, descriptor) pairs written, or a negative code.
+ * out[2i] = %globaltimer (ns), out[2i+1] = kind<<56 | mode<<52 | sm<<40 | object<<24 | tile (or iteration, solve phase);
+ * tools/mega_timeline.py decodes it. */
 int dspgn_debug_events(DspgnSolver* s, long long* out, int max_events);
 
 /* Test hook for the wgmma operand paths: D[128][n_mma] = A[128][16*k_steps] * B[n_mma][16*k_steps]^T

@@ -51,7 +51,7 @@ def test_hgmma_waits_are_batched(kernel):
 @pytest.mark.parametrize("kernel", [
     pytest.param("k_gn_persistent_render", marks=pytest.mark.xfail(strict=True, reason="6 LDL/STL left in the span")),
     "k_gn_persistentENS",
-    pytest.param("k_decoder_tc", marks=pytest.mark.xfail(strict=True, reason="15 LDL/STL left in the span")),
+    pytest.param("k_decoder_tc", marks=pytest.mark.xfail(strict=True, reason="4 LDL/STL left in the span")),
 ])
 def test_hgmma_span_has_no_local_memory_traffic(kernel):
     span, _ = _hgmma_span(kernel)
