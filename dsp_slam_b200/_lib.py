@@ -101,6 +101,10 @@ SYMBOLS = [
     ("dspgn_keyframe_batch_gated", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(GateIn),
                                              C.POINTER(ObjectOut)]),
     ("dspgn_decode_sdf", C.c_int, [_VP, C.c_int, _FP, _FP, C.c_int, C.c_int, C.c_int, _FP]),
+    ("dspgn_mesh_batch", C.c_int, [_VP, C.c_int, _FP, C.c_int, C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32),
+                                   C.POINTER(C.c_int32)]),
+    ("dspgn_mesh_results", C.c_int, [_VP, _FP, C.POINTER(C.c_int32), _FP]),
+    ("dspgn_debug_mesh_grid", C.c_int, [_VP, C.c_int, C.c_int, _FP, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("dspgn_counters", C.c_int, [_VP, C.POINTER(Counters)]),
     ("dspgn_enable_timing", C.c_int, [_VP, C.c_int]),
     ("dspgn_gather_create", C.c_int, [_VP, C.c_int, C.c_int, C.POINTER(IpcHandle)]),

@@ -9,10 +9,13 @@
 #include <new>
 #include <algorithm>
 
+#include <cub/device/device_scan.cuh>
+
 #include "dspgn_common.cuh"
 #include "dspgn_simt.cuh"
 #include "dspgn_solve.cuh"
 #include "dspgn_tc.cuh"
+#include "dspgn_mesh.cuh"
 
 using namespace dspgn;
 
@@ -139,6 +142,12 @@ struct DspgnSolver {
     int bound_n = -1;
   } gather;
   GatherDev gdev{};                  // exchange arguments of the run being enqueued (slots == nullptr: off)
+  // mesh calls (dspgn_mesh_batch): query points and scan workspace of one chunk, the grids of the whole call
+  DevBuf d_grid_pts, d_mgrid, d_mws, d_mscan_tmp, d_mout;
+  HostBuf h_mbase;
+  int mesh_n = 0, mesh_dim = 0;      // objects / grid size of the last mesh call (0: none)
+  std::vector<float> mesh_v;         // its meshes, object after object
+  std::vector<int32_t> mesh_f;
 };
 
 namespace {
@@ -353,8 +362,10 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   dspgn_gather_close(s);
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
-                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_run}) b->release();
+                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_run,
+                    &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout}) b->release();
   s->h_stage.release();
+  s->h_mbase.release();
   s->h_results.release();
   s->h_run.release();
   for (auto e : s->ev) cudaEventDestroy(e);
@@ -399,8 +410,10 @@ int dspgn_counters(DspgnSolver* s, DspgnCounters* out) {
 // ---------------------------------------------------------------------------------------------
 namespace {
 
-// decode_only: forward-only use (dspgn_decode_sdf) -- no J^T J partials, no band buffers
-int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool decode_only) {
+// decode_only: forward-only use (dspgn_decode_sdf) -- no J^T J partials, no band buffers.
+// grid_dim > 0 (mesh calls, decode_only): every object's points are the dim^3 query grid, written on the device into a
+// block of their own (in[o].pts is ignored, in[o].n_pts must be dim^3).
+int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool decode_only, int grid_dim = 0) {
   if (!s || !in) return fail(DSPGN_E_ARG, "null argument");
   if (n_obj < 1 || n_obj > kMaxObjScan) return fail(DSPGN_E_ARG, "n_obj must be in [1,1024] per resident batch");
   CU(cudaSetDevice(s->device));
@@ -415,7 +428,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
     // its batch neighbours nor raise inside the embedded interpreter
     if (!I.t_cam_obj) return fail(DSPGN_E_ARG, "object without a pose");
     if (I.class_id < 0 || I.class_id >= (int)s->classes.size()) return fail(DSPGN_E_ARG, "bad class_id");
-    const bool bad = I.n_pts < 1 || !I.pts || I.n_rays < 0 || I.n_depth < 0 || I.n_depth > I.n_rays ||
+    const bool bad = I.n_pts < 1 || (!I.pts && grid_dim == 0) || I.n_rays < 0 || I.n_depth < 0 || I.n_depth > I.n_rays ||
                      I.n_rays > kScanMaxRays || (I.n_rays > 0 && I.n_depth > 0 && !I.depth) || (I.pixels && !I.inv_k);
     const float* ray_src = I.pixels ? I.pixels : I.rays;
     ObjMeta& M = s->h_meta[o];
@@ -435,7 +448,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
   // one staging block: meta | T_init | code | pts | rays | depth
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   const size_t o_meta = 0, o_T = al(o_meta + sizeof(ObjMeta) * n_obj), o_code = al(o_T + 64 * n_obj),
-               o_pts = al(o_code + 4 * kMaxCode * (size_t)n_obj), o_rays = al(o_pts + 12 * (size_t)tp),
+               o_pts = al(o_code + 4 * kMaxCode * (size_t)n_obj), o_rays = al(o_pts + (grid_dim ? 0 : 12 * (size_t)tp)),
                o_depth = al(o_rays + 12 * (size_t)tr), o_tb = al(o_depth + 4 * (size_t)tf),
                o_aux = al(o_tb + 2 * 4 * (size_t)n_obj),
                total = al(o_aux + (any_build ? 4 * (size_t)kAuxFloats * n_obj : 0));
@@ -471,8 +484,9 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
       for (int c = 0; c < 4; ++c) hT[o * 16 + r * 4 + c] = I.t_cam_obj[(size_t)r * I.t_rs + (size_t)c * I.t_cs];
     for (int i = 0; i < kMaxCode; ++i) hC[o * kMaxCode + i] = (I.code && i < s->cfg.code_len) ? I.code[i] : 0.f;
     float* p = hP + 3 * (size_t)M.pts_off;
-    if (M.n_pts > 0 && I.pts_cs == 1 && I.pts_rs == 3) memcpy(p, I.pts, 12 * (size_t)M.n_pts);
-    else for (int r = 0; r < M.n_pts; ++r)
+    const int n_host_pts = grid_dim ? 0 : M.n_pts;
+    if (n_host_pts > 0 && I.pts_cs == 1 && I.pts_rs == 3) memcpy(p, I.pts, 12 * (size_t)M.n_pts);
+    else for (int r = 0; r < n_host_pts; ++r)
       for (int c = 0; c < 3; ++c) p[3 * (size_t)r + c] = I.pts[(size_t)r * I.pts_rs + (size_t)c * I.pts_cs];
     float* q = hR + 3 * (size_t)M.ray_off;
     if (M.build & 1) {                      // pixel coordinates: the device turns (u, v, 1) into inv_k [u, v, 1]
@@ -503,10 +517,19 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
     k_build_inputs<<<n_obj, 256, 0, s->stream>>>(ba);
     CU(cudaGetLastError());
   }
+  if (grid_dim) {
+    if (s->d_grid_pts.cap < 12 * (size_t)tp) CU(cudaStreamSynchronize(s->stream));
+    if (s->d_grid_pts.reserve(12 * (size_t)tp)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
+    const long long R = (long long)grid_dim * grid_dim * grid_dim;
+    k_mesh_grid_points<<<dim3((unsigned)((R + 255) / 256), (unsigned)std::min(n_obj, 65535)), 256, 0, s->stream>>>(
+        s->d_grid_pts.as<float>(), n_obj, grid_dim);
+    s->ctr.kernel_launches++;
+    CU(cudaGetLastError());
+  }
   s->d_meta = reinterpret_cast<ObjMeta*>(db + o_meta);
   s->d_Tinit = reinterpret_cast<float*>(db + o_T);
   s->d_code = reinterpret_cast<float*>(db + o_code);
-  s->d_pts = reinterpret_cast<float*>(db + o_pts);
+  s->d_pts = grid_dim ? s->d_grid_pts.as<float>() : reinterpret_cast<float*>(db + o_pts);
   s->d_rays = reinterpret_cast<float*>(db + o_rays);
   s->d_depth = reinterpret_cast<float*>(db + o_depth);
   s->d_tbase_static = reinterpret_cast<int*>(db + o_tb);
@@ -1230,6 +1253,158 @@ int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const floa
   s->ctr.rows_fwd_only += n;
   CU(cudaMemcpyAsync(sdf_out, s->d_sdf.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
   CU(cudaStreamSynchronize(s->stream));
+  return 0;
+}
+
+namespace {
+
+// The iso-surface of the chunk's grids g (dspgn_mesh.cuh), appended to s->mesh_v / mesh_f; per-object counts into nV / nF.
+int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF) {
+  const size_t nv = (size_t)g.n * g.R, nf = 4 * (size_t)g.n * g.C;
+  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
+  // workspace: vertex counts -> scan [nv + 1] | face counts -> scan [nf + 1] | edge masks [nv] | cube flags [n C] |
+  // per-object bases [n + 1][2]
+  const size_t o_fc = al(4 * (nv + 1)), o_mask = o_fc + al(4 * (nf + 1)), o_ok = o_mask + al(nv),
+               o_base = o_ok + al((size_t)g.n * g.C), total = o_base + al(8 * ((size_t)g.n + 1));
+  if (s->d_mws.cap < total) CU(cudaStreamSynchronize(s->stream));
+  if (s->d_mws.reserve(total)) return fail(DSPGN_E_ALLOC, "mesh workspace allocation failed");
+  unsigned char* w = s->d_mws.as<unsigned char>();
+  int* vscan = reinterpret_cast<int*>(w);
+  int* fscan = reinterpret_cast<int*>(w + o_fc);
+  uint8_t* mask = w + o_mask;
+  uint8_t* ok = w + o_ok;
+  int* bases = reinterpret_cast<int*>(w + o_base);
+  size_t tmp_v = 0, tmp_f = 0;
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_v, vscan, vscan, (int)(nv + 1), s->stream));
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_f, fscan, fscan, (int)(nf + 1), s->stream));
+  if (s->d_mscan_tmp.cap < std::max(tmp_v, tmp_f)) CU(cudaStreamSynchronize(s->stream));
+  if (s->d_mscan_tmp.reserve(std::max(tmp_v, tmp_f)) || s->h_mbase.reserve(8 * ((size_t)g.n + 1)))
+    return fail(DSPGN_E_ALLOC, "mesh workspace allocation failed");
+  // the slot after the last count: the scans' totals
+  CU(cudaMemsetAsync(vscan + nv, 0, 4, s->stream));
+  CU(cudaMemsetAsync(fscan + nf, 0, 4, s->stream));
+  const unsigned bc = (unsigned)(((size_t)g.n * g.C + 255) / 256), bv = (unsigned)((nv + 255) / 256);
+  k_mesh_cubes<<<bc, 256, 0, s->stream>>>(g, ok, fscan);
+  k_mesh_verts<<<bv, 256, 0, s->stream>>>(g, ok, mask, vscan);
+  CU(cudaGetLastError());
+  size_t tb = s->d_mscan_tmp.cap;
+  CU(cub::DeviceScan::ExclusiveSum(s->d_mscan_tmp.p, tb, vscan, vscan, (int)(nv + 1), s->stream));
+  tb = s->d_mscan_tmp.cap;
+  CU(cub::DeviceScan::ExclusiveSum(s->d_mscan_tmp.p, tb, fscan, fscan, (int)(nf + 1), s->stream));
+  // per object: first vertex and first face (object n: the totals); the counts come back here (one read-back)
+  k_mesh_bases<<<(g.n + 1 + 127) / 128, 128, 0, s->stream>>>(g, vscan, fscan, bases);
+  CU(cudaGetLastError());
+  int* hb = s->h_mbase.as<int>();
+  CU(cudaMemcpyAsync(hb, bases, 8 * ((size_t)g.n + 1), cudaMemcpyDeviceToHost, s->stream));
+  CU(cudaStreamSynchronize(s->stream));
+  for (int o = 0; o < g.n; ++o) { nV[o] = hb[2 * o + 2] - hb[2 * o]; nF[o] = hb[2 * o + 3] - hb[2 * o + 1]; }
+  const size_t V = (size_t)hb[2 * g.n], F = (size_t)hb[2 * g.n + 1];
+  s->ctr.kernel_launches += 2 + 2 * 2 + 1;                    // classify passes, two scans (two kernels each), bases
+  if (V == 0 && F == 0) return 0;
+  if (s->d_mout.reserve(12 * (V + F))) return fail(DSPGN_E_ALLOC, "mesh output allocation failed");
+  float* dv = s->d_mout.as<float>();
+  int32_t* df = reinterpret_cast<int32_t*>(dv + 3 * V);
+  k_mesh_emit_verts<<<bv, 256, 0, s->stream>>>(g, mask, vscan, dv);
+  k_mesh_emit_faces<<<bc, 256, 0, s->stream>>>(g, mask, vscan, fscan, df);
+  CU(cudaGetLastError());
+  s->ctr.kernel_launches += 2;
+  const size_t v0 = s->mesh_v.size(), f0 = s->mesh_f.size();
+  s->mesh_v.resize(v0 + 3 * V);
+  s->mesh_f.resize(f0 + 3 * F);
+  CU(cudaMemcpyAsync(s->mesh_v.data() + v0, dv, 12 * V, cudaMemcpyDeviceToHost, s->stream));
+  CU(cudaMemcpyAsync(s->mesh_f.data() + f0, df, 12 * F, cudaMemcpyDeviceToHost, s->stream));
+  CU(cudaStreamSynchronize(s->stream));
+  return 0;
+}
+
+// One mesh call: grids decoded from codes (sdf_in == nullptr) or given by the caller, meshed chunk after chunk.  The
+// grids of the whole call stay in HBM for dspgn_mesh_results (4 B per grid row); the rest of the device memory is per
+// chunk of at most kMeshChunkRows grid rows, about 34 B per row (query points 12, vertex scan 4, face scans 16, flags 2),
+// plus the chunk's meshes.
+int mesh_impl(DspgnSolver* s, int n, int dim, const float* codes, int code_stride, const int32_t* class_ids,
+              const float* sdf_in, int32_t* n_vertices, int32_t* n_faces) {
+  if (!s || n < 1 || !n_vertices || !n_faces) return fail(DSPGN_E_ARG, "bad argument");
+  if (dim < 2 || dim > kMeshMaxDim) return fail(DSPGN_E_ARG, "voxels_dim must be in [2,128]");
+  if (!codes && !sdf_in) return fail(DSPGN_E_ARG, "null codes");
+  if (codes && code_stride < s->cfg.code_len) return fail(DSPGN_E_ARG, "code_stride must be >= code_len");
+  for (int o = 0; class_ids && o < n; ++o)
+    if (class_ids[o] < 0 || class_ids[o] >= (int)s->classes.size()) return fail(DSPGN_E_ARG, "bad class_id");
+  CU(cudaSetDevice(s->device));
+  const long long R = (long long)dim * dim * dim, C = (long long)(dim - 1) * (dim - 1) * (dim - 1);
+  const int per_chunk = (int)std::max<long long>(1, std::min<long long>(kMaxObjScan, kMeshChunkRows / R));
+  s->mesh_n = 0;
+  s->mesh_v.clear(); s->mesh_f.clear();
+  if (s->d_mgrid.cap < 4 * (size_t)n * R) CU(cudaStreamSynchronize(s->stream));
+  if (s->d_mgrid.reserve(4 * (size_t)n * R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
+  s->ctr = DspgnCounters{};
+  s->ev_used = 0;
+  s->gdev = GatherDev{};
+  CU(cudaEventRecord(s->ev_run0, s->stream));
+  if (sdf_in) CU(cudaMemcpyAsync(s->d_mgrid.p, sdf_in, 4 * (size_t)n * R, cudaMemcpyHostToDevice, s->stream));
+  const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  std::vector<DspgnObjectIn> ins;
+  const std::vector<int32_t> joint(per_chunk, DSPGN_MODE_JOINT);
+  for (int o0 = 0; o0 < n; o0 += per_chunk) {
+    const int nc = std::min(per_chunk, n - o0);
+    float* grid = s->d_mgrid.as<float>() + (size_t)o0 * R;
+    if (codes) {            // dspgn_decode_sdf of the query grid, every object of the chunk in one launch
+      ins.assign(nc, DspgnObjectIn{});
+      for (int k = 0; k < nc; ++k) {
+        DspgnObjectIn& I = ins[k];
+        I.t_cam_obj = I4; I.t_rs = 4; I.t_cs = 1;
+        I.n_pts = (int)R;
+        I.code = codes + (size_t)(o0 + k) * code_stride; I.scale = 1.f; I.class_id = class_ids ? class_ids[o0 + k] : 0;
+      }
+      if (int rc = upload_batch_impl(s, nc, ins.data(), true, dim)) return rc;
+      RunPlan p;
+      if (int rc = plan_run(s, joint.data(), p)) return rc;
+      BatchDev b = batch_dev(s);
+      b.sdf = grid;
+      if (int rc = launch_init(s, b, p)) return rc;
+      if (int rc = launch_term(s, b, base_term(s, MODE_PTSFWD), (long long)nc * R)) return rc;
+      s->ctr.rows_fwd_only += (long long)nc * R;
+    }
+    const MeshGrid g{grid, nc, dim, R, C, 2.0 / (dim - 1)};
+    if (int rc = mesh_chunk(s, g, n_vertices + o0, n_faces + o0)) return rc;
+  }
+  CU(cudaEventRecord(s->ev_run1, s->stream));
+  CU(cudaStreamSynchronize(s->stream));
+  if (s->timing) {
+    float dec = 0.f;
+    for (size_t i = 0; i + 1 < s->ev_used; i += 2) { float ms = 0.f; cudaEventElapsedTime(&ms, s->ev[i], s->ev[i + 1]); dec += ms; }
+    s->ctr.decoder_ms = dec;
+  }
+  float tot = 0.f;
+  if (cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot; else cudaGetLastError();
+  s->mesh_n = n; s->mesh_dim = dim;
+  return 0;
+}
+
+}  // namespace
+
+int dspgn_mesh_batch(DspgnSolver* s, int n, const float* codes, int code_stride, const int32_t* class_ids,
+                     int voxels_dim, int32_t* n_vertices, int32_t* n_faces) {
+  if (!codes) return fail(DSPGN_E_ARG, "null codes");
+  return mesh_impl(s, n, voxels_dim, codes, code_stride, class_ids, nullptr, n_vertices, n_faces);
+}
+
+int dspgn_debug_mesh_grid(DspgnSolver* s, int n, int voxels_dim, const float* sdf, int32_t* n_vertices, int32_t* n_faces) {
+  if (!sdf) return fail(DSPGN_E_ARG, "null sdf");
+  return mesh_impl(s, n, voxels_dim, nullptr, 0, nullptr, sdf, n_vertices, n_faces);
+}
+
+int dspgn_mesh_results(DspgnSolver* s, float* vertices, int32_t* faces, float* sdf) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  if (s->mesh_n < 1) return fail(DSPGN_E_ARG, "no mesh call to return");
+  if ((!vertices && !s->mesh_v.empty()) || (!faces && !s->mesh_f.empty())) return fail(DSPGN_E_ARG, "null output");
+  if (!s->mesh_v.empty()) memcpy(vertices, s->mesh_v.data(), 4 * s->mesh_v.size());
+  if (!s->mesh_f.empty()) memcpy(faces, s->mesh_f.data(), 4 * s->mesh_f.size());
+  if (sdf) {
+    CU(cudaSetDevice(s->device));
+    const size_t R = (size_t)s->mesh_dim * s->mesh_dim * s->mesh_dim;
+    CU(cudaMemcpyAsync(sdf, s->d_mgrid.p, 4 * (size_t)s->mesh_n * R, cudaMemcpyDeviceToHost, s->stream));
+    CU(cudaStreamSynchronize(s->stream));
+  }
   return 0;
 }
 

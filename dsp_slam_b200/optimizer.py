@@ -295,6 +295,43 @@ class BatchSolver:
                                                 out.ctypes.data_as(_FP)))
         return out
 
+    def mesh(self, codes, voxels_dim, class_ids=None, want_sdf=False):
+        """dspgn_mesh_batch: codes (n, >= code_len) -> list of (vertices (V,3) f32, faces (F,3) int32), one per code,
+        exactly MeshExtractor.extract_mesh_from_code's marching-tetrahedra mesh of each code's grid; with want_sdf also
+        the grids (n, dim, dim, dim)."""
+        codes = np.asarray(codes, dtype=np.float32)
+        if codes.ndim != 2:
+            raise ValueError("codes must be (n, code_len)")
+        if codes.shape[1] < self.cfg.code_len:      # zero-pad (optimizer.py:97-100 slices code[:code_len])
+            codes = np.concatenate([codes, np.zeros((codes.shape[0], self.cfg.code_len - codes.shape[1]), np.float32)], 1)
+        codes = np.ascontiguousarray(codes)
+        n = codes.shape[0]
+        cls = None if class_ids is None else (C.c_int32 * n)(*[int(c) for c in class_ids])
+        nv, nf = (C.c_int32 * max(n, 1))(), (C.c_int32 * max(n, 1))()
+        _lib.check(_lib.load().dspgn_mesh_batch(self.handle, n, codes.ctypes.data_as(_FP), codes.shape[1], cls,
+                                                int(voxels_dim), nv, nf))
+        return self._mesh_results(n, voxels_dim, nv, nf, want_sdf)
+
+    def debug_mesh_grid(self, sdf):
+        """dspgn_debug_mesh_grid: the device iso-surface of caller-given grids (n, dim, dim, dim) -> list of (V, F)."""
+        sdf = np.ascontiguousarray(sdf, dtype=np.float32)
+        n, dim = sdf.shape[0], sdf.shape[1]
+        nv, nf = (C.c_int32 * max(n, 1))(), (C.c_int32 * max(n, 1))()
+        _lib.check(_lib.load().dspgn_debug_mesh_grid(self.handle, n, dim, sdf.ctypes.data_as(_FP), nv, nf))
+        return self._mesh_results(n, dim, nv, nf, False)
+
+    def _mesh_results(self, n, dim, nv, nf, want_sdf):
+        nv, nf = np.array(nv[:n], np.int64), np.array(nf[:n], np.int64)
+        V = np.empty((int(nv.sum()), 3), np.float32)
+        F = np.empty((int(nf.sum()), 3), np.int32)
+        sdf = np.empty((n, dim, dim, dim), np.float32) if want_sdf else None
+        _lib.check(_lib.load().dspgn_mesh_results(self.handle, V.ctypes.data_as(_FP),
+                                                  F.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                  sdf.ctypes.data_as(_FP) if want_sdf else None))
+        ov, of = np.concatenate([[0], np.cumsum(nv)]), np.concatenate([[0], np.cumsum(nf)])
+        meshes = [(V[ov[i]:ov[i + 1]], F[of[i]:of[i + 1]]) for i in range(n)]
+        return (meshes, sdf) if want_sdf else meshes
+
     def debug_system(self, obj=0, mode=0, want_rows=False, n_pts=0, iteration=0):
         P = 6 if mode else 7 + self.cfg.code_len
         H = np.zeros((P, P), np.float32); b = np.zeros(P, np.float32); dx = np.zeros(P, np.float32)
@@ -506,7 +543,8 @@ def create_voxel_grid(vol_dim=128):
 
 class MeshExtractor(object):
     """Drop-in for reconstruct.optimizer.MeshExtractor (optimizer.py:206-223): the SDF grid is
-    decoded on the GPU; marching cubes stays on the host (skimage, as in the reference)."""
+    decoded on the GPU; marching cubes by scikit-image on the host when it is installed (as in the reference),
+    marching tetrahedra on the GPU otherwise (extract_meshes)."""
 
     def __init__(self, decoder, code_len=64, voxels_dim=64, device=0, engine=None):
         self.decoder = decoder
@@ -528,20 +566,27 @@ class MeshExtractor(object):
         s = self.solver.decode_sdf(code, self.voxel_points)
         return s.reshape(self.voxels_dim, self.voxels_dim, self.voxels_dim)
 
+    def extract_meshes(self, codes, class_ids=None):
+        """extract_mesh_from_code for several codes in one device call (dspgn_mesh_batch): a list of
+        ResultDict(vertices, faces), each bit-identical to dsp_slam_b200.mesh.marching_tetrahedra of the code's
+        grid shifted by -1 (what extract_mesh_from_code returns without scikit-image)."""
+        codes = np.stack([np.asarray(c, dtype=np.float32).reshape(-1)[:self.code_len] for c in codes])
+        return [ResultDict(vertices=v, faces=f) for v, f in self.solver.mesh(codes, self.voxels_dim, class_ids)]
+
     def extract_mesh_from_code(self, code):
         """optimizer.py:214-223.  Marching cubes by scikit-image exactly like the reference when it is installed
-        (DSP-SLAM's own environment); otherwise the dependency-free marching-tetrahedra fallback of
-        dsp_slam_b200.mesh (same level set, different triangulation)."""
+        (DSP-SLAM's own environment); otherwise marching tetrahedra on the device (extract_meshes), which returns
+        exactly what the dependency-free host fallback dsp_slam_b200.mesh returns (same level set, different
+        triangulation from scikit-image's)."""
         try:
-            sdf = self.sdf_grid(code)
-            voxel_size = 2.0 / (self.voxels_dim - 1)
             try:
                 from skimage import measure
-                mc = getattr(measure, "marching_cubes_lewiner", None) or measure.marching_cubes
-                verts, faces, _, _ = mc(sdf, level=0.0, spacing=[voxel_size] * 3)
             except ImportError:
-                from .mesh import marching_tetrahedra
-                verts, faces = marching_tetrahedra(sdf, level=0.0, spacing=[voxel_size] * 3)
+                return self.extract_meshes([code])[0]
+            sdf = self.sdf_grid(code)
+            voxel_size = 2.0 / (self.voxels_dim - 1)
+            mc = getattr(measure, "marching_cubes_lewiner", None) or measure.marching_cubes
+            verts, faces, _, _ = mc(sdf, level=0.0, spacing=[voxel_size] * 3)
             verts = verts + np.array([-1.0, -1.0, -1.0])          # reconstruct/utils.py:131-137
             return ResultDict(vertices=verts.astype("float32"), faces=faces.astype("int32"))
         except Exception as e:            # noqa: BLE001 -- called from C++ with no handler (LocalMapping_util.cc:194-196)

@@ -18,6 +18,7 @@
  *   ... with GetNewObservations' map check (LocalMapping_util.cc:104-147) and the demoted detections'
  *       reconstruction in CreateNewMapObjects (:179)             dspgn_keyframe_batch_gated
  *   loss_utils.decode_sdf        (reconstruct/loss_utils.py:51) dspgn_decode_sdf
+ *   MeshExtractor.extract_mesh_from_code (optimizer.py:214)     dspgn_mesh_batch + dspgn_mesh_results
  *   loss.compute_sdf_loss / compute_render_loss (loss.py:22,46) dspgn_debug_system (test hook)
  *
  * Conventions: every function returns 0 on success or a negative DSPGN_E_* code; per-object soft
@@ -217,6 +218,22 @@ int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* i
 /* Forward-only decode (loss_utils.decode_sdf): x (n,3) host, strides in elements -> sdf (n,) host. */
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n,
                      int x_rs, int x_cs, float* sdf_out);
+
+/* MeshExtractor.extract_mesh_from_code (reconstruct/optimizer.py:214-223) for n codes at once, on the device: the
+ * voxels_dim^3 grid of create_voxel_grid (written on the device) decoded like dspgn_decode_sdf, then the iso-surface
+ * sdf = 0 by marching tetrahedra, bit-identical in vertex and face order to dsp_slam_b200/mesh.py's
+ * marching_tetrahedra(grid, 0, h = 2/(dim-1)) with every vertex shifted by -1 as extract_mesh_from_code does.
+ * Replaces the solver's resident batch (like dspgn_decode_sdf).  codes: n x code_stride floats, the first code_len
+ * used.  class_ids NULL = class 0.  2 <= voxels_dim <= 128, else DSPGN_E_ARG; misuse returns DSPGN_E_ARG before anything
+ * is enqueued.  Objects are meshed in chunks of at most 2^24 grid rows; the grids of the call stay in HBM.
+ * Counters: rows_fwd_only += n * dim^3, and the call's launches. */
+int dspgn_mesh_batch(DspgnSolver* s, int n, const float* codes, int code_stride, const int32_t* class_ids,
+                     int voxels_dim, int32_t* n_vertices, int32_t* n_faces);
+/* the meshes of the last mesh call, object after object: vertices (sum n_vertices x 3, f32, object frame),
+ * faces (sum n_faces x 3, int32, indices local to the object's own vertices), sdf (n x dim^3, may be NULL) */
+int dspgn_mesh_results(DspgnSolver* s, float* vertices, int32_t* faces, float* sdf);
+/* test hook: the same iso-surface on n caller-given grids (n x dim^3 host floats) */
+int dspgn_debug_mesh_grid(DspgnSolver* s, int n, int voxels_dim, const float* sdf, int32_t* n_vertices, int32_t* n_faces);
 
 /* Counters of the last run (for roofline arithmetic): decoder rows evaluated fwd+bwd (SDF rows + band rows) and
  * fwd-only, and the number of kernel launches issued.  Persistent schedule: fwd-only rows = the sum of V over objects
