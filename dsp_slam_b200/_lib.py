@@ -14,6 +14,7 @@ ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC = 0, 1, 2
 SCHED_AUTO, SCHED_LAUNCHES, SCHED_PERSISTENT = 0, 1, 2
 MODE_JOINT, MODE_POSE = 0, 1
 GATE_OFF, GATE_KEPT, GATE_REJECTED = 0, 1, 2
+MESH_OFF, MESH_DONE, MESH_FAILED, MESH_LOST = 0, 1, 2, 3
 ST_OK, ST_SDF_NAN, ST_RENDER_FEW, ST_RENDER_NAN, ST_SOLVE, ST_BAD_INPUT = 0, 1, 2, 3, 4, 5
 E_ARG, E_CUDA, E_NOGPU, E_ALLOC, E_PEER = -1, -2, -3, -4, -5
 IPC_HANDLE_BYTES = 64
@@ -57,11 +58,20 @@ class ObjectOut(C.Structure):
                 ("status", C.c_int32), ("n_valid", C.c_int32), ("n_band", C.c_int32),
                 ("iters_done", C.c_int32), ("gate", C.c_int32), ("pad_", C.c_int32 * 2)]
 
+    @property
+    def mesh(self):
+        """DSPGN_MESH_* of dspgn_keyframe_batch_meshed (the header's `mesh`, the first word of pad_); 0 elsewhere."""
+        return self.pad_[0]
+
 
 class GateIn(C.Structure):
     _fields_ = [("t_cam_obj_map", _FP), ("map_rs", C.c_int32), ("map_cs", C.c_int32),
                 ("t_cam_obj_sim3", _FP), ("sim3_rs", C.c_int32), ("sim3_cs", C.c_int32),
                 ("gate", C.c_int32)]
+
+
+class MeshSpec(C.Structure):
+    _fields_ = [("voxels_dim", C.c_int32), ("pair", C.POINTER(C.c_int32))]
 
 
 class Counters(C.Structure):
@@ -100,6 +110,9 @@ SYMBOLS = [
     ("dspgn_keyframe_batch", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(ObjectOut)]),
     ("dspgn_keyframe_batch_gated", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(GateIn),
                                              C.POINTER(ObjectOut)]),
+    ("dspgn_keyframe_batch_meshed", C.c_int, [_VP, C.c_int, C.POINTER(ObjectIn), C.POINTER(C.c_int32), C.POINTER(GateIn),
+                                              C.POINTER(MeshSpec), C.POINTER(ObjectOut), C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int32)]),
     ("dspgn_decode_sdf", C.c_int, [_VP, C.c_int, _FP, _FP, C.c_int, C.c_int, C.c_int, _FP]),
     ("dspgn_mesh_batch", C.c_int, [_VP, C.c_int, _FP, C.c_int, C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32),
                                    C.POINTER(C.c_int32)]),

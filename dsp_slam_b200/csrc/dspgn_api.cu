@@ -148,6 +148,8 @@ struct DspgnSolver {
   int mesh_n = 0, mesh_dim = 0;      // objects / grid size of the last mesh call (0: none)
   std::vector<float> mesh_v;         // its meshes, object after object
   std::vector<int32_t> mesh_f;
+  std::vector<int32_t> mesh_grid_of; // meshed keyframe call: grid of each object in d_mgrid (-1: none); empty: grid o is object o's
+  DevBuf d_mesh_sel;                 // meshed keyframe call, per chunk: grid slot | pair partner of each resident slot
 };
 
 namespace {
@@ -363,7 +365,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
                     &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_run,
-                    &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout}) b->release();
+                    &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout, &s->d_mesh_sel}) b->release();
   s->h_stage.release();
   s->h_mbase.release();
   s->h_results.release();
@@ -1159,12 +1161,16 @@ int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in
   return 0;
 }
 
-int dspgn_keyframe_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, DspgnObjectOut* out) {
-  return dspgn_keyframe_batch_gated(s, n_obj, in, modes, nullptr, out);
-}
+namespace {
 
-int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
-                               const DspgnGateIn* gates, DspgnObjectOut* out) {
+int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF);
+
+// dspgn_keyframe_batch_gated, and with mesh != nullptr dspgn_keyframe_batch_meshed.  The objects are walked in units --
+// one object, or a mono pair (its two hypotheses next to each other) -- packed into resident chunks of at most
+// kMaxObjScan slots; a gated object's joint slot is appended after the chunk's objects.  When meshing, a chunk also holds
+// at most kMeshChunkRows grid rows of candidates, and its grids sit in walk order in the call's grid block.
+int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, const DspgnGateIn* gates,
+                  const DspgnMeshSpec* mesh, DspgnObjectOut* out, int32_t* n_vertices, int32_t* n_faces) {
   if (!s || !in || !modes || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
   if (int rc = check_modes(s, modes, n_obj, in)) return rc;
   auto gated = [&](int o) { return gates != nullptr && gates[o].gate != 0; };
@@ -1176,58 +1182,185 @@ int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* i
     if (!g.t_cam_obj_map || !g.t_cam_obj_sim3) return fail(DSPGN_E_ARG, "a gate needs t_cam_obj_map and t_cam_obj_sim3");
     if (in[o].t_cam_world) return fail(DSPGN_E_ARG, "a gated object takes camera-frame inputs (no t_cam_world)");
   }
-  // resident chunks of at most kMaxObjScan slots; a gated object and its joint slot (appended after the chunk's
-  // objects) always share a chunk
+  const int32_t* pair = mesh ? mesh->pair : nullptr;
+  const int dim = mesh ? mesh->voxels_dim : 0;
+  if (mesh) {
+    if (dim < 2 || dim > kMeshMaxDim) return fail(DSPGN_E_ARG, "voxels_dim must be in [2,128]");
+    for (int o = 0; pair && o < n_obj; ++o) {
+      const int j = pair[o];
+      if (j == -1) continue;
+      if (j < 0 || j >= n_obj || j == o || pair[j] != o) return fail(DSPGN_E_ARG, "pair must be symmetric, in range and never an object with itself");
+      if (modes[o] != DSPGN_MODE_JOINT || gated(o)) return fail(DSPGN_E_ARG, "a pair needs two ungated joint objects");
+    }
+  }
+  auto paired = [&](int o) { return pair != nullptr && pair[o] >= 0; };
+  auto candidate = [&](int o) { return modes[o] == DSPGN_MODE_JOINT || gated(o); };
+  const long long R = mesh ? (long long)dim * dim * dim : 0;
+  // walk order: every object once, the flipped hypothesis j right after its map-pose hypothesis i < j
+  std::vector<int> order;
+  order.reserve(n_obj);
+  int n_cand = 0;
+  for (int o = 0; o < n_obj; ++o) {
+    n_cand += candidate(o) ? 1 : 0;
+    if (paired(o) && pair[o] < o) continue;
+    order.push_back(o);
+    if (paired(o)) order.push_back(pair[o]);
+  }
+  std::vector<int32_t> gV, gF, grid_of(mesh ? n_obj : 0, -1);
+  if (mesh) {
+    CU(cudaSetDevice(s->device));
+    s->mesh_n = 0;
+    s->mesh_v.clear(); s->mesh_f.clear();
+    const size_t grid_bytes = 4 * (size_t)n_cand * R;
+    if (s->d_mgrid.cap < grid_bytes || s->d_grid_pts.cap < 12 * (size_t)R) CU(cudaStreamSynchronize(s->stream));
+    if (s->d_mgrid.reserve(grid_bytes) || s->d_grid_pts.reserve(12 * (size_t)R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
+    gV.assign(n_cand, 0); gF.assign(n_cand, 0);
+  }
   std::vector<DspgnObjectIn> ins;
-  std::vector<int32_t> cm, link;
+  std::vector<int32_t> cm, link, sel;
   std::vector<float> t_map;
   std::vector<DspgnObjectOut> res;
-  for (int o0 = 0; o0 < n_obj;) {
-    int o1 = o0, slots = 0;
-    while (o1 < n_obj && slots + 1 + (gated(o1) ? 1 : 0) <= kMaxObjScan) slots += 1 + (gated(o1++) ? 1 : 0);
-    const int n = o1 - o0;
+  int g0 = 0;                                          // grids of the chunks before this one
+  for (size_t u0 = 0; u0 < order.size();) {
+    size_t u1 = u0;
+    int slots = 0;
+    long long cands = 0;
+    while (u1 < order.size()) {
+      const int o = order[u1], m = paired(o) ? 2 : 1;
+      const int sl = m + (gated(o) ? 1 : 0), cd = m == 2 ? 2 : (candidate(o) ? 1 : 0);
+      if (slots + sl > kMaxObjScan || (cands + cd) * R > kMeshChunkRows) break;
+      slots += sl; cands += cd; u1 += m;
+    }
+    const int n = (int)(u1 - u0);
     s->gdev = GatherDev{};
-    if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
-      if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
-      if (int rc = run_batch_impl(s, modes + o0)) return rc;
-      if (int rc = dspgn_results(s, out + o0)) return rc;
-      o0 = o1;
-      continue;
-    }
-    ins.assign(in + o0, in + o1);
-    cm.assign(modes + o0, modes + o1);
+    ins.clear(); cm.clear();
+    for (int k = 0; k < n; ++k) { ins.push_back(in[order[u0 + k]]); cm.push_back(modes[order[u0 + k]]); }
     link.assign(n, -1);
-    t_map.assign(16 * (size_t)slots, 0.f);
-    for (int k = 0; k < n; ++k) {
-      if (!gated(o0 + k)) continue;
-      const DspgnGateIn& g = gates[o0 + k];
-      DspgnObjectIn J = in[o0 + k];                    // the detection as reconstruct_object(Sim3Tco, pts, rays, depth) sees it
-      J.t_cam_obj = g.t_cam_obj_sim3; J.t_rs = g.sim3_rs; J.t_cs = g.sim3_cs;
-      J.code = nullptr;
-      link[k] = (int)ins.size();
-      link.push_back(k);
-      ins.push_back(J);
-      cm.push_back(DSPGN_MODE_JOINT);
-      for (int r = 0; r < 4; ++r)
-        for (int c = 0; c < 4; ++c) t_map[16 * (size_t)k + 4 * r + c] = g.t_cam_obj_map[(size_t)r * g.map_rs + (size_t)c * g.map_cs];
+    if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
+      if (int rc = dspgn_upload_batch(s, n, ins.data())) return rc;
+      if (int rc = run_batch_impl(s, cm.data())) return rc;
+    } else {
+      t_map.assign(16 * (size_t)slots, 0.f);
+      for (int k = 0; k < n; ++k) {
+        const int o = order[u0 + k];
+        if (!gated(o)) continue;
+        const DspgnGateIn& g = gates[o];
+        DspgnObjectIn J = in[o];                       // the detection as reconstruct_object(Sim3Tco, pts, rays, depth) sees it
+        J.t_cam_obj = g.t_cam_obj_sim3; J.t_rs = g.sim3_rs; J.t_cs = g.sim3_cs;
+        J.code = nullptr;
+        link[k] = (int)ins.size();
+        link.push_back(k);
+        ins.push_back(J);
+        cm.push_back(DSPGN_MODE_JOINT);
+        for (int r = 0; r < 4; ++r)
+          for (int c = 0; c < 4; ++c) t_map[16 * (size_t)k + 4 * r + c] = g.t_cam_obj_map[(size_t)r * g.map_rs + (size_t)c * g.map_cs];
+      }
+      if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
+      if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data())) return rc;
     }
-    if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
-    if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data())) return rc;
     const bool mega = s->mega_ran;
+    int gc = 0;                                        // grids of this chunk
+    if (mesh) {
+      // per slot: its grid in the chunk's block (-1: not a candidate) | the slot of the other hypothesis of its pair
+      sel.assign(2 * (size_t)slots, -1);
+      for (int k = 0; k < n; ++k) {
+        const int o = order[u0 + k];
+        if (!candidate(o)) continue;
+        sel[cm[k] == DSPGN_MODE_JOINT ? k : link[k]] = gc;
+        grid_of[o] = g0 + gc++;
+        if (paired(o)) sel[(size_t)slots + k] = pair[o] > o ? k + 1 : k - 1;
+      }
+      if (s->d_mesh_sel.cap < 4 * sel.size()) CU(cudaStreamSynchronize(s->stream));
+      if (s->d_mesh_sel.reserve(4 * sel.size())) return fail(DSPGN_E_ALLOC, "cudaMalloc");
+      int* d_sel = s->d_mesh_sel.as<int>();
+      CU(cudaMemcpyAsync(d_sel, sel.data(), 4 * sel.size(), cudaMemcpyHostToDevice, s->stream));
+      if (u0 == 0) {                                   // the call-wide query grid of create_voxel_grid
+        k_mesh_grid_points<<<(unsigned)((R + 255) / 256), 256, 0, s->stream>>>(s->d_grid_pts.as<float>(), 1, dim);
+        s->ctr.kernel_launches++;
+      }
+      BatchDev b = batch_dev(s);
+      k_mesh_select<<<slots, 128, 0, s->stream>>>(b, d_sel, d_sel + slots);
+      s->ctr.kernel_launches++;
+      CU(cudaGetLastError());
+      if (gc > 0) {
+        // grids of the candidates that get no mesh stay NaN: no cube of theirs is on the surface
+        b.sdf = s->d_mgrid.as<float>() + (size_t)g0 * R;
+        CU(cudaMemsetAsync(b.sdf, 0xff, 4 * (size_t)gc * R, s->stream));
+        TermArgs a = base_term(s, MODE_GRIDFWD);
+        a.grid = s->d_grid_pts.as<float>(); a.grid_slot = d_sel; a.grid_rows = (int)R;
+        if (int rc = launch_term(s, b, a, (long long)gc * R)) return rc;
+      }
+    }
     res.resize(slots);
     if (int rc = dspgn_results(s, res.data())) return rc;
+    int done = 0;
     for (int k = 0; k < n; ++k) {
-      DspgnObjectOut& r = out[o0 + k];
+      DspgnObjectOut& r = out[order[u0 + k]];
       r = res[k];
       if (link[k] >= 0 && res[k].gate == DSPGN_GATE_REJECTED) {
         r = res[link[k]];
         r.gate = DSPGN_GATE_REJECTED;
         if (mega) s->ctr.rows_fwd_bwd += (long long)s->h_meta[link[k]].n_pts * s->cfg.num_iterations;   // the woken slot's SDF rows
       }
+      done += r.mesh == DSPGN_MESH_DONE ? 1 : 0;
     }
-    o0 = o1;
+    if (gc > 0) {
+      s->ctr.rows_fwd_only += (long long)done * R;
+      const MeshGrid g{s->d_mgrid.as<float>() + (size_t)g0 * R, gc, dim, R, (long long)(dim - 1) * (dim - 1) * (dim - 1), 2.0 / (dim - 1)};
+      if (int rc = mesh_chunk(s, g, gV.data() + g0, gF.data() + g0)) return rc;
+    }
+    g0 += gc;
+    u0 = u1;
   }
+  if (!mesh) return 0;
+  // the meshes came out in walk order: put them in object order (they differ only where a pair is not adjacent)
+  bool in_order = true;
+  for (int o = 0, last = -1; o < n_obj; ++o)
+    if (grid_of[o] >= 0) { in_order = in_order && grid_of[o] > last; last = grid_of[o]; }
+  if (!in_order) {
+    std::vector<size_t> ov(n_cand + 1, 0), of(n_cand + 1, 0);
+    for (int g = 0; g < n_cand; ++g) { ov[g + 1] = ov[g] + 3 * (size_t)gV[g]; of[g + 1] = of[g] + 3 * (size_t)gF[g]; }
+    std::vector<float> v; std::vector<int32_t> f;
+    v.reserve(s->mesh_v.size()); f.reserve(s->mesh_f.size());
+    for (int o = 0; o < n_obj; ++o) {
+      const int g = grid_of[o];
+      if (g < 0) continue;
+      v.insert(v.end(), s->mesh_v.begin() + ov[g], s->mesh_v.begin() + ov[g + 1]);
+      f.insert(f.end(), s->mesh_f.begin() + of[g], s->mesh_f.begin() + of[g + 1]);
+    }
+    s->mesh_v.swap(v); s->mesh_f.swap(f);
+  }
+  for (int o = 0; o < n_obj; ++o) {
+    n_vertices[o] = grid_of[o] >= 0 ? gV[grid_of[o]] : 0;
+    n_faces[o] = grid_of[o] >= 0 ? gF[grid_of[o]] : 0;
+  }
+  s->mesh_n = n_obj; s->mesh_dim = dim;
+  s->mesh_grid_of.swap(grid_of);
   return 0;
+}
+
+}  // namespace
+
+int dspgn_keyframe_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, DspgnObjectOut* out) {
+  return dspgn_keyframe_batch_gated(s, n_obj, in, modes, nullptr, out);
+}
+
+int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
+                               const DspgnGateIn* gates, DspgnObjectOut* out) {
+  if (!modes) return fail(DSPGN_E_ARG, "bad argument");
+  return keyframe_impl(s, n_obj, in, modes, gates, nullptr, out, nullptr, nullptr);
+}
+
+int dspgn_keyframe_batch_meshed(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
+                                const DspgnGateIn* gates, const DspgnMeshSpec* mesh, DspgnObjectOut* out,
+                                int32_t* n_vertices, int32_t* n_faces) {
+  if (!mesh || !n_vertices || !n_faces) return fail(DSPGN_E_ARG, "bad argument");
+  std::vector<int32_t> joint;
+  if (!modes && n_obj > 0) {
+    joint.assign(n_obj, DSPGN_MODE_JOINT);
+    modes = joint.data();
+  }
+  return keyframe_impl(s, n_obj, in, modes, gates, mesh, out, n_vertices, n_faces);
 }
 
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n, int x_rs, int x_cs,
@@ -1333,7 +1466,7 @@ int mesh_impl(DspgnSolver* s, int n, int dim, const float* codes, int code_strid
   const long long R = (long long)dim * dim * dim, C = (long long)(dim - 1) * (dim - 1) * (dim - 1);
   const int per_chunk = (int)std::max<long long>(1, std::min<long long>(kMaxObjScan, kMeshChunkRows / R));
   s->mesh_n = 0;
-  s->mesh_v.clear(); s->mesh_f.clear();
+  s->mesh_v.clear(); s->mesh_f.clear(); s->mesh_grid_of.clear();
   if (s->d_mgrid.cap < 4 * (size_t)n * R) CU(cudaStreamSynchronize(s->stream));
   if (s->d_mgrid.reserve(4 * (size_t)n * R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
   s->ctr = DspgnCounters{};
@@ -1402,7 +1535,15 @@ int dspgn_mesh_results(DspgnSolver* s, float* vertices, int32_t* faces, float* s
   if (sdf) {
     CU(cudaSetDevice(s->device));
     const size_t R = (size_t)s->mesh_dim * s->mesh_dim * s->mesh_dim;
-    CU(cudaMemcpyAsync(sdf, s->d_mgrid.p, 4 * (size_t)s->mesh_n * R, cudaMemcpyDeviceToHost, s->stream));
+    if (s->mesh_grid_of.empty()) {
+      CU(cudaMemcpyAsync(sdf, s->d_mgrid.p, 4 * (size_t)s->mesh_n * R, cudaMemcpyDeviceToHost, s->stream));
+    } else {
+      for (int o = 0; o < s->mesh_n; ++o) {
+        const int g = s->mesh_grid_of[o];
+        if (g >= 0) CU(cudaMemcpyAsync(sdf + (size_t)o * R, s->d_mgrid.as<float>() + (size_t)g * R, 4 * R, cudaMemcpyDeviceToHost, s->stream));
+        else memset(sdf + (size_t)o * R, 0xff, 4 * R);     // no grid: NaN, the bit pattern of the device's unmeshed grids
+      }
+    }
     CU(cudaStreamSynchronize(s->stream));
   }
   return 0;

@@ -34,7 +34,16 @@ struct DecoderDev {
   TcPlan tc_plan;
 };
 
-enum { MODE_SDF = 0, MODE_BAND = 1, MODE_RAYFWD = 2, MODE_PTSFWD = 3 };
+// MODE_GRIDFWD (per-launch kernels only): forward-only decode of the call-wide mesh query grid (TermArgs.grid, no pose
+// transform) with each object's final code, for the objects whose record's mesh word is DSPGN_MESH_DONE; the sdf of grid
+// row r of object o goes to b.sdf[grid_slot[o] * grid_rows + r]
+enum { MODE_SDF = 0, MODE_BAND = 1, MODE_RAYFWD = 2, MODE_PTSFWD = 3, MODE_GRIDFWD = 4 };
+
+// the record word that carries DSPGN_MESH_* (DspgnObjectOut.mesh)
+constexpr int kRecMeshWord = 86;
+__device__ __forceinline__ int record_mesh(const float* results, int o) {
+  return reinterpret_cast<const int*>(results + (size_t)o * DSPGN_RESULT_FLOATS)[kRecMeshWord];
+}
 
 // The resident batch and its run, as every kernel of the run sees it (one by-value kernel parameter; the persistent
 // kernel keeps a copy in shared memory for its out-of-line solve step).
@@ -81,6 +90,8 @@ struct TermArgs {
   float* ln_scratch;         // SIMT engine, LayerNorm decoders: per-CTA [layer][256][kTP] normalised activations
   // debug dump of Jacobian rows (external order [pose | code]) for one object
   float* dbg_J; float* dbg_res; int dbg_obj; int dbg_P;
+  // MODE_GRIDFWD: query points [grid_rows][3], grid slot of each object (-1: none)
+  const float* grid; const int* grid_slot; int grid_rows;
 };
 
 // Device work queue of the persistent object-pipelined kernel (dspgn_tc.cuh).
@@ -151,6 +162,7 @@ struct MegaArgs {
 // ---------------------------------------------------------------------------------------------
 // tile scheduling shared by all decoder kernels: rows per object -> tiles, scanned per CTA
 __device__ __forceinline__ int term_rows(const BatchDev& b, const TermArgs& a, int o) {
+  if (a.mode == MODE_GRIDFWD) return (record_mesh(b.results, o) == DSPGN_MESH_DONE) ? a.grid_rows : 0;
   const ObjState& st = b.state[o];
   if (st.status != 0 || a.iter >= st.n_iter) return 0;
   if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) return b.meta[o].n_pts;
@@ -326,6 +338,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
           const float* q = b.pts + 3 * (size_t)(M.pts_off + r);
           xform_point(st.T_oc, q[0], q[1], q[2], x, y, z);
           sc = (mask_in == nullptr || mask_in[M.pts_off + r]) ? 1.f : 0.f;
+        } else if (a.mode == MODE_GRIDFWD) {
+          const float* q = a.grid + 3 * (size_t)r;
+          x = q[0]; y = q[1]; z = q[2]; sc = 1.f;
         } else if (a.mode == MODE_BAND) {
           const size_t s = (size_t)M.smp_off + r;
           x = b.band_x[3 * s]; y = b.band_x[3 * s + 1]; z = b.band_x[3 * s + 2];
@@ -461,11 +476,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       }
       __syncthreads();
     }
-    if (a.mode == MODE_RAYFWD || a.mode == MODE_PTSFWD) {
+    if (a.mode == MODE_RAYFWD || a.mode == MODE_PTSFWD || a.mode == MODE_GRIDFWD) {
       int cnt = 0;
       if (tid < nrows) {
         const bool valid = S.rscale[tid] != 0.f;
-        const size_t base = (a.mode == MODE_RAYFWD) ? (size_t)M.smp_off : (size_t)M.pts_off;
+        const size_t base = (a.mode == MODE_RAYFWD) ? (size_t)M.smp_off
+                            : (a.mode == MODE_GRIDFWD ? (size_t)a.grid_slot[o] * a.grid_rows : (size_t)M.pts_off);
         b.sdf[base + row0 + tid] = valid ? S.yv[tid] : INFINITY;
         cnt = valid ? 1 : 0;
       }

@@ -782,6 +782,36 @@ __global__ void k_gate_wake(BatchDev b, int n_iter_joint) {
   b.state[o].n_iter = wake ? n_iter_joint : 0;
 }
 
+// dspgn_keyframe_batch_meshed, after the run's last iteration (both schedules): which objects get a mesh.  One CTA per
+// object.  grid_slot[o] >= 0 marks a candidate (a joint object, including the joint slot of a gated object); pair[o] is the
+// other hypothesis of a mono pair (-1: none).  Writes the record's mesh word, and for a DSPGN_MESH_DONE object the layer-0
+// bias folded from its final code (the solve does not refresh zb0 after the last iteration) for the MODE_GRIDFWD decode.
+__global__ void k_mesh_select(BatchDev b, const int* grid_slot, const int* pair) {
+  const int o = blockIdx.x, tid = threadIdx.x;
+  __shared__ int s_word;
+  if (tid == 0) {
+    const int* rec = reinterpret_cast<const int*>(b.results);
+    const float* recf = b.results;
+    const size_t RF = DSPGN_RESULT_FLOATS;
+    int word = DSPGN_MESH_OFF;
+    const int lk = (b.link != nullptr) ? b.link[o] : -1;
+    // the joint slot of a gated object is a candidate only when the device rejected its pose-only record
+    const bool woken = lk < 0 || rec[(size_t)lk * RF + 85] == DSPGN_GATE_REJECTED;
+    if (grid_slot[o] >= 0 && woken) {
+      const int p = pair[o];
+      // the pair rule of ProcessDetectedObjects (src/LocalMapping_util.cc:403-407): hypothesis j > i wins iff
+      // loss[i] > loss[j]; a tie keeps i
+      const bool lost = p >= 0 && (p > o ? recf[(size_t)o * RF + 80] > recf[(size_t)p * RF + 80]
+                                         : !(recf[(size_t)p * RF + 80] > recf[(size_t)o * RF + 80]));
+      word = lost ? DSPGN_MESH_LOST : (rec[(size_t)o * RF + 81] != DSPGN_ST_OK ? DSPGN_MESH_FAILED : DSPGN_MESH_DONE);
+    }
+    reinterpret_cast<int*>(b.results + (size_t)o * RF)[kRecMeshWord] = word;
+    s_word = word;
+  }
+  __syncthreads();
+  if (s_word == DSPGN_MESH_DONE) refresh_zb0(b.state[o], b.decs[b.meta[o].class_id], tid, blockDim.x);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Render term, per-ray part (loss.py:84-141).  One CTA per object, one warp per ray, two passes:
 // pass 1 counts the band samples each ray keeps, a block scan turns counts into row offsets, pass 2

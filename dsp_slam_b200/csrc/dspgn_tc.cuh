@@ -492,7 +492,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         const int cls = b.meta[o].class_id;
         const TcPlan& plan = S.plans[cls];
         const unsigned char* blob = b.decs[cls].tc_blob;
-        const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD);
+        const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD || (!MEGA && tr.mode == MODE_GRIDFWD));
         const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
         for (int s = 0; s < ns; ++s)
           produce_step(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full,
@@ -559,7 +559,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       const TcPlan& plan = S.plans[M.class_id];
       const int L = dec.L, in0 = dec.in0, n_lin = dec.n_lin;
       const bool has_skip = dec.latent_in >= 0;
-      const bool fwd_only = (mode == MODE_RAYFWD || mode == MODE_PTSFWD);
+      const bool grid_mode = !MEGA && mode == MODE_GRIDFWD;
+      const bool fwd_only = (mode == MODE_RAYFWD || mode == MODE_PTSFWD || grid_mode);
       const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
       const float huber_b = term_huber(a, mode, ost.mode, (RENDER && mode == MODE_BAND) ? a.huber_b1 : a.huber_b);
       float* const part = (RENDER && mode == MODE_BAND) ? a.part_r : a.part;
@@ -569,7 +570,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       // for the same two L2 lines -- and on few-object batches every SM asks for them at the same moment.
       if (tid < 12) S.ost[tid] = ldv(&ost.T_oc[tid]);
       else if (tid < 16) S.ost[tid] = ldv(&ost.dmin + (tid - 12));          // dmin, dmax, dstep, dfar
-      const bool pts_mode = (mode == MODE_SDF || mode == MODE_PTSFWD);
+      const bool pts_mode = (mode == MODE_SDF || mode == MODE_PTSFWD || grid_mode);
       if (MEGA && !pts_mode && tid == 16) S.ost_rows = mega_rows(b, q, M, o, mode);   // band / ray-sample rows: a counter
 
       // per-class constants in smem (bias, last row, xyz rows of layer 0), the tile's latent code
@@ -610,9 +611,9 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       if (pts_mode) {
         nrows = min(kTcRows, (MEGA ? M.n_pts : term_rows(b, a, o)) - row0);
         if (r < nrows) {
-          const float* pq = b.pts + 3 * (size_t)(M.pts_off + row0 + r);
+          const float* pq = grid_mode ? a.grid + 3 * (size_t)(row0 + r) : b.pts + 3 * (size_t)(M.pts_off + row0 + r);
           p0 = pq[0]; p1 = pq[1]; p2 = pq[2];
-          sc = (mask_in == nullptr || ldv(mask_in + M.pts_off + row0 + r)) ? 1.f : 0.f;
+          sc = (grid_mode || mask_in == nullptr || ldv(mask_in + M.pts_off + row0 + r)) ? 1.f : 0.f;
         }
       }
       epi_bar_sync();      // (per-iteration schedule: Jp / rr of the previous tile are not written before the barrier further down;
@@ -625,7 +626,9 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       float x0 = 0.f, x1 = 0.f, x2 = 0.f, res_in = 0.f;
       if (r < nrows) {
         const int rr_ = row0 + r;
-        if (pts_mode) {
+        if (grid_mode) {
+          x0 = p0; x1 = p1; x2 = p2;
+        } else if (pts_mode) {
           xform_point(Toc, p0, p1, p2, x0, x1, x2);
         } else if (mode == MODE_BAND) {
           // band rows were written by the CTAs that ran this object's scan: L2 is the point of coherence
@@ -732,7 +735,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           yv = S.yrow[r];
           if (fwd_only) {
             if (grp == 0 && r < nrows) {
-              const size_t base = (mode == MODE_RAYFWD) ? (size_t)M.smp_off : (size_t)M.pts_off;
+              const size_t base = (mode == MODE_RAYFWD) ? (size_t)M.smp_off
+                                  : (grid_mode ? (size_t)a.grid_slot[o] * a.grid_rows : (size_t)M.pts_off);
               b.sdf[base + row0 + r] = (sc != 0.f) ? yv : INFINITY;
             }
             if (!RENDER && mode == MODE_RAYFWD) {        // (persistent kernel: counted by the scan items, dspgn_solve.cuh)

@@ -256,22 +256,31 @@ class BatchSolver:
         self.n_obj = len(objs)
         return out
 
-    def keyframe(self, objs, modes, gates=None):
+    def keyframe(self, objs, modes, gates=None, voxels_dim=None, pairs=None, want_sdf=False):
         """Joint and pose-only objects in one call: modes[i] = _lib.MODE_JOINT (reconstruct) or MODE_POSE (estimate_pose).
         gates: None, or one entry per object: None (not gated) or dict(t_cam_obj_map, t_cam_obj_sim3) for a pose-only
         object checked against the map's prediction (dspgn_keyframe_batch_gated); the record's `gate` word tells
-        _lib.GATE_KEPT (pose-only record) from _lib.GATE_REJECTED (the joint record of the detection from t_cam_obj_sim3)."""
+        _lib.GATE_KEPT (pose-only record) from _lib.GATE_REJECTED (the joint record of the detection from t_cam_obj_sim3).
+
+        voxels_dim: also mesh every object the call creates (dspgn_keyframe_batch_meshed) and return (records, meshes),
+        meshes[i] = (vertices (V,3) f32, faces (F,3) int32) where the record's `mesh` word is _lib.MESH_DONE, else None;
+        with want_sdf also the (n, dim, dim, dim) grids (NaN where there is none).  pairs (with voxels_dim): one entry
+        per object, pairs[i] = j and pairs[j] = i for the two hypotheses i < j of a mono detection, -1 otherwise."""
         m = _modes_array(modes)
-        if len(m) != len(objs):
-            raise ValueError(f"{len(m)} modes for {len(objs)} objects")
+        n = len(objs)
+        if len(m) != n:
+            raise ValueError(f"{len(m)} modes for {n} objects")
+        if gates is not None and len(gates) != n:
+            raise ValueError(f"{len(gates)} gates for {n} objects")
+        if voxels_dim is None and pairs is not None:
+            raise ValueError("pairs only apply to a meshed call (voxels_dim)")
+        if pairs is not None and len(pairs) != n:
+            raise ValueError(f"{len(pairs)} pairs for {n} objects")
         arr, keep = self._pack(objs)
-        out = (_lib.ObjectOut * len(objs))()
-        if gates is None:
-            _lib.check(_lib.load().dspgn_keyframe_batch(self.handle, len(objs), arr, m, out))
-        else:
-            if len(gates) != len(objs):
-                raise ValueError(f"{len(gates)} gates for {len(objs)} objects")
-            g = (_lib.GateIn * len(objs))()
+        out = (_lib.ObjectOut * n)()
+        g = None
+        if gates is not None:
+            g = (_lib.GateIn * n)()
             for i, d in enumerate(gates):
                 if d is None:
                     continue
@@ -281,8 +290,24 @@ class BatchSolver:
                 g[i].t_cam_obj_map = Tm.ctypes.data_as(_FP); g[i].map_rs = 4; g[i].map_cs = 1
                 g[i].t_cam_obj_sim3 = Ts.ctypes.data_as(_FP); g[i].sim3_rs = 4; g[i].sim3_cs = 1
                 g[i].gate = 1
-            _lib.check(_lib.load().dspgn_keyframe_batch_gated(self.handle, len(objs), arr, m, g, out))
-        self.n_obj = len(objs)
+        lib = _lib.load()
+        if voxels_dim is not None:
+            spec = _lib.MeshSpec()
+            spec.voxels_dim = int(voxels_dim)
+            pr = None if pairs is None else (C.c_int32 * n)(*[-1 if p is None else int(p) for p in pairs])
+            spec.pair = pr
+            nv, nf = (C.c_int32 * n)(), (C.c_int32 * n)()
+            _lib.check(lib.dspgn_keyframe_batch_meshed(self.handle, n, arr, m, g, C.byref(spec), out, nv, nf))
+            self.n_obj = n
+            res = self._mesh_results(n, int(voxels_dim), nv, nf, want_sdf)
+            meshes, sdf = res if want_sdf else (res, None)
+            meshes = [mm if out[i].mesh == _lib.MESH_DONE else None for i, mm in enumerate(meshes)]
+            return (out, meshes, sdf) if want_sdf else (out, meshes)
+        if g is None:
+            _lib.check(lib.dspgn_keyframe_batch(self.handle, n, arr, m, out))
+        else:
+            _lib.check(lib.dspgn_keyframe_batch_gated(self.handle, n, arr, m, g, out))
+        self.n_obj = n
         return out
 
     def decode_sdf(self, code, x, class_id=0):
@@ -359,6 +384,14 @@ class BatchSolver:
 
 def _modes_array(modes):
     return (C.c_int32 * len(modes))(*[int(m) for m in modes])
+
+
+def _with_meshes(results, meshes):
+    """Attach each mesh (vertices, faces) to its ResultDict (objects without a mesh get no keys)."""
+    for r, m in zip(results, meshes):
+        if m is not None:
+            r.vertices, r.faces = m
+    return results
 
 
 def _records(out, n):
@@ -457,18 +490,58 @@ class Optimizer(object):
             return T0
 
     # -- batched extension ----------------------------------------------------------------------
-    def reconstruct_batch(self, objs, strict=True):
+    def reconstruct_batch(self, objs, strict=True, voxels_dim=None):
         """objs: list of dicts(t_cam_obj, pts, rays, depth, [code], [class_id]) -> list of ResultDict.
         Any number of objects (the library walks resident batches of 1024).  Per-object problems are
-        per-object soft failures; strict=False additionally turns call-level errors into all-failed results."""
+        per-object soft failures; strict=False additionally turns call-level errors into all-failed results.
+        voxels_dim: the same call also meshes every good result (CreateNewMapObjects, src/LocalMapping_util.cc:179-196):
+        its ResultDict carries vertices (V,3) f32 and faces (F,3) int32 exactly as MeshExtractor(voxels_dim)
+        .extract_meshes returns them for its code."""
         try:
-            out = self.solver.reconstruct(objs)
-            return _unpack_all(out, len(objs), self.code_len)
+            if voxels_dim is None:
+                out = self.solver.reconstruct(objs)
+                return _unpack_all(out, len(objs), self.code_len)
+            if not objs:
+                return []
+            out, meshes = self.solver.keyframe(objs, [_lib.MODE_JOINT] * len(objs), voxels_dim=voxels_dim)
+            return _with_meshes(_unpack_all(out, len(objs), self.code_len), meshes)
         except Exception as e:            # noqa: BLE001
             if strict:
                 raise
             _warn_once(("reconstruct_batch", type(e).__name__), f"reconstruct_batch failed softly: {e!r}")
             return [self._failed() for _ in objs]
+
+    def reconstruct_mono_batch(self, objs, voxels_dim=None):
+        """The mono path's reconstruction of ProcessDetectedObjects (src/LocalMapping_util.cc:390-428) for a list of
+        dicts(t_cam_obj, pts, rays, depth, [code], [class_id], [t_cam_obj_flipped]) in one call.  A dict with
+        t_cam_obj_flipped (the map pose turned 180 degrees about y) runs both hypotheses and keeps the flipped one iff
+        loss(map pose) > loss(flipped).  Returns one ResultDict per dict: the kept result plus `flipped` (bool); with
+        voxels_dim the kept good result also carries vertices and faces, decided and meshed on the device."""
+        run, pairs, first = [], [], []
+        for o in objs:
+            first.append(len(run))
+            run.append(o)
+            pairs.append(-1)
+            if o.get("t_cam_obj_flipped") is not None:
+                i = len(run) - 1
+                run.append(dict(o, t_cam_obj=o["t_cam_obj_flipped"]))
+                pairs[i] = i + 1
+                pairs.append(i)
+        if not run:
+            return []
+        if voxels_dim is None:
+            res = _unpack_all(self.solver.reconstruct(run), len(run), self.code_len)
+        else:
+            out, meshes = self.solver.keyframe(run, [_lib.MODE_JOINT] * len(run), voxels_dim=voxels_dim, pairs=pairs)
+            res = _with_meshes(_unpack_all(out, len(run), self.code_len), meshes)
+        kept = []
+        for i in first:
+            j = pairs[i]
+            flip = j >= 0 and res[i].loss > res[j].loss        # LocalMapping_util.cc:403-407 (a tie keeps the map pose)
+            r = res[j] if flip else res[i]
+            r.flipped = bool(flip)
+            kept.append(r)
+        return kept
 
     def estimate_pose_batch(self, objs, return_status=False):
         """Batched estimate_pose_cam_obj.  Failed objects keep their input pose; return_status=True also returns
@@ -482,7 +555,7 @@ class Optimizer(object):
                       else np.array(o["t_cam_obj"], dtype=np.float32).reshape(4, 4))
         return (Ts, st) if return_status else Ts
 
-    def keyframe_batch(self, new_objects, tracked_objects, return_status=False):
+    def keyframe_batch(self, new_objects, tracked_objects, return_status=False, voxels_dim=None):
         """The stereo keyframe's two passes (src/LocalMapping.cc:88-95) as ONE library call: reconstruct_batch(new_objects)
         (CreateNewMapObjects) and estimate_pose_batch(tracked_objects) (GetNewObservations; dicts with t_cam_obj, pts,
         code, scale).  Returns (results, poses) or (results, poses, status) with exactly the values of those two calls:
@@ -493,7 +566,10 @@ class Optimizer(object):
         observations (src/LocalMapping_util.cc:104-147) runs on the device, and a detection that fails it is
         reconstructed in the same call like CreateNewMapObjects does (:179).  Then the call returns one more list,
         `rejected`: per tracked object None, or the reconstruct_object-shaped result of the rejected detection (whose
-        pose and status entries are None)."""
+        pose and status entries are None).
+
+        voxels_dim: the same call also meshes every good new object and every good rejected detection: their
+        ResultDicts carry vertices (V,3) f32 and faces (F,3) int32 (dspgn_keyframe_batch_meshed)."""
         objs = list(new_objects) + list(tracked_objects)
         n_new = len(new_objects)
         gate_keys = ("t_cam_obj_map", "t_cam_obj_sim3", "rays", "depth")
@@ -502,16 +578,23 @@ class Optimizer(object):
         gated = any(g is not None for g in gates)
         if not objs:
             return ([], [], []) if return_status else ([], [])
-        out = self.solver.keyframe(objs, [_lib.MODE_JOINT] * n_new + [_lib.MODE_POSE] * (len(objs) - n_new),
-                                   [None] * n_new + gates if gated else None)
+        modes = [_lib.MODE_JOINT] * n_new + [_lib.MODE_POSE] * (len(objs) - n_new)
+        meshes = None
+        if voxels_dim is None:
+            out = self.solver.keyframe(objs, modes, [None] * n_new + gates if gated else None)
+        else:
+            out, meshes = self.solver.keyframe(objs, modes, [None] * n_new + gates if gated else None, voxels_dim=voxels_dim)
         results = _unpack_all(out, n_new, self.code_len) if n_new else []
+        if meshes is not None:
+            results = _with_meshes(results, meshes[:n_new])
         Ts, st, rejected = [], [], []
         for i, o in enumerate(tracked_objects):
             rec = out[n_new + i]
             if rec.gate == _lib.GATE_REJECTED:
                 from .distributed import records_to_results
                 raw = np.frombuffer(rec, dtype=np.float32, count=_lib.RESULT_FLOATS).reshape(1, -1)
-                rejected.append(records_to_results(raw, self.code_len)[0])
+                r = records_to_results(raw, self.code_len)[0]
+                rejected.append(r if meshes is None else _with_meshes([r], [meshes[n_new + i]])[0])
                 Ts.append(None)
                 st.append(None)
                 continue

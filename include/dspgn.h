@@ -17,6 +17,8 @@
  *   one stereo keyframe's two passes (LocalMapping.cc:88-95)     dspgn_keyframe_batch
  *   ... with GetNewObservations' map check (LocalMapping_util.cc:104-147) and the demoted detections'
  *       reconstruction in CreateNewMapObjects (:179)             dspgn_keyframe_batch_gated
+ *   ... and the meshes of every object it creates (:179-196), incl. the mono path's map-pose / flipped pair
+ *       (ProcessDetectedObjects, :390-428)                       dspgn_keyframe_batch_meshed + dspgn_mesh_results
  *   loss_utils.decode_sdf        (reconstruct/loss_utils.py:51) dspgn_decode_sdf
  *   MeshExtractor.extract_mesh_from_code (optimizer.py:214)     dspgn_mesh_batch + dspgn_mesh_results
  *   loss.compute_sdf_loss / compute_render_loss (loss.py:22,46) dspgn_debug_system (test hook)
@@ -140,7 +142,13 @@ typedef struct {
   int32_t n_band;                 /* m: band rows kept, last iteration */
   int32_t iters_done;
   int32_t gate;                   /* dspgn_keyframe_batch_gated: DSPGN_GATE_*; 0 everywhere else */
-  int32_t pad_[2];
+  union {
+    int32_t pad_[2];
+    struct {
+      int32_t mesh;               /* dspgn_keyframe_batch_meshed: DSPGN_MESH_*; 0 everywhere else */
+      int32_t reserved_;
+    };
+  };
 } DspgnObjectOut;                 /* 88 floats */
 
 /* device-side result record (same layout), for callers that keep results on the GPU */
@@ -214,6 +222,32 @@ typedef struct {
 } DspgnGateIn;
 int dspgn_keyframe_batch_gated(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
                                const DspgnGateIn* gates /* n_obj entries, or NULL */, DspgnObjectOut* out);
+
+/* The gated keyframe call that also meshes every object it creates, as CreateNewMapObjects (:179-196) and
+ * ProcessDetectedObjects (:390-428) store them: pose, code and mesh from one call.  The records are bit-identical to
+ * dspgn_keyframe_batch_gated's with the same arguments, except for out.mesh.  Candidates are the joint objects and the
+ * gated objects the device rejects (the mesh of a rejected detection goes to the gated object's index).  A pair
+ * (pair[i] = j, pair[j] = i, i < j, both joint) is the mono path's two hypotheses, map pose i and flipped pose j: j wins
+ * iff loss[i] > loss[j], whatever the statuses; the loser is DSPGN_MESH_LOST.  A candidate (or a pair's winner) whose
+ * status is not DSPGN_ST_OK is DSPGN_MESH_FAILED.  The decision and the grid decode run on the device after the last
+ * GN iteration, in the run's own resident batch; every DSPGN_MESH_DONE mesh is bit-identical to dspgn_mesh_batch of
+ * the record's code and class_id at the same voxels_dim on the same engine.  dspgn_mesh_results then returns the meshes
+ * object after object over all n_obj objects (0 vertices / faces without a mesh) and n_obj x dim^3 grids (NaN for
+ * objects without one).  modes = NULL: every object joint.  A bad voxels_dim, a pair on a pose-only or gated object, or
+ * a pair array that is not symmetric, pairs an object with itself or points out of range returns DSPGN_E_ARG before
+ * anything is enqueued.  Counters: rows_fwd_only += dim^3 per meshed object; the mesh launches are counted. */
+#define DSPGN_MESH_OFF 0      /* not a mesh candidate (pose-only record, kept gated object) */
+#define DSPGN_MESH_DONE 1     /* the object's mesh is in this call's dspgn_mesh_results */
+#define DSPGN_MESH_FAILED 2   /* candidate whose record has status != DSPGN_ST_OK: no mesh (CreateNewMapObjects skips it) */
+#define DSPGN_MESH_LOST 3     /* the other hypothesis of its pair has the lower loss: no mesh */
+typedef struct {
+  int32_t voxels_dim;         /* 2..128, as dspgn_mesh_batch */
+  const int32_t* pair;        /* n_obj entries or NULL: pair[i] = j and pair[j] = i make joint objects i < j the two
+                                 hypotheses of one mono detection (i = map pose, j = flipped); -1 = unpaired */
+} DspgnMeshSpec;
+int dspgn_keyframe_batch_meshed(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes /* or NULL */,
+                                const DspgnGateIn* gates /* or NULL */, const DspgnMeshSpec* mesh, DspgnObjectOut* out,
+                                int32_t* n_vertices, int32_t* n_faces /* n_obj entries each */);
 
 /* Forward-only decode (loss_utils.decode_sdf): x (n,3) host, strides in elements -> sdf (n,) host. */
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n,
