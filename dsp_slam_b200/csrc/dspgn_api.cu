@@ -150,9 +150,56 @@ struct DspgnSolver {
   std::vector<int32_t> mesh_f;
   std::vector<int32_t> mesh_grid_of; // meshed keyframe call: grid of each object in d_mgrid (-1: none); empty: grid o is object o's
   DevBuf d_mesh_sel;                 // meshed keyframe call, per chunk: grid slot | pair partner of each resident slot
+  HostBuf h_mesh_sel;                // ... its pinned staging (rewritten only after the chunk's results came back)
+  // a submitted keyframe call (dspgn_keyframe_submit .. dspgn_keyframe_wait)
+  struct Flight {
+    bool active = false;
+    bool mesh = false;               // a mesh spec was given
+    bool mega = false;               // the run used the persistent kernel
+    bool render = false;             // ... and the per-iteration schedule's woken slots run the render term
+    bool device_wake = false;        // the per-iteration schedule's second round was enqueued for every gated slot
+    int n_obj = 0, slots = 0, n = 0, dim = 0, n_cand = 0, gc = 0;
+    long long cap_v = 0, cap_f = 0;  // mesh arena (vertices | faces)
+    size_t o_ctr = 0, o_base = 0, o_arena = 0;   // h_flight: records | queue counters | mesh bases | arena
+    std::vector<int> order;          // walk order of the objects
+    std::vector<int32_t> link, grid_of;
+    MeshGrid g{};
+    uint8_t* mask = nullptr; int* vscan = nullptr; int* fscan = nullptr;   // the chunk's scans, kept for an overflow
+  } flight;
+  HostBuf h_flight;
+  cudaEvent_t ev_flight = nullptr;
+  double arena_v = 4.0, arena_f = 8.0;     // arena estimate: vertices / faces per object and per dim^2 (grows)
+  long long arena_force_v = 0, arena_force_f = 0;   // dspgn_debug_mesh_arena
+  long long host_syncs = 0;          // dspgn_debug_host_syncs
 };
 
 namespace {
+
+// Every wait of the calling thread on the device goes through these (dspgn_debug_host_syncs counts them).
+cudaError_t sync_stream(DspgnSolver* s) {
+  ++s->host_syncs;
+  return cudaStreamSynchronize(s->stream);
+}
+
+// Before a buffer the stream's earlier work may still read is freed or rewritten: waits only if that work is unfinished.
+cudaError_t settle_stream(DspgnSolver* s) {
+  const cudaError_t q = cudaStreamQuery(s->stream);
+  if (q != cudaErrorNotReady) return q;
+  return sync_stream(s);
+}
+
+cudaError_t settle_event(DspgnSolver* s, cudaEvent_t e) {
+  const cudaError_t q = cudaEventQuery(e);
+  if (q != cudaErrorNotReady) return q;
+  ++s->host_syncs;
+  return cudaEventSynchronize(e);
+}
+
+#define BUSY(s)                                                                                              \
+  do {                                                                                                       \
+    if ((s) && (s)->flight.active)                                                                           \
+      return fail(DSPGN_E_BUSY, "the solver has a submitted keyframe call that has not been collected (dspgn_keyframe_wait)"); \
+  } while (0)
 
 // what is concatenated at the input of layer k (latent_in_layer is shorthand for one kind-1 layer)
 int cat_kind_of(const DspgnDecoderSpec& s, int k) {
@@ -360,7 +407,8 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
 void dspgn_solver_destroy(DspgnSolver* s) {
   if (!s) return;
   cudaSetDevice(s->device);
-  cudaDeviceSynchronize();
+  cudaDeviceSynchronize();                 // also the work of a submitted call that was never collected
+  s->flight.active = false;
   dspgn_gather_close(s);
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
@@ -370,6 +418,9 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   s->h_mbase.release();
   s->h_results.release();
   s->h_run.release();
+  s->h_mesh_sel.release();
+  s->h_flight.release();
+  if (s->ev_flight) cudaEventDestroy(s->ev_flight);
   for (auto e : s->ev) cudaEventDestroy(e);
   for (auto e : s->ev_solve) cudaEventDestroy(e);
   if (s->ev_upload) cudaEventDestroy(s->ev_upload);
@@ -384,6 +435,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
 
 int dspgn_solver_set_stream(DspgnSolver* s, void* cuda_stream) {
   if (!s) return fail(DSPGN_E_ARG, "null solver");
+  BUSY(s);
   s->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
   return 0;
 }
@@ -393,14 +445,20 @@ int dspgn_solver_engine(const DspgnSolver* s) { return s ? s->engine : DSPGN_E_A
 int dspgn_solver_sync(DspgnSolver* s) {
   if (!s) return fail(DSPGN_E_ARG, "null solver");
   CU(cudaSetDevice(s->device));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   return 0;
 }
 
-int dspgn_enable_timing(DspgnSolver* s, int on) { if (!s) return fail(DSPGN_E_ARG, "null solver"); s->timing = on != 0; return 0; }
+int dspgn_enable_timing(DspgnSolver* s, int on) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  BUSY(s);
+  s->timing = on != 0;
+  return 0;
+}
 
 int dspgn_counters(DspgnSolver* s, DspgnCounters* out) {
   if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
+  BUSY(s);
   // device time of the last run's kernels, if they have finished (events on the solver's stream)
   float tot = 0.f;
   if (s->ev_run0 && s->ev_run1 && cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot;
@@ -454,8 +512,8 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
                o_depth = al(o_rays + 12 * (size_t)tr), o_tb = al(o_depth + 4 * (size_t)tf),
                o_aux = al(o_tb + 2 * 4 * (size_t)n_obj),
                total = al(o_aux + (any_build ? 4 * (size_t)kAuxFloats * n_obj : 0));
-  if (s->upload_pending) { CU(cudaEventSynchronize(s->ev_upload)); s->upload_pending = false; }
-  if (s->d_stage.cap < total) CU(cudaStreamSynchronize(s->stream));      // kernels of an earlier batch may still read the old block
+  if (s->upload_pending) { CU(settle_event(s, s->ev_upload)); s->upload_pending = false; }
+  if (s->d_stage.cap < total) CU(settle_stream(s));      // kernels of an earlier batch may still read the old block
   if (s->h_stage.reserve(total) || s->d_stage.reserve(total)) return fail(DSPGN_E_ALLOC, "staging allocation failed");
   unsigned char* hb = s->h_stage.as<unsigned char>();
   memcpy(hb + o_meta, s->h_meta.data(), sizeof(ObjMeta) * n_obj);
@@ -520,7 +578,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
     CU(cudaGetLastError());
   }
   if (grid_dim) {
-    if (s->d_grid_pts.cap < 12 * (size_t)tp) CU(cudaStreamSynchronize(s->stream));
+    if (s->d_grid_pts.cap < 12 * (size_t)tp) CU(settle_stream(s));
     if (s->d_grid_pts.reserve(12 * (size_t)tp)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
     const long long R = (long long)grid_dim * grid_dim * grid_dim;
     k_mesh_grid_points<<<dim3((unsigned)((R + 255) / 256), (unsigned)std::min(n_obj, 65535)), 256, 0, s->stream>>>(
@@ -570,6 +628,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
 }  // namespace
 
 int dspgn_upload_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in) {
+  BUSY(s);
   return upload_batch_impl(s, n_obj, in, false);
 }
 
@@ -669,12 +728,12 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
   p.iters[DSPGN_MODE_JOINT] = unlimited ? (1 << 30) : c.num_iterations;
   p.iters[DSPGN_MODE_POSE] = unlimited ? (1 << 30) : c.pose_only_iterations;
   p.render = (p.any[DSPGN_MODE_JOINT] || p.any_dormant) && !c.sdf_only;
-  if (s->run_upload_pending) { CU(cudaEventSynchronize(s->ev_run_upload)); s->run_upload_pending = false; }
+  if (s->run_upload_pending) { CU(settle_event(s, s->ev_run_upload)); s->run_upload_pending = false; }
   const size_t bytes = run_table_bytes(n, p.gated);
   const bool same = s->run_table_valid && !p.gated && !s->run_table_gated &&
                     memcmp(run_table(s->h_run.p, n, false).modes, modes, 4 * (size_t)n) == 0;
   if (!same) {
-    if (s->d_run.cap < bytes) CU(cudaStreamSynchronize(s->stream));      // kernels of an earlier run may still read it
+    if (s->d_run.cap < bytes) CU(settle_stream(s));      // kernels of an earlier run may still read it
     if (s->h_run.reserve(bytes) || s->d_run.reserve(bytes)) return fail(DSPGN_E_ALLOC, "run table allocation failed");
   }
   const RunTable h = run_table(s->h_run.p, n, p.gated);
@@ -812,8 +871,11 @@ namespace {
 // terms and update and finishes after its own last iteration; dspgn_run_batch(s, m) is the uniform case.
 // A gated run (link != nullptr, see plan_run) also checks every gated pose-only object at its last solve and runs the joint
 // slots of the rejected ones: woken on the device by the persistent kernel; in the per-iteration schedule as a second
-// phase after a readback of the verdicts.
-int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = nullptr, const float* t_map = nullptr) {
+// phase after a readback of the verdicts, or (device_wake, a submitted call) as a second phase enqueued for every gated
+// slot: k_gate_wake reads the verdicts itself and the slots it does not wake have n_iter 0, so they contribute no rows
+// (term_rows) and k_solve skips them -- the same records.  Their rows are counted when the records come back.
+int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = nullptr, const float* t_map = nullptr,
+                   bool device_wake = false) {
   CU(cudaSetDevice(s->device));
   RunPlan p;
   if (int rc = plan_run(s, modes, p, false, link, t_map)) return rc;
@@ -873,12 +935,20 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     return 0;
   };
   if (int rc = iterate(p, max_iters)) return rc;
-  if (p.any_dormant) {
+  if (p.any_dormant && device_wake) {
+    RunPlan pb = p;
+    pb.any[DSPGN_MODE_POSE] = false; pb.any[DSPGN_MODE_JOINT] = true;
+    pb.pts[DSPGN_MODE_POSE] = 0; pb.pts[DSPGN_MODE_JOINT] = 0; pb.smp_joint = 0;
+    k_gate_wake<<<(s->n_obj + 127) / 128, 128, 0, s->stream>>>(b, p.iters[DSPGN_MODE_JOINT]);
+    s->ctr.kernel_launches++;
+    CU(cudaGetLastError());
+    if (int rc = iterate(pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
+  } else if (p.any_dormant) {
     // second phase: the verdicts of the first (record gate words) decide which joint slots run
     const int n = s->n_obj;
     if (s->h_results.reserve(4 * DSPGN_RESULT_FLOATS * (size_t)n + 512)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
     CU(cudaMemcpyAsync(s->h_results.p, s->d_results.p, 4 * DSPGN_RESULT_FLOATS * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
-    CU(cudaStreamSynchronize(s->stream));
+    CU(sync_stream(s));
     const int* rec = s->h_results.as<int>();
     RunPlan pb = p;
     pb.any[DSPGN_MODE_POSE] = false; pb.any[DSPGN_MODE_JOINT] = false;
@@ -949,12 +1019,14 @@ int gather_layout(DspgnSolver* s, int n_slots, int world, int rank) {
 }  // namespace
 
 int dspgn_run_batch(DspgnSolver* s, int mode) {
+  BUSY(s);
   if (s) s->gdev = GatherDev{};
   return run_uniform(s, mode);
 }
 
 int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes) {
   if (!s || !modes) return fail(DSPGN_E_ARG, "null argument");
+  BUSY(s);
   if (s->n_obj < 1) return fail(DSPGN_E_ARG, "no batch uploaded");
   if (int rc = check_modes(s, modes, s->n_obj, nullptr)) return rc;
   s->gdev = GatherDev{};
@@ -964,6 +1036,7 @@ int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes) {
 // ---- multi-GPU result exchange ----------------------------------------------------------------------------------
 int dspgn_gather_create(DspgnSolver* s, int n_slots, int world, DspgnIpcHandle* handle_out) {
   if (!s || !handle_out || n_slots < 1 || world < 1 || world > 1024) return fail(DSPGN_E_ARG, "bad gather arguments");
+  BUSY(s);
   static_assert(sizeof(cudaIpcMemHandle_t) <= DSPGN_IPC_HANDLE_BYTES, "IPC handle size");
   CU(cudaSetDevice(s->device));
   dspgn_gather_close(s);
@@ -986,6 +1059,7 @@ int dspgn_gather_create(DspgnSolver* s, int n_slots, int world, DspgnIpcHandle* 
 
 int dspgn_gather_open(DspgnSolver* s, const DspgnIpcHandle* handle, int n_slots, int world, int rank) {
   if (!s || !handle || n_slots < 1 || world < 2 || rank < 1 || rank >= world) return fail(DSPGN_E_ARG, "bad gather arguments");
+  BUSY(s);
   CU(cudaSetDevice(s->device));
   dspgn_gather_close(s);
   if (int rc = gather_layout(s, n_slots, world, rank)) return rc;
@@ -1001,10 +1075,11 @@ int dspgn_gather_open(DspgnSolver* s, const DspgnIpcHandle* handle, int n_slots,
 
 void dspgn_gather_close(DspgnSolver* s) {
   if (!s) return;
+  if (s->flight.active) { fail(DSPGN_E_BUSY, "a submitted keyframe call is in flight"); return; }
   DspgnSolver::Gather& G = s->gather;
   if (G.base) {
     cudaSetDevice(s->device);
-    cudaStreamSynchronize(s->stream);
+    sync_stream(s);
     if (G.owner) cudaFree(G.base); else cudaIpcCloseMemHandle(G.base);
     cudaGetLastError();
   }
@@ -1015,6 +1090,7 @@ void dspgn_gather_close(DspgnSolver* s) {
 
 int dspgn_gather_bind(DspgnSolver* s, const int32_t* slots, int n) {
   if (!s || n < 0 || (n > 0 && !slots)) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   DspgnSolver::Gather& G = s->gather;
   if (!G.active) return fail(DSPGN_E_ARG, "no gather buffer (dspgn_gather_create / dspgn_gather_open first)");
   if (n > 0 && n != s->n_obj) return fail(DSPGN_E_ARG, "gather_bind: n must equal the resident batch size");
@@ -1022,7 +1098,7 @@ int dspgn_gather_bind(DspgnSolver* s, const int32_t* slots, int n) {
     if (slots[i] < 0 || slots[i] >= G.n_slots) return fail(DSPGN_E_ARG, "gather_bind: slot out of range");
   CU(cudaSetDevice(s->device));
   if (n > 0) {
-    if (G.d_slot_of.cap < 4 * (size_t)n) CU(cudaStreamSynchronize(s->stream));
+    if (G.d_slot_of.cap < 4 * (size_t)n) CU(settle_stream(s));
     if (G.d_slot_of.reserve(4 * (size_t)n)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
     CU(cudaMemcpyAsync(G.d_slot_of.p, slots, 4 * (size_t)n, cudaMemcpyHostToDevice, s->stream));   // pageable source: returns after staging
   }
@@ -1032,6 +1108,7 @@ int dspgn_gather_bind(DspgnSolver* s, const int32_t* slots, int n) {
 
 int dspgn_run_batch_gather(DspgnSolver* s, int mode, int seq) {
   if (!s || seq < 1) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   DspgnSolver::Gather& G = s->gather;
   if (!G.active || G.bound_n < 0) return fail(DSPGN_E_ARG, "gather not bound for the resident batch");
   CU(cudaSetDevice(s->device));
@@ -1051,11 +1128,13 @@ int dspgn_run_batch_gather(DspgnSolver* s, int mode, int seq) {
 
 const float* dspgn_gather_device(DspgnSolver* s, int seq) {
   if (!s || !s->gather.active) return nullptr;
+  if (s->flight.active) { fail(DSPGN_E_BUSY, "a submitted keyframe call is in flight"); return nullptr; }
   return reinterpret_cast<const float*>(s->gather.base) + (size_t)(seq & 1) * s->gather.n_slots * DSPGN_RESULT_FLOATS;
 }
 
 int dspgn_gather_results(DspgnSolver* s, int seq, int n, DspgnObjectOut* out) {
   if (!s || !out || n < 1) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   DspgnSolver::Gather& G = s->gather;
   if (!G.active || G.rank != 0 || n > G.n_slots) return fail(DSPGN_E_ARG, "gather_results: rank 0 only, n <= n_slots");
   CU(cudaSetDevice(s->device));
@@ -1063,7 +1142,7 @@ int dspgn_gather_results(DspgnSolver* s, int seq, int n, DspgnObjectOut* out) {
   if (G.h_out.reserve(bytes + 64)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
   CU(cudaMemcpyAsync(G.h_out.p, dspgn_gather_device(s, seq), bytes, cudaMemcpyDeviceToHost, s->stream));
   CU(cudaMemcpyAsync(G.h_out.as<unsigned char>() + bytes, G.d_local.p, 4, cudaMemcpyDeviceToHost, s->stream));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   memcpy(out, G.h_out.p, bytes);
   int err = 0;
   memcpy(&err, G.h_out.as<unsigned char>() + bytes, 4);
@@ -1073,9 +1152,10 @@ int dspgn_gather_results(DspgnSolver* s, int seq, int n, DspgnObjectOut* out) {
 
 long long dspgn_gather_wait_ns(DspgnSolver* s) {
   if (!s || !s->gather.active) return -1;
+  if (s->flight.active) { fail(DSPGN_E_BUSY, "a submitted keyframe call is in flight"); return -1; }
   long long v[2] = {0, 0};
   cudaSetDevice(s->device);
-  if (cudaStreamSynchronize(s->stream) != cudaSuccess) return -1;
+  if (sync_stream(s) != cudaSuccess) return -1;
   if (cudaMemcpy(v, s->gather.d_local.p, 16, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
   return v[1];
 }
@@ -1099,29 +1179,23 @@ int dspgn_debug_exp(int device, int sim3, const float* x, int n, float* out) {
   return 0;
 }
 
-const float* dspgn_results_device(DspgnSolver* s) { return s ? s->d_results.as<float>() : nullptr; }
+const float* dspgn_results_device(DspgnSolver* s) {
+  if (s && s->flight.active) { fail(DSPGN_E_BUSY, "a submitted keyframe call is in flight"); return nullptr; }
+  return s ? s->d_results.as<float>() : nullptr;
+}
 
-int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
-  if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
-  CU(cudaSetDevice(s->device));
-  static_assert(sizeof(DspgnObjectOut) == 4 * DSPGN_RESULT_FLOATS, "result record layout");
-  const size_t bytes = sizeof(DspgnObjectOut) * (size_t)s->n_obj;
-  const bool mega = s->mega_ran;           // the queue counters (abort flag, band-row total) ride on the same copy + sync
-  const size_t ctr_off = (bytes + 63) / 64 * 64;
-  if (s->h_results.reserve(ctr_off + sizeof(QueueCounters))) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
-  const QueueCounters& hq = *reinterpret_cast<const QueueCounters*>(s->h_results.as<unsigned char>() + ctr_off);
-  CU(cudaMemcpyAsync(s->h_results.p, s->d_results.p, bytes, cudaMemcpyDeviceToHost, s->stream));
-  if (mega) CU(cudaMemcpyAsync(s->h_results.as<unsigned char>() + ctr_off, s->d_q_ctr.p, sizeof(QueueCounters), cudaMemcpyDeviceToHost, s->stream));
-  CU(cudaStreamSynchronize(s->stream));
-  memcpy(out, s->h_results.p, bytes);
-  if (mega) {
+namespace {
+// The host side of a run's end, once its records and (persistent kernel) queue counters hq are on the host: the kernel's
+// row totals and abort flag, and the timings.
+int collect_run(DspgnSolver* s, const QueueCounters* hq) {
+  if (hq) {
     s->mega_ran = false;
     if (s->band_rows_pending) {              // roofline accounting: what the reference decodes (loss.py:77-78, :143-144)
-      s->ctr.rows_fwd_bwd += hq.band_rows_total;                  // band rows of all iterations
-      s->ctr.rows_fwd_only += (long long)hq.valid_rows_total;     // V: ray samples inside the unit sphere, all iterations
+      s->ctr.rows_fwd_bwd += hq->band_rows_total;                 // band rows of all iterations
+      s->ctr.rows_fwd_only += (long long)hq->valid_rows_total;    // V: ray samples inside the unit sphere, all iterations
     }
     s->band_rows_pending = false;
-    if (hq.abort_flag) return fail(DSPGN_E_CUDA, "persistent kernel: a work-queue wait timed out (aborted softly; results incomplete)");
+    if (hq->abort_flag) return fail(DSPGN_E_CUDA, "persistent kernel: a work-queue wait timed out (aborted softly; results incomplete)");
   }
   if (s->timing) {
     float dec = 0.f;
@@ -1135,9 +1209,28 @@ int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
   if (cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot; else cudaGetLastError();
   return 0;
 }
+}  // namespace
+
+int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
+  if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
+  BUSY(s);
+  CU(cudaSetDevice(s->device));
+  static_assert(sizeof(DspgnObjectOut) == 4 * DSPGN_RESULT_FLOATS, "result record layout");
+  const size_t bytes = sizeof(DspgnObjectOut) * (size_t)s->n_obj;
+  const bool mega = s->mega_ran;           // the queue counters (abort flag, band-row total) ride on the same copy + sync
+  const size_t ctr_off = (bytes + 63) / 64 * 64;
+  if (s->h_results.reserve(ctr_off + sizeof(QueueCounters))) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
+  const QueueCounters& hq = *reinterpret_cast<const QueueCounters*>(s->h_results.as<unsigned char>() + ctr_off);
+  CU(cudaMemcpyAsync(s->h_results.p, s->d_results.p, bytes, cudaMemcpyDeviceToHost, s->stream));
+  if (mega) CU(cudaMemcpyAsync(s->h_results.as<unsigned char>() + ctr_off, s->d_q_ctr.p, sizeof(QueueCounters), cudaMemcpyDeviceToHost, s->stream));
+  CU(sync_stream(s));
+  memcpy(out, s->h_results.p, bytes);
+  return collect_run(s, mega ? &hq : nullptr);
+}
 
 int dspgn_reconstruct_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out) {
   if (!s || !in || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   // any number of objects: resident batches of at most kMaxObjScan, one after the other
   for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
     const int n = std::min(kMaxObjScan, n_obj - o0);
@@ -1150,6 +1243,7 @@ int dspgn_reconstruct_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, 
 
 int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out) {
   if (!s || !in || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   for (int o = 0; o < n_obj; ++o)
     if (!in[o].code || !(in[o].scale > 0.f)) return fail(DSPGN_E_ARG, "estimate_pose needs a code and a positive scale per object");
   for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
@@ -1163,166 +1257,192 @@ int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in
 
 namespace {
 
+struct MeshWs {                      // one chunk's mesh workspace (mesh_count)
+  uint8_t* mask; uint8_t* ok; int* vscan; int* fscan; int* bases;
+  unsigned bv, bc;                   // blocks of the per-lattice-vertex / per-cube passes
+};
+int mesh_count(DspgnSolver* s, const MeshGrid& g, MeshWs& w);
+int mesh_emit(DspgnSolver* s, const MeshGrid& g, const MeshWs& w, size_t V, size_t F);
 int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF);
 
-// dspgn_keyframe_batch_gated, and with mesh != nullptr dspgn_keyframe_batch_meshed.  The objects are walked in units --
-// one object, or a mono pair (its two hypotheses next to each other) -- packed into resident chunks of at most
-// kMaxObjScan slots; a gated object's joint slot is appended after the chunk's objects.  When meshing, a chunk also holds
-// at most kMeshChunkRows grid rows of candidates, and its grids sit in walk order in the call's grid block.
-int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, const DspgnGateIn* gates,
-                  const DspgnMeshSpec* mesh, DspgnObjectOut* out, int32_t* n_vertices, int32_t* n_faces) {
-  if (!s || !in || !modes || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
+// A keyframe call (dspgn_keyframe_batch_gated / _meshed / _submit) after its argument checks.  The objects are walked in
+// units -- one object, or a mono pair (its two hypotheses next to each other) -- packed into resident chunks of at most
+// kMaxObjScan slots; a gated object's joint slot is appended after the chunk's objects.  When meshing, a chunk also
+// holds at most kMeshChunkRows grid rows of candidates, and its grids sit in walk order in the call's grid block.
+struct KfWalk {
+  const DspgnObjectIn* in = nullptr; const int32_t* modes = nullptr; const DspgnGateIn* gates = nullptr;
+  const int32_t* pair = nullptr;
+  bool mesh = false;
+  int n_obj = 0, dim = 0, n_cand = 0;
+  long long R = 0;                   // grid rows of one candidate
+  std::vector<int> order;            // every object once, the flipped hypothesis j right after its map-pose hypothesis i < j
+  bool gated(int o) const { return gates != nullptr && gates[o].gate != 0; }
+  bool paired(int o) const { return pair != nullptr && pair[o] >= 0; }
+  bool candidate(int o) const { return modes[o] == DSPGN_MODE_JOINT || gated(o); }
+};
+
+int kf_walk(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, const DspgnGateIn* gates,
+            const DspgnMeshSpec* mesh, KfWalk& w) {
+  if (!s || !in || !modes || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
   if (int rc = check_modes(s, modes, n_obj, in)) return rc;
-  auto gated = [&](int o) { return gates != nullptr && gates[o].gate != 0; };
+  w.in = in; w.modes = modes; w.gates = gates; w.n_obj = n_obj; w.mesh = mesh != nullptr;
   for (int o = 0; gates && o < n_obj; ++o) {
     const DspgnGateIn& g = gates[o];
     if (g.gate != 0 && g.gate != 1) return fail(DSPGN_E_ARG, "gate must be 0 or 1");
-    if (!gated(o)) continue;
+    if (!w.gated(o)) continue;
     if (modes[o] != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "a gate needs a pose-only object");
     if (!g.t_cam_obj_map || !g.t_cam_obj_sim3) return fail(DSPGN_E_ARG, "a gate needs t_cam_obj_map and t_cam_obj_sim3");
     if (in[o].t_cam_world) return fail(DSPGN_E_ARG, "a gated object takes camera-frame inputs (no t_cam_world)");
   }
-  const int32_t* pair = mesh ? mesh->pair : nullptr;
-  const int dim = mesh ? mesh->voxels_dim : 0;
+  w.pair = mesh ? mesh->pair : nullptr;
+  w.dim = mesh ? mesh->voxels_dim : 0;
   if (mesh) {
-    if (dim < 2 || dim > kMeshMaxDim) return fail(DSPGN_E_ARG, "voxels_dim must be in [2,128]");
-    for (int o = 0; pair && o < n_obj; ++o) {
-      const int j = pair[o];
+    if (w.dim < 2 || w.dim > kMeshMaxDim) return fail(DSPGN_E_ARG, "voxels_dim must be in [2,128]");
+    for (int o = 0; w.pair && o < n_obj; ++o) {
+      const int j = w.pair[o];
       if (j == -1) continue;
-      if (j < 0 || j >= n_obj || j == o || pair[j] != o) return fail(DSPGN_E_ARG, "pair must be symmetric, in range and never an object with itself");
-      if (modes[o] != DSPGN_MODE_JOINT || gated(o)) return fail(DSPGN_E_ARG, "a pair needs two ungated joint objects");
+      if (j < 0 || j >= n_obj || j == o || w.pair[j] != o) return fail(DSPGN_E_ARG, "pair must be symmetric, in range and never an object with itself");
+      if (modes[o] != DSPGN_MODE_JOINT || w.gated(o)) return fail(DSPGN_E_ARG, "a pair needs two ungated joint objects");
     }
   }
-  auto paired = [&](int o) { return pair != nullptr && pair[o] >= 0; };
-  auto candidate = [&](int o) { return modes[o] == DSPGN_MODE_JOINT || gated(o); };
-  const long long R = mesh ? (long long)dim * dim * dim : 0;
-  // walk order: every object once, the flipped hypothesis j right after its map-pose hypothesis i < j
-  std::vector<int> order;
-  order.reserve(n_obj);
-  int n_cand = 0;
+  w.R = mesh ? (long long)w.dim * w.dim * w.dim : 0;
+  w.order.reserve(n_obj);
   for (int o = 0; o < n_obj; ++o) {
-    n_cand += candidate(o) ? 1 : 0;
-    if (paired(o) && pair[o] < o) continue;
-    order.push_back(o);
-    if (paired(o)) order.push_back(pair[o]);
+    w.n_cand += w.candidate(o) ? 1 : 0;
+    if (w.paired(o) && w.pair[o] < o) continue;
+    w.order.push_back(o);
+    if (w.paired(o)) w.order.push_back(w.pair[o]);
   }
-  std::vector<int32_t> gV, gF, grid_of(mesh ? n_obj : 0, -1);
-  if (mesh) {
-    CU(cudaSetDevice(s->device));
-    s->mesh_n = 0;
-    s->mesh_v.clear(); s->mesh_f.clear();
-    const size_t grid_bytes = 4 * (size_t)n_cand * R;
-    if (s->d_mgrid.cap < grid_bytes || s->d_grid_pts.cap < 12 * (size_t)R) CU(cudaStreamSynchronize(s->stream));
-    if (s->d_mgrid.reserve(grid_bytes) || s->d_grid_pts.reserve(12 * (size_t)R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
-    gV.assign(n_cand, 0); gF.assign(n_cand, 0);
+  return 0;
+}
+
+// the end of the chunk that starts at walk position u0, and its resident slots
+size_t kf_chunk_end(const KfWalk& w, size_t u0, int& slots) {
+  size_t u1 = u0;
+  long long cands = 0;
+  slots = 0;
+  while (u1 < w.order.size()) {
+    const int o = w.order[u1], m = w.paired(o) ? 2 : 1;
+    const int sl = m + (w.gated(o) ? 1 : 0), cd = m == 2 ? 2 : (w.candidate(o) ? 1 : 0);
+    if (slots + sl > kMaxObjScan || (cands + cd) * w.R > kMeshChunkRows) break;
+    slots += sl; cands += cd; u1 += m;
   }
+  return u1;
+}
+
+// the call's grid block and query grid; no mesh of an earlier call is returned any more
+int kf_grids(DspgnSolver* s, const KfWalk& w) {
+  CU(cudaSetDevice(s->device));
+  s->mesh_n = 0;
+  s->mesh_v.clear(); s->mesh_f.clear();
+  const size_t grid_bytes = 4 * (size_t)w.n_cand * w.R;
+  if (s->d_mgrid.cap < grid_bytes || s->d_grid_pts.cap < 12 * (size_t)w.R) CU(settle_stream(s));
+  if (s->d_mgrid.reserve(grid_bytes) || s->d_grid_pts.reserve(12 * (size_t)w.R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
+  return 0;
+}
+
+// Enqueues the chunk of walk units [u0, u0 + n) with `slots` resident slots: upload, run and, when meshing, the mesh
+// selection and the decode of the chunk's grids (from grid g0 of the call).  link: per slot, as the run table has it;
+// gc: grids of the chunk; grid_of[o]: the call-wide grid of each candidate object.
+int kf_enqueue_chunk(DspgnSolver* s, const KfWalk& w, size_t u0, int n, int slots, int g0, bool device_wake,
+                     std::vector<int32_t>& link, int& gc, std::vector<int32_t>& grid_of) {
+  s->gdev = GatherDev{};
   std::vector<DspgnObjectIn> ins;
-  std::vector<int32_t> cm, link, sel;
-  std::vector<float> t_map;
-  std::vector<DspgnObjectOut> res;
-  int g0 = 0;                                          // grids of the chunks before this one
-  for (size_t u0 = 0; u0 < order.size();) {
-    size_t u1 = u0;
-    int slots = 0;
-    long long cands = 0;
-    while (u1 < order.size()) {
-      const int o = order[u1], m = paired(o) ? 2 : 1;
-      const int sl = m + (gated(o) ? 1 : 0), cd = m == 2 ? 2 : (candidate(o) ? 1 : 0);
-      if (slots + sl > kMaxObjScan || (cands + cd) * R > kMeshChunkRows) break;
-      slots += sl; cands += cd; u1 += m;
-    }
-    const int n = (int)(u1 - u0);
-    s->gdev = GatherDev{};
-    ins.clear(); cm.clear();
-    for (int k = 0; k < n; ++k) { ins.push_back(in[order[u0 + k]]); cm.push_back(modes[order[u0 + k]]); }
-    link.assign(n, -1);
-    if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
-      if (int rc = dspgn_upload_batch(s, n, ins.data())) return rc;
-      if (int rc = run_batch_impl(s, cm.data())) return rc;
-    } else {
-      t_map.assign(16 * (size_t)slots, 0.f);
-      for (int k = 0; k < n; ++k) {
-        const int o = order[u0 + k];
-        if (!gated(o)) continue;
-        const DspgnGateIn& g = gates[o];
-        DspgnObjectIn J = in[o];                       // the detection as reconstruct_object(Sim3Tco, pts, rays, depth) sees it
-        J.t_cam_obj = g.t_cam_obj_sim3; J.t_rs = g.sim3_rs; J.t_cs = g.sim3_cs;
-        J.code = nullptr;
-        link[k] = (int)ins.size();
-        link.push_back(k);
-        ins.push_back(J);
-        cm.push_back(DSPGN_MODE_JOINT);
-        for (int r = 0; r < 4; ++r)
-          for (int c = 0; c < 4; ++c) t_map[16 * (size_t)k + 4 * r + c] = g.t_cam_obj_map[(size_t)r * g.map_rs + (size_t)c * g.map_cs];
-      }
-      if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
-      if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data())) return rc;
-    }
-    const bool mega = s->mega_ran;
-    int gc = 0;                                        // grids of this chunk
-    if (mesh) {
-      // per slot: its grid in the chunk's block (-1: not a candidate) | the slot of the other hypothesis of its pair
-      sel.assign(2 * (size_t)slots, -1);
-      for (int k = 0; k < n; ++k) {
-        const int o = order[u0 + k];
-        if (!candidate(o)) continue;
-        sel[cm[k] == DSPGN_MODE_JOINT ? k : link[k]] = gc;
-        grid_of[o] = g0 + gc++;
-        if (paired(o)) sel[(size_t)slots + k] = pair[o] > o ? k + 1 : k - 1;
-      }
-      if (s->d_mesh_sel.cap < 4 * sel.size()) CU(cudaStreamSynchronize(s->stream));
-      if (s->d_mesh_sel.reserve(4 * sel.size())) return fail(DSPGN_E_ALLOC, "cudaMalloc");
-      int* d_sel = s->d_mesh_sel.as<int>();
-      CU(cudaMemcpyAsync(d_sel, sel.data(), 4 * sel.size(), cudaMemcpyHostToDevice, s->stream));
-      if (u0 == 0) {                                   // the call-wide query grid of create_voxel_grid
-        k_mesh_grid_points<<<(unsigned)((R + 255) / 256), 256, 0, s->stream>>>(s->d_grid_pts.as<float>(), 1, dim);
-        s->ctr.kernel_launches++;
-      }
-      BatchDev b = batch_dev(s);
-      k_mesh_select<<<slots, 128, 0, s->stream>>>(b, d_sel, d_sel + slots);
-      s->ctr.kernel_launches++;
-      CU(cudaGetLastError());
-      if (gc > 0) {
-        // grids of the candidates that get no mesh stay NaN: no cube of theirs is on the surface
-        b.sdf = s->d_mgrid.as<float>() + (size_t)g0 * R;
-        CU(cudaMemsetAsync(b.sdf, 0xff, 4 * (size_t)gc * R, s->stream));
-        TermArgs a = base_term(s, MODE_GRIDFWD);
-        a.grid = s->d_grid_pts.as<float>(); a.grid_slot = d_sel; a.grid_rows = (int)R;
-        if (int rc = launch_term(s, b, a, (long long)gc * R)) return rc;
-      }
-    }
-    res.resize(slots);
-    if (int rc = dspgn_results(s, res.data())) return rc;
-    int done = 0;
+  std::vector<int32_t> cm;
+  for (int k = 0; k < n; ++k) { ins.push_back(w.in[w.order[u0 + k]]); cm.push_back(w.modes[w.order[u0 + k]]); }
+  link.assign(n, -1);
+  if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
+    if (int rc = dspgn_upload_batch(s, n, ins.data())) return rc;
+    if (int rc = run_batch_impl(s, cm.data())) return rc;
+  } else {
+    std::vector<float> t_map(16 * (size_t)slots, 0.f);
     for (int k = 0; k < n; ++k) {
-      DspgnObjectOut& r = out[order[u0 + k]];
-      r = res[k];
-      if (link[k] >= 0 && res[k].gate == DSPGN_GATE_REJECTED) {
-        r = res[link[k]];
-        r.gate = DSPGN_GATE_REJECTED;
-        if (mega) s->ctr.rows_fwd_bwd += (long long)s->h_meta[link[k]].n_pts * s->cfg.num_iterations;   // the woken slot's SDF rows
-      }
-      done += r.mesh == DSPGN_MESH_DONE ? 1 : 0;
+      const int o = w.order[u0 + k];
+      if (!w.gated(o)) continue;
+      const DspgnGateIn& g = w.gates[o];
+      DspgnObjectIn J = w.in[o];                     // the detection as reconstruct_object(Sim3Tco, pts, rays, depth) sees it
+      J.t_cam_obj = g.t_cam_obj_sim3; J.t_rs = g.sim3_rs; J.t_cs = g.sim3_cs;
+      J.code = nullptr;
+      link[k] = (int)ins.size();
+      link.push_back(k);
+      ins.push_back(J);
+      cm.push_back(DSPGN_MODE_JOINT);
+      for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) t_map[16 * (size_t)k + 4 * r + c] = g.t_cam_obj_map[(size_t)r * g.map_rs + (size_t)c * g.map_cs];
     }
-    if (gc > 0) {
-      s->ctr.rows_fwd_only += (long long)done * R;
-      const MeshGrid g{s->d_mgrid.as<float>() + (size_t)g0 * R, gc, dim, R, (long long)(dim - 1) * (dim - 1) * (dim - 1), 2.0 / (dim - 1)};
-      if (int rc = mesh_chunk(s, g, gV.data() + g0, gF.data() + g0)) return rc;
-    }
-    g0 += gc;
-    u0 = u1;
+    if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
+    if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data(), device_wake)) return rc;
   }
-  if (!mesh) return 0;
-  // the meshes came out in walk order: put them in object order (they differ only where a pair is not adjacent)
+  gc = 0;
+  if (!w.mesh) return 0;
+  // per slot: its grid in the chunk's block (-1: not a candidate) | the slot of the other hypothesis of its pair
+  const size_t sel_bytes = 4 * 2 * (size_t)slots;
+  if (s->d_mesh_sel.cap < sel_bytes) CU(settle_stream(s));
+  if (s->d_mesh_sel.reserve(sel_bytes) || s->h_mesh_sel.reserve(sel_bytes)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
+  int* sel = s->h_mesh_sel.as<int>();
+  std::fill(sel, sel + 2 * (size_t)slots, -1);
+  for (int k = 0; k < n; ++k) {
+    const int o = w.order[u0 + k];
+    if (!w.candidate(o)) continue;
+    sel[cm[k] == DSPGN_MODE_JOINT ? k : link[k]] = gc;
+    grid_of[o] = g0 + gc++;
+    if (w.paired(o)) sel[(size_t)slots + k] = w.pair[o] > o ? k + 1 : k - 1;
+  }
+  int* d_sel = s->d_mesh_sel.as<int>();
+  CU(cudaMemcpyAsync(d_sel, sel, sel_bytes, cudaMemcpyHostToDevice, s->stream));
+  if (u0 == 0) {                                     // the call-wide query grid of create_voxel_grid
+    k_mesh_grid_points<<<(unsigned)((w.R + 255) / 256), 256, 0, s->stream>>>(s->d_grid_pts.as<float>(), 1, w.dim);
+    s->ctr.kernel_launches++;
+  }
+  BatchDev b = batch_dev(s);
+  k_mesh_select<<<slots, 128, 0, s->stream>>>(b, d_sel, d_sel + slots);
+  s->ctr.kernel_launches++;
+  CU(cudaGetLastError());
+  if (gc > 0) {
+    // grids of the candidates that get no mesh stay NaN: no cube of theirs is on the surface
+    b.sdf = s->d_mgrid.as<float>() + (size_t)g0 * w.R;
+    CU(cudaMemsetAsync(b.sdf, 0xff, 4 * (size_t)gc * w.R, s->stream));
+    TermArgs a = base_term(s, MODE_GRIDFWD);
+    a.grid = s->d_grid_pts.as<float>(); a.grid_slot = d_sel; a.grid_rows = (int)w.R;
+    if (int rc = launch_term(s, b, a, (long long)gc * w.R)) return rc;
+  }
+  return 0;
+}
+
+// The chunk's records (res, one per slot) into the caller's out in object order; a rejected gated object gets its joint
+// slot's record.  woken_rows: the woken slots' rows are not in the counters yet (1: SDF rows, 2: also ray-sample rows,
+// when the run had the render term).  Returns the number of DSPGN_MESH_DONE records.
+int kf_records(DspgnSolver* s, const KfWalk& w, size_t u0, int n, const std::vector<int32_t>& link,
+               const DspgnObjectOut* res, DspgnObjectOut* out, int woken_rows) {
+  int done = 0;
+  for (int k = 0; k < n; ++k) {
+    DspgnObjectOut& r = out[w.order[u0 + k]];
+    r = res[k];
+    if (link[k] >= 0 && res[k].gate == DSPGN_GATE_REJECTED) {
+      r = res[link[k]];
+      r.gate = DSPGN_GATE_REJECTED;
+      const ObjMeta& M = s->h_meta[link[k]];
+      if (woken_rows >= 1) s->ctr.rows_fwd_bwd += (long long)M.n_pts * s->cfg.num_iterations;
+      if (woken_rows >= 2) s->ctr.rows_fwd_only += (long long)M.n_rays * s->cfg.num_depth_samples * s->cfg.num_iterations;
+    }
+    done += r.mesh == DSPGN_MESH_DONE ? 1 : 0;
+  }
+  return done;
+}
+
+// The call's meshes, in walk order in mesh_v / mesh_f with gV / gF per grid, into object order; the per-object counts.
+void kf_meshes(DspgnSolver* s, const KfWalk& w, std::vector<int32_t>& grid_of, const std::vector<int32_t>& gV,
+               const std::vector<int32_t>& gF, int32_t* n_vertices, int32_t* n_faces) {
+  // they differ only where a pair is not adjacent
   bool in_order = true;
-  for (int o = 0, last = -1; o < n_obj; ++o)
+  for (int o = 0, last = -1; o < w.n_obj; ++o)
     if (grid_of[o] >= 0) { in_order = in_order && grid_of[o] > last; last = grid_of[o]; }
   if (!in_order) {
-    std::vector<size_t> ov(n_cand + 1, 0), of(n_cand + 1, 0);
-    for (int g = 0; g < n_cand; ++g) { ov[g + 1] = ov[g] + 3 * (size_t)gV[g]; of[g + 1] = of[g] + 3 * (size_t)gF[g]; }
+    std::vector<size_t> ov(w.n_cand + 1, 0), of(w.n_cand + 1, 0);
+    for (int g = 0; g < w.n_cand; ++g) { ov[g + 1] = ov[g] + 3 * (size_t)gV[g]; of[g + 1] = of[g] + 3 * (size_t)gF[g]; }
     std::vector<float> v; std::vector<int32_t> f;
     v.reserve(s->mesh_v.size()); f.reserve(s->mesh_f.size());
-    for (int o = 0; o < n_obj; ++o) {
+    for (int o = 0; o < w.n_obj; ++o) {
       const int g = grid_of[o];
       if (g < 0) continue;
       v.insert(v.end(), s->mesh_v.begin() + ov[g], s->mesh_v.begin() + ov[g + 1]);
@@ -1330,12 +1450,49 @@ int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int3
     }
     s->mesh_v.swap(v); s->mesh_f.swap(f);
   }
-  for (int o = 0; o < n_obj; ++o) {
+  for (int o = 0; o < w.n_obj; ++o) {
     n_vertices[o] = grid_of[o] >= 0 ? gV[grid_of[o]] : 0;
     n_faces[o] = grid_of[o] >= 0 ? gF[grid_of[o]] : 0;
   }
-  s->mesh_n = n_obj; s->mesh_dim = dim;
+  s->mesh_n = w.n_obj; s->mesh_dim = w.dim;
   s->mesh_grid_of.swap(grid_of);
+}
+
+// dspgn_keyframe_batch_gated, and with mesh != nullptr dspgn_keyframe_batch_meshed: chunk after chunk, each collected
+// (dspgn_results) before the next.
+int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes, const DspgnGateIn* gates,
+                  const DspgnMeshSpec* mesh, DspgnObjectOut* out, int32_t* n_vertices, int32_t* n_faces) {
+  if (!out) return fail(DSPGN_E_ARG, "bad argument");
+  KfWalk w;
+  if (int rc = kf_walk(s, n_obj, in, modes, gates, mesh, w)) return rc;
+  BUSY(s);
+  std::vector<int32_t> gV, gF, grid_of(mesh ? n_obj : 0, -1);
+  if (mesh) {
+    if (int rc = kf_grids(s, w)) return rc;
+    gV.assign(w.n_cand, 0); gF.assign(w.n_cand, 0);
+  }
+  std::vector<int32_t> link;
+  std::vector<DspgnObjectOut> res;
+  int g0 = 0;                                          // grids of the chunks before this one
+  for (size_t u0 = 0; u0 < w.order.size();) {
+    int slots = 0;
+    const size_t u1 = kf_chunk_end(w, u0, slots);
+    const int n = (int)(u1 - u0);
+    int gc = 0;                                        // grids of this chunk
+    if (int rc = kf_enqueue_chunk(s, w, u0, n, slots, g0, false, link, gc, grid_of)) return rc;
+    const bool mega = s->mega_ran;
+    res.resize(slots);
+    if (int rc = dspgn_results(s, res.data())) return rc;
+    const int done = kf_records(s, w, u0, n, link, res.data(), out, mega ? 1 : 0);   // the woken slots' SDF rows
+    if (gc > 0) {
+      s->ctr.rows_fwd_only += (long long)done * w.R;
+      const MeshGrid g{s->d_mgrid.as<float>() + (size_t)g0 * w.R, gc, w.dim, w.R, (long long)(w.dim - 1) * (w.dim - 1) * (w.dim - 1), 2.0 / (w.dim - 1)};
+      if (int rc = mesh_chunk(s, g, gV.data() + g0, gF.data() + g0)) return rc;
+    }
+    g0 += gc;
+    u0 = u1;
+  }
+  if (mesh) kf_meshes(s, w, grid_of, gV, gF, n_vertices, n_faces);
   return 0;
 }
 
@@ -1363,9 +1520,151 @@ int dspgn_keyframe_batch_meshed(DspgnSolver* s, int n_obj, const DspgnObjectIn* 
   return keyframe_impl(s, n_obj, in, modes, gates, mesh, out, n_vertices, n_faces);
 }
 
+// ---- submitted keyframe calls ------------------------------------------------------------------------------------
+// Submit enqueues what keyframe_impl does for one chunk, with two changes that keep the host out of the call: the
+// per-iteration schedule wakes the rejected slots on the device (run_batch_impl, device_wake), and the meshes go into an
+// arena sized beforehand (k_mesh_emit_*_arena) instead of buffers sized from a read-back of the counts.  Then the
+// records, the queue counters, the mesh bases and the arena are copied into h_flight and ev_flight is recorded.
+int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes,
+                          const DspgnGateIn* gates, const DspgnMeshSpec* mesh) {
+  std::vector<int32_t> joint;
+  if (!modes && n_obj > 0) {
+    joint.assign(n_obj, DSPGN_MODE_JOINT);
+    modes = joint.data();
+  }
+  KfWalk w;
+  if (int rc = kf_walk(s, n_obj, in, modes, gates, mesh, w)) return rc;
+  BUSY(s);
+  int slots = 0;
+  const size_t u1 = kf_chunk_end(w, 0, slots);
+  if (u1 < w.order.size())
+    return fail(DSPGN_E_ARG, "a submitted keyframe must fit one resident chunk: at most 1024 slots (a gated object takes two) "
+                             "and 2^24 candidate grid rows (the blocking calls take any size)");
+  CU(cudaSetDevice(s->device));
+  if (!s->ev_flight) CU(cudaEventCreateWithFlags(&s->ev_flight, cudaEventDisableTiming));
+  DspgnSolver::Flight& F = s->flight;
+  F = DspgnSolver::Flight{};
+  F.grid_of.assign(mesh ? n_obj : 0, -1);
+  if (mesh)
+    if (int rc = kf_grids(s, w)) return rc;
+  s->mega_ran = false;
+  int gc = 0;
+  if (int rc = kf_enqueue_chunk(s, w, 0, (int)u1, slots, 0, true, F.link, gc, F.grid_of)) return rc;
+  F.mega = s->mega_ran;
+  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
+  F.o_ctr = al(sizeof(DspgnObjectOut) * (size_t)slots);
+  F.o_base = F.o_ctr + al(sizeof(QueueCounters));
+  F.o_arena = F.o_base + al(8 * ((size_t)gc + 1));
+  MeshWs mw{};
+  if (gc > 0) {
+    F.g = MeshGrid{s->d_mgrid.as<float>(), gc, w.dim, w.R, (long long)(w.dim - 1) * (w.dim - 1) * (w.dim - 1), 2.0 / (w.dim - 1)};
+    if (int rc = mesh_count(s, F.g, mw)) return rc;
+    const double d2 = (double)w.dim * w.dim;
+    F.cap_v = s->arena_force_v > 0 ? s->arena_force_v : gc * (long long)std::ceil(s->arena_v * d2);
+    F.cap_f = s->arena_force_f > 0 ? s->arena_force_f : gc * (long long)std::ceil(s->arena_f * d2);
+    const size_t arena_bytes = 12 * (size_t)(F.cap_v + F.cap_f);
+    if (s->d_mout.cap < arena_bytes) CU(settle_stream(s));
+    if (s->d_mout.reserve(arena_bytes)) return fail(DSPGN_E_ALLOC, "mesh arena allocation failed");
+    const int* totals = mw.bases + 2 * gc;
+    k_mesh_emit_verts_arena<<<mw.bv, 256, 0, s->stream>>>(F.g, mw.mask, mw.vscan, totals, F.cap_v, F.cap_f, s->d_mout.as<float>());
+    k_mesh_emit_faces_arena<<<mw.bc, 256, 0, s->stream>>>(F.g, mw.mask, mw.vscan, mw.fscan, totals, F.cap_v, F.cap_f,
+                                                          s->d_mout.as<float>());
+    CU(cudaGetLastError());
+    s->ctr.kernel_launches += 2;
+    F.mask = mw.mask; F.vscan = mw.vscan; F.fscan = mw.fscan;
+  }
+  const size_t total = F.o_arena + 12 * (size_t)(F.cap_v + F.cap_f);
+  if (s->h_flight.reserve(total)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
+  unsigned char* h = s->h_flight.as<unsigned char>();
+  CU(cudaMemcpyAsync(h, s->d_results.p, sizeof(DspgnObjectOut) * (size_t)slots, cudaMemcpyDeviceToHost, s->stream));
+  if (F.mega) CU(cudaMemcpyAsync(h + F.o_ctr, s->d_q_ctr.p, sizeof(QueueCounters), cudaMemcpyDeviceToHost, s->stream));
+  if (gc > 0) {
+    CU(cudaMemcpyAsync(h + F.o_base, mw.bases, 8 * ((size_t)gc + 1), cudaMemcpyDeviceToHost, s->stream));
+    CU(cudaMemcpyAsync(h + F.o_arena, s->d_mout.p, 12 * (size_t)(F.cap_v + F.cap_f), cudaMemcpyDeviceToHost, s->stream));
+  }
+  CU(cudaEventRecord(s->ev_flight, s->stream));
+  F.mesh = mesh != nullptr;
+  F.device_wake = !F.mega;
+  F.render = !s->cfg.sdf_only;
+  F.n_obj = n_obj; F.slots = slots; F.n = (int)u1; F.dim = w.dim; F.n_cand = w.n_cand; F.gc = gc;
+  F.order.swap(w.order);
+  F.active = true;
+  return 0;
+}
+
+int dspgn_keyframe_query(DspgnSolver* s) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  if (!s->flight.active) return fail(DSPGN_E_ARG, "no submitted keyframe call");
+  CU(cudaSetDevice(s->device));
+  const cudaError_t e = cudaEventQuery(s->ev_flight);
+  if (e == cudaSuccess) return 1;
+  if (e == cudaErrorNotReady) return 0;
+  return fail(DSPGN_E_CUDA, std::string("keyframe_query: ") + cudaGetErrorString(e));
+}
+
+int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices, int32_t* n_faces) {
+  if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
+  DspgnSolver::Flight& F = s->flight;
+  if (!F.active) return fail(DSPGN_E_ARG, "no submitted keyframe call");
+  if ((n_vertices == nullptr) == F.mesh || (n_faces == nullptr) == F.mesh)
+    return fail(DSPGN_E_ARG, "n_vertices and n_faces must be given iff the submitted call had a mesh spec");
+  F.active = false;                                  // collected from here on, whatever happens below
+  CU(cudaSetDevice(s->device));
+  CU(settle_event(s, s->ev_flight));
+  s->upload_pending = false;                         // the event follows every copy of the call
+  s->run_upload_pending = false;
+  const unsigned char* h = s->h_flight.as<unsigned char>();
+  if (int rc = collect_run(s, F.mega ? reinterpret_cast<const QueueCounters*>(h + F.o_ctr) : nullptr)) return rc;
+  KfWalk w;                                          // the walk's bookkeeping (the inputs are not read again)
+  w.n_obj = F.n_obj; w.n_cand = F.n_cand; w.dim = F.dim; w.R = (long long)F.dim * F.dim * F.dim; w.mesh = F.mesh;
+  w.order.swap(F.order);
+  const int done = kf_records(s, w, 0, F.n, F.link, reinterpret_cast<const DspgnObjectOut*>(h), out,
+                              F.mega ? 1 : (F.render ? 2 : 1));
+  if (!F.mesh) return 0;
+  std::vector<int32_t> gV(F.n_cand, 0), gF(F.n_cand, 0);
+  s->mesh_v.clear(); s->mesh_f.clear();
+  if (F.gc > 0) {
+    s->ctr.rows_fwd_only += (long long)done * w.R;
+    const int* hb = reinterpret_cast<const int*>(h + F.o_base);
+    const double d2 = (double)F.dim * F.dim;
+    for (int g = 0; g < F.gc; ++g) {
+      gV[g] = hb[2 * g + 2] - hb[2 * g]; gF[g] = hb[2 * g + 3] - hb[2 * g + 1];
+      s->arena_v = std::max(s->arena_v, 1.25 * gV[g] / d2);     // the next calls' arena: a margin over the largest mesh
+      s->arena_f = std::max(s->arena_f, 1.25 * gF[g] / d2);
+    }
+    const size_t V = (size_t)hb[2 * F.gc], Fc = (size_t)hb[2 * F.gc + 1];
+    if ((long long)V <= F.cap_v && (long long)Fc <= F.cap_f) {
+      const float* hv = reinterpret_cast<const float*>(h + F.o_arena);
+      const int32_t* hf = reinterpret_cast<const int32_t*>(hv + 3 * F.cap_v);
+      s->mesh_v.assign(hv, hv + 3 * V);
+      s->mesh_f.assign(hf, hf + 3 * Fc);
+    } else {                                         // the arena was too small: emit again at the exact size
+      const MeshWs mw{F.mask, nullptr, F.vscan, F.fscan, nullptr, (unsigned)(((size_t)F.g.n * F.g.R + 255) / 256),
+                      (unsigned)(((size_t)F.g.n * F.g.C + 255) / 256)};
+      if (int rc = mesh_emit(s, F.g, mw, V, Fc)) return rc;
+    }
+  }
+  kf_meshes(s, w, F.grid_of, gV, gF, n_vertices, n_faces);
+  return 0;
+}
+
+int dspgn_debug_host_syncs(DspgnSolver* s, int64_t* out) {
+  if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
+  *out = s->host_syncs;
+  return 0;
+}
+
+int dspgn_debug_mesh_arena(DspgnSolver* s, int64_t max_vertices, int64_t max_faces) {
+  if (!s || max_vertices < 0 || max_faces < 0 || (max_vertices == 0) != (max_faces == 0)) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
+  s->arena_force_v = max_vertices; s->arena_force_f = max_faces;
+  return 0;
+}
+
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n, int x_rs, int x_cs,
                      float* sdf_out) {
   if (!s || !code || !x || !sdf_out || n < 1) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   DspgnObjectIn in{};
   in.t_cam_obj = I4; in.t_rs = 4; in.t_cs = 1;
@@ -1385,21 +1684,22 @@ int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const floa
   if (int rc = launch_term(s, b, base_term(s, MODE_PTSFWD), n)) return rc;
   s->ctr.rows_fwd_only += n;
   CU(cudaMemcpyAsync(sdf_out, s->d_sdf.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   return 0;
 }
 
 namespace {
 
-// The iso-surface of the chunk's grids g (dspgn_mesh.cuh), appended to s->mesh_v / mesh_f; per-object counts into nV / nF.
-int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF) {
+// The passes of the iso-surface of the chunk's grids g (dspgn_mesh.cuh) up to the per-object bases (w.bases: first vertex
+// and face of every object, entry g.n the totals), enqueued.
+int mesh_count(DspgnSolver* s, const MeshGrid& g, MeshWs& ws) {
   const size_t nv = (size_t)g.n * g.R, nf = 4 * (size_t)g.n * g.C;
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   // workspace: vertex counts -> scan [nv + 1] | face counts -> scan [nf + 1] | edge masks [nv] | cube flags [n C] |
   // per-object bases [n + 1][2]
   const size_t o_fc = al(4 * (nv + 1)), o_mask = o_fc + al(4 * (nf + 1)), o_ok = o_mask + al(nv),
                o_base = o_ok + al((size_t)g.n * g.C), total = o_base + al(8 * ((size_t)g.n + 1));
-  if (s->d_mws.cap < total) CU(cudaStreamSynchronize(s->stream));
+  if (s->d_mws.cap < total) CU(settle_stream(s));
   if (s->d_mws.reserve(total)) return fail(DSPGN_E_ALLOC, "mesh workspace allocation failed");
   unsigned char* w = s->d_mws.as<unsigned char>();
   int* vscan = reinterpret_cast<int*>(w);
@@ -1410,9 +1710,8 @@ int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF) {
   size_t tmp_v = 0, tmp_f = 0;
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_v, vscan, vscan, (int)(nv + 1), s->stream));
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_f, fscan, fscan, (int)(nf + 1), s->stream));
-  if (s->d_mscan_tmp.cap < std::max(tmp_v, tmp_f)) CU(cudaStreamSynchronize(s->stream));
-  if (s->d_mscan_tmp.reserve(std::max(tmp_v, tmp_f)) || s->h_mbase.reserve(8 * ((size_t)g.n + 1)))
-    return fail(DSPGN_E_ALLOC, "mesh workspace allocation failed");
+  if (s->d_mscan_tmp.cap < std::max(tmp_v, tmp_f)) CU(settle_stream(s));
+  if (s->d_mscan_tmp.reserve(std::max(tmp_v, tmp_f))) return fail(DSPGN_E_ALLOC, "mesh workspace allocation failed");
   // the slot after the last count: the scans' totals
   CU(cudaMemsetAsync(vscan + nv, 0, 4, s->stream));
   CU(cudaMemsetAsync(fscan + nf, 0, 4, s->stream));
@@ -1424,21 +1723,22 @@ int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF) {
   CU(cub::DeviceScan::ExclusiveSum(s->d_mscan_tmp.p, tb, vscan, vscan, (int)(nv + 1), s->stream));
   tb = s->d_mscan_tmp.cap;
   CU(cub::DeviceScan::ExclusiveSum(s->d_mscan_tmp.p, tb, fscan, fscan, (int)(nf + 1), s->stream));
-  // per object: first vertex and first face (object n: the totals); the counts come back here (one read-back)
+  // per object: first vertex and first face (object n: the totals)
   k_mesh_bases<<<(g.n + 1 + 127) / 128, 128, 0, s->stream>>>(g, vscan, fscan, bases);
   CU(cudaGetLastError());
-  int* hb = s->h_mbase.as<int>();
-  CU(cudaMemcpyAsync(hb, bases, 8 * ((size_t)g.n + 1), cudaMemcpyDeviceToHost, s->stream));
-  CU(cudaStreamSynchronize(s->stream));
-  for (int o = 0; o < g.n; ++o) { nV[o] = hb[2 * o + 2] - hb[2 * o]; nF[o] = hb[2 * o + 3] - hb[2 * o + 1]; }
-  const size_t V = (size_t)hb[2 * g.n], F = (size_t)hb[2 * g.n + 1];
   s->ctr.kernel_launches += 2 + 2 * 2 + 1;                    // classify passes, two scans (two kernels each), bases
+  ws = MeshWs{mask, ok, vscan, fscan, bases, bv, bc};
+  return 0;
+}
+
+// The emit passes of mesh_count's chunk at V vertices and F faces, appended to s->mesh_v / mesh_f (synchronous).
+int mesh_emit(DspgnSolver* s, const MeshGrid& g, const MeshWs& w, size_t V, size_t F) {
   if (V == 0 && F == 0) return 0;
   if (s->d_mout.reserve(12 * (V + F))) return fail(DSPGN_E_ALLOC, "mesh output allocation failed");
   float* dv = s->d_mout.as<float>();
   int32_t* df = reinterpret_cast<int32_t*>(dv + 3 * V);
-  k_mesh_emit_verts<<<bv, 256, 0, s->stream>>>(g, mask, vscan, dv);
-  k_mesh_emit_faces<<<bc, 256, 0, s->stream>>>(g, mask, vscan, fscan, df);
+  k_mesh_emit_verts<<<w.bv, 256, 0, s->stream>>>(g, w.mask, w.vscan, dv);
+  k_mesh_emit_faces<<<w.bc, 256, 0, s->stream>>>(g, w.mask, w.vscan, w.fscan, df);
   CU(cudaGetLastError());
   s->ctr.kernel_launches += 2;
   const size_t v0 = s->mesh_v.size(), f0 = s->mesh_f.size();
@@ -1446,8 +1746,20 @@ int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF) {
   s->mesh_f.resize(f0 + 3 * F);
   CU(cudaMemcpyAsync(s->mesh_v.data() + v0, dv, 12 * V, cudaMemcpyDeviceToHost, s->stream));
   CU(cudaMemcpyAsync(s->mesh_f.data() + f0, df, 12 * F, cudaMemcpyDeviceToHost, s->stream));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   return 0;
+}
+
+// The iso-surface of the chunk's grids g, appended to s->mesh_v / mesh_f; per-object counts into nV / nF (one read-back).
+int mesh_chunk(DspgnSolver* s, const MeshGrid& g, int32_t* nV, int32_t* nF) {
+  MeshWs w;
+  if (int rc = mesh_count(s, g, w)) return rc;
+  if (s->h_mbase.reserve(8 * ((size_t)g.n + 1))) return fail(DSPGN_E_ALLOC, "mesh workspace allocation failed");
+  int* hb = s->h_mbase.as<int>();
+  CU(cudaMemcpyAsync(hb, w.bases, 8 * ((size_t)g.n + 1), cudaMemcpyDeviceToHost, s->stream));
+  CU(sync_stream(s));
+  for (int o = 0; o < g.n; ++o) { nV[o] = hb[2 * o + 2] - hb[2 * o]; nF[o] = hb[2 * o + 3] - hb[2 * o + 1]; }
+  return mesh_emit(s, g, w, (size_t)hb[2 * g.n], (size_t)hb[2 * g.n + 1]);
 }
 
 // One mesh call: grids decoded from codes (sdf_in == nullptr) or given by the caller, meshed chunk after chunk.  The
@@ -1462,12 +1774,13 @@ int mesh_impl(DspgnSolver* s, int n, int dim, const float* codes, int code_strid
   if (codes && code_stride < s->cfg.code_len) return fail(DSPGN_E_ARG, "code_stride must be >= code_len");
   for (int o = 0; class_ids && o < n; ++o)
     if (class_ids[o] < 0 || class_ids[o] >= (int)s->classes.size()) return fail(DSPGN_E_ARG, "bad class_id");
+  BUSY(s);
   CU(cudaSetDevice(s->device));
   const long long R = (long long)dim * dim * dim, C = (long long)(dim - 1) * (dim - 1) * (dim - 1);
   const int per_chunk = (int)std::max<long long>(1, std::min<long long>(kMaxObjScan, kMeshChunkRows / R));
   s->mesh_n = 0;
   s->mesh_v.clear(); s->mesh_f.clear(); s->mesh_grid_of.clear();
-  if (s->d_mgrid.cap < 4 * (size_t)n * R) CU(cudaStreamSynchronize(s->stream));
+  if (s->d_mgrid.cap < 4 * (size_t)n * R) CU(settle_stream(s));
   if (s->d_mgrid.reserve(4 * (size_t)n * R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
   s->ctr = DspgnCounters{};
   s->ev_used = 0;
@@ -1501,7 +1814,7 @@ int mesh_impl(DspgnSolver* s, int n, int dim, const float* codes, int code_strid
     if (int rc = mesh_chunk(s, g, n_vertices + o0, n_faces + o0)) return rc;
   }
   CU(cudaEventRecord(s->ev_run1, s->stream));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   if (s->timing) {
     float dec = 0.f;
     for (size_t i = 0; i + 1 < s->ev_used; i += 2) { float ms = 0.f; cudaEventElapsedTime(&ms, s->ev[i], s->ev[i + 1]); dec += ms; }
@@ -1528,6 +1841,7 @@ int dspgn_debug_mesh_grid(DspgnSolver* s, int n, int voxels_dim, const float* sd
 
 int dspgn_mesh_results(DspgnSolver* s, float* vertices, int32_t* faces, float* sdf) {
   if (!s) return fail(DSPGN_E_ARG, "null solver");
+  BUSY(s);
   if (s->mesh_n < 1) return fail(DSPGN_E_ARG, "no mesh call to return");
   if ((!vertices && !s->mesh_v.empty()) || (!faces && !s->mesh_f.empty())) return fail(DSPGN_E_ARG, "null output");
   if (!s->mesh_v.empty()) memcpy(vertices, s->mesh_v.data(), 4 * s->mesh_v.size());
@@ -1544,7 +1858,7 @@ int dspgn_mesh_results(DspgnSolver* s, float* vertices, int32_t* faces, float* s
         else memset(sdf + (size_t)o * R, 0xff, 4 * R);     // no grid: NaN, the bit pattern of the device's unmeshed grids
       }
     }
-    CU(cudaStreamSynchronize(s->stream));
+    CU(sync_stream(s));
   }
   return 0;
 }
@@ -1557,6 +1871,7 @@ int dspgn_debug_system(DspgnSolver* s, int obj, int mode, float* H, float* b, fl
 int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* H, float* b, float* dx, float* J_rows,
                             float* res_rows, float* losses) {
   if (!s || !H || !b || !dx) return fail(DSPGN_E_ARG, "null argument");
+  BUSY(s);
   if (obj < 0 || obj >= s->n_obj) return fail(DSPGN_E_ARG, "bad object index");
   if (iter < 0 || iter > 1000) return fail(DSPGN_E_ARG, "bad iteration index");
   if (mode != DSPGN_MODE_JOINT && mode != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
@@ -1601,7 +1916,7 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
       if (res_rows) cudaMemcpyAsync(res_rows, dres, 4 * (size_t)npts, cudaMemcpyDeviceToHost, s->stream);
     }
   }
-  cudaError_t e = cudaStreamSynchronize(s->stream);
+  cudaError_t e = sync_stream(s);
   dJ.release();
   if (rc) return rc;
   if (e != cudaSuccess) return fail(DSPGN_E_CUDA, std::string("debug_system: ") + cudaGetErrorString(e));
@@ -1610,8 +1925,9 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
 
 int dspgn_debug_inputs(DspgnSolver* s, int obj, float* t_cam_obj, float* pts, float* rays) {
   if (!s || obj < 0 || obj >= s->n_obj) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   CU(cudaSetDevice(s->device));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   const ObjMeta& M = s->h_meta[obj];
   if (t_cam_obj) CU(cudaMemcpy(t_cam_obj, s->d_Tinit + 16 * (size_t)obj, 64, cudaMemcpyDeviceToHost));
   if (pts && M.n_pts) CU(cudaMemcpy(pts, s->d_pts + 3 * (size_t)M.pts_off, 12 * (size_t)M.n_pts, cudaMemcpyDeviceToHost));
@@ -1623,9 +1939,10 @@ int dspgn_debug_events(DspgnSolver* s, long long* out, int max_events) {
   // event log of the last persistent-kernel run (env DSPGN_CLK=1 at solver creation): returns the number of events,
   // out[2*i] = %globaltimer (ns), out[2*i+1] = kind<<56 | mode<<52 | sm<<40 | object<<24 | tile (or iteration)
   if (!s || !out || max_events < 1) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
   if (!s->events_on || !s->d_ev.p) return fail(DSPGN_E_ARG, "event log not enabled (DSPGN_CLK)");
   CU(cudaSetDevice(s->device));
-  CU(cudaStreamSynchronize(s->stream));
+  CU(sync_stream(s));
   long long n = 0;
   CU(cudaMemcpy(&n, s->d_ev.p, 8, cudaMemcpyDeviceToHost));
   if (n > kEvCap) n = kEvCap;

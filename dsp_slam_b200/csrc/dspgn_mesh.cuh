@@ -14,7 +14,8 @@
 // 2-inside quads -- each in cube order, then tetrahedron order; a triangle is flipped when its fp64 normal points against
 // (mean of the outside corners - mean of the inside corners) and dropped when its squared area is <= 1e-30.
 // Passes: k_mesh_cubes (per-cube NaN flag and group counts) -> k_mesh_verts (edge masks) -> integer scans -> one
-// read-back of the per-object totals -> k_mesh_emit_verts / k_mesh_emit_faces.
+// read-back of the per-object totals -> k_mesh_emit_verts / k_mesh_emit_faces (or, in a submitted keyframe call, no
+// read-back and the *_arena variants below).
 // Every fp64 step is an explicit _rn intrinsic: numpy rounds each operation, and the build's --fmad=true must not
 // contract them.
 #pragma once
@@ -230,7 +231,7 @@ __global__ void k_mesh_bases(MeshGrid g, const int* vscan, const int* fscan, int
 }
 
 // pass 3a, one thread per lattice vertex: its vertices, f32(f32(p) + (-1.0)) as extract_mesh_from_code returns them
-__global__ void k_mesh_emit_verts(MeshGrid g, const uint8_t* mask, const int* vscan, float* verts) {
+__device__ __forceinline__ void mesh_emit_verts(const MeshGrid& g, const uint8_t* mask, const int* vscan, float* verts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)g.n * g.R) return;
   unsigned bits = mask[i];
@@ -251,7 +252,8 @@ __global__ void k_mesh_emit_verts(MeshGrid g, const uint8_t* mask, const int* vs
 
 // pass 3b, one thread per cube: its kept triangles at their place in the object's four groups; indices local to the
 // object's vertices
-__global__ void k_mesh_emit_faces(MeshGrid g, const uint8_t* mask, const int* vscan, const int* fscan, int32_t* faces) {
+__device__ __forceinline__ void mesh_emit_faces(const MeshGrid& g, const uint8_t* mask, const int* vscan, const int* fscan,
+                                                int32_t* faces) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)g.n * g.C) return;
   const int o = (int)(i / g.C);
@@ -283,6 +285,34 @@ __global__ void k_mesh_emit_faces(MeshGrid g, const uint8_t* mask, const int* vs
       f[0] = id[0]; f[1] = T.flip ? id[2] : id[1]; f[2] = T.flip ? id[1] : id[2];
     }
   }
+}
+
+__global__ void k_mesh_emit_verts(MeshGrid g, const uint8_t* mask, const int* vscan, float* verts) {
+  mesh_emit_verts(g, mask, vscan, verts);
+}
+
+__global__ void k_mesh_emit_faces(MeshGrid g, const uint8_t* mask, const int* vscan, const int* fscan, int32_t* faces) {
+  mesh_emit_faces(g, mask, vscan, fscan, faces);
+}
+
+// The emit passes of a submitted keyframe call (dspgn_keyframe_submit), which places its meshes without reading the
+// counts back: vertices and faces go into an arena of cap_v vertices | cap_f faces sized on the host beforehand.  When
+// the chunk's totals (k_mesh_bases' entry n) do not fit, nothing is written and dspgn_keyframe_wait re-runs
+// k_mesh_emit_verts / k_mesh_emit_faces at the exact sizes from the same grids and scans.
+__device__ __forceinline__ bool mesh_arena_fits(const int* totals, long long cap_v, long long cap_f) {
+  return totals[0] <= cap_v && totals[1] <= cap_f;
+}
+
+__global__ void k_mesh_emit_verts_arena(MeshGrid g, const uint8_t* mask, const int* vscan, const int* totals, long long cap_v,
+                                        long long cap_f, float* arena) {
+  if (!mesh_arena_fits(totals, cap_v, cap_f)) return;
+  mesh_emit_verts(g, mask, vscan, arena);
+}
+
+__global__ void k_mesh_emit_faces_arena(MeshGrid g, const uint8_t* mask, const int* vscan, const int* fscan,
+                                        const int* totals, long long cap_v, long long cap_f, float* arena) {
+  if (!mesh_arena_fits(totals, cap_v, cap_f)) return;
+  mesh_emit_faces(g, mask, vscan, fscan, reinterpret_cast<int32_t*>(arena + 3 * cap_v));
 }
 
 }  // namespace dspgn

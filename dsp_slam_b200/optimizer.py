@@ -266,6 +266,24 @@ class BatchSolver:
         meshes[i] = (vertices (V,3) f32, faces (F,3) int32) where the record's `mesh` word is _lib.MESH_DONE, else None;
         with want_sdf also the (n, dim, dim, dim) grids (NaN where there is none).  pairs (with voxels_dim): one entry
         per object, pairs[i] = j and pairs[j] = i for the two hypotheses i < j of a mono detection, -1 otherwise."""
+        n = len(objs)
+        arr, m, g, spec, keep = self._keyframe_args(objs, modes, gates, voxels_dim, pairs)
+        out = (_lib.ObjectOut * n)()
+        lib = _lib.load()
+        if voxels_dim is not None:
+            nv, nf = (C.c_int32 * n)(), (C.c_int32 * n)()
+            _lib.check(lib.dspgn_keyframe_batch_meshed(self.handle, n, arr, m, g, C.byref(spec), out, nv, nf))
+            self.n_obj = n
+            return self._meshed(out, n, int(voxels_dim), nv, nf, want_sdf)
+        if g is None:
+            _lib.check(lib.dspgn_keyframe_batch(self.handle, n, arr, m, out))
+        else:
+            _lib.check(lib.dspgn_keyframe_batch_gated(self.handle, n, arr, m, g, out))
+        self.n_obj = n
+        return out
+
+    def _keyframe_args(self, objs, modes, gates, voxels_dim, pairs):
+        """The C arguments of a keyframe call: (objects, modes, gates or None, mesh spec or None, arrays to keep alive)."""
         m = _modes_array(modes)
         n = len(objs)
         if len(m) != n:
@@ -277,7 +295,6 @@ class BatchSolver:
         if pairs is not None and len(pairs) != n:
             raise ValueError(f"{len(pairs)} pairs for {n} objects")
         arr, keep = self._pack(objs)
-        out = (_lib.ObjectOut * n)()
         g = None
         if gates is not None:
             g = (_lib.GateIn * n)()
@@ -290,25 +307,62 @@ class BatchSolver:
                 g[i].t_cam_obj_map = Tm.ctypes.data_as(_FP); g[i].map_rs = 4; g[i].map_cs = 1
                 g[i].t_cam_obj_sim3 = Ts.ctypes.data_as(_FP); g[i].sim3_rs = 4; g[i].sim3_cs = 1
                 g[i].gate = 1
-        lib = _lib.load()
+        spec = None
         if voxels_dim is not None:
             spec = _lib.MeshSpec()
             spec.voxels_dim = int(voxels_dim)
             pr = None if pairs is None else (C.c_int32 * n)(*[-1 if p is None else int(p) for p in pairs])
             spec.pair = pr
-            nv, nf = (C.c_int32 * n)(), (C.c_int32 * n)()
-            _lib.check(lib.dspgn_keyframe_batch_meshed(self.handle, n, arr, m, g, C.byref(spec), out, nv, nf))
+            keep.append(pr)
+        return arr, m, g, spec, keep
+
+    def _meshed(self, out, n, dim, nv, nf, want_sdf):
+        res = self._mesh_results(n, dim, nv, nf, want_sdf)
+        meshes, sdf = res if want_sdf else (res, None)
+        meshes = [mm if out[i].mesh == _lib.MESH_DONE else None for i, mm in enumerate(meshes)]
+        return (out, meshes, sdf) if want_sdf else (out, meshes)
+
+    # non-blocking keyframe call ----------------------------------------------------------------
+    def keyframe_submit(self, objs, modes, gates=None, voxels_dim=None, pairs=None):
+        """keyframe() split in two (dspgn_keyframe_submit): enqueue the call and return without waiting for the device.
+        Every input array may change as soon as this returns.  Collect with keyframe_wait(); until then every other
+        library call on this solver raises DspgnError with code _lib.E_BUSY."""
+        n = len(objs)
+        arr, m, g, spec, keep = self._keyframe_args(objs, modes, gates, voxels_dim, pairs)
+        _lib.check(_lib.load().dspgn_keyframe_submit(self.handle, n, arr, m, g, None if spec is None else C.byref(spec)))
+        self._flight = (n, voxels_dim)
+
+    def keyframe_query(self):
+        """True once the submitted call has finished (never blocks)."""
+        rc = _lib.load().dspgn_keyframe_query(self.handle)
+        if rc < 0:
+            _lib.check(rc)
+        return rc == 1
+
+    def keyframe_wait(self, want_sdf=False):
+        """Block (without the GIL) until the submitted call has finished; returns what keyframe() returns for it."""
+        n, voxels_dim = self._flight
+        self._flight = None
+        out = (_lib.ObjectOut * n)()
+        lib = _lib.load()
+        if voxels_dim is None:
+            _lib.check(lib.dspgn_keyframe_wait(self.handle, out, None, None))
             self.n_obj = n
-            res = self._mesh_results(n, int(voxels_dim), nv, nf, want_sdf)
-            meshes, sdf = res if want_sdf else (res, None)
-            meshes = [mm if out[i].mesh == _lib.MESH_DONE else None for i, mm in enumerate(meshes)]
-            return (out, meshes, sdf) if want_sdf else (out, meshes)
-        if g is None:
-            _lib.check(lib.dspgn_keyframe_batch(self.handle, n, arr, m, out))
-        else:
-            _lib.check(lib.dspgn_keyframe_batch_gated(self.handle, n, arr, m, g, out))
+            return out
+        nv, nf = (C.c_int32 * n)(), (C.c_int32 * n)()
+        _lib.check(lib.dspgn_keyframe_wait(self.handle, out, nv, nf))
         self.n_obj = n
-        return out
+        return self._meshed(out, n, int(voxels_dim), nv, nf, want_sdf)
+
+    def host_syncs(self):
+        """dspgn_debug_host_syncs: how often the solver's calls have blocked the calling thread on the device."""
+        v = C.c_int64()
+        _lib.check(_lib.load().dspgn_debug_host_syncs(self.handle, C.byref(v)))
+        return v.value
+
+    def set_mesh_arena(self, max_vertices=0, max_faces=0):
+        """Test hook (dspgn_debug_mesh_arena): the mesh arena of later submits; 0, 0 = automatic."""
+        _lib.check(_lib.load().dspgn_debug_mesh_arena(self.handle, int(max_vertices), int(max_faces)))
 
     def decode_sdf(self, code, x, class_id=0):
         x = _f32(x)
@@ -406,6 +460,50 @@ def _unpack_all(out, n, code_len):
     return records_to_results(rec, code_len)
 
 
+class KeyframeFuture(object):
+    """The outcome of Optimizer.keyframe_batch_async / reconstruct_mono_batch_async: the library call runs on the device
+    while the caller does other work.  done() never blocks; result() blocks with the GIL released and returns exactly
+    what the blocking method returns.  Like the reference surface, result() never raises: a call-level failure (which
+    the blocking method would raise) is logged once on stderr and every object comes back failed."""
+
+    def __init__(self, owner, finish, failed, label):
+        self._owner, self._finish, self._failed, self._label = owner, finish, failed, label
+        self._settled = owner is None
+        self._value = None
+
+    @classmethod
+    def resolved(cls, value):
+        f = cls(None, None, None, None)
+        f._value = value
+        return f
+
+    def done(self):
+        if self._settled:
+            return True
+        try:
+            return self._owner.solver.keyframe_query()
+        except Exception:                 # noqa: BLE001 -- result() reports it
+            return True
+
+    def result(self):
+        self._settle()
+        return self._value
+
+    def _settle(self):
+        if self._settled:
+            return
+        self._settled = True
+        owner = self._owner
+        if getattr(owner, "_pending", None) is self:
+            owner._pending = None
+        try:
+            self._value = self._finish(owner.solver.keyframe_wait())
+        except Exception as e:            # noqa: BLE001 -- see the class comment
+            _warn_once((self._label, type(e).__name__), f"{self._label} failed softly: {e!r}")
+            self._value = self._failed()
+        self._owner = self._finish = self._failed = None
+
+
 class Optimizer(object):
     """Drop-in for reconstruct.optimizer.Optimizer (reconstruct/optimizer.py:26-203)."""
 
@@ -446,6 +544,24 @@ class Optimizer(object):
         c.schedule = {None: _lib.SCHED_AUTO, "auto": _lib.SCHED_AUTO, "launches": _lib.SCHED_LAUNCHES,
                       "persistent": _lib.SCHED_PERSISTENT}[schedule]
         self.solver = BatchSolver(self._dev_decoders, c, device)
+        self._pending = None
+
+    def _collect(self):
+        """A method called while a KeyframeFuture is outstanding collects it first (the solver has one call in flight)."""
+        f = getattr(self, "_pending", None)
+        if f is not None:
+            f._settle()
+
+    def _submit(self, label, objs, modes, gates, voxels_dim, pairs, finish, failed):
+        """Submit one keyframe call and return its KeyframeFuture (a failure to submit is a settled, failed future)."""
+        self._collect()
+        try:
+            self.solver.keyframe_submit(objs, modes, gates, voxels_dim=voxels_dim, pairs=pairs)
+        except Exception as e:            # noqa: BLE001 -- see KeyframeFuture
+            _warn_once((label, type(e).__name__), f"{label} failed softly: {e!r}")
+            return KeyframeFuture.resolved(failed())
+        self._pending = KeyframeFuture(self, finish, failed, label)
+        return self._pending
 
     # -- reference surface --------------------------------------------------------------------
     # These three are called from C++ through pybind11 with no handler above them
@@ -459,6 +575,7 @@ class Optimizer(object):
     def reconstruct_object(self, t_cam_obj, pts, rays, depth, code=None):
         """optimizer.py:88-203.  Returns ResultDict(t_cam_obj (4,4) f32 | None, code (L,) f32 | None,
         is_good, loss)."""
+        self._collect()
         try:
             out = self.solver.reconstruct([dict(t_cam_obj=t_cam_obj, pts=pts, rays=rays, depth=depth,
                                                 code=None if code is None else np.asarray(code)[:self.code_len])])
@@ -472,6 +589,7 @@ class Optimizer(object):
         The C++ caller casts the return value to Eigen::Matrix4f unconditionally
         (src/LocalMapping_util.cc:109-110), so a failed optimisation (non-finite residuals, singular system,
         unusable input) returns the INPUT pose unchanged (logged once) instead of garbage or an exception."""
+        self._collect()
         try:
             T0 = np.array(t_co_se3, dtype=np.float32).reshape(4, 4)
         except Exception as e:            # noqa: BLE001
@@ -497,6 +615,7 @@ class Optimizer(object):
         voxels_dim: the same call also meshes every good result (CreateNewMapObjects, src/LocalMapping_util.cc:179-196):
         its ResultDict carries vertices (V,3) f32 and faces (F,3) int32 exactly as MeshExtractor(voxels_dim)
         .extract_meshes returns them for its code."""
+        self._collect()
         try:
             if voxels_dim is None:
                 out = self.solver.reconstruct(objs)
@@ -517,6 +636,38 @@ class Optimizer(object):
         t_cam_obj_flipped (the map pose turned 180 degrees about y) runs both hypotheses and keeps the flipped one iff
         loss(map pose) > loss(flipped).  Returns one ResultDict per dict: the kept result plus `flipped` (bool); with
         voxels_dim the kept good result also carries vertices and faces, decided and meshed on the device."""
+        self._collect()
+        run, pairs, first = self._mono_run(objs)
+        if not run:
+            return []
+        if voxels_dim is None:
+            res = _unpack_all(self.solver.reconstruct(run), len(run), self.code_len)
+        else:
+            out, meshes = self.solver.keyframe(run, [_lib.MODE_JOINT] * len(run), voxels_dim=voxels_dim, pairs=pairs)
+            res = _with_meshes(_unpack_all(out, len(run), self.code_len), meshes)
+        return self._mono_kept(res, pairs, first)
+
+    def reconstruct_mono_batch_async(self, objs, voxels_dim=None):
+        """reconstruct_mono_batch without waiting for the device: returns a KeyframeFuture whose result() is what
+        reconstruct_mono_batch(objs, voxels_dim) returns.  The arrays of objs may change as soon as this returns."""
+        run, pairs, first = self._mono_run(objs)
+        if not run:
+            return KeyframeFuture.resolved([])
+
+        def finish(ret):
+            out, meshes = (ret, None) if voxels_dim is None else ret
+            res = _unpack_all(out, len(run), self.code_len)
+            return self._mono_kept(res if meshes is None else _with_meshes(res, meshes), pairs, first)
+
+        def failed():
+            return [ResultDict(self._failed(), flipped=False) for _ in first]
+
+        return self._submit("reconstruct_mono_batch_async", run, [_lib.MODE_JOINT] * len(run), None, voxels_dim,
+                            None if voxels_dim is None else pairs, finish, failed)
+
+    @staticmethod
+    def _mono_run(objs):
+        """The hypotheses of the mono dicts: (run, pairs, index of each dict's map-pose hypothesis)."""
         run, pairs, first = [], [], []
         for o in objs:
             first.append(len(run))
@@ -527,13 +678,10 @@ class Optimizer(object):
                 run.append(dict(o, t_cam_obj=o["t_cam_obj_flipped"]))
                 pairs[i] = i + 1
                 pairs.append(i)
-        if not run:
-            return []
-        if voxels_dim is None:
-            res = _unpack_all(self.solver.reconstruct(run), len(run), self.code_len)
-        else:
-            out, meshes = self.solver.keyframe(run, [_lib.MODE_JOINT] * len(run), voxels_dim=voxels_dim, pairs=pairs)
-            res = _with_meshes(_unpack_all(out, len(run), self.code_len), meshes)
+        return run, pairs, first
+
+    @staticmethod
+    def _mono_kept(res, pairs, first):
         kept = []
         for i in first:
             j = pairs[i]
@@ -546,6 +694,7 @@ class Optimizer(object):
     def estimate_pose_batch(self, objs, return_status=False):
         """Batched estimate_pose_cam_obj.  Failed objects keep their input pose; return_status=True also returns
         the per-object DSPGN_ST_* codes so that a native caller can skip them."""
+        self._collect()
         out = self.solver.estimate_pose(objs)
         Ts, st = [], []
         for i, o in enumerate(objs):
@@ -570,20 +719,54 @@ class Optimizer(object):
 
         voxels_dim: the same call also meshes every good new object and every good rejected detection: their
         ResultDicts carry vertices (V,3) f32 and faces (F,3) int32 (dspgn_keyframe_batch_meshed)."""
+        self._collect()
+        objs, modes, gates, gated = self._keyframe_inputs(new_objects, tracked_objects)
+        if not objs:
+            return ([], [], []) if return_status else ([], [])
+        meshes = None
+        if voxels_dim is None:
+            out = self.solver.keyframe(objs, modes, gates)
+        else:
+            out, meshes = self.solver.keyframe(objs, modes, gates, voxels_dim=voxels_dim)
+        return self._keyframe_outputs(out, meshes, new_objects, tracked_objects, gated, return_status)
+
+    def keyframe_batch_async(self, new_objects, tracked_objects, voxels_dim=None, return_status=False):
+        """keyframe_batch without waiting for the device: returns a KeyframeFuture whose result() is what
+        keyframe_batch(new_objects, tracked_objects, return_status, voxels_dim) returns.  Every input (detections,
+        poses, codes, the map's predictions) is read before this returns; the arrays may change afterwards."""
+        objs, modes, gates, gated = self._keyframe_inputs(new_objects, tracked_objects)
+        if not objs:
+            return KeyframeFuture.resolved(([], [], []) if return_status else ([], []))
+        new_objects, tracked_objects = list(new_objects), list(tracked_objects)
+        poses = [np.array(o["t_cam_obj"], dtype=np.float32).reshape(4, 4) for o in tracked_objects]
+
+        def finish(ret):
+            out, meshes = (ret, None) if voxels_dim is None else ret
+            # the failed-pose fallback returns the input pose as it was at submit time
+            tracked = [dict(t_cam_obj=T) for T in poses]
+            return self._keyframe_outputs(out, meshes, new_objects, tracked, gated, return_status)
+
+        def failed():
+            ret = ([self._failed() for _ in new_objects], [T.copy() for T in poses])
+            ret = ret + ([-1] * len(poses),) if return_status else ret
+            return ret + ([None] * len(poses),) if gated else ret
+
+        return self._submit("keyframe_batch_async", objs, modes, gates, voxels_dim, None, finish, failed)
+
+    def _keyframe_inputs(self, new_objects, tracked_objects):
+        """The one call of a keyframe: (objects, modes, gates or None, whether any tracked object is gated)."""
         objs = list(new_objects) + list(tracked_objects)
         n_new = len(new_objects)
         gate_keys = ("t_cam_obj_map", "t_cam_obj_sim3", "rays", "depth")
         gates = [dict(t_cam_obj_map=o["t_cam_obj_map"], t_cam_obj_sim3=o["t_cam_obj_sim3"])
                  if all(o.get(k) is not None for k in gate_keys) else None for o in tracked_objects]
         gated = any(g is not None for g in gates)
-        if not objs:
-            return ([], [], []) if return_status else ([], [])
         modes = [_lib.MODE_JOINT] * n_new + [_lib.MODE_POSE] * (len(objs) - n_new)
-        meshes = None
-        if voxels_dim is None:
-            out = self.solver.keyframe(objs, modes, [None] * n_new + gates if gated else None)
-        else:
-            out, meshes = self.solver.keyframe(objs, modes, [None] * n_new + gates if gated else None, voxels_dim=voxels_dim)
+        return objs, modes, [None] * n_new + gates if gated else None, gated
+
+    def _keyframe_outputs(self, out, meshes, new_objects, tracked_objects, gated, return_status):
+        """keyframe_batch's return value from the call's records (and meshes)."""
+        n_new = len(new_objects)
         results = _unpack_all(out, n_new, self.code_len) if n_new else []
         if meshes is not None:
             results = _with_meshes(results, meshes[:n_new])

@@ -21,6 +21,8 @@
  *       (ProcessDetectedObjects, :390-428)                       dspgn_keyframe_batch_meshed + dspgn_mesh_results
  *   loss_utils.decode_sdf        (reconstruct/loss_utils.py:51) dspgn_decode_sdf
  *   MeshExtractor.extract_mesh_from_code (optimizer.py:214)     dspgn_mesh_batch + dspgn_mesh_results
+ *   the same keyframe call, collected after LocalMapping's own   dspgn_keyframe_submit + dspgn_keyframe_wait
+ *       mapping steps (LocalMapping.cc:72-96)
  *   loss.compute_sdf_loss / compute_render_loss (loss.py:22,46) dspgn_debug_system (test hook)
  *
  * Conventions: every function returns 0 on success or a negative DSPGN_E_* code; per-object soft
@@ -50,6 +52,7 @@ extern "C" {
 #define DSPGN_E_NOGPU (-3)    /* no usable sm_90 device */
 #define DSPGN_E_ALLOC (-4)
 #define DSPGN_E_PEER (-5)     /* multi-GPU exchange: a peer never published its results (timeout) */
+#define DSPGN_E_BUSY (-6)     /* the solver has a submitted call that has not been collected */
 
 /* DspgnObjectOut.status (per-object soft failure = the reference's is_good=False exits) */
 #define DSPGN_ST_OK 0
@@ -248,6 +251,36 @@ typedef struct {
 int dspgn_keyframe_batch_meshed(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes /* or NULL */,
                                 const DspgnGateIn* gates /* or NULL */, const DspgnMeshSpec* mesh, DspgnObjectOut* out,
                                 int32_t* n_vertices, int32_t* n_faces /* n_obj entries each */);
+
+/* The meshed (or gated) keyframe call without blocking the calling thread: submit a keyframe's object work, do other
+ * work (LocalMapping's own mapping steps), collect the records and meshes afterwards.
+ *   submit  validates, packs every input into the solver's pinned staging, enqueues the upload, the run, the mesh passes
+ *           and asynchronous copies of the records, the mesh counts and the meshes into pinned memory, records an event
+ *           and returns.  It never waits for the device once the solver's buffers are large enough for the keyframe
+ *           (a call that grows one frees the old buffer, which waits).  Every input array may be freed or overwritten as
+ *           soon as it returns.  Arguments as dspgn_keyframe_batch_meshed; mesh = NULL is dspgn_keyframe_batch_gated,
+ *           modes = NULL: every object joint.  Scope: one resident chunk -- at most 1024 slots (a gated object takes
+ *           two) and at most 2^24 candidate grid rows (64 objects at 64^3); a larger keyframe returns DSPGN_E_ARG (the
+ *           blocking calls take any size).
+ *   query   1 when the submitted call has finished, 0 while it runs, < 0 on error; never blocks.
+ *   wait    blocks until the call has finished and writes what the blocking call writes: n_obj records, and with a mesh
+ *           spec n_vertices / n_faces (NULL iff the submit had no mesh spec); dspgn_mesh_results then returns the
+ *           meshes.  Records, counts and meshes are bit-identical to dspgn_keyframe_batch_meshed / _gated.
+ * One call in flight per solver: until wait, every other entry point on the solver returns DSPGN_E_BUSY (results_device
+ * and gather_device return NULL, gather_close does nothing) and leaves the call intact, except query, wait,
+ * dspgn_solver_sync, dspgn_solver_engine and dspgn_debug_host_syncs; dspgn_solver_destroy waits for the call first.
+ * Solvers on different streams may each have a call in flight.  The multi-GPU exchange does not apply. */
+int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes /* or NULL: all joint */,
+                          const DspgnGateIn* gates /* or NULL */, const DspgnMeshSpec* mesh /* or NULL */);
+int dspgn_keyframe_query(DspgnSolver* s);
+int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices, int32_t* n_faces);
+/* Debug: the number of times the solver's calls have blocked the calling thread on the device so far (stream and event
+ * synchronisations, counted only when the device still had work to finish). */
+int dspgn_debug_host_syncs(DspgnSolver* s, int64_t* out);
+/* Test hook: the mesh arena of the following submits holds max_vertices vertices and max_faces faces (both 0: the
+ * automatic size, a per-object estimate that grows with the meshes the solver has seen).  A keyframe whose meshes do not
+ * fit is meshed again at the exact size inside dspgn_keyframe_wait: slower, never different. */
+int dspgn_debug_mesh_arena(DspgnSolver* s, int64_t max_vertices, int64_t max_faces);
 
 /* Forward-only decode (loss_utils.decode_sdf): x (n,3) host, strides in elements -> sdf (n,) host. */
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n,
