@@ -1972,4 +1972,20 @@ int dspgn_tc_selftest(int device, int n_mma, int k_steps, const float* A, const 
   return 0;
 }
 
+#ifdef DSPGN_STALL_PROBE
+// probe build only (tools/tile_probe.py): copies the per-CTA cycle counters of the tensor-core tile loop into out
+// (kProbeCtas x 3 x kProbeSlots), then zeroes them when `reset`.  Returns the number of values.
+int dspgn_debug_stall_probe(int device, unsigned long long* out, int reset) {
+  CU(cudaSetDevice(device));
+  CU(cudaDeviceSynchronize());
+  constexpr size_t n = (size_t)kProbeCtas * 3 * kProbeSlots;
+  if (out) CU(cudaMemcpyFromSymbol(out, g_stall_probe, 8 * n));
+  if (reset) {
+    std::vector<unsigned long long> zero(n, 0ull);
+    CU(cudaMemcpyToSymbol(g_stall_probe, zero.data(), 8 * n));
+  }
+  return (int)n;
+}
+#endif
+
 }  // extern "C"

@@ -145,6 +145,30 @@ DSPGN_WGMMA(80, DSPGN_D40, DSPGN_ACC_OPS40, 40, 41, 42, 43, 44, 45, 40, 41, 42)
 
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
+// ---- cycle accounting of the tile (probe build only: -DDSPGN_STALL_PROBE, tools/tile_probe.py) ----------------------
+// Lane 0 of consumer warp 0 of each warpgroup and the producer lane add the clock64 cycles they spend in each part of
+// the tile loop to per-CTA counters: row 0 / 1 = consumer warpgroup 0 / 1, row 2 = producer.  The shipped library
+// compiles none of it.
+enum ProbeSlot {
+  PR_WFULL, PR_WGWAIT, PR_GEMM, PR_EPI, PR_PROLOGUE, PR_JTJ, PR_TILE_END, PR_SOLVE, PR_FIFO, PR_LOOP, PR_TILES, PR_SOLVES,
+  PR_WEMPTY, PR_POP, PR_PROD_LOOP, kProbeSlots = 16
+};
+constexpr int kProbeCtas = 256;
+#ifdef DSPGN_STALL_PROBE
+__device__ unsigned long long g_stall_probe[kProbeCtas * 3 * kProbeSlots];
+__device__ __forceinline__ void probe_add(int slot, unsigned long long v) {
+  if ((threadIdx.x & 127) == 0 && blockIdx.x < kProbeCtas)
+    atomicAdd(&g_stall_probe[(blockIdx.x * 3 + (threadIdx.x >> 7)) * kProbeSlots + slot], v);
+}
+#define DSPGN_PROBE_T(t0) const long long t0 = clock64()
+#define DSPGN_PROBE_ADD(slot, t0) probe_add(slot, (unsigned long long)(clock64() - (t0)))
+#define DSPGN_PROBE_COUNT(slot) probe_add(slot, 1ull)
+#else
+#define DSPGN_PROBE_T(t0)
+#define DSPGN_PROBE_ADD(slot, t0)
+#define DSPGN_PROBE_COUNT(slot)
+#endif
+
 // K-major, 128B-swizzled shared-memory matrix descriptor (sm90 GMMA descriptor):
 // start>>4 [0,14) | LBO>>4 [16,30) = 1 (unused for swizzled K-major) | SBO>>4 [32,46) = 64 (8 rows x 128 B) |
 // base offset [49,52) = 0 (1024 B aligned atoms) | layout [62,64) = 1 (SWIZZLE_128B)
@@ -205,6 +229,7 @@ struct TcSmemTail {
 };
 constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail);
 static_assert(kTcSmemBytes <= 227 * 1024, "tensor-core engine shared memory exceeds the 227 KB per block of sm_90");
+static_assert(offsetof(TcSmemTail, bias) % 8 == 0, "the hidden-layer epilogue reads bias column pairs as float2");
 
 // ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
 // 8-column block j = e >> 2 at row 16w + l/4 (+8 when e & 2), column 8j + 2(l%4) + (e & 1).
@@ -264,7 +289,9 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[
       const uint32_t ph = phase ^ (uint32_t)(c & 1);
 #pragma unroll
       for (int s = 0; s < kTcStages; ++s) {
+        DSPGN_PROBE_T(tf);
         mbar_wait(w_full + 8u * s, ph);
+        DSPGN_PROBE_ADD(PR_WFULL, tf);
         wg_fence();
         const uint32_t bw = ring + (uint32_t)s * kTcStageBytes;
 #pragma unroll
@@ -276,18 +303,24 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[
         }
         wg_commit();
         if (s == 1) {
+          DSPGN_PROBE_T(tw);
           wg_wait1();
+          DSPGN_PROBE_ADD(PR_WGWAIT, tw);
           release_stage(w_empty, 0);
           if (c > 0) release_stage(w_empty, 3);
         } else if (s == 3) {
+          DSPGN_PROBE_T(tw);
           wg_wait1();
+          DSPGN_PROBE_ADD(PR_WGWAIT, tw);
           release_stage(w_empty, 1);
           release_stage(w_empty, 2);
         }
       }
     }
   }
+  DSPGN_PROBE_T(tw);
   wg_wait0();
+  DSPGN_PROBE_ADD(PR_WGWAIT, tw);
   release_stage(w_empty, 3);
   phase ^= (uint32_t)(nch & 1);
 }
@@ -297,7 +330,9 @@ __device__ __forceinline__ void produce_step(const unsigned char* src, int nch, 
                                              uint64_t* w_full, uint64_t* w_empty, uint32_t& phase) {
   for (int c = 0; c < nch; ++c) {
     for (int s = 0; s < kTcStages; ++s) {
+      DSPGN_PROBE_T(te);
       mbar_wait(&w_empty[s], phase ^ 1);
+      DSPGN_PROBE_ADD(PR_WEMPTY, te);
       mbar_expect_tx(&w_full[s], img_bytes);
       bulk_g2s(ring + (size_t)s * kTcStageBytes, src + (size_t)(kTcStages * c + s) * img_bytes, img_bytes, &w_full[s]);
     }
@@ -475,12 +510,15 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
     setmaxnreg_dec<kTcProducerRegs>();
     if (warp == 8 && lane == 0) {
       uint32_t phase = 0;
+      DSPGN_PROBE_T(tloop);
       for (int seq = 0;; ++seq) {
         if (MEGA) {
           // scheduler: fetch this CTA's next tile into the local FIFO (at most 3 entries ahead of the epilogue)
+          DSPGN_PROBE_T(tp);
           volatile int* es = &S.epi_seq;
           while (seq - *es >= 3) __nanosleep(64);   // the epilogue warps always make progress (bounded tile work)
           const int item = mega_pop(q, b.n_obj);
+          DSPGN_PROBE_ADD(PR_POP, tp);
           if (item >= 0) log_event(q.log, ev_desc(EV_POPPED, item >> kItemKindShift, (item >> kItemObjShift) & kItemObjMask, item & kItemTileMask));
           reinterpret_cast<volatile int*>(S.fifo)[seq & 3] = item;
           __threadfence_block();
@@ -498,6 +536,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           produce_step(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full,
                        S.w_empty, phase);
       }
+      DSPGN_PROBE_ADD(PR_PROD_LOOP, tloop);
     }
   } else {
     // ===================== consumer warpgroups =================================================
@@ -514,9 +553,13 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
     uint32_t phase = 0;
     float acc[128];
     uint32_t ah[64];
+    DSPGN_PROBE_T(tloop);
     for (int seq = 0;; ++seq) {
       TileRef tr;
+      DSPGN_PROBE_T(tq);
       if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
+      DSPGN_PROBE_ADD(PR_FIFO, tq);
+      DSPGN_PROBE_T(tpro);
       if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = seq + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
       if (RENDER && tr.mode == kKindScan) {
         // ---- scan item: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141); no GEMM steps ----------
@@ -690,6 +733,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         for (int w = 0; w < 4; ++w) maskw[w * kTcEpiThreads] = mw[w];
         store_operand(acc, ah, alo, rl, qd, grp);
       }
+      DSPGN_PROBE_ADD(PR_PROLOGUE, tpro);
+      DSPGN_PROBE_COUNT(PR_TILES);
 
       float yv = 0.f;
       for (int s = 0; s < ns; ++s) {
@@ -699,9 +744,12 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         const int nm = st.n_mma;
         if (MEGA && tid == 0 && s == 0) log_event(q.log, ev_desc(EV_FIRST_MMA, tr.mode, tr.o, tr.tile));
         const int nch = st.k_steps / 4;
+        DSPGN_PROBE_T(tg);
         if (nm == 80) wg_gemm<80>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
         else if (nm == 192) wg_gemm<192>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
         else wg_gemm<256>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
+        DSPGN_PROBE_ADD(PR_GEMM, tg);
+        DSPGN_PROBE_T(tepi);
         wg_bar_sync(grp);                                // every MMA of the warpgroup has read the A lo image
         const int qs = opaque_int(qd);
 
@@ -757,17 +805,35 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         } else if (st.kind == TK_FWD_HIDDEN) {
           const float* bb = S.bias + st.layer * kHid;
           uint32_t mw[4] = {0u, 0u, 0u, 0u};
+          if (SCHED == 1 && st.cat_off < 0) {
+            // SDF-tile kernel, every layer but the one before latent_in: the same values without a branch per element
+            // (the concat below makes the loop a chain of small blocks the scheduler cannot interleave), and the bias
+            // of the fragment's column pair 8j + 2q, +1 in one 8-byte load
 #pragma unroll
-          for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qs);
-            float t = 0.f;
-            if (c < nm) {
-              const float w = acc[e] + bb[c];
-              mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
-              t = fmaxf(w, 0.f);
+            for (int j = 0; j < 32; ++j) {
+              const float2 bj = *reinterpret_cast<const float2*>(bb + 8 * j + 2 * qs);
+#pragma unroll
+              for (int h = 0; h < 4; ++h) {
+                const int e = 4 * j + h, c = frag_col(e, qs);
+                const float w = acc[e] + ((h & 1) ? bj.y : bj.x);
+                const bool live = c < nm;
+                mw[e >> 5] |= ((live && w > 0.f) ? 1u : 0u) << (e & 31);
+                acc[e] = (live && c < k_next) ? fmaxf(w, 0.f) : 0.f;
+              }
             }
-            if (st.cat_off >= 0 && c >= st.cat_off) t = inp(c - st.cat_off, (e & 2) ? rowB : rowA);   // deep_sdf_decoder.py:87-88
-            acc[e] = (c < k_next) ? t : 0.f;
+          } else {
+#pragma unroll
+            for (int e = 0; e < 128; ++e) {
+              const int c = frag_col(e, qs);
+              float t = 0.f;
+              if (c < nm) {
+                const float w = acc[e] + bb[c];
+                mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
+                t = fmaxf(w, 0.f);
+              }
+              if (st.cat_off >= 0 && c >= st.cat_off) t = inp(c - st.cat_off, (e & 2) ? rowB : rowA);   // deep_sdf_decoder.py:87-88
+              acc[e] = (c < k_next) ? t : 0.f;
+            }
           }
 #pragma unroll
           for (int w = 0; w < 4; ++w) maskw[(4 * st.layer + w) * kTcEpiThreads] = mw[w];
@@ -776,20 +842,30 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           uint32_t mw[4];
 #pragma unroll
           for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
+          if (SCHED == 1 && st.cat_off < 0) {
+            // SDF-tile kernel, every layer but latent_in: the same values without a branch per element (as TK_FWD_HIDDEN)
 #pragma unroll
-          for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qs);
-            float t = 0.f;
-            if (c < nm) {
-              const float v = acc[e];
-              t = ((mw[e >> 5] >> (e & 31)) & 1u) ? v : 0.f;
-              if (st.cat_off >= 0 && c >= st.cat_off) {      // latent_in skip path -> d/d(input)
-                const int ii = c - st.cat_off;
-                if (ii < in0) S.Jp[((e & 2) ? rowB : rowA) * kJpStride + ((ii < L) ? ii : (kMaxCode + ii - L))] = v;
-                t = 0.f;
-              }
+            for (int e = 0; e < 128; ++e) {
+              const int c = frag_col(e, qs);
+              const bool on = c < nm && c < k_next && ((mw[e >> 5] >> (e & 31)) & 1u);
+              acc[e] = on ? acc[e] : 0.f;
             }
-            acc[e] = (c < k_next) ? t : 0.f;
+          } else {
+#pragma unroll
+            for (int e = 0; e < 128; ++e) {
+              const int c = frag_col(e, qs);
+              float t = 0.f;
+              if (c < nm) {
+                const float v = acc[e];
+                t = ((mw[e >> 5] >> (e & 31)) & 1u) ? v : 0.f;
+                if (st.cat_off >= 0 && c >= st.cat_off) {      // latent_in skip path -> d/d(input)
+                  const int ii = c - st.cat_off;
+                  if (ii < in0) S.Jp[((e & 2) ? rowB : rowA) * kJpStride + ((ii < L) ? ii : (kMaxCode + ii - L))] = v;
+                  t = 0.f;
+                }
+              }
+              acc[e] = (c < k_next) ? t : 0.f;
+            }
           }
           if (more) store_operand(acc, ah, alo, rl, qd, grp);
         } else {
@@ -812,7 +888,9 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
 #pragma unroll
           for (int i = 0; i < 64; ++i) ah[i] = 0u;
         }
+        DSPGN_PROBE_ADD(PR_EPI, tepi);
       }
+      DSPGN_PROBE_T(tjtj);
       if (!fwd_only) {
       // ---- pose columns, residual (thread = row; needs every d/d(input) column of the row) -----------
       epi_bar_sync();
@@ -891,7 +969,9 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         if (k == 0) { accp[kAccLoss] = sacc; accp[kAccLoss + 1] = n; }
       }
       }   // !fwd_only
+      DSPGN_PROBE_ADD(PR_JTJ, tjtj);
       if (MEGA) {
+        DSPGN_PROBE_T(tend);
         // ---- object pipeline.  Per object and iteration:  ray-sample tiles (forward only) -> [last one] per-ray scan +
         // band compaction -> band tiles (fwd+bwd) ;  SDF tiles (fwd+bwd) ;  [last SDF / band tile] solve, pose / code
         // update, tiles of the next iteration.  The CTA that finishes the last tile of a stage runs the serial step
@@ -916,10 +996,17 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
             mega_push(q, kKindScan, o, nch);
           }
         }
-        if (act == 2) mega_solve_and_advance(S, o, tid);
+        DSPGN_PROBE_ADD(PR_TILE_END, tend);
+        if (act == 2) {
+          DSPGN_PROBE_T(tsv);
+          mega_solve_and_advance(S, o, tid);
+          DSPGN_PROBE_ADD(PR_SOLVE, tsv);
+          DSPGN_PROBE_COUNT(PR_SOLVES);
+        }
       }
       // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
     }
+    DSPGN_PROBE_ADD(PR_LOOP, tloop);
   }
 }
 
