@@ -84,6 +84,21 @@ class IpcHandle(C.Structure):
     _fields_ = [("bytes", C.c_ubyte * IPC_HANDLE_BYTES)]
 
 
+class LidarSpec(C.Structure):
+    _fields_ = [("k", C.c_float * 9), ("inv_k", C.c_float * 9), ("t_cam_velo", C.c_float * 16),
+                ("img_h", C.c_int32), ("img_w", C.c_int32), ("num_lidar_max", C.c_int32),
+                ("min_mask_area", C.c_int32), ("downsample_ratio", C.c_int32), ("reserved_", C.c_int32)]
+
+
+class LidarBox(C.Structure):
+    _fields_ = [("t_obj_velo", C.c_float * 12), ("trans", C.c_float * 3), ("size", C.c_float * 3),
+                ("front", C.c_int32)]
+
+
+class LidarBoxOut(C.Structure):
+    _fields_ = [("n_pts", C.c_int32), ("n_rays", C.c_int32), ("mask", C.c_int32), ("n_selected", C.c_int32)]
+
+
 assert C.sizeof(ObjectOut) == 4 * RESULT_FLOATS
 
 # every symbol include/dspgn.h declares: (name, restype, argtypes)
@@ -140,6 +155,12 @@ SYMBOLS = [
     ("dspgn_debug_inputs", C.c_int, [_VP, C.c_int, _FP, _FP, _FP]),
     ("dspgn_debug_events", C.c_int, [_VP, C.POINTER(C.c_longlong), C.c_int]),
     ("dspgn_tc_selftest", C.c_int, [C.c_int, C.c_int, C.c_int, _FP, _FP, _FP]),
+    ("dspgn_lidar_frame_create", C.c_int, [C.POINTER(LidarSpec), C.c_int, C.POINTER(_VP)]),
+    ("dspgn_lidar_frame_destroy", None, [_VP]),
+    ("dspgn_lidar_frame_set_stream", C.c_int, [_VP, _VP]),
+    ("dspgn_lidar_frame_run", C.c_int, [_VP, _FP, C.c_int, C.POINTER(LidarBox), C.c_int, C.POINTER(C.c_uint8),
+                                        C.POINTER(C.c_int32), C.c_int, C.POINTER(LidarBoxOut)]),
+    ("dspgn_lidar_frame_results", C.c_int, [_VP, _FP, _FP, _FP]),
 ]
 
 _lib = None

@@ -16,6 +16,7 @@
 #include "dspgn_solve.cuh"
 #include "dspgn_tc.cuh"
 #include "dspgn_mesh.cuh"
+#include "dspgn_frame.cuh"
 
 using namespace dspgn;
 
@@ -1987,5 +1988,195 @@ int dspgn_debug_stall_probe(int device, unsigned long long* out, int reset) {
   return (int)n;
 }
 #endif
+
+}  // extern "C"
+
+// ---- LiDAR keyframe detections (dspgn_frame.cuh) ----
+
+struct DspgnLidarFrame {
+  int device = 0;
+  DspgnLidarSpec spec{};
+  cudaStream_t stream = nullptr;
+  cudaStream_t own = nullptr;  // the handle's non-blocking stream (the default), so LocalMapping's work never orders it
+  HostBuf h_in, h_out;        // pinned: staged inputs, downloaded outputs
+  DevBuf d_in, d_work, d_out;
+  int n_boxes = 0;            // of the last run
+  std::vector<DspgnLidarBoxOut> last;
+};
+
+namespace {
+
+size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+// the output block of a run: header, points [box][num_max][3], rays [box][num_max + 200][3]
+struct FrameOutLayout {
+  size_t hdr, pts, rays, bytes;
+  FrameOutLayout(int n_boxes, int num_max) {
+    hdr = 0;
+    pts = align16(4 * (size_t)n_boxes * kFrameHdr);
+    rays = pts + align16(12 * (size_t)n_boxes * num_max);
+    bytes = rays + 12 * (size_t)n_boxes * (num_max + kFrameBackground);
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+int dspgn_lidar_frame_create(const DspgnLidarSpec* spec, int device, DspgnLidarFrame** out) {
+  if (!spec || !out) return fail(DSPGN_E_ARG, "null argument");
+  if (spec->img_h < 1 || spec->img_h > 4096 || spec->img_w < 1 || spec->img_w > 4096) return fail(DSPGN_E_ARG, "image size must be in [1,4096]^2");
+  if (spec->num_lidar_max < 1 || spec->num_lidar_max > kFrameMaxLidar) return fail(DSPGN_E_ARG, "num_lidar_max must be in [1,4096]");
+  if (spec->downsample_ratio < 1) return fail(DSPGN_E_ARG, "downsample_ratio must be >= 1");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPGN_E_NOGPU, "no CUDA device"); }
+  if (device < 0 || device >= ndev) return fail(DSPGN_E_ARG, "bad device index");
+  CU(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CU(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only");
+  DspgnLidarFrame* f = new (std::nothrow) DspgnLidarFrame();
+  if (!f) return fail(DSPGN_E_ALLOC, "oom");
+  f->device = device;
+  f->spec = *spec;
+  if (cudaStreamCreateWithFlags(&f->own, cudaStreamNonBlocking) != cudaSuccess) {
+    cudaGetLastError();
+    delete f;
+    return fail(DSPGN_E_CUDA, "cudaStreamCreateWithFlags");
+  }
+  f->stream = f->own;
+  *out = f;
+  return 0;
+}
+
+void dspgn_lidar_frame_destroy(DspgnLidarFrame* f) {
+  if (!f) return;
+  cudaSetDevice(f->device);
+  cudaStreamSynchronize(f->stream);
+  f->h_in.release(); f->h_out.release();
+  f->d_in.release(); f->d_work.release(); f->d_out.release();
+  if (f->own) cudaStreamDestroy(f->own);
+  delete f;
+}
+
+int dspgn_lidar_frame_set_stream(DspgnLidarFrame* f, void* cuda_stream) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  f->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+  return 0;
+}
+
+int dspgn_lidar_frame_run(DspgnLidarFrame* f, const float* scan, int n_points, const DspgnLidarBox* boxes, int n_boxes,
+                          const uint8_t* masks, const int32_t* bboxes, int n_masks, DspgnLidarBoxOut* out) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  const DspgnLidarSpec& sp = f->spec;
+  if (n_points < 0 || n_points > (1 << 22)) return fail(DSPGN_E_ARG, "n_points must be in [0, 2^22]");
+  if (n_boxes < 0 || n_boxes > kFrameMaxBoxes) return fail(DSPGN_E_ARG, "n_boxes must be in [0, 256]");
+  if (n_masks < 0 || n_masks > kFrameMaxMasks) return fail(DSPGN_E_ARG, "n_masks must be in [0, 64]");
+  if ((n_points > 0 && !scan) || (n_boxes > 0 && (!boxes || !out)) || (n_masks > 0 && (!masks || !bboxes)))
+    return fail(DSPGN_E_ARG, "null pointer where data is required");
+  for (int m = 0; m < n_masks; ++m) {
+    const int32_t* bb = bboxes + 4 * m;
+    if (!(0 <= bb[0] && bb[0] <= bb[2] && bb[2] <= sp.img_w && 0 <= bb[1] && bb[1] <= bb[3] && bb[3] <= sp.img_h))
+      return fail(DSPGN_E_ARG, "bbox " + std::to_string(m) + " outside 0 <= l <= r <= img_w, 0 <= t <= b <= img_h");
+  }
+  CU(cudaSetDevice(f->device));
+  f->n_boxes = n_boxes;
+  f->last.assign(n_boxes, DspgnLidarBoxOut{0, -1, -1, 0});
+  if (n_boxes == 0) return 0;
+  // staged input block: boxes | bboxes | scan | masks (each mask padded to 16 bytes)
+  const size_t mstride = align16((size_t)sp.img_h * sp.img_w);
+  const size_t o_bb = align16(4 * (size_t)n_boxes * kFrameBoxWords);
+  const size_t o_scan = o_bb + align16(16 * (size_t)n_masks);
+  const size_t o_mask = o_scan + align16(16 * (size_t)n_points);
+  const size_t in_bytes = o_mask + mstride * n_masks;
+  const int n_chunks = (n_points + kFrameChunk - 1) / kFrameChunk;
+  const size_t o_tot = align16(4 * (size_t)n_boxes * std::max(n_chunks, 1));
+  const size_t o_area = o_tot + align16(4 * (size_t)n_boxes);
+  const size_t work_bytes = o_area + 4 * (size_t)kFrameMaxMasks;
+  const FrameOutLayout L(n_boxes, sp.num_lidar_max);
+  if (f->h_in.reserve(in_bytes) || f->h_out.reserve(L.bytes)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
+  if (f->d_in.reserve(in_bytes) || f->d_work.reserve(work_bytes) || f->d_out.reserve(L.bytes)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
+  unsigned char* h = f->h_in.as<unsigned char>();
+  float* hb = reinterpret_cast<float*>(h);
+  for (int b = 0; b < n_boxes; ++b) {
+    float* w = hb + (size_t)b * kFrameBoxWords;
+    memcpy(w, boxes[b].t_obj_velo, 12 * sizeof(float));
+    memcpy(w + 12, boxes[b].trans, 3 * sizeof(float));
+    memcpy(w + 15, boxes[b].size, 3 * sizeof(float));
+    const int32_t front = boxes[b].front != 0;
+    memcpy(w + 18, &front, 4);
+    w[19] = 0.f;
+  }
+  if (n_masks) memcpy(h + o_bb, bboxes, 16 * (size_t)n_masks);
+  if (n_points) memcpy(h + o_scan, scan, 16 * (size_t)n_points);
+  const size_t hw = (size_t)sp.img_h * sp.img_w;
+  for (int m = 0; m < n_masks; ++m) {
+    memcpy(h + o_mask + m * mstride, masks + m * hw, hw);
+    memset(h + o_mask + m * mstride + hw, 0, mstride - hw);
+  }
+  FrameParams P{};
+  memcpy(P.K, sp.k, sizeof(P.K));
+  memcpy(P.inv_k, sp.inv_k, sizeof(P.inv_k));
+  memcpy(P.tcv, sp.t_cam_velo, sizeof(P.tcv));
+  P.img_h = sp.img_h; P.img_w = sp.img_w; P.num_max = sp.num_lidar_max; P.min_area = sp.min_mask_area;
+  P.alpha = sp.downsample_ratio; P.n_pts = n_points; P.n_boxes = n_boxes; P.n_masks = n_masks; P.n_chunks = n_chunks;
+  P.mask_stride = (long long)mstride;
+  unsigned char* d = f->d_in.as<unsigned char>();
+  const float* d_boxes = reinterpret_cast<const float*>(d);
+  const int* d_bb = reinterpret_cast<const int*>(d + o_bb);
+  const float4* d_scan = reinterpret_cast<const float4*>(d + o_scan);
+  const unsigned char* d_masks = d + o_mask;
+  unsigned char* wk = f->d_work.as<unsigned char>();
+  int* d_cnt = reinterpret_cast<int*>(wk);
+  int* d_tot = reinterpret_cast<int*>(wk + o_tot);
+  int* d_area = reinterpret_cast<int*>(wk + o_area);
+  unsigned char* o = f->d_out.as<unsigned char>();
+  int* d_hdr = reinterpret_cast<int*>(o + L.hdr);
+  float* d_pts = reinterpret_cast<float*>(o + L.pts);
+  float* d_rays = reinterpret_cast<float*>(o + L.rays);
+  cudaStream_t st = f->stream;
+  CU(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
+  const int sel_blocks = std::max((n_chunks + kFrameWarps - 1) / kFrameWarps, 1);
+  k_frame_select<0><<<sel_blocks, kFrameWarps * 32, 0, st>>>(P, d_boxes, d_scan, d_cnt, d_tot, d_pts);
+  k_frame_scan_area<<<n_boxes + n_masks, 1024, 0, st>>>(P, d_cnt, d_tot, d_hdr, d_masks, d_area);
+  k_frame_select<1><<<sel_blocks, kFrameWarps * 32, 0, st>>>(P, d_boxes, d_scan, d_cnt, d_tot, d_pts);
+  k_frame_box<<<n_boxes, kFrameBoxThreads, 0, st>>>(P, d_boxes, d_pts, d_masks, d_bb, d_area, d_hdr, d_rays);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(f->h_out.p, o, L.bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const int* hh = f->h_out.as<int>();
+  for (int b = 0; b < n_boxes; ++b) {
+    DspgnLidarBoxOut r;
+    r.n_pts = hh[b * kFrameHdr + 0];
+    r.n_rays = hh[b * kFrameHdr + 1];
+    r.mask = hh[b * kFrameHdr + 2];
+    r.n_selected = hh[b * kFrameHdr + 3];
+    f->last[b] = r;
+    out[b] = r;
+  }
+  return 0;
+}
+
+int dspgn_lidar_frame_results(DspgnLidarFrame* f, float* points, float* depth, float* rays) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  const int num_max = f->spec.num_lidar_max;
+  const FrameOutLayout L(f->n_boxes, num_max);
+  const unsigned char* h = f->h_out.as<unsigned char>();
+  size_t np_ = 0, nr = 0;
+  for (int b = 0; b < f->n_boxes; ++b) {
+    const DspgnLidarBoxOut& r = f->last[b];
+    const float* p = reinterpret_cast<const float*>(h + L.pts) + (size_t)b * num_max * 3;
+    if (points) memcpy(points + 3 * np_, p, 12 * (size_t)r.n_pts);
+    if (depth)
+      for (int i = 0; i < r.n_pts; ++i) depth[np_ + i] = p[3 * i + 2];
+    np_ += r.n_pts;
+    if (r.n_rays > 0) {
+      const float* q = reinterpret_cast<const float*>(h + L.rays) + (size_t)b * (num_max + kFrameBackground) * 3;
+      if (rays) memcpy(rays + 3 * nr, q, 12 * (size_t)r.n_rays);
+      nr += r.n_rays;
+    }
+  }
+  return 0;
+}
 
 }  // extern "C"

@@ -102,3 +102,67 @@ def make_batch(n_obj, n_pts, n_fg_rays=None, n_bg_rays=0, cls="cars", seed0=0, *
     clss = cls if isinstance(cls, (list, tuple)) else [cls] * n_obj
     return [make_object(seed0 + i, n_pts, n_fg_rays, n_bg_rays, cls=clss[i], **kw)
             for i in range(n_obj)]
+
+
+KITTI_K = np.array([[721.5377, 0.0, 609.5593], [0.0, 721.5377, 172.854], [0.0, 0.0, 1.0]], F32)
+KITTI_T_CAM_VELO = np.array([[0.000427, -0.999967, -0.008084, 0.048489], [-0.007211, 0.008081, -0.999941, -0.073220],
+                             [0.999974, 0.000485, -0.007206, -0.333997], [0.0, 0.0, 0.0, 1.0]], F32)
+
+
+def make_lidar_frame(seed, n_points=127000, n_boxes=20, n_masks=10, img_hw=(375, 1242)):
+    """A KITTI-sized LiDAR keyframe as FrameWithLiDAR.get_detections receives it (kitti_sequence.py:99-216):
+    scan (n, 4) f32 with dense clusters inside the boxes, boxes (k, 7) f32 (x, y, z, w, l, h, theta, velodyne frame),
+    masks (m, H, W) bool over the projections of the nearest front boxes (one pair shares a mask, one mask misses),
+    bboxes (m, 4) f32 clipped to the image."""
+    rng = np.random.default_rng(seed)
+    H, W = img_hw
+    x = rng.uniform(-15, 45, n_boxes)
+    y = rng.uniform(-12, 12, n_boxes)
+    size = np.stack([rng.uniform(1.4, 2.0, n_boxes), rng.uniform(3.4, 4.8, n_boxes), rng.uniform(1.3, 1.8, n_boxes)], -1)
+    th = rng.uniform(-np.pi, np.pi, n_boxes)
+    dets = np.concatenate([np.stack([x, y, np.full(n_boxes, -1.7)], -1), size, th[:, None]], -1)
+    cl, per_box = [], []
+    n_dense = int(n_points * 0.25)
+    counts = rng.multinomial(n_dense, rng.dirichlet(np.ones(n_boxes)))
+    for b in range(n_boxes):
+        o = (rng.random((counts[b], 3)) - 0.5) * np.array([size[b, 0], size[b, 2], size[b, 1]]) * 1.05
+        c, s = np.cos(th[b]), np.sin(th[b])
+        R = np.array([[c, 0, -s], [-s, 0, -c], [0, 1, 0]])
+        p = o @ R.T + np.array([x[b], y[b], -1.7 + size[b, 2] / 2])
+        cl.append(p)
+        per_box.append(p)
+    n_bg = n_points - n_dense
+    bg = np.stack([rng.uniform(-40, 60, n_bg), rng.uniform(-30, 30, n_bg), rng.uniform(-2.5, 1.0, n_bg)], -1)
+    pts = np.concatenate([bg] + cl, 0)
+    pts = pts[rng.permutation(pts.shape[0])]
+    scan = np.concatenate([pts, rng.random((pts.shape[0], 1))], -1).astype(F32)
+    # masks over the projected clusters of the front boxes, nearest first
+    T = KITTI_T_CAM_VELO.astype(np.float64)
+    K = KITTI_K.astype(np.float64)
+    rects = []
+    for b in np.argsort(x):
+        pc = per_box[b] @ T[:3, :3].T + T[:3, 3]
+        pc = pc[pc[:, 2] > 0.5]
+        if pc.shape[0] < 10:
+            continue
+        uv = (pc @ K.T)[:, :2] / (pc @ K.T)[:, 2:3]
+        u0, v0 = np.clip(uv.min(0), 0, [W, H])
+        u1, v1 = np.clip(uv.max(0), 0, [W, H])
+        if u1 - u0 > 2 and v1 - v0 > 2:
+            rects.append((u0, v0, u1, v1))
+    masks = np.zeros((n_masks, H, W), bool)
+    bboxes = np.zeros((n_masks, 4), F32)
+    for m in range(n_masks):
+        if m < len(rects) and m != n_masks - 1:
+            u0, v0, u1, v1 = rects[m]
+            if m == 1 and len(rects) > 2:          # one mask covering two boxes
+                u0, v0 = min(u0, rects[2][0]), min(v0, rects[2][1])
+                u1, v1 = max(u1, rects[2][2]), max(v1, rects[2][3])
+        else:                                      # a mask where no box projects
+            u0, v0 = rng.uniform(0, W - 60), rng.uniform(0, H - 40)
+            u1, v1 = u0 + 50, v0 + 30
+        masks[m, int(v0):int(np.ceil(v1)), int(u0):int(np.ceil(u1))] = True
+        bboxes[m] = np.clip([u0 - rng.uniform(0, 30), v0 - rng.uniform(0, 15), u1 + rng.uniform(0, 30), v1 + rng.uniform(0, 15)],
+                            0, [W, H, W, H])
+    return dict(scan=scan, dets=dets.astype(F32), masks=masks, bboxes=bboxes, K=KITTI_K, T_cam_velo=KITTI_T_CAM_VELO,
+                img_hw=(H, W))

@@ -370,6 +370,60 @@ int dspgn_debug_inputs(DspgnSolver* s, int obj, float* t_cam_obj, float* pts, fl
  * tools/mega_timeline.py decodes it. */
 int dspgn_debug_events(DspgnSolver* s, long long* out, int max_events);
 
+/* ---- A KITTI LiDAR keyframe's detections (FrameWithLiDAR.get_detections, reconstruct/kitti_sequence.py:99-216),
+ * built on the device from the raw scan, the 3D boxes and the 2D masks.  Its own handle: Tracking builds detections
+ * in another thread than LocalMapping's solver calls (src/Tracking_util.cc:31-57), and a solver is one host thread.
+ * Per box (the caller keeps the boxes in depth order, np.argsort(detections_3d[:, 0])):
+ *   points  the scan points with x-3 < px < x+3 on all three axes (float32), transformed by t_obj_velo and strictly
+ *           inside +-1.1 w/2, +-h/2, +-1.1 l/2, in scan order; more than num_lidar_max of them are subsampled at the
+ *           ranks np.linspace(0, N-1, num_lidar_max).astype(int32); then transformed by T_cam_velo.
+ *   mask    front boxes of a frame with masks: the points projected with K (float32 division), the pixels strictly
+ *           inside the image truncated to int, one vote per pixel per mask containing it; the first mask with the
+ *           most votes matches iff votes > 0.5 * (pixels inside).
+ *   rays    a matched mask with area > min_mask_area: the background grid of its bbox (truncated, expanded by 5 px,
+ *           clamped; np.linspace(t, b, int(H/alpha)) x np.linspace(l, r, int(W/alpha)), row-major) outside the mask,
+ *           200 of them at np.linspace(0, n-1, 200) ranks when more, appended to the projected (u, v) of every point
+ *           (including those outside the image); rays = inv_k [u, v, 1] in float64, cast to float32.  depth = z.
+ * Every float step is rounded as numpy rounds it, so the arrays are bit-identical to the reference's.
+ *   run      validates (DSPGN_E_ARG before anything is enqueued), stages the scan and the masks in pinned memory, one
+ *            H2D copy, four kernels and one D2H copy on the handle's stream, then waits for that copy (the only host
+ *            synchronisation) and writes one DspgnLidarBoxOut per box.  Limits: scan <= 2^22 points, <= 256 boxes,
+ *            <= 64 masks, each bbox 0 <= l <= r <= img_w and 0 <= t <= b <= img_h after truncation.
+ *   results  the arrays of the last run, box after box: points (sum n_pts x 3), depth (sum n_pts), rays
+ *            (sum of n_rays > 0, x 3).  Any pointer may be NULL. */
+typedef struct DspgnLidarFrame DspgnLidarFrame;
+typedef struct {
+  float k[9];                 /* K (3x3 row-major, float32 as the loader casts it) */
+  float inv_k[9];             /* inv(K) as float32 */
+  float t_cam_velo[16];       /* 4x4 row-major */
+  int32_t img_h, img_w;       /* 1..4096 */
+  int32_t num_lidar_max;      /* 1..4096 */
+  int32_t min_mask_area;
+  int32_t downsample_ratio;   /* int(configs.downsample_ratio), >= 1 */
+  int32_t reserved_;
+} DspgnLidarSpec;
+typedef struct {
+  float t_obj_velo[12];       /* rows 0..2 of inv(T_velo_obj) (float32 LAPACK on the host) */
+  float trans[3];             /* box centre x, y, z (velodyne frame) */
+  float size[3];              /* w, l, h */
+  int32_t front;              /* T_cam_obj[2][3] > 0 as the caller computed T_cam_obj = T_cam_velo T_velo_obj */
+} DspgnLidarBox;
+typedef struct {
+  int32_t n_pts;              /* surface points after subsampling */
+  int32_t n_rays;             /* -1: no rays (None) */
+  int32_t mask;               /* matched mask index, -1: none */
+  int32_t n_selected;         /* points inside the box before subsampling */
+} DspgnLidarBoxOut;
+int dspgn_lidar_frame_create(const DspgnLidarSpec* spec, int device, DspgnLidarFrame** out);
+void dspgn_lidar_frame_destroy(DspgnLidarFrame* f);
+/* the handle enqueues on a non-blocking stream of its own; stream = a cudaStream_t replaces it (NULL = legacy default) */
+int dspgn_lidar_frame_set_stream(DspgnLidarFrame* f, void* cuda_stream);
+/* scan: n_points x 4 float32 (x, y, z, reflectance); masks: n_masks x img_h x img_w bytes (numpy bool, nonzero =
+ * inside); bboxes: n_masks x 4 int32 (l, t, r, b), the masks' boxes truncated like astype(int32) */
+int dspgn_lidar_frame_run(DspgnLidarFrame* f, const float* scan, int n_points, const DspgnLidarBox* boxes, int n_boxes,
+                          const uint8_t* masks, const int32_t* bboxes, int n_masks, DspgnLidarBoxOut* out);
+int dspgn_lidar_frame_results(DspgnLidarFrame* f, float* points, float* depth, float* rays);
+
 /* Test hook for the wgmma operand paths: D[128][n_mma] = A[128][16*k_steps] * B[n_mma][16*k_steps]^T
  * (A through the register / shared-memory split-fp16 path, B through the pre-swizzled shared-memory images). Host buffers. */
 int dspgn_tc_selftest(int device, int n_mma, int k_steps, const float* A, const float* B, float* D);
