@@ -148,11 +148,16 @@ __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;"
 // ---- cycle accounting of the tile (probe build only: -DDSPGN_STALL_PROBE, tools/tile_probe.py) ----------------------
 // Lane 0 of consumer warp 0 of each warpgroup and the producer lane add the clock64 cycles they spend in each part of
 // the tile loop to per-CTA counters: row 0 / 1 = consumer warpgroup 0 / 1, row 2 = producer.  The shipped library
-// compiles none of it.
+// compiles none of it.  The epilogue (PR_EPI) is split further: the barrier that opens it (PR_EPI_ENTRY), then per step
+// kind (EpiKind) three slots from PR_EPI_KIND + 3 * kind: the value loop, the split and stores of store_operand, and its
+// proxy fence + warpgroup barrier.
 enum ProbeSlot {
   PR_WFULL, PR_WGWAIT, PR_GEMM, PR_EPI, PR_PROLOGUE, PR_JTJ, PR_TILE_END, PR_SOLVE, PR_FIFO, PR_LOOP, PR_TILES, PR_SOLVES,
-  PR_WEMPTY, PR_POP, PR_PROD_LOOP, kProbeSlots = 16
+  PR_WEMPTY, PR_POP, PR_PROD_LOOP, PR_EPI_ENTRY, PR_EPI_KIND, kProbeSlots = PR_EPI_KIND + 3 * 6
 };
+// hidden forward, the same before latent_in (concat), last hidden layer, backward, the same at latent_in (skip gradient),
+// first layer backward
+enum EpiKind { EK_FWD, EK_FWD_CAT, EK_PENULT, EK_BWD, EK_BWD_SKIP, EK_BWD_FIRST };
 constexpr int kProbeCtas = 256;
 #ifdef DSPGN_STALL_PROBE
 __device__ unsigned long long g_stall_probe[kProbeCtas * 3 * kProbeSlots];
@@ -163,10 +168,12 @@ __device__ __forceinline__ void probe_add(int slot, unsigned long long v) {
 #define DSPGN_PROBE_T(t0) const long long t0 = clock64()
 #define DSPGN_PROBE_ADD(slot, t0) probe_add(slot, (unsigned long long)(clock64() - (t0)))
 #define DSPGN_PROBE_COUNT(slot) probe_add(slot, 1ull)
+#define DSPGN_PROBE_ADD_IF(cond, slot, t0) do { if (cond) DSPGN_PROBE_ADD(slot, t0); } while (0)
 #else
 #define DSPGN_PROBE_T(t0)
 #define DSPGN_PROBE_ADD(slot, t0)
 #define DSPGN_PROBE_COUNT(slot)
+#define DSPGN_PROBE_ADD_IF(cond, slot, t0)
 #endif
 
 // K-major, 128B-swizzled shared-memory matrix descriptor (sm90 GMMA descriptor):
@@ -244,8 +251,11 @@ __device__ __forceinline__ int opaque_int(int v) {
 
 // accumulator-shaped values -> A operand of the next GEMM step: hi halves into `ah` (the register A fragment of
 // K-step t is columns [16t, 16t+16) of the accumulator fragment), lo halves into this warpgroup's swizzled image.
-// Ends with the proxy fence and the warpgroup barrier the wgmma reads need.
-__device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&ah)[64], unsigned char* alo, int rl, int q, int grp) {
+// Ends with the proxy fence and the warpgroup barrier the wgmma reads need.  pslot: probe build only, the step kind's
+// first probe slot (PR_EPI_KIND + 3 * kind), or -1.
+__device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&ah)[64], unsigned char* alo, int rl, int q, int grp,
+                                              int pslot = -1) {
+  DSPGN_PROBE_T(ts);
 #pragma unroll
   for (int t = 0; t < 16; ++t) {
 #pragma unroll
@@ -258,8 +268,131 @@ __device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&
       *reinterpret_cast<uint32_t*>(alo + off) = lo;
     }
   }
+  DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 1, ts);
+  DSPGN_PROBE_T(tf);
   fence_proxy_async();
   wg_bar_sync(grp);
+  DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 2, tf);
+}
+
+// store_operand of the SDF-tile kernel: the same registers and bytes, the lo image written with 16 stmatrix.x4 instead of
+// 64 scalar stores.  The lo halves of K-step t form an m16k16 fragment whose four 8 x 8 matrices, (rows rl / rl + 8) x
+// (columns 16t.. / 16t+8..), are exactly the values h = 0..3 above; lane l gives the swizzled address of row l % 8 of
+// matrix l / 8.  In that row's 16-byte chunk  ((kk & 63) >> 3) ^ (row & 7)  the K-step enters only as 2(t & 3), so a lane
+// needs one base address and one xor per t.
+__device__ __forceinline__ void store_operand_stsm(const float (&v)[128], uint32_t (&ah)[64], uint32_t alo, int grp, int pslot = -1) {
+  DSPGN_PROBE_T(ts);
+  const int lane = threadIdx.x & 31;
+  const int srow = 16 * ((threadIdx.x >> 5) & 3) + (lane & 7) + 8 * ((lane >> 3) & 1);
+  const uint32_t base = alo + 128u * (uint32_t)srow;
+  const uint32_t xo = (uint32_t)(((lane >> 4) & 1) ^ (lane & 7)) << 4;
+#pragma unroll
+  for (int t = 0; t < 16; ++t) {
+    uint32_t lo[4];
+#pragma unroll
+    for (int h = 0; h < 4; ++h) split_pack(v[8 * t + 2 * h], v[8 * t + 2 * h + 1], ah[4 * t + h], lo[h]);
+    const uint32_t addr = base + 8192u * (uint32_t)(t >> 2) + (xo ^ (32u * (uint32_t)(t & 3)));
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(lo[0]), "r"(lo[1]),
+                 "r"(lo[2]), "r"(lo[3]) : "memory");
+  }
+  DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 1, ts);
+  DSPGN_PROBE_T(tf);
+  fence_proxy_async();
+  wg_bar_sync(grp);
+  DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 2, tf);
+}
+
+// ---- epilogue value loops of the SDF-tile kernel (k_gn_persistent).  They give the values of the general loops in
+// tc_body, element by element and in the same order, without a branch per element.  Fragment element e = 4j + h covers
+// columns 8j + 2q + (h & 1) with q < 4, and n_mma and k_next are multiples of 8: a column is below either bound iff 8j
+// is.  NM / KNEXT are the step's n_mma / k_next at compile time, so for the pairs the 8 x 256 decoders produce every live
+// / zero decision is fixed per j.  NM = KNEXT = 0 is the fallback for other pairs: the runtime values nm / k_next.
+// Steps with more to do than bias + ReLU or the mask run it as a separate pass over the fragment: folded into one loop,
+// the extra loads, stores and dot-product chain are scheduled across the whole fragment and the tile loop spills.
+template <int NM, int KNEXT>
+__device__ __forceinline__ void epi_fwd_hidden(float (&acc)[128], uint32_t (&mw)[4], const float* bb, int qs, int nm, int k_next) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const bool live = 8 * j < (NM ? NM : nm), nxt = 8 * j < (KNEXT ? KNEXT : k_next);
+    const float2 bj = *reinterpret_cast<const float2*>(bb + 8 * j + 2 * qs);
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int e = 4 * j + h;
+      const float w = acc[e] + ((h & 1) ? bj.y : bj.x);
+      mw[e >> 5] |= ((live && w > 0.f) ? 1u : 0u) << (e & 31);
+      acc[e] = (live && nxt) ? fmaxf(w, 0.f) : 0.f;
+    }
+  }
+}
+
+// the layer before latent_in, after epi_fwd_hidden: columns >= cat_off below k_next take the decoder input
+// [z | x | 0...] (deep_sdf_decoder.py:87-88), read from clamped shared-memory indices and selected.  Column blocks
+// below cat_off are skipped whole (a branch per block, not per element).
+__device__ __forceinline__ void epi_concat_input(float (&acc)[128], int qs, int k_next, int cat_off, int L, const float* zs,
+                                                 const float* xr, int rowA, int rowB) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    if (8 * j + 8 <= cat_off) continue;
+    const bool nxt = 8 * j < k_next;
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int e = 4 * j + h, i = 8 * j + 2 * qs + (h & 1) - cat_off, ix = i - L;
+      const float zv = zs[(unsigned)i < (unsigned)L ? i : 0];
+      const float xv = xr[((unsigned)ix < 3u ? ix : 0) * kTcRows + ((h & 2) ? rowB : rowA)];
+      acc[e] = (nxt && i >= 0) ? (i < L ? zv : ((unsigned)ix < 3u ? xv : 0.f)) : acc[e];
+    }
+  }
+}
+
+// the layer at latent_in, before epi_bwd_mid: the gradient of its skip columns (>= cat_off) goes to the Jacobian tile
+// (the first in0 of them, predicated stores) instead of to the next layer.  Column blocks below cat_off are skipped
+// whole.
+__device__ __forceinline__ void epi_skip_grad(float (&acc)[128], int qs, int nm, int cat_off, int in0, int L, float* Jp, int rowA,
+                                              int rowB) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    if (8 * j + 8 <= cat_off) continue;
+    const bool live = 8 * j < nm;
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int e = 4 * j + h, ii = 8 * j + 2 * qs + (h & 1) - cat_off;
+      if (live && ii >= 0 && ii < in0) Jp[((h & 2) ? rowB : rowA) * kJpStride + ((ii < L) ? ii : (kMaxCode + ii - L))] = acc[e];
+      acc[e] = (ii >= 0) ? 0.f : acc[e];
+    }
+  }
+}
+
+// backward through a hidden layer: the saved ReLU mask
+template <int NM, int KNEXT>
+__device__ __forceinline__ void epi_bwd_mid(float (&acc)[128], const uint32_t (&mw)[4], int nm, int k_next) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const bool live = 8 * j < (NM ? NM : nm), nxt = 8 * j < (KNEXT ? KNEXT : k_next);
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int e = 4 * j + h;
+      acc[e] = (live && nxt && ((mw[e >> 5] >> (e & 31)) & 1u)) ? acc[e] : 0.f;
+    }
+  }
+}
+
+// d/d(input) of the first layer: the Jacobian row, plus the skip gradient stored before (loss.py:34-41 / :143-150).
+// The step's wgmma N is always 80: tc_pack_decoder takes decoders with in0 <= 80 only, so the 10 column blocks below 80
+// are the whole fragment the step computes.
+__device__ __forceinline__ void epi_bwd_first(const float (&acc)[128], int qs, int in0, int L, bool has_skip, float* Jp,
+                                              const float* scr, int rowA, int rowB) {
+  const float sa = scr[rowA], sb = scr[rowB];
+#pragma unroll
+  for (int j = 0; j < 10; ++j) {
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int c = 8 * j + 2 * qs + (h & 1);
+      const bool st = c < in0;
+      float* pj = Jp + ((h & 2) ? rowB : rowA) * kJpStride + (st ? ((c < L) ? c : (kMaxCode + c - L)) : 0);
+      const float g = has_skip ? acc[4 * j + h] + *pj : acc[4 * j + h];
+      if (st) *pj = g * ((h & 2) ? sb : sa);                       // loss.py:145 (de_ds) / inactive rows
+    }
+  }
 }
 
 // every consumer warp has finished reading ring stage s (its wgmma groups have completed)
@@ -706,6 +839,10 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         return (j < 0) ? S.zs[i] : ((unsigned)j < 3u ? S.xr[j * kTcRows + row] : 0.f);
       };
       uint32_t* const maskw = S.maskw + tid;           // word w of layer l: maskw[(4 * l + w) * kTcEpiThreads]
+      auto put_operand = [&](int pslot) {
+        if (SCHED == 1) store_operand_stsm(acc, ah, alo_s, grp, pslot);
+        else store_operand(acc, ah, alo, rl, qd, grp, pslot);
+      };
 
       // ---- A operand of the first GEMM step (= layer 1): layer 0 on the CUDA cores.  With W0[:, :L] z folded into
       // zb0, layer 0 is 3 FMAs per output:  h0[j] = relu(zb0[j] + W0[j][L..L+2] . x)  (deep_sdf_decoder.py:91,103).
@@ -731,7 +868,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         }
 #pragma unroll
         for (int w = 0; w < 4; ++w) maskw[w * kTcEpiThreads] = mw[w];
-        store_operand(acc, ah, alo, rl, qd, grp);
+        put_operand(-1);
       }
       DSPGN_PROBE_ADD(PR_PROLOGUE, tpro);
       DSPGN_PROBE_COUNT(PR_TILES);
@@ -751,6 +888,15 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         DSPGN_PROBE_ADD(PR_GEMM, tg);
         DSPGN_PROBE_T(tepi);
         wg_bar_sync(grp);                                // every MMA of the warpgroup has read the A lo image
+        DSPGN_PROBE_ADD(PR_EPI_ENTRY, tepi);
+        DSPGN_PROBE_T(tval);
+#ifdef DSPGN_STALL_PROBE
+        const int pk = PR_EPI_KIND + 3 * (st.kind == TK_FWD_PENULT ? EK_PENULT
+                                          : st.kind == TK_FWD_HIDDEN ? (st.cat_off >= 0 ? EK_FWD_CAT : EK_FWD)
+                                          : st.kind == TK_BWD_MID ? (st.cat_off >= 0 ? EK_BWD_SKIP : EK_BWD) : EK_BWD_FIRST);
+#else
+        constexpr int pk = -1;
+#endif
         const int qs = opaque_int(qd);
 
         if (st.kind == TK_FWD_PENULT) {
@@ -800,27 +946,19 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
               const int c = frag_col(e, qs);
               acc[e] = ((mw[e >> 5] >> (e & 31)) & 1u) ? ((e & 2) ? gb : ga) * S.wlast[c] : 0.f;
             }
-            store_operand(acc, ah, alo, rl, qd, grp);
+            DSPGN_PROBE_ADD(pk, tval);
+            put_operand(pk);
+          } else {
+            DSPGN_PROBE_ADD(pk, tval);
           }
         } else if (st.kind == TK_FWD_HIDDEN) {
           const float* bb = S.bias + st.layer * kHid;
           uint32_t mw[4] = {0u, 0u, 0u, 0u};
-          if (SCHED == 1 && st.cat_off < 0) {
-            // SDF-tile kernel, every layer but the one before latent_in: the same values without a branch per element
-            // (the concat below makes the loop a chain of small blocks the scheduler cannot interleave), and the bias
-            // of the fragment's column pair 8j + 2q, +1 in one 8-byte load
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float2 bj = *reinterpret_cast<const float2*>(bb + 8 * j + 2 * qs);
-#pragma unroll
-              for (int h = 0; h < 4; ++h) {
-                const int e = 4 * j + h, c = frag_col(e, qs);
-                const float w = acc[e] + ((h & 1) ? bj.y : bj.x);
-                const bool live = c < nm;
-                mw[e >> 5] |= ((live && w > 0.f) ? 1u : 0u) << (e & 31);
-                acc[e] = (live && c < k_next) ? fmaxf(w, 0.f) : 0.f;
-              }
-            }
+          if (SCHED == 1) {
+            if (nm == 256 && k_next == 256) epi_fwd_hidden<256, 256>(acc, mw, bb, qs, nm, k_next);
+            else if (nm == 192 && k_next == 256) epi_fwd_hidden<192, 256>(acc, mw, bb, qs, nm, k_next);
+            else epi_fwd_hidden<0, 0>(acc, mw, bb, qs, nm, k_next);
+            if (st.cat_off >= 0) epi_concat_input(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
           } else {
 #pragma unroll
             for (int e = 0; e < 128; ++e) {
@@ -837,19 +975,17 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           }
 #pragma unroll
           for (int w = 0; w < 4; ++w) maskw[(4 * st.layer + w) * kTcEpiThreads] = mw[w];
-          store_operand(acc, ah, alo, rl, qd, grp);
+          DSPGN_PROBE_ADD(pk, tval);
+          put_operand(pk);
         } else if (st.kind == TK_BWD_MID) {
           uint32_t mw[4];
 #pragma unroll
           for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
-          if (SCHED == 1 && st.cat_off < 0) {
-            // SDF-tile kernel, every layer but latent_in: the same values without a branch per element (as TK_FWD_HIDDEN)
-#pragma unroll
-            for (int e = 0; e < 128; ++e) {
-              const int c = frag_col(e, qs);
-              const bool on = c < nm && c < k_next && ((mw[e >> 5] >> (e & 31)) & 1u);
-              acc[e] = on ? acc[e] : 0.f;
-            }
+          if (SCHED == 1) {
+            if (st.cat_off >= 0) epi_skip_grad(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
+            if (nm == 256 && k_next == 256) epi_bwd_mid<256, 256>(acc, mw, nm, k_next);
+            else if (nm == 256 && k_next == 192) epi_bwd_mid<256, 192>(acc, mw, nm, k_next);
+            else epi_bwd_mid<0, 0>(acc, mw, nm, k_next);
           } else {
 #pragma unroll
             for (int e = 0; e < 128; ++e) {
@@ -867,20 +1003,26 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
               acc[e] = (c < k_next) ? t : 0.f;
             }
           }
-          if (more) store_operand(acc, ah, alo, rl, qd, grp);
+          DSPGN_PROBE_ADD(pk, tval);
+          if (more) put_operand(pk);
         } else {
           // ---- TK_BWD_FIRST: d/d(input) complete -> Jacobian row (loss.py:34-41 / :143-150) -------------
+          if (SCHED == 1) {
+            epi_bwd_first(acc, qs, in0, L, has_skip, S.Jp, S.scr, rowA, rowB);
+          } else {
 #pragma unroll
-          for (int e = 0; e < 128; ++e) {
-            const int c = frag_col(e, qs);
-            if (c < nm && c < in0) {
-              const int row = (e & 2) ? rowB : rowA;
-              float* pj = S.Jp + row * kJpStride + ((c < L) ? c : (kMaxCode + c - L));
-              float g = acc[e];
-              if (has_skip) g += *pj;
-              *pj = g * S.scr[row];                                  // loss.py:145 (de_ds) / inactive rows
+            for (int e = 0; e < 128; ++e) {
+              const int c = frag_col(e, qs);
+              if (c < nm && c < in0) {
+                const int row = (e & 2) ? rowB : rowA;
+                float* pj = S.Jp + row * kJpStride + ((c < L) ? c : (kMaxCode + c - L));
+                float g = acc[e];
+                if (has_skip) g += *pj;
+                *pj = g * S.scr[row];                                  // loss.py:145 (de_ds) / inactive rows
+              }
             }
           }
+          DSPGN_PROBE_ADD(pk, tval);
         }
         if (!more || st.kind == TK_BWD_FIRST) {
           // no next operand: overwriting the register A fragment ends its live range at the GEMM above.  Otherwise it

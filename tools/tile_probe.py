@@ -25,8 +25,12 @@ sys.path.insert(0, ROOT)
 
 # dspgn_tc.cuh: enum ProbeSlot, kProbeCtas
 SLOTS = ["wfull_wait", "wgmma_wait", "gemm", "epilogue", "prologue_layer0", "jtj", "tile_end", "solve", "fifo_wait",
-         "loop", "tiles", "solves", "wempty_wait", "pop", "producer_loop"]
-N_SLOTS, N_CTAS = 16, 256
+         "loop", "tiles", "solves", "wempty_wait", "pop", "producer_loop", "epi_entry_bar"]
+# enum EpiKind; per kind: value loop, store_operand split + stores, store_operand proxy fence + warpgroup barrier
+EPI_KINDS = ["fwd", "fwd_concat", "penult", "bwd", "bwd_skip", "bwd_first"]
+EPI_PARTS = ["values", "split_store", "fence_bar"]
+SLOTS += [f"epi_{k}_{p}" for k in EPI_KINDS for p in EPI_PARTS]
+N_SLOTS, N_CTAS = len(SLOTS), 256
 
 
 def card():
@@ -99,6 +103,7 @@ def main():
         "cycles_per_tile": {k: s[k] / s["tiles"] for k in parts + ["gemm"]} | {"loop": loop / s["tiles"]},
         "cycles_per_solve": s["solve"] / max(s["solves"], 1),
         "producer_share": {k: sp[k] / max(sp["producer_loop"], 1) for k in ("wempty_wait", "pop")},
+        "epilogue_cycles_per_tile": {k: s[k] / s["tiles"] for k in SLOTS if k.startswith("epi_")},
     }
     print(f"{args.workload} on {gpu}: {ctas} CTAs, {res['tiles_per_run']:.0f} tiles and {res['solves_per_run']:.0f} "
           f"solves per run, {ms:.2f} ms per run (probe build)")
@@ -107,6 +112,14 @@ def main():
         per = res["cycles_per_tile"].get(k, v * loop / s["tiles"])
         print(f"  {k:18s} {100 * v:6.2f} %  {per:10.0f}")
     print(f"  {'loop':18s} {100.0:6.2f} %  {loop / s['tiles']:10.0f}")
+    print("epilogue by step kind, cycles per tile (share of the epilogue):")
+    ept = res["epilogue_cycles_per_tile"]
+    epi = s["epilogue"] / s["tiles"]
+    print(f"  {'entry barrier':18s} {ept['epi_entry_bar']:10.0f}  ({100 * ept['epi_entry_bar'] / epi:5.1f} %)")
+    print(f"  {'kind':12s} " + " ".join(f"{p:>12s}" for p in EPI_PARTS) + f" {'total':>12s}")
+    for k in EPI_KINDS:
+        v = [ept[f"epi_{k}_{p}"] for p in EPI_PARTS]
+        print(f"  {k:12s} " + " ".join(f"{x:12.0f}" for x in v) + f" {sum(v):12.0f}  ({100 * sum(v) / epi:5.1f} %)")
     print(f"producer: waiting for free ring stages {100 * res['producer_share']['wempty_wait']:.2f} %, "
           f"popping / FIFO full {100 * res['producer_share']['pop']:.2f} % of its loop")
     print(f"cycles per solve {res['cycles_per_solve']:.0f}")
