@@ -99,6 +99,15 @@ class LidarBoxOut(C.Structure):
     _fields_ = [("n_pts", C.c_int32), ("n_rays", C.c_int32), ("mask", C.c_int32), ("n_selected", C.c_int32)]
 
 
+class MonoSpec(C.Structure):
+    _fields_ = [("k", C.c_double * 9), ("inv_k", C.c_double * 9), ("k1", C.c_double), ("k2", C.c_double),
+                ("img_h", C.c_int32), ("img_w", C.c_int32), ("downsample_ratio", C.c_int32), ("mask_erosion", C.c_int32)]
+
+
+class MonoOut(C.Structure):
+    _fields_ = [("mask", C.c_int32), ("n_nonsurface", C.c_int32), ("n_rays", C.c_int32), ("n_feature", C.c_int32)]
+
+
 assert C.sizeof(ObjectOut) == 4 * RESULT_FLOATS
 
 # every symbol include/dspgn.h declares: (name, restype, argtypes)
@@ -161,6 +170,12 @@ SYMBOLS = [
     ("dspgn_lidar_frame_run", C.c_int, [_VP, _FP, C.c_int, C.POINTER(LidarBox), C.c_int, C.POINTER(C.c_uint8),
                                         C.POINTER(C.c_int32), C.c_int, C.POINTER(LidarBoxOut)]),
     ("dspgn_lidar_frame_results", C.c_int, [_VP, _FP, _FP, _FP]),
+    ("dspgn_mono_frame_create", C.c_int, [C.POINTER(MonoSpec), C.c_int, C.POINTER(_VP)]),
+    ("dspgn_mono_frame_destroy", None, [_VP]),
+    ("dspgn_mono_frame_set_stream", C.c_int, [_VP, _VP]),
+    ("dspgn_mono_frame_run", C.c_int, [_VP, C.POINTER(C.c_uint8), C.POINTER(C.c_int32), C.c_int, _FP, C.c_int,
+                                       C.POINTER(MonoOut)]),
+    ("dspgn_mono_frame_results", C.c_int, [_VP, _FP, C.POINTER(C.c_int32)]),
 ]
 
 _lib = None

@@ -17,6 +17,7 @@
 #include "dspgn_tc.cuh"
 #include "dspgn_mesh.cuh"
 #include "dspgn_frame.cuh"
+#include "dspgn_mono.cuh"
 
 using namespace dspgn;
 
@@ -2174,6 +2175,176 @@ int dspgn_lidar_frame_results(DspgnLidarFrame* f, float* points, float* depth, f
       const float* q = reinterpret_cast<const float*>(h + L.rays) + (size_t)b * (num_max + kFrameBackground) * 3;
       if (rays) memcpy(rays + 3 * nr, q, 12 * (size_t)r.n_rays);
       nr += r.n_rays;
+    }
+  }
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- A monocular keyframe's detection (dspgn_mono.cuh) ----
+
+struct DspgnMonoFrame {
+  int device = 0;
+  DspgnMonoSpec spec{};
+  cudaStream_t stream = nullptr;
+  cudaStream_t own = nullptr;  // the handle's non-blocking stream (the default), as DspgnLidarFrame's
+  HostBuf h_in, h_out;
+  DevBuf d_in, d_work, d_out;
+  int n_kp_blocks = 0;         // of the last run
+  DspgnMonoOut last{-1, 0, -1, 0};
+};
+
+namespace {
+
+// the output block of a run: header, rays [200][3], per keypoint block: count, then its passing indices
+struct MonoOutLayout {
+  size_t rays, cnt, idx, bytes;
+  explicit MonoOutLayout(int n_kp_blocks) {
+    rays = align16(4 * (size_t)kMonoHdr);
+    cnt = rays + align16(12 * (size_t)kFrameBackground);
+    idx = cnt + align16(4 * (size_t)n_kp_blocks);
+    bytes = idx + 4 * (size_t)n_kp_blocks * kMonoKpPerBlock;
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+int dspgn_mono_frame_create(const DspgnMonoSpec* spec, int device, DspgnMonoFrame** out) {
+  if (!spec || !out) return fail(DSPGN_E_ARG, "null argument");
+  if (spec->img_h < 1 || spec->img_h > 4096 || spec->img_w < 1 || spec->img_w > 4096) return fail(DSPGN_E_ARG, "image size must be in [1,4096]^2");
+  if (spec->downsample_ratio < 1) return fail(DSPGN_E_ARG, "downsample_ratio must be >= 1");
+  if (spec->mask_erosion < 0 || spec->mask_erosion > kMonoMaxErosion) return fail(DSPGN_E_ARG, "mask_erosion must be in [0,63]");
+  if (!(spec->k[0] != 0.0 && spec->k[4] != 0.0)) return fail(DSPGN_E_ARG, "fx and fy must be nonzero");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPGN_E_NOGPU, "no CUDA device"); }
+  if (device < 0 || device >= ndev) return fail(DSPGN_E_ARG, "bad device index");
+  CU(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CU(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only");
+  DspgnMonoFrame* f = new (std::nothrow) DspgnMonoFrame();
+  if (!f) return fail(DSPGN_E_ALLOC, "oom");
+  f->device = device;
+  f->spec = *spec;
+  if (cudaStreamCreateWithFlags(&f->own, cudaStreamNonBlocking) != cudaSuccess) {
+    cudaGetLastError();
+    delete f;
+    return fail(DSPGN_E_CUDA, "cudaStreamCreateWithFlags");
+  }
+  f->stream = f->own;
+  *out = f;
+  return 0;
+}
+
+void dspgn_mono_frame_destroy(DspgnMonoFrame* f) {
+  if (!f) return;
+  cudaSetDevice(f->device);
+  cudaStreamSynchronize(f->stream);
+  f->h_in.release(); f->h_out.release();
+  f->d_in.release(); f->d_work.release(); f->d_out.release();
+  if (f->own) cudaStreamDestroy(f->own);
+  delete f;
+}
+
+int dspgn_mono_frame_set_stream(DspgnMonoFrame* f, void* cuda_stream) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  f->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+  return 0;
+}
+
+int dspgn_mono_frame_run(DspgnMonoFrame* f, const uint8_t* masks, const int32_t* bboxes, int n_masks,
+                         const float* keypoints, int n_kp, DspgnMonoOut* out) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  const DspgnMonoSpec& sp = f->spec;
+  if (n_masks < 0 || n_masks > kFrameMaxMasks) return fail(DSPGN_E_ARG, "n_masks must be in [0, 64]");
+  if (n_kp < 0 || n_kp > (1 << 20)) return fail(DSPGN_E_ARG, "n_kp must be in [0, 2^20]");
+  if (!out || (n_masks > 0 && (!masks || !bboxes)) || (n_kp > 0 && !keypoints))
+    return fail(DSPGN_E_ARG, "null pointer where data is required");
+  for (int m = 0; m < n_masks; ++m) {
+    const int32_t* bb = bboxes + 4 * m;
+    if (!(0 <= bb[0] && bb[0] <= bb[2] && bb[2] <= sp.img_w && 0 <= bb[1] && bb[1] <= bb[3] && bb[3] <= sp.img_h))
+      return fail(DSPGN_E_ARG, "bbox " + std::to_string(m) + " outside 0 <= l <= r <= img_w, 0 <= t <= b <= img_h");
+  }
+  for (int i = 0; i < n_kp; ++i) {       // cv::Mat::at reads ((int)y, (int)x): both truncations inside the image
+    const float x = keypoints[2 * i], y = keypoints[2 * i + 1];
+    if (!(x > -1.f && x < (float)sp.img_w && y > -1.f && y < (float)sp.img_h))
+      return fail(DSPGN_E_ARG, "keypoint " + std::to_string(i) + " does not truncate to a pixel inside the image");
+  }
+  CU(cudaSetDevice(f->device));
+  f->last = DspgnMonoOut{-1, 0, -1, 0};
+  f->n_kp_blocks = 0;
+  *out = f->last;
+  if (n_masks == 0) return 0;              // the reference returns no instance; nothing reads the keypoints
+  const int n_kp_blocks = (n_kp + kMonoKpPerBlock - 1) / kMonoKpPerBlock;
+  // staged input block: bboxes | keypoints | masks (each mask padded to 16 bytes)
+  const size_t mstride = align16((size_t)sp.img_h * sp.img_w);
+  const size_t o_kp = align16(16 * (size_t)n_masks);
+  const size_t o_mask = o_kp + align16(8 * (size_t)n_kp);
+  const size_t in_bytes = o_mask + mstride * n_masks;
+  const MonoOutLayout L(n_kp_blocks);
+  if (f->h_in.reserve(in_bytes) || f->h_out.reserve(L.bytes)) return fail(DSPGN_E_ALLOC, "cudaMallocHost");
+  if (f->d_in.reserve(in_bytes) || f->d_work.reserve(4 * kFrameMaxMasks) || f->d_out.reserve(L.bytes))
+    return fail(DSPGN_E_ALLOC, "cudaMalloc");
+  unsigned char* h = f->h_in.as<unsigned char>();
+  memcpy(h, bboxes, 16 * (size_t)n_masks);
+  if (n_kp) memcpy(h + o_kp, keypoints, 8 * (size_t)n_kp);
+  const size_t hw = (size_t)sp.img_h * sp.img_w;
+  for (int m = 0; m < n_masks; ++m) {
+    memcpy(h + o_mask + m * mstride, masks + m * hw, hw);
+    memset(h + o_mask + m * mstride + hw, 0, mstride - hw);
+  }
+  FrameParams A{};                         // the LiDAR call's area blocks: n_boxes = 0, one block per mask
+  A.n_masks = n_masks;
+  A.mask_stride = (long long)mstride;
+  MonoParams P{};
+  memcpy(P.P, sp.k, sizeof(P.P));
+  memcpy(P.inv_k, sp.inv_k, sizeof(P.inv_k));
+  P.fx = sp.k[0]; P.fy = sp.k[4]; P.cx = sp.k[2]; P.cy = sp.k[5];
+  P.ifx = 1. / P.fx; P.ify = 1. / P.fy;
+  P.k1 = sp.k1; P.k2 = sp.k2;
+  P.img_h = sp.img_h; P.img_w = sp.img_w; P.alpha = sp.downsample_ratio; P.erosion = sp.mask_erosion;
+  P.n_masks = n_masks; P.n_kp = n_kp; P.mask_stride = (long long)mstride;
+  unsigned char* d = f->d_in.as<unsigned char>();
+  const int* d_bb = reinterpret_cast<const int*>(d);
+  const float2* d_kp = reinterpret_cast<const float2*>(d + o_kp);
+  const unsigned char* d_masks = d + o_mask;
+  int* d_area = f->d_work.as<int>();
+  unsigned char* o = f->d_out.as<unsigned char>();
+  cudaStream_t st = f->stream;
+  CU(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
+  k_frame_scan_area<<<n_masks, 1024, 0, st>>>(A, nullptr, nullptr, nullptr, d_masks, d_area);
+  k_mono_frame<<<1 + n_kp_blocks, kFrameBoxThreads, 0, st>>>(P, d_masks, d_bb, d_kp, d_area, reinterpret_cast<int*>(o),
+                                                             reinterpret_cast<float*>(o + L.rays),
+                                                             reinterpret_cast<int*>(o + L.cnt),
+                                                             reinterpret_cast<int*>(o + L.idx));
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(f->h_out.p, o, L.bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const int* hh = f->h_out.as<int>();
+  const int* cnt = reinterpret_cast<const int*>(f->h_out.as<unsigned char>() + L.cnt);
+  DspgnMonoOut r{hh[0], hh[1], hh[2], 0};
+  for (int b = 0; b < n_kp_blocks; ++b) r.n_feature += cnt[b];
+  f->n_kp_blocks = n_kp_blocks;
+  f->last = r;
+  *out = r;
+  return 0;
+}
+
+int dspgn_mono_frame_results(DspgnMonoFrame* f, float* background_rays, int32_t* feature_idx) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  const MonoOutLayout L(f->n_kp_blocks);
+  const unsigned char* h = f->h_out.as<unsigned char>();
+  if (background_rays && f->last.n_rays > 0) memcpy(background_rays, h + L.rays, 12 * (size_t)f->last.n_rays);
+  if (feature_idx) {
+    const int* cnt = reinterpret_cast<const int*>(h + L.cnt);
+    const int* idx = reinterpret_cast<const int*>(h + L.idx);
+    size_t n = 0;
+    for (int b = 0; b < f->n_kp_blocks; ++b) {
+      memcpy(feature_idx + n, idx + (size_t)b * kMonoKpPerBlock, 4 * (size_t)cnt[b]);
+      n += cnt[b];
     }
   }
   return 0;

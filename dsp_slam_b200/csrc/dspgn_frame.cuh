@@ -211,6 +211,59 @@ __device__ __forceinline__ int frame_block_rank(bool f, int* s_w, int* rank) {
   return total;
 }
 
+// The background sampler of one mask's bbox (kitti_sequence.py:70-92, mono_sequence.py:51-73), for a block of
+// kFrameBoxThreads threads: the bbox (l, t, r, b) expanded by 5 px and clamped to the image, the grid
+// np.linspace(t, b, int(H/alpha)) x np.linspace(l, r, int(W/alpha)) in row-major order, its pixels outside the mask,
+// and, when there are more than 200, the ranks np.linspace(0, n-1, 200).astype(int32).  Writes the kept (u, v) to
+// s_samp in order and returns n, the count before subsampling, to every thread.
+// Params: FrameParams or MonoParams (img_h, img_w, alpha).
+template <class Params>
+__device__ __forceinline__ int frame_background(const Params& P, const int* bbox, const unsigned char* mk, int* s_w,
+                                                int (*s_samp)[2]) {
+  const int max_w = P.img_w - 1, max_h = P.img_h - 1;
+  int l = bbox[0], t = bbox[1], r = bbox[2], bt = bbox[3];
+  l = l > kFrameExpand ? l - kFrameExpand : 0;
+  t = t > kFrameExpand ? t - kFrameExpand : 0;
+  r = r < max_w - kFrameExpand ? r + kFrameExpand : max_w;
+  bt = bt < max_h - kFrameExpand ? bt + kFrameExpand : max_h;
+  const int nh = (bt - t + 1) / P.alpha, nw = (r - l + 1) / P.alpha;    // int(crop / alpha), crop >= 1
+  const long long ng = (long long)nh * nw;
+  // pass 1: the number of grid pixels outside the mask; pass 2: their ranks, kept by the 200-of-n subsample
+  int ns = 0;
+  for (long long g = threadIdx.x; g < ng; g += blockDim.x) {
+    const int vv = (int)np_linspace((double)t, (double)bt, nh, (int)(g / nw));
+    const int uu = (int)np_linspace((double)l, (double)r, nw, (int)(g % nw));
+    ns += mk[(size_t)vv * P.img_w + uu] == 0;
+  }
+  ns = __reduce_add_sync(0xffffffffu, ns);
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = ns;
+  __syncthreads();
+  int n_bg = 0;
+  for (int i = 0; i < kFrameBoxThreads / 32; ++i) n_bg += s_w[i];
+  __syncthreads();
+  int base = 0;
+  for (long long g0 = 0; g0 < ng; g0 += blockDim.x) {
+    const long long g = g0 + threadIdx.x;
+    int vv = 0, uu = 0;
+    bool f = false;
+    if (g < ng) {
+      vv = (int)np_linspace((double)t, (double)bt, nh, (int)(g / nw));
+      uu = (int)np_linspace((double)l, (double)r, nw, (int)(g % nw));
+      f = mk[(size_t)vv * P.img_w + uu] == 0;
+    }
+    int rank;
+    const int tile = frame_block_rank(f, s_w, &rank);
+    if (f) {
+      const int q = base + rank;
+      const int slot = n_bg <= kFrameBackground ? q : np_subsample_slot(q, n_bg, kFrameBackground);
+      if (slot >= 0) { s_samp[slot][0] = uu; s_samp[slot][1] = vv; }
+    }
+    base += tile;
+  }
+  __syncthreads();
+  return n_bg;
+}
+
 // the projection of a camera-frame point with K (float32 division; a point behind the camera still yields a value)
 __device__ __forceinline__ void frame_project(const FrameParams& P, const float* q, float* u, float* v) {
   const float h0 = f3dot(q[0], q[1], q[2], P.K[0], P.K[1], P.K[2]);
@@ -284,49 +337,7 @@ __global__ void __launch_bounds__(kFrameBoxThreads) k_frame_box(FrameParams P, c
   __syncthreads();
   const int m = s_match;
   if (m < 0) return;
-  // the sampler's crop (kitti_sequence.py:70-92): expanded by 5 px, clamped to the image
-  const int max_w = P.img_w - 1, max_h = P.img_h - 1;
-  int l = bboxes[4 * m], t = bboxes[4 * m + 1], r = bboxes[4 * m + 2], bt = bboxes[4 * m + 3];
-  l = l > kFrameExpand ? l - kFrameExpand : 0;
-  t = t > kFrameExpand ? t - kFrameExpand : 0;
-  r = r < max_w - kFrameExpand ? r + kFrameExpand : max_w;
-  bt = bt < max_h - kFrameExpand ? bt + kFrameExpand : max_h;
-  const int nh = (bt - t + 1) / P.alpha, nw = (r - l + 1) / P.alpha;    // int(crop / alpha), crop >= 1
-  const long long ng = (long long)nh * nw;
-  const unsigned char* mk = masks + (size_t)m * P.mask_stride;
-  // pass 1: the number of grid pixels outside the mask; pass 2: their ranks, kept by the 200-of-n subsample
-  int ns = 0;
-  for (long long g = threadIdx.x; g < ng; g += blockDim.x) {
-    const int vv = (int)np_linspace((double)t, (double)bt, nh, (int)(g / nw));
-    const int uu = (int)np_linspace((double)l, (double)r, nw, (int)(g % nw));
-    ns += mk[(size_t)vv * P.img_w + uu] == 0;
-  }
-  ns = __reduce_add_sync(0xffffffffu, ns);
-  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = ns;
-  __syncthreads();
-  int n_bg = 0;
-  for (int i = 0; i < kFrameBoxThreads / 32; ++i) n_bg += s_w[i];
-  __syncthreads();
-  int base = 0;
-  for (long long g0 = 0; g0 < ng; g0 += blockDim.x) {
-    const long long g = g0 + threadIdx.x;
-    int vv = 0, uu = 0;
-    bool f = false;
-    if (g < ng) {
-      vv = (int)np_linspace((double)t, (double)bt, nh, (int)(g / nw));
-      uu = (int)np_linspace((double)l, (double)r, nw, (int)(g % nw));
-      f = mk[(size_t)vv * P.img_w + uu] == 0;
-    }
-    int rank;
-    const int tile = frame_block_rank(f, s_w, &rank);
-    if (f) {
-      const int q = base + rank;
-      const int slot = n_bg <= kFrameBackground ? q : np_subsample_slot(q, n_bg, kFrameBackground);
-      if (slot >= 0) { s_samp[slot][0] = uu; s_samp[slot][1] = vv; }
-    }
-    base += tile;
-  }
-  __syncthreads();
+  const int n_bg = frame_background(P, bboxes + 4 * m, masks + (size_t)m * P.mask_stride, s_w, s_samp);
   const int n_s = min(n_bg, kFrameBackground);
   float* ro = rays + (size_t)b * (P.num_max + kFrameBackground) * 3;
   for (int i = threadIdx.x; i < n + n_s; i += blockDim.x) {

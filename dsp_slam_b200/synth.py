@@ -166,3 +166,43 @@ def make_lidar_frame(seed, n_points=127000, n_boxes=20, n_masks=10, img_hw=(375,
                             0, [W, H, W, H])
     return dict(scan=scan, dets=dets.astype(F32), masks=masks, bboxes=bboxes, K=KITTI_K, T_cam_velo=KITTI_T_CAM_VELO,
                 img_hw=(H, W))
+
+
+# Redwood 01053 and Freiburg 002 cameras (Camera.fx, fy, cx, cy, k1, k2 of their ORB-SLAM yamls) and image sizes
+MONO_CAMERAS = {"redwood": ((538.204343, 538.204343, 320.0, 240.0), 0.023896, -0.067078, (480, 640)),
+                "freiburg": ((984.697, 984.697, 480.0, 270.0), -0.133543, -0.15436, (540, 960))}
+
+
+def make_mono_frame(seed, camera="redwood", n_masks=12, n_kp=2000):
+    """A full-size monocular keyframe as Frame.get_detections and GetObjectDetectionsMono receive it
+    (mono_sequence.py:75-114, Tracking_util.cc:176-201): masks (m, H, W) bool (ellipses with ragged edges, one large
+    object in the middle), bboxes (m, 4) f32 around them, keypoints (n, 2) f32 (pt.x, pt.y; a third on the largest
+    mask, fractional, some on the image border), K (3, 3) f64, k1, k2."""
+    rng = np.random.default_rng(seed)
+    (fx, fy, cx, cy), k1, k2, (H, W) = MONO_CAMERAS[camera]
+    v, u = np.mgrid[0:H, 0:W]
+    masks = np.zeros((n_masks, H, W), bool)
+    bboxes = np.zeros((n_masks, 4), F32)
+    for m in range(n_masks):
+        big = m == n_masks // 2
+        cu = W / 2 + rng.uniform(-30, 30) if big else rng.uniform(0, W)
+        cv = H / 2 + rng.uniform(-20, 20) if big else rng.uniform(0, H)
+        au = rng.uniform(0.2, 0.3) * W if big else rng.uniform(10, 0.15 * W)
+        av = rng.uniform(0.25, 0.35) * H if big else rng.uniform(10, 0.15 * H)
+        r = ((u - cu) / au) ** 2 + ((v - cv) / av) ** 2
+        mk = r <= 1.0 + 0.08 * rng.standard_normal((H, W))
+        masks[m] = mk
+        vv, uu = np.nonzero(mk)
+        if vv.size == 0:
+            continue
+        bboxes[m] = np.clip([uu.min() - rng.uniform(0, 4), vv.min() - rng.uniform(0, 4), uu.max() + rng.uniform(0, 4),
+                             vv.max() + rng.uniform(0, 4)], 0, [W, H, W, H])
+    big = masks[int(np.argmax(masks.sum(-1).sum(-1)))]
+    vv, uu = np.nonzero(big)
+    n_in = n_kp // 3
+    pick = rng.integers(0, vv.size, n_in)
+    kp = np.concatenate([np.stack([uu[pick] + rng.random(n_in), vv[pick] + rng.random(n_in)], -1),
+                         np.stack([rng.uniform(-0.99, W - 0.01, n_kp - n_in - 4), rng.uniform(-0.99, H - 0.01, n_kp - n_in - 4)], -1),
+                         [[0.0, 0.0], [W - 0.5, H - 0.5], [-0.5, H / 2], [W / 2, H - 0.01]]]).astype(F32)
+    K = np.array([[fx, 0.0, cx], [0.0, fy, cy], [0.0, 0.0, 1.0]])
+    return dict(masks=masks, bboxes=bboxes, keypoints=kp, K=K, k1=k1, k2=k2, img_hw=(H, W))

@@ -424,6 +424,52 @@ int dspgn_lidar_frame_run(DspgnLidarFrame* f, const float* scan, int n_points, c
                           const uint8_t* masks, const int32_t* bboxes, int n_masks, DspgnLidarBoxOut* out);
 int dspgn_lidar_frame_results(DspgnLidarFrame* f, float* points, float* depth, float* rays);
 
+/* ---- A monocular (Redwood / Freiburg) keyframe's detection (mono_sequence.Frame.get_detections,
+ * reconstruct/mono_sequence.py:75-114) and its keypoint test (Tracking::GetObjectDetectionsMono,
+ * src/Tracking_util.cc:176-201), built on the device from the 2D masks and the keyframe's keypoints.  Its own handle,
+ * like DspgnLidarFrame: Tracking is a different thread from LocalMapping's solver calls.
+ *   mask      the first mask with the most set pixels (np.argmax of the areas); -1 when there are no masks.
+ *   rays      the background grid of its bbox (truncated, expanded by 5 px, clamped; np.linspace(t, b, int(H/alpha))
+ *             x np.linspace(l, r, int(W/alpha)), row-major) outside the mask, 200 of them at np.linspace(0, n-1, 200)
+ *             ranks when more; undistorted as cv2.undistortPoints(pixels, K, (k1, k2, 0, 0, 0), P=K) (fp64, 5
+ *             iterations, float32 result); rays = inv_k [u, v, 1] in float64, cast to float32.  Fewer than 2 such
+ *             pixels is a frame the reference fails on (cv2 asserts on none, get_rays raises on one): n_rays = -1.
+ *   features  the indices, ascending, of the keypoints whose pixel ((int)pt.y, (int)pt.x) is set in the mask eroded
+ *             by getStructuringElement(MORPH_ELLIPSE, (2e+1)^2): every mask pixel of the ellipse around it that lies
+ *             inside the image is set.  The image is not eroded: only the keypoints' footprints are read.
+ * Every float step is rounded as numpy / OpenCV round it, so the arrays are bit-identical to the reference's.
+ *   run      validates (DSPGN_E_ARG before anything is enqueued), stages the masks, bboxes and keypoints in pinned
+ *            memory, one H2D copy, two kernels and one D2H copy on the handle's stream, then waits for that copy (the
+ *            only host synchronisation) and writes the DspgnMonoOut.  Limits: <= 64 masks, each bbox 0 <= l <= r <=
+ *            img_w and 0 <= t <= b <= img_h after truncation, <= 2^20 keypoints, each finite with -1 < x < img_w and
+ *            -1 < y < img_h (its truncation inside the image).
+ *   results  the arrays of the last run: background_rays (n_rays x 3, when n_rays > 0), feature_idx (n_feature).
+ *            Either pointer may be NULL. */
+typedef struct DspgnMonoFrame DspgnMonoFrame;
+typedef struct {
+  double k[9];                /* K_cam (3x3 row-major, float64 from the yaml's Camera.fx/fy/cx/cy) */
+  double inv_k[9];            /* np.linalg.inv(K_cam), float64 */
+  double k1, k2;              /* Camera.k1, Camera.k2 */
+  int32_t img_h, img_w;       /* 1..4096 */
+  int32_t downsample_ratio;   /* int(configs.downsample_ratio), >= 1 */
+  int32_t mask_erosion;       /* Objects.maskErrosion, 0..63 */
+} DspgnMonoSpec;
+typedef struct {
+  int32_t mask;               /* the largest mask's index, -1: no masks */
+  int32_t n_nonsurface;       /* background pixels before subsampling */
+  int32_t n_rays;             /* background rays, -1: none (no masks, or fewer than 2 pixels) */
+  int32_t n_feature;          /* keypoints inside the eroded mask (the detection is good iff >= 20) */
+} DspgnMonoOut;
+int dspgn_mono_frame_create(const DspgnMonoSpec* spec, int device, DspgnMonoFrame** out);
+void dspgn_mono_frame_destroy(DspgnMonoFrame* f);
+/* as dspgn_lidar_frame_set_stream */
+int dspgn_mono_frame_set_stream(DspgnMonoFrame* f, void* cuda_stream);
+/* masks: n_masks x img_h x img_w bytes (numpy bool, nonzero = inside); bboxes: n_masks x 4 int32 (l, t, r, b), the
+ * boxes truncated like astype(int32); keypoints: n_kp x 2 float32 (pt.x, pt.y of KeyFrame::mvKeys) */
+int dspgn_mono_frame_run(DspgnMonoFrame* f, const uint8_t* masks, const int32_t* bboxes, int n_masks,
+                         const float* keypoints, int n_kp, DspgnMonoOut* out);
+int dspgn_mono_frame_results(DspgnMonoFrame* f, float* background_rays, int32_t* feature_idx);
+
 /* Test hook for the wgmma operand paths: D[128][n_mma] = A[128][16*k_steps] * B[n_mma][16*k_steps]^T
  * (A through the register / shared-memory split-fp16 path, B through the pre-swizzled shared-memory images). Host buffers. */
 int dspgn_tc_selftest(int device, int n_mma, int k_steps, const float* A, const float* B, float* D);
