@@ -18,6 +18,7 @@ MESH_OFF, MESH_DONE, MESH_FAILED, MESH_LOST = 0, 1, 2, 3
 ST_OK, ST_SDF_NAN, ST_RENDER_FEW, ST_RENDER_NAN, ST_SOLVE, ST_BAD_INPUT = 0, 1, 2, 3, 4, 5
 E_ARG, E_CUDA, E_NOGPU, E_ALLOC, E_PEER, E_BUSY = -1, -2, -3, -4, -5, -6
 IPC_HANDLE_BYTES = 64
+FRAME_RESERVE_SMS = 4      # DSPGN_FRAME_RESERVE_SMS: SMs the solvers leave free while a frame handle is alive
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdspgn.so")
@@ -143,6 +144,7 @@ SYMBOLS = [
     ("dspgn_keyframe_wait", C.c_int, [_VP, C.POINTER(ObjectOut), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("dspgn_debug_host_syncs", C.c_int, [_VP, C.POINTER(C.c_int64)]),
     ("dspgn_debug_mesh_arena", C.c_int, [_VP, C.c_int64, C.c_int64]),
+    ("dspgn_debug_sm_budget", C.c_int, [_VP, C.c_int, C.POINTER(C.c_int32)]),
     ("dspgn_decode_sdf", C.c_int, [_VP, C.c_int, _FP, _FP, C.c_int, C.c_int, C.c_int, _FP]),
     ("dspgn_mesh_batch", C.c_int, [_VP, C.c_int, _FP, C.c_int, C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32),
                                    C.POINTER(C.c_int32)]),

@@ -8,6 +8,7 @@
 #include <vector>
 #include <new>
 #include <algorithm>
+#include <atomic>
 
 #include <cub/device/device_scan.cuh>
 
@@ -173,9 +174,31 @@ struct DspgnSolver {
   double arena_v = 4.0, arena_f = 8.0;     // arena estimate: vertices / faces per object and per dim^2 (grows)
   long long arena_force_v = 0, arena_force_f = 0;   // dspgn_debug_mesh_arena
   long long host_syncs = 0;          // dspgn_debug_host_syncs
+  int sm_force = 0;                  // dspgn_debug_sm_budget (0: the automatic budget, grid_sms)
 };
 
 namespace {
+
+// ---- SM budget of the solver's grid-sized launches ----------------------------------------------------------------
+// The persistent kernels fill a whole SM per CTA (registers and shared memory), so while one runs on every SM no block
+// of another kernel can start anywhere.  A live frame handle (DspgnLidarFrame / DspgnMonoFrame) on the device means a
+// Tracking thread may build a keyframe's detections while LocalMapping's keyframe runs: the grid-sized launches then
+// leave kFrameReserveSms SMs to it.  Counted per device, read at every launch (the builder may be created after the
+// solver).  DESIGN §5 has the measurement this value comes from.
+constexpr int kFrameReserveSms = DSPGN_FRAME_RESERVE_SMS;
+constexpr int kMaxDevices = 64;
+std::atomic<int> g_live_frames[kMaxDevices];
+
+void count_frame(int device, int delta) {
+  if (device >= 0 && device < kMaxDevices) g_live_frames[device].fetch_add(delta, std::memory_order_relaxed);
+}
+
+// CTAs of the next grid-sized launch (k_gn_persistent*, k_decoder_tc, k_decoder_simt): at most this many
+int grid_sms(const DspgnSolver* s) {
+  if (s->sm_force > 0) return s->sm_force;
+  const bool frames = s->device < kMaxDevices && g_live_frames[s->device].load(std::memory_order_relaxed) > 0;
+  return frames ? std::max(s->num_sms - kFrameReserveSms, 1) : s->num_sms;
+}
 
 // Every wait of the calling thread on the device goes through these (dspgn_debug_host_syncs counts them).
 cudaError_t sync_stream(DspgnSolver* s) {
@@ -649,9 +672,9 @@ int launch_term(DspgnSolver* s, const BatchDev& b, const TermArgs& a, long long 
   const long long tile_rows = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
   long long tiles = (rows_upper + tile_rows - 1) / tile_rows + s->n_obj;
   if (s->engine == DSPGN_ENGINE_TC) {
-    if (int rc = tc_launch_term(b, a, s->num_sms, tiles, st, g_err)) return rc;
+    if (int rc = tc_launch_term(b, a, grid_sms(s), tiles, st, g_err)) return rc;
   } else {
-    int grid = (int)std::min<long long>(tiles, s->num_sms);
+    int grid = (int)std::min<long long>(tiles, grid_sms(s));
     if (grid < 1) grid = 1;
     k_decoder_simt<<<grid, kThreads, sizeof(SimtSmem), st>>>(b, a);
   }
@@ -907,9 +930,10 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     if (q.log.ev) CU(cudaMemsetAsync(q.log.ev, 0, 8, s->stream));
     SolveArgs v = base_solve(s);
     v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0;
+    const int grid = grid_sms(s);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
-    if (render) k_gn_persistent_render<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
-    else k_gn_persistent<<<s->num_sms, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
+    if (render) k_gn_persistent_render<<<grid, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
+    else k_gn_persistent<<<grid, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
     s->ctr.kernel_launches += 1;
     for (int m = 0; m < 2; ++m) s->ctr.rows_fwd_bwd += p.pts[m] * p.iters[m];
@@ -1663,6 +1687,15 @@ int dspgn_debug_mesh_arena(DspgnSolver* s, int64_t max_vertices, int64_t max_fac
   return 0;
 }
 
+int dspgn_debug_sm_budget(DspgnSolver* s, int n, int32_t* current) {
+  if (!s || n < 0) return fail(DSPGN_E_ARG, "bad argument");
+  BUSY(s);
+  if (n > s->num_sms) return fail(DSPGN_E_ARG, "n must be 0 (automatic) or in [1, number of SMs]");
+  s->sm_force = n;
+  if (current) *current = grid_sms(s);
+  return 0;
+}
+
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n, int x_rs, int x_cs,
                      float* sdf_out) {
   if (!s || !code || !x || !sdf_out || n < 1) return fail(DSPGN_E_ARG, "bad argument");
@@ -2009,6 +2042,18 @@ namespace {
 
 size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
+// A frame handle's own stream: non-blocking, at the device's greatest priority, so that the frame's blocks are
+// dispatched ahead of the solver's queued short kernels (mesh passes, scans, per-iteration launches).
+int frame_stream(cudaStream_t* out) {
+  int least = 0, greatest = 0;
+  if (cudaDeviceGetStreamPriorityRange(&least, &greatest) != cudaSuccess ||
+      cudaStreamCreateWithPriority(out, cudaStreamNonBlocking, greatest) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(DSPGN_E_CUDA, "cudaStreamCreateWithPriority");
+  }
+  return 0;
+}
+
 // the output block of a run: header, points [box][num_max][3], rays [box][num_max + 200][3]
 struct FrameOutLayout {
   size_t hdr, pts, rays, bytes;
@@ -2040,12 +2085,12 @@ int dspgn_lidar_frame_create(const DspgnLidarSpec* spec, int device, DspgnLidarF
   if (!f) return fail(DSPGN_E_ALLOC, "oom");
   f->device = device;
   f->spec = *spec;
-  if (cudaStreamCreateWithFlags(&f->own, cudaStreamNonBlocking) != cudaSuccess) {
-    cudaGetLastError();
+  if (int rc = frame_stream(&f->own)) {
     delete f;
-    return fail(DSPGN_E_CUDA, "cudaStreamCreateWithFlags");
+    return rc;
   }
   f->stream = f->own;
+  count_frame(device, 1);
   *out = f;
   return 0;
 }
@@ -2057,6 +2102,7 @@ void dspgn_lidar_frame_destroy(DspgnLidarFrame* f) {
   f->h_in.release(); f->h_out.release();
   f->d_in.release(); f->d_work.release(); f->d_out.release();
   if (f->own) cudaStreamDestroy(f->own);
+  count_frame(f->device, -1);
   delete f;
 }
 
@@ -2229,12 +2275,12 @@ int dspgn_mono_frame_create(const DspgnMonoSpec* spec, int device, DspgnMonoFram
   if (!f) return fail(DSPGN_E_ALLOC, "oom");
   f->device = device;
   f->spec = *spec;
-  if (cudaStreamCreateWithFlags(&f->own, cudaStreamNonBlocking) != cudaSuccess) {
-    cudaGetLastError();
+  if (int rc = frame_stream(&f->own)) {
     delete f;
-    return fail(DSPGN_E_CUDA, "cudaStreamCreateWithFlags");
+    return rc;
   }
   f->stream = f->own;
+  count_frame(device, 1);
   *out = f;
   return 0;
 }
@@ -2246,6 +2292,7 @@ void dspgn_mono_frame_destroy(DspgnMonoFrame* f) {
   f->h_in.release(); f->h_out.release();
   f->d_in.release(); f->d_work.release(); f->d_out.release();
   if (f->own) cudaStreamDestroy(f->own);
+  count_frame(f->device, -1);
   delete f;
 }
 

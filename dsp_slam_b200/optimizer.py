@@ -364,6 +364,13 @@ class BatchSolver:
         """Test hook (dspgn_debug_mesh_arena): the mesh arena of later submits; 0, 0 = automatic."""
         _lib.check(_lib.load().dspgn_debug_mesh_arena(self.handle, int(max_vertices), int(max_faces)))
 
+    def debug_sm_budget(self, n=None):
+        """Test hook (dspgn_debug_sm_budget): force the grid-sized launches onto n SMs; None or 0 = the automatic budget
+        (every SM, or FRAME_RESERVE_SMS fewer while a frame builder is alive).  Returns the SM count of the next launch."""
+        cur = C.c_int32()
+        _lib.check(_lib.load().dspgn_debug_sm_budget(self.handle, int(n or 0), C.byref(cur)))
+        return cur.value
+
     def decode_sdf(self, code, x, class_id=0):
         x = _f32(x)
         code = np.ascontiguousarray(_f32(code)).reshape(-1)

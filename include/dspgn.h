@@ -44,6 +44,8 @@ extern "C" {
 #define DSPGN_MAX_CODE 64
 #define DSPGN_MAX_LINEAR 12
 #define DSPGN_MAX_CLASSES 4
+/* SMs a solver's grid-sized launches leave free while a frame handle is alive on its device (dspgn_keyframe_submit) */
+#define DSPGN_FRAME_RESERVE_SMS 4
 
 /* return codes */
 #define DSPGN_OK 0
@@ -269,7 +271,14 @@ int dspgn_keyframe_batch_meshed(DspgnSolver* s, int n_obj, const DspgnObjectIn* 
  * One call in flight per solver: until wait, every other entry point on the solver returns DSPGN_E_BUSY (results_device
  * and gather_device return NULL, gather_close does nothing) and leaves the call intact, except query, wait,
  * dspgn_solver_sync, dspgn_solver_engine and dspgn_debug_host_syncs; dspgn_solver_destroy waits for the call first.
- * Solvers on different streams may each have a call in flight.  The multi-GPU exchange does not apply. */
+ * Solvers on different streams may each have a call in flight.  The multi-GPU exchange does not apply.
+ * SM budget: the persistent kernels fill a whole SM per CTA, so while one runs on every SM no block of another kernel
+ * starts anywhere.  While at least one frame handle (DspgnLidarFrame, DspgnMonoFrame) is alive on the solver's device,
+ * every grid-sized launch of every solver there -- the persistent kernels and the per-iteration schedule's decoder
+ * launches, of this call and of the blocking ones -- uses DSPGN_FRAME_RESERVE_SMS fewer CTAs than the device has SMs,
+ * so a Tracking thread's frame call runs beside the keyframe instead of after it.  The budget is read at each launch
+ * (a frame handle may be created after the solver); with no frame handle the launches use every SM.  Records and
+ * meshes do not depend on the budget: they are bit-identical at every SM count. */
 int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* modes /* or NULL: all joint */,
                           const DspgnGateIn* gates /* or NULL */, const DspgnMeshSpec* mesh /* or NULL */);
 int dspgn_keyframe_query(DspgnSolver* s);
@@ -281,6 +290,10 @@ int dspgn_debug_host_syncs(DspgnSolver* s, int64_t* out);
  * automatic size, a per-object estimate that grows with the meshes the solver has seen).  A keyframe whose meshes do not
  * fit is meshed again at the exact size inside dspgn_keyframe_wait: slower, never different. */
 int dspgn_debug_mesh_arena(DspgnSolver* s, int64_t max_vertices, int64_t max_faces);
+/* Test hook: the SM budget of the solver's grid-sized launches (dspgn_keyframe_submit).  n = 0 restores the automatic
+ * budget, 1 <= n <= the device's SM count forces n SMs, anything else returns DSPGN_E_ARG.  current (may be NULL)
+ * receives the SM count the next grid-sized launch would use. */
+int dspgn_debug_sm_budget(DspgnSolver* s, int n, int32_t* current);
 
 /* Forward-only decode (loss_utils.decode_sdf): x (n,3) host, strides in elements -> sdf (n,) host. */
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n,
@@ -390,7 +403,12 @@ int dspgn_debug_events(DspgnSolver* s, long long* out, int max_events);
  *            synchronisation) and writes one DspgnLidarBoxOut per box.  Limits: scan <= 2^22 points, <= 256 boxes,
  *            <= 64 masks, each bbox 0 <= l <= r <= img_w and 0 <= t <= b <= img_h after truncation.
  *   results  the arrays of the last run, box after box: points (sum n_pts x 3), depth (sum n_pts), rays
- *            (sum of n_rays > 0, x 3).  Any pointer may be NULL. */
+ *            (sum of n_rays > 0, x 3).  Any pointer may be NULL.
+ * Beside a running keyframe: while the handle is alive, the solvers on its device leave DSPGN_FRAME_RESERVE_SMS SMs
+ * free (dspgn_keyframe_submit), and the handle's own stream has the device's greatest priority, so its blocks are
+ * dispatched ahead of a solver's queued kernels: a run does not wait for LocalMapping's keyframe.  A run allocates
+ * nothing once its buffers are large enough; the first run with more scan points, boxes or masks than any before may
+ * grow them (+25 % headroom), and freeing the old buffer waits for all work on the device, the keyframe included. */
 typedef struct DspgnLidarFrame DspgnLidarFrame;
 typedef struct {
   float k[9];                 /* K (3x3 row-major, float32 as the loader casts it) */
@@ -416,7 +434,8 @@ typedef struct {
 } DspgnLidarBoxOut;
 int dspgn_lidar_frame_create(const DspgnLidarSpec* spec, int device, DspgnLidarFrame** out);
 void dspgn_lidar_frame_destroy(DspgnLidarFrame* f);
-/* the handle enqueues on a non-blocking stream of its own; stream = a cudaStream_t replaces it (NULL = legacy default) */
+/* the handle enqueues on a non-blocking stream of its own (greatest priority); stream = a cudaStream_t replaces it
+ * (NULL = legacy default; the caller's stream keeps the caller's priority) */
 int dspgn_lidar_frame_set_stream(DspgnLidarFrame* f, void* cuda_stream);
 /* scan: n_points x 4 float32 (x, y, z, reflectance); masks: n_masks x img_h x img_w bytes (numpy bool, nonzero =
  * inside); bboxes: n_masks x 4 int32 (l, t, r, b), the masks' boxes truncated like astype(int32) */
@@ -444,7 +463,9 @@ int dspgn_lidar_frame_results(DspgnLidarFrame* f, float* points, float* depth, f
  *            img_w and 0 <= t <= b <= img_h after truncation, <= 2^20 keypoints, each finite with -1 < x < img_w and
  *            -1 < y < img_h (its truncation inside the image).
  *   results  the arrays of the last run: background_rays (n_rays x 3, when n_rays > 0), feature_idx (n_feature).
- *            Either pointer may be NULL. */
+ *            Either pointer may be NULL.
+ * Beside a running keyframe: as DspgnLidarFrame (the SM reserve, the stream priority, and growth only on the first run
+ * with more masks or keypoints than any before). */
 typedef struct DspgnMonoFrame DspgnMonoFrame;
 typedef struct {
   double k[9];                /* K_cam (3x3 row-major, float64 from the yaml's Camera.fx/fy/cx/cy) */

@@ -8,7 +8,14 @@ config's num_lidar_max 250, min_mask_area 1000, downsample_ratio 4.  Legs, alter
                 device time of its stream work (CUDA events around the call: H2D, kernels, D2H; separate pass); and
                 the four kernels' time from torch.profiler (separate pass)
   c  busy       leg b issued right after keyframe_batch_async submitted tools/keyframe_bench.py's gated keyframe
-                (meshed at 32), which is still running; the keyframe is collected after the timed call
+                (meshed at 32), which is still running; the keyframe is collected after the timed call.  The solver's
+                SM budget is forced to every SM (dspgn_debug_sm_budget): the launches as they are without a frame handle
+  d<k>          leg c with the budget forced to k SMs fewer (k = 4, 8, 16): what a live frame handle does with
+                DSPGN_FRAME_RESERVE_SMS = k
+
+Legs c and d<k> alternate step by step.  Each reports the frame call's time, the fraction of steps in which the keyframe
+was still running when the call returned, and the keyframe's submit->collect time beside the frame call against the
+same keyframe alone at the same budget (submitted and collected just before).
 
 Every leg's instances are compared bit for bit with leg a's.  Prints one JSON line with medians and spreads (p10-p90)
 in ms, and the card's name, power limit and max SM clock read in the same run.
@@ -51,6 +58,42 @@ def same(got, want):
             assert np.array_equal(a["rays"], b["rays"]) and np.array_equal(a["depth"], b["depth"])
 
 
+RESERVES = (4, 8, 16)
+
+
+def busy_budgets(n_sms):
+    """leg -> forced SM budget: c every SM, d<k> k SMs left free"""
+    return dict([("c", n_sms)] + [(f"d{k}", n_sms - k) for k in RESERVES])
+
+
+def busy_step(opt, new, tracked, call, leg, budget, t, keep):
+    """One step of a busy leg: the keyframe alone, then again with `call` issued right after its submit.  Returns what
+    `call` returned."""
+    opt.solver.debug_sm_budget(budget)
+    k0 = time.perf_counter()
+    opt.keyframe_batch_async(new, tracked, voxels_dim=32).result()
+    k1 = time.perf_counter()
+    fut = opt.keyframe_batch_async(new, tracked, voxels_dim=32)
+    t0 = time.perf_counter(); got = call(); t1 = time.perf_counter()
+    pending = not fut.done()
+    fut.result()
+    k2 = time.perf_counter()
+    opt.solver.debug_sm_budget(None)
+    if keep:
+        t.setdefault(f"{leg}_device_busy_ms", []).append(1e3 * (t1 - t0))
+        t.setdefault(f"{leg}_keyframe_busy_ms", []).append(1e3 * (k2 - k1))
+        t.setdefault(f"{leg}_keyframe_alone_ms", []).append(1e3 * (k1 - k0))
+        t.setdefault(f"{leg}_still_running", []).append(int(pending))
+    return got
+
+
+def busy_report(t):
+    """legs' stats, with the still-running flags as fractions"""
+    legs = {k: stats(v) for k, v in t.items() if not k.endswith("_still_running")}
+    frac = {k[:-len("_still_running")]: float(np.mean(v)) for k, v in t.items() if k.endswith("_still_running")}
+    return legs, frac
+
+
 def stats(v):
     v = np.asarray(v)
     return {"median": float(np.median(v)), "p10": float(np.percentile(v, 10)), "p90": float(np.percentile(v, 90)),
@@ -90,25 +133,19 @@ def main():
     def dev(f):
         return b.detections(f["scan"], f["dets"], f["masks"], f["bboxes"])
 
-    t = {"a_numpy_ms": [], "b_device_ms": [], "c_device_busy_ms": [], "b_stream_ms": [], "keyframe_ms": []}
+    n_sms = torch.cuda.get_device_properties(0).multi_processor_count
+    budgets = list(busy_budgets(n_sms).items())
+    t = {"a_numpy_ms": [], "b_device_ms": [], "b_stream_ms": []}
     for step in range(args.warmup + args.steps):
         f = frames[step % len(frames)]
         t0 = time.perf_counter(); want = host(f); t1 = time.perf_counter()
         got = dev(f); t2 = time.perf_counter()
         same(got, want)
-        k0 = time.perf_counter()
-        fut = opt.keyframe_batch_async(new, tracked, voxels_dim=32)
-        t3 = time.perf_counter(); busy = dev(f); t4 = time.perf_counter()
-        busy_pending = not fut.done()
-        fut.result()
-        k1 = time.perf_counter()
-        same(busy, want)
+        for leg, budget in budgets[step % len(budgets):] + budgets[:step % len(budgets)]:
+            same(busy_step(opt, new, tracked, lambda: dev(f), leg, budget, t, step >= args.warmup), want)
         if step >= args.warmup:
             t["a_numpy_ms"].append(1e3 * (t1 - t0))
             t["b_device_ms"].append(1e3 * (t2 - t1))
-            t["c_device_busy_ms"].append(1e3 * (t4 - t3))
-            t["keyframe_ms"].append(1e3 * (k1 - k0))
-            t.setdefault("c_keyframe_still_running", []).append(int(busy_pending))
     # device time of the call's stream work (events around the call on the handle's stream)
     s = torch.cuda.Stream()
     b.set_stream(s.cuda_stream)
@@ -127,9 +164,9 @@ def main():
         for f in frames:
             dev(f)
     kern = [e for e in prof.key_averages() if "k_frame" in e.key]
-    res = {"card": card(), "points": args.points, "steps": args.steps,
-           "legs": {k: stats(v) for k, v in t.items() if k != "c_keyframe_still_running"},
-           "c_keyframe_still_running_frac": float(np.mean(t["c_keyframe_still_running"])),
+    legs, frac = busy_report(t)
+    res = {"card": card(), "points": args.points, "steps": args.steps, "sms": n_sms, "budgets": dict(budgets),
+           "legs": legs, "keyframe_still_running_frac": frac,
            "kernels_us_per_call": {e.key: getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0)) / len(frames) for e in kern},
            "outputs": "bit-identical in every leg"}
     line = json.dumps(res)

@@ -8,6 +8,10 @@ Seeded frames (synth.make_mono_frame) at the Redwood (640 x 480, erosion 5) and 
   b  device     MonoFrameBuilder.detections end to end (host clock: staging, H2D, two kernels, D2H, unpacking); the
                 device time of its stream work (CUDA events around the call, separate pass); and the kernels' time from
                 torch.profiler (separate pass)
+  c, d<k>       leg b issued right after the solver submitted tools/keyframe_bench.py's gated keyframe (meshed at 32),
+                at a forced SM budget of every SM (c) or k SMs fewer (d4, d8, d16), as in tools/frame_bench.py: the
+                call's time, the fraction of steps in which the keyframe still ran when it returned, and the keyframe's
+                submit->collect time against its time alone at the same budget
 
 Every step's rays and feature indices are compared bit for bit with leg a's.  Prints one JSON line with medians and
 spreads (p10-p90) in ms, and the card's name, power limit and max SM clock read in the same run.
@@ -62,7 +66,14 @@ def main():
     g.build()
     from dsp_slam_b200 import synth
     from dsp_slam_b200.mono_frame import MonoFrameBuilder
-    from frame_bench import card, stats
+    from dsp_slam_b200.optimizer import Optimizer
+    from frame_bench import busy_budgets, busy_report, busy_step, card
+    from keyframe_bench import N_TRACKED, keyframe_inputs
+    kcfg, objs, _ = keyframe_inputs()
+    opt = Optimizer(os.path.join(ROOT, "tests", "golden", "decoder_cars.npz"), kcfg)
+    tracked, new = objs[:N_TRACKED], objs[N_TRACKED:]
+    n_sms = torch.cuda.get_device_properties(0).multi_processor_count
+    budgets = list(busy_budgets(n_sms).items())
     res = {"card": card(), "steps": args.steps, "cv2": cv2.__version__, "cv2_threads": cv2.getNumThreads(), "sizes": {}}
     for cam, e in SIZES.items():
         frames = [synth.make_mono_frame(200 + i, cam, 12, 2000) for i in range(4)]
@@ -80,6 +91,9 @@ def main():
             t0 = time.perf_counter(); want = host_leg(cv2, f, invK, e); t1 = time.perf_counter()
             got = dev(f); t2 = time.perf_counter()
             assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1])
+            for leg, budget in budgets[step % len(budgets):] + budgets[:step % len(budgets)]:
+                busy = busy_step(opt, new, tracked, lambda: dev(f), leg, budget, t, step >= args.warmup)
+                assert np.array_equal(busy[0], want[0]) and np.array_equal(busy[1], want[1])
             if step >= args.warmup:
                 t["a_host_ms"].append(1e3 * (t1 - t0))
                 t["b_device_ms"].append(1e3 * (t2 - t1))
@@ -100,8 +114,9 @@ def main():
                 dev(f)
         kern = [ev for ev in prof.key_averages() if "k_mono" in ev.key or "k_frame" in ev.key]
         H, W = frames[0]["img_hw"]
-        res["sizes"][cam] = {"img_hw": [H, W], "erosion": e, "masks": 12, "keypoints": 2000,
-                             "legs": {k: stats(v) for k, v in t.items()},
+        legs, frac = busy_report(t)
+        res["sizes"][cam] = {"img_hw": [H, W], "erosion": e, "masks": 12, "keypoints": 2000, "sms": n_sms,
+                             "budgets": dict(budgets), "legs": legs, "keyframe_still_running_frac": frac,
                              "kernels_us_per_call": {ev.key: getattr(ev, "device_time_total", getattr(ev, "cuda_time_total", 0)) / len(frames)
                                                      for ev in kern},
                              "outputs": "bit-identical in every step"}
