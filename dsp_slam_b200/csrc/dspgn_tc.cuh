@@ -150,10 +150,14 @@ __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;"
 // the tile loop to per-CTA counters: row 0 / 1 = consumer warpgroup 0 / 1, row 2 = producer.  The shipped library
 // compiles none of it.  The epilogue (PR_EPI) is split further: the barrier that opens it (PR_EPI_ENTRY), then per step
 // kind (EpiKind) three slots from PR_EPI_KIND + 3 * kind: the value loop, the split and stores of store_operand, and its
-// proxy fence + warpgroup barrier.
+// proxy fence + warpgroup barrier.  The prologue (PR_PROLOGUE) is split into its global reads with the two barriers
+// (PR_PRO_GLOBAL) and the layer-0 loop with its store_operand (PR_PRO_L0); the tile's final step (PR_JTJ) into the pose
+// columns and residual with their two barriers (PR_JTJ_POSE), the J^T J chains (PR_JTJ_LOOP) and the partial stores
+// (PR_JTJ_STORE).  The probed lanes run J^T J, not J^T r: a J^T r that outlasts J^T J shows up in PR_TILE_END's barrier.
 enum ProbeSlot {
   PR_WFULL, PR_WGWAIT, PR_GEMM, PR_EPI, PR_PROLOGUE, PR_JTJ, PR_TILE_END, PR_SOLVE, PR_FIFO, PR_LOOP, PR_TILES, PR_SOLVES,
-  PR_WEMPTY, PR_POP, PR_PROD_LOOP, PR_EPI_ENTRY, PR_EPI_KIND, kProbeSlots = PR_EPI_KIND + 3 * 6
+  PR_WEMPTY, PR_POP, PR_PROD_LOOP, PR_EPI_ENTRY, PR_EPI_KIND, PR_PRO_GLOBAL = PR_EPI_KIND + 3 * 6, PR_PRO_L0, PR_JTJ_POSE,
+  PR_JTJ_LOOP, PR_JTJ_STORE, kProbeSlots
 };
 // hidden forward, the same before latent_in (concat), last hidden layer, backward, the same at latent_in (skip gradient),
 // first layer backward
@@ -236,7 +240,8 @@ struct TcSmemTail {
 };
 constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail);
 static_assert(kTcSmemBytes <= 227 * 1024, "tensor-core engine shared memory exceeds the 227 KB per block of sm_90");
-static_assert(offsetof(TcSmemTail, bias) % 8 == 0, "the hidden-layer epilogue reads bias column pairs as float2");
+static_assert(offsetof(TcSmemTail, bias) % 8 == 0 && offsetof(TcSmemTail, w0x) % 8 == 0,
+              "the SDF-tile epilogues read bias and W0 column pairs as float2");
 
 // ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
 // 8-column block j = e >> 2 at row 16w + l/4 (+8 when e & 2), column 8j + 2(l%4) + (e & 1).
@@ -327,13 +332,23 @@ __device__ __forceinline__ void epi_fwd_hidden(float (&acc)[128], uint32_t (&mw)
 
 // the layer before latent_in, after epi_fwd_hidden: columns >= cat_off below k_next take the decoder input
 // [z | x | 0...] (deep_sdf_decoder.py:87-88), read from clamped shared-memory indices and selected.  Column blocks
-// below cat_off are skipped whole (a branch per block, not per element).
-__device__ __forceinline__ void epi_concat_input(float (&acc)[128], int qs, int k_next, int cat_off, int L, const float* zs,
+// below cat_off are skipped whole (a branch per block, not per element).  CAT / LL: cat_off and L at compile time (189
+// and 64 for the 8 x 256 decoders with a 64-wide code): the blocks that lie wholly inside the code then read it at a
+// fixed offset from one lane address, and only the blocks that straddle cat_off or L select per element.  CAT = 0: the
+// runtime cat_off_ / L_.
+template <int CAT, int LL>
+__device__ __forceinline__ void epi_concat_input(float (&acc)[128], int qs, int k_next, int cat_off_, int L_, const float* zs,
                                                  const float* xr, int rowA, int rowB) {
+  const int cat_off = CAT ? CAT : cat_off_, L = CAT ? LL : L_;
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     if (8 * j + 8 <= cat_off) continue;
     const bool nxt = 8 * j < k_next;
+    if (CAT && 8 * j >= cat_off && 8 * j + 8 - cat_off <= L) {
+#pragma unroll
+      for (int h = 0; h < 4; ++h) acc[4 * j + h] = nxt ? zs[2 * qs + (8 * j + (h & 1) - cat_off)] : acc[4 * j + h];
+      continue;
+    }
 #pragma unroll
     for (int h = 0; h < 4; ++h) {
       const int e = 4 * j + h, i = 8 * j + 2 * qs + (h & 1) - cat_off, ix = i - L;
@@ -346,13 +361,27 @@ __device__ __forceinline__ void epi_concat_input(float (&acc)[128], int qs, int 
 
 // the layer at latent_in, before epi_bwd_mid: the gradient of its skip columns (>= cat_off) goes to the Jacobian tile
 // (the first in0 of them, predicated stores) instead of to the next layer.  Column blocks below cat_off are skipped
-// whole.
-__device__ __forceinline__ void epi_skip_grad(float (&acc)[128], int qs, int nm, int cat_off, int in0, int L, float* Jp, int rowA,
+// whole.  CAT / LL as in epi_concat_input (in0 = LL + 3, and nm = 256: every column is live): the blocks wholly inside
+// the code store unpredicated at a fixed offset from one lane address.
+template <int CAT, int LL>
+__device__ __forceinline__ void epi_skip_grad(float (&acc)[128], int qs, int nm, int cat_off_, int in0_, int L_, float* Jp, int rowA,
                                               int rowB) {
+  const int cat_off = CAT ? CAT : cat_off_, L = CAT ? LL : L_, in0 = CAT ? LL + 3 : in0_;
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     if (8 * j + 8 <= cat_off) continue;
-    const bool live = 8 * j < nm;
+    const bool live = 8 * j < (CAT ? kHid : nm);
+    if (CAT && 8 * j >= cat_off && 8 * j + 8 - cat_off <= L) {
+      float* pa = Jp + rowA * kJpStride + 2 * qs;
+      float* pb = Jp + rowB * kJpStride + 2 * qs;
+#pragma unroll
+      for (int h = 0; h < 4; ++h) {
+        const int e = 4 * j + h, off = 8 * j + (h & 1) - cat_off;
+        ((h & 2) ? pb : pa)[off] = acc[e];
+        acc[e] = 0.f;
+      }
+      continue;
+    }
 #pragma unroll
     for (int h = 0; h < 4; ++h) {
       const int e = 4 * j + h, ii = 8 * j + 2 * qs + (h & 1) - cat_off;
@@ -391,6 +420,32 @@ __device__ __forceinline__ void epi_bwd_first(const float (&acc)[128], int qs, i
       float* pj = Jp + ((h & 2) ? rowB : rowA) * kJpStride + (st ? ((c < L) ? c : (kMaxCode + c - L)) : 0);
       const float g = has_skip ? acc[4 * j + h] + *pj : acc[4 * j + h];
       if (st) *pj = g * ((h & 2) ? sb : sa);                       // loss.py:145 (de_ds) / inactive rows
+    }
+  }
+}
+
+// layer 0 of a decoder whose first GEMM step takes all 256 of its outputs (k_steps * 16 = out_dim[0] = 256): every
+// column is live, bias (zb0) and the xyz rows of W0 are read as column pairs.  The fmaf order is that of the general
+// loop in tc_body:  bias -> x0 -> x1 -> x2.
+__device__ __forceinline__ void epi_layer0_256(float (&acc)[128], uint32_t (&mw)[4], const float* bias, const float* w0x, int qs,
+                                               float xa0, float xa1, float xa2, float xb0, float xb1, float xb2) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const int c = 8 * j + 2 * qs;
+    const float2 bj = *reinterpret_cast<const float2*>(bias + c);
+    const float2 w0 = *reinterpret_cast<const float2*>(w0x + c);
+    const float2 w1 = *reinterpret_cast<const float2*>(w0x + kHid + c);
+    const float2 w2 = *reinterpret_cast<const float2*>(w0x + 2 * kHid + c);
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int e = 4 * j + h;
+      const bool hb = (h & 2) != 0, hy = (h & 1) != 0;
+      float w = hy ? bj.y : bj.x;
+      w = fmaf(hy ? w0.y : w0.x, hb ? xb0 : xa0, w);
+      w = fmaf(hy ? w1.y : w1.x, hb ? xb1 : xa1, w);
+      w = fmaf(hy ? w2.y : w2.x, hb ? xb2 : xa2, w);
+      mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
+      acc[e] = w > 0.f ? w : 0.f;
     }
   }
 }
@@ -831,6 +886,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       }
       if (grp == 0) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; S.scr[r] = sc; }
       epi_bar_sync();                                // zs / xr / bias visible; previous tile fully drained
+      DSPGN_PROBE_ADD(PR_PRO_GLOBAL, tpro);
+      DSPGN_PROBE_T(tl0);
       if (tid == 0) S.cur_class = M.class_id;
 
       // decoder input element i of tile row `row`: [z | x | 0...]
@@ -854,22 +911,27 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         const float xb0 = S.xr[rowB], xb1 = S.xr[kTcRows + rowB], xb2 = S.xr[2 * kTcRows + rowB];
         const int qs = opaque_int(qd);
         uint32_t mw[4] = {0u, 0u, 0u, 0u};
+        if (SCHED == 1 && kk == kHid && n0out == kHid) {
+          epi_layer0_256(acc, mw, S.bias, w0x, qs, xa0, xa1, xa2, xb0, xb1, xb2);
+        } else {
 #pragma unroll
-        for (int e = 0; e < 128; ++e) {
-          const int c = frag_col(e, qs);
-          const bool hb = (e & 2) != 0;
-          float w = S.bias[c];
-          w = fmaf(w0x[c], hb ? xb0 : xa0, w);
-          w = fmaf(w0x[kHid + c], hb ? xb1 : xa1, w);
-          w = fmaf(w0x[2 * kHid + c], hb ? xb2 : xa2, w);
-          const bool on = (c < kk) && (c < n0out) && (w > 0.f);
-          mw[e >> 5] |= (on ? 1u : 0u) << (e & 31);
-          acc[e] = on ? w : 0.f;
+          for (int e = 0; e < 128; ++e) {
+            const int c = frag_col(e, qs);
+            const bool hb = (e & 2) != 0;
+            float w = S.bias[c];
+            w = fmaf(w0x[c], hb ? xb0 : xa0, w);
+            w = fmaf(w0x[kHid + c], hb ? xb1 : xa1, w);
+            w = fmaf(w0x[2 * kHid + c], hb ? xb2 : xa2, w);
+            const bool on = (c < kk) && (c < n0out) && (w > 0.f);
+            mw[e >> 5] |= (on ? 1u : 0u) << (e & 31);
+            acc[e] = on ? w : 0.f;
+          }
         }
 #pragma unroll
         for (int w = 0; w < 4; ++w) maskw[w * kTcEpiThreads] = mw[w];
         put_operand(-1);
       }
+      DSPGN_PROBE_ADD(PR_PRO_L0, tl0);
       DSPGN_PROBE_ADD(PR_PROLOGUE, tpro);
       DSPGN_PROBE_COUNT(PR_TILES);
 
@@ -958,7 +1020,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
             if (nm == 256 && k_next == 256) epi_fwd_hidden<256, 256>(acc, mw, bb, qs, nm, k_next);
             else if (nm == 192 && k_next == 256) epi_fwd_hidden<192, 256>(acc, mw, bb, qs, nm, k_next);
             else epi_fwd_hidden<0, 0>(acc, mw, bb, qs, nm, k_next);
-            if (st.cat_off >= 0) epi_concat_input(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
+            if (st.cat_off == 189 && L == 64) epi_concat_input<189, 64>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
+            else if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
           } else {
 #pragma unroll
             for (int e = 0; e < 128; ++e) {
@@ -982,7 +1045,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
 #pragma unroll
           for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
           if (SCHED == 1) {
-            if (st.cat_off >= 0) epi_skip_grad(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
+            if (st.cat_off == 189 && L == 64 && in0 == 67 && nm == kHid) epi_skip_grad<189, 64>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
+            else if (st.cat_off >= 0) epi_skip_grad<0, 0>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
             if (nm == 256 && k_next == 256) epi_bwd_mid<256, 256>(acc, mw, nm, k_next);
             else if (nm == 256 && k_next == 192) epi_bwd_mid<256, 192>(acc, mw, nm, k_next);
             else epi_bwd_mid<0, 0>(acc, mw, nm, k_next);
@@ -1051,10 +1115,12 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         if (mask_out != nullptr && mode == MODE_SDF && r < nrows)
           mask_out[M.pts_off + row0 + r] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;      // optimizer.py:76-78
         S.rr[r] = huber_weight(fabsf(res), huber_b) * res;
+        if (SCHED == 1) jr[kMaxCode + 7] = S.rr[r];      // the J^T J chains of column block 17 give J^T (rho r) as well
         S.rsc[r] = (mode == MODE_SDF) ? sc : (r < nrows ? 1.f : 0.f);
         if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF && r < nrows) a.dbg_res[row0 + r] = res;
       }
       epi_bar_sync();
+      DSPGN_PROBE_ADD(PR_JTJ_POSE, tjtj);
       if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF) {
         const int P = a.dbg_P, npose = (ost.mode == DSPGN_MODE_POSE) ? 6 : 7;
         for (int idx = tid; idx < nrows * P; idx += kTcEpiThreads) {
@@ -1066,6 +1132,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       // ---- J^T J, J^T (rho r), loss over the 128 rows of the tile (optimizer.py:161-167) -------------
       float* accp = part + (size_t)tile * kAccStride;
       if (tid < 171) {
+        DSPGN_PROBE_T(tjl);
         int bi = 0, rem = tid;
         while (rem >= 18 - bi) { rem -= 18 - bi; ++bi; }
         const int bj = bi + rem;
@@ -1086,6 +1153,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
 #pragma unroll
             for (int v = 0; v < 4; ++v) h[u][v] = fmaf(av[u], bv[v], h[u][v]);
         }
+        DSPGN_PROBE_ADD(PR_JTJ_LOOP, tjl);
+        DSPGN_PROBE_T(tjs);
 #pragma unroll
         for (int u = 0; u < 4; ++u)
 #pragma unroll
@@ -1093,7 +1162,14 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
             const int rI = 4 * bi + u, cI = 4 * bj + v;
             if (cI >= rI && cI < kMaxCode + 7) accp[tri_index(rI, cI)] = h[u][v];
           }
-      } else if (tid < 171 + kMaxCode + 7) {
+        if (SCHED == 1 && bj == 17) {
+          // column 71 holds rho r: the same fmaf chains over p as the J^T r loop below
+#pragma unroll
+          for (int u = 0; u < 4; ++u)
+            if (4 * bi + u < kMaxCode + 7) accp[kAccB + 4 * bi + u] = h[u][3];
+        }
+        DSPGN_PROBE_ADD(PR_JTJ_STORE, tjs);
+      } else if (SCHED != 1 && tid < 171 + kMaxCode + 7) {
         const int c = tid - 171;
         float sacc = 0.f;
         for (int p = 0; p < kTcRows; ++p) sacc = fmaf(S.Jp[p * kJpStride + c], S.rr[p], sacc);

@@ -30,6 +30,9 @@ SLOTS = ["wfull_wait", "wgmma_wait", "gemm", "epilogue", "prologue_layer0", "jtj
 EPI_KINDS = ["fwd", "fwd_concat", "penult", "bwd", "bwd_skip", "bwd_first"]
 EPI_PARTS = ["values", "split_store", "fence_bar"]
 SLOTS += [f"epi_{k}_{p}" for k in EPI_KINDS for p in EPI_PARTS]
+# sub-parts of prologue_layer0 and jtj (J^T r runs on lanes the probe does not read: its excess lands in tile_end)
+SUB_PARTS = {"prologue_layer0": ["prologue_global", "prologue_l0"], "jtj": ["jtj_pose", "jtj_loop", "jtj_store"]}
+SLOTS += [p for v in SUB_PARTS.values() for p in v]
 N_SLOTS, N_CTAS = len(SLOTS), 256
 
 
@@ -104,6 +107,7 @@ def main():
         "cycles_per_solve": s["solve"] / max(s["solves"], 1),
         "producer_share": {k: sp[k] / max(sp["producer_loop"], 1) for k in ("wempty_wait", "pop")},
         "epilogue_cycles_per_tile": {k: s[k] / s["tiles"] for k in SLOTS if k.startswith("epi_")},
+        "sub_part_cycles_per_tile": {p: s[p] / s["tiles"] for v in SUB_PARTS.values() for p in v},
     }
     print(f"{args.workload} on {gpu}: {ctas} CTAs, {res['tiles_per_run']:.0f} tiles and {res['solves_per_run']:.0f} "
           f"solves per run, {ms:.2f} ms per run (probe build)")
@@ -112,6 +116,9 @@ def main():
         per = res["cycles_per_tile"].get(k, v * loop / s["tiles"])
         print(f"  {k:18s} {100 * v:6.2f} %  {per:10.0f}")
     print(f"  {'loop':18s} {100.0:6.2f} %  {loop / s['tiles']:10.0f}")
+    print("prologue and final step by part, cycles per tile:")
+    for whole, subs in SUB_PARTS.items():
+        print(f"  {whole:18s} " + "  ".join(f"{p} {res['sub_part_cycles_per_tile'][p]:.0f}" for p in subs))
     print("epilogue by step kind, cycles per tile (share of the epilogue):")
     ept = res["epilogue_cycles_per_tile"]
     epi = s["epilogue"] / s["tiles"]
