@@ -117,6 +117,7 @@ struct DspgnSolver {
   bool mega_enabled = true;
   bool compact_rays = true;        // persistent kernel, render term: forward-only tiles over the valid-sample hulls only (env DSPGN_COMPACT_RAYS=0: all n_rays x D samples)
   DevBuf d_ev, d_seg, d_ln, d_vpre;
+  DevBuf d_masks;                  // k_gn_persistent: per-CTA ReLU mask scratch (kTcMaskLayers x kTcEpiThreads uint4 per SM)
   bool events_on = false;          // env DSPGN_CLK: the persistent kernel writes its event log (dspgn_debug_events)
   HostBuf h_results;
   // counters
@@ -404,6 +405,8 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
       if (s->d_ln.reserve(4 * (size_t)s->num_sms * DSPGN_MAX_LINEAR * kHid * kTP)) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
       break;
     }
+  if (eng == DSPGN_ENGINE_TC &&
+      s->d_masks.reserve(sizeof(uint4) * (size_t)s->num_sms * kTcMaskLayers * kTcEpiThreads)) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
   if (int rc = tc_setup_kernels(g_err)) { dspgn_solver_destroy(s); return rc; }
   if (const char* m = getenv("DSPGN_MEGA")) s->mega_enabled = (m[0] != '0');
   if (const char* m = getenv("DSPGN_COMPACT_RAYS")) s->compact_rays = (m[0] != '0');   // A/B switch of the valid-sample hulls
@@ -437,7 +440,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   dspgn_gather_close(s);
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
-                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_run,
+                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_masks, &s->d_run,
                     &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout, &s->d_mesh_sel}) b->release();
   s->h_stage.release();
   s->h_mbase.release();
@@ -932,8 +935,8 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0;
     const int grid = grid_sms(s);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
-    if (render) k_gn_persistent_render<<<grid, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
-    else k_gn_persistent<<<grid, kTcThreads, kTcSmemBytes, s->stream>>>(b, a, q, v);
+    if (render) k_gn_persistent_render<<<grid, kTcThreads, kTcSmemBytes<2>, s->stream>>>(b, a, q, v);
+    else k_gn_persistent<<<grid, kTcThreads, kTcSmemBytes<1>, s->stream>>>(b, a, q, v, s->d_masks.as<uint4>());
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
     s->ctr.kernel_launches += 1;
     for (int m = 0; m < 2; ++m) s->ctr.rows_fwd_bwd += p.pts[m] * p.iters[m];

@@ -44,6 +44,10 @@ constexpr int kTcThreads = 384;          // 2 consumer warpgroups + 1 producer w
 constexpr int kTcEpiThreads = 256;
 constexpr int kTcStages = 4;              // one 64-wide K chunk: hi[k 0..31], hi[k 32..63], lo[k 0..31], lo[k 32..63]
 constexpr int kTcStageBytes = 16384;      // one ring stage: up to 256 rows x 32 K x fp16 (64 B rows, SWIZZLE_64B)
+// Stages of the weight ring of a schedule (tc_body SCHED): one K chunk, or one and a half in the SDF-tile kernel, whose
+// ReLU masks live in global memory (TcSmemTail) to make room.  Deeper, the ring keeps refills further ahead of the MMAs
+// and holds more of the next step while an epilogue runs.
+template <int SCHED> constexpr int kTcRing = SCHED == 1 ? 6 : kTcStages;
 constexpr int kTcAloBytes = 32768;        // lo halves of one warpgroup's A operand: 4 x (64 rows x 128 B)
 // Registers are allocated per warpgroup: the producer warpgroup hands most of its share to the two consumer
 // warpgroups (setmaxnreg), which hold the fp32 accumulator (128) and the register A fragment (64).  The pair must fit
@@ -89,6 +93,12 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+
+// 16 bytes global -> shared, bypassing L1; cp_async_wait_all: every earlier cp_async_16 of this thread has landed
+__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gmem_src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // generic-proxy shared-memory writes (the A lo image) before the async proxy (wgmma) reads them
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -215,9 +225,13 @@ __device__ __forceinline__ void split_pack(float a, float b, uint32_t& hi, uint3
 // shared-memory carve-up
 // ------------------------------------------------------------------------------------------------
 constexpr int kJpStride = 76;             // floats per row of the point-major Jacobian tile (72 + pad, 16B aligned)
+constexpr int kTcMaskLayers = 8;          // hidden layers with a saved ReLU mask (layers 0 .. 7 of the 8 x 256 decoders)
+template <int SCHED>
 struct TcSmemTail {
   float Jp[kTcRows * kJpStride];          // [row][72+4]: J row of each point; cols 0..66 double as latent_in skip gradient
-  uint32_t maskw[8 * 4 * kTcEpiThreads];  // ReLU masks [layer][word][consumer thread]: bit e of word w = fragment element 32w+e
+  // ReLU masks [layer][word][consumer thread]: bit e of word w = fragment element 32w+e.  SCHED 1 keeps them in a per-CTA
+  // global scratch ([layer][consumer thread] of uint4) and stages here only the layer a backward step reads: [thread] of uint4.
+  uint32_t maskw[(SCHED == 1 ? 1 : kTcMaskLayers) * 4 * kTcEpiThreads];
   float bias[9 * kHid];
   float wlast[kHid];
   float w0x[3 * kHid];                    // xyz rows of the layer-0 matrix (the latent rows are folded into ObjState.zb0)
@@ -225,9 +239,9 @@ struct TcSmemTail {
   float xr[3 * kTcRows];                  // object-frame point of every row
   float rr[kTcRows], rsc[kTcRows];
   float yrow[kTcRows], scr[kTcRows];      // decoder output and row weight (0 = inactive row) of every row
-  int prefix[kMaxObjScan + 1];
+  int prefix[SCHED == 1 ? 1 : kMaxObjScan + 1];     // tile prefix of the per-iteration schedule (unused by SCHED 1)
   int warp_tmp[32];
-  uint64_t w_full[kTcStages], w_empty[kTcStages];   // adjacent: wg_gemm addresses both from w_full
+  uint64_t w_full[kTcRing<SCHED>], w_empty[kTcRing<SCHED>];   // adjacent: wg_gemm addresses both from w_full
   int cur_class;
   int fifo[4]; int fifo_pub; int epi_seq; int last_flag;   // persistent mode: CTA-local tile FIFO (scheduler = producer warp)
   TcPlan plans[DSPGN_MAX_CLASSES];        // step plans of every decoder class (read by all warp roles)
@@ -238,10 +252,14 @@ struct TcSmemTail {
   int push_base, push_nF, push_nS, push_o;   // cooperative publication of an object's next-iteration tiles
   float ost[16]; int ost_rows;            // the tile's object: T_oc[12], dmin, dmax, dstep, dfar; rows of its term (counter)
 };
-constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail);
-static_assert(kTcSmemBytes <= 227 * 1024, "tensor-core engine shared memory exceeds the 227 KB per block of sm_90");
-static_assert(offsetof(TcSmemTail, bias) % 8 == 0 && offsetof(TcSmemTail, w0x) % 8 == 0,
+template <int SCHED>
+constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcRing<SCHED> * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail<SCHED>);
+static_assert(kTcSmemBytes<0> <= 227 * 1024, "k_decoder_tc: shared memory exceeds the 227 KB per block of sm_90");
+static_assert(kTcSmemBytes<1> <= 227 * 1024, "k_gn_persistent: shared memory exceeds the 227 KB per block of sm_90");
+static_assert(kTcSmemBytes<2> <= 227 * 1024, "k_gn_persistent_render: shared memory exceeds the 227 KB per block of sm_90");
+static_assert(offsetof(TcSmemTail<1>, bias) % 8 == 0 && offsetof(TcSmemTail<1>, w0x) % 8 == 0,
               "the SDF-tile epilogues read bias and W0 column pairs as float2");
+static_assert(offsetof(TcSmemTail<1>, maskw) % 16 == 0, "the SDF-tile kernel stages one uint4 of masks per thread");
 
 // ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
 // 8-column block j = e >> 2 at row 16w + l/4 (+8 when e & 2), column 8j + 2(l%4) + (e & 1).
@@ -456,32 +474,47 @@ __device__ __forceinline__ void release_stage(uint32_t w_empty, int s) {
   if ((threadIdx.x & 31) == 0) mbar_arrive(w_empty + 8u * s);
 }
 
-// One GEMM step of a consumer warpgroup: acc = A * W^T over nch K chunks of 64, W streamed through the 4-stage ring.  The
-// stages of a chunk arrive as hi[k 0..31], hi[k 32..63], lo[k 0..31], lo[k 32..63], so every output element accumulates in
-// the order  A_hi W_hi, A_lo W_hi  per K-step, then  A_hi W_lo  per K-step,  as when the chunk was one image pair.  Each
-// chunk is a fixed, unrolled MMA sequence (only the chunk count varies), one commit group per stage.  Behind every
-// second stage `wgmma.wait_group 1` retires all but the newest group and their stages go back to the producer, which
-// refills them while the newest group runs.  Every step consumes whole chunks, so the ring is at stage 0 on entry.
+// Position in a ring of RING stages: the ring stage `k` stages after (stage, phase), and the parity of that lap.  Producer
+// and consumers each carry (stage, phase) across steps and tiles; they visit the stages in the same order.
+template <int RING>
+__device__ __forceinline__ void ring_at(uint32_t stage, uint32_t phase, uint32_t k, uint32_t& slot, uint32_t& par) {
+  const uint32_t g = stage + k, laps = g / RING;
+  slot = g - RING * laps;
+  par = phase ^ (laps & 1u);
+}
+
+// One GEMM step of a consumer warpgroup: acc = A * W^T over nch K chunks of 64, W streamed through the weight ring of
+// RING stages.  The stages of a chunk arrive as hi[k 0..31], hi[k 32..63], lo[k 0..31], lo[k 32..63], so every output
+// element accumulates in the order  A_hi W_hi, A_lo W_hi  per K-step, then  A_hi W_lo  per K-step,  as when the chunk was
+// one image pair.  Each chunk is a fixed, unrolled MMA sequence (only the chunk count varies), one commit group per stage.
+// Behind every second stage `wgmma.wait_group 1` retires all but the newest group and their stages go back to the
+// producer, which refills them while the newest group runs.  Stage s of chunk c sits in ring stage (stage + 4c + s) mod
+// RING; a 4-stage ring holds exactly one chunk, so there every step starts at stage 0.
 // alo, ring, bars: shared-space addresses (32-bit: the MMA sequence runs with few registers to spare); bars holds the
-// kTcStages full barriers followed by the kTcStages empty barriers.
-template <int N>
+// RING full barriers followed by the RING empty barriers.
+template <int N, int RING>
 __device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[64], uint32_t alo, uint32_t ring,
-                                        uint32_t bars, uint32_t& phase, int nch) {
-  static_assert(kTcStages == 4, "one ring lap per K chunk");
-  const uint32_t w_full = bars, w_empty = bars + 8u * kTcStages;
+                                        uint32_t bars, uint32_t& stage, uint32_t& phase, int nch) {
+  static_assert(RING >= kTcStages, "the ring holds at least one K chunk");
+  const uint32_t w_full = bars, w_empty = bars + 8u * RING;
+  const uint32_t st0 = (RING == kTcStages) ? 0u : stage;
+  // Every ring stage is recomputed from the step's start position: a stage index carried from one chunk to the next
+  // makes ptxas serialize the wgmma (C7515).
+  auto slot_of = [&](int k) { uint32_t sl, p; ring_at<RING>(st0, phase, (uint32_t)k, sl, p); return sl; };
 #pragma unroll
   for (int i = 0; i < 128; ++i) acc[i] = 0.f;
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
     if (c < nch) {
-      const uint32_t ph = phase ^ (uint32_t)(c & 1);
 #pragma unroll
       for (int s = 0; s < kTcStages; ++s) {
+        uint32_t slot, ph;
+        ring_at<RING>(st0, phase, (uint32_t)(kTcStages * c + s), slot, ph);
         DSPGN_PROBE_T(tf);
-        mbar_wait(w_full + 8u * s, ph);
+        mbar_wait(w_full + 8u * slot, ph);
         DSPGN_PROBE_ADD(PR_WFULL, tf);
         wg_fence();
-        const uint32_t bw = ring + (uint32_t)s * kTcStageBytes;
+        const uint32_t bw = ring + slot * kTcStageBytes;
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
           const int t = 4 * c + 2 * (s & 1) + k;             // K-step of the step
@@ -494,14 +527,14 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[
           DSPGN_PROBE_T(tw);
           wg_wait1();
           DSPGN_PROBE_ADD(PR_WGWAIT, tw);
-          release_stage(w_empty, 0);
-          if (c > 0) release_stage(w_empty, 3);
+          release_stage(w_empty, slot_of(kTcStages * c));
+          if (c > 0) release_stage(w_empty, slot_of(kTcStages * c - 1));
         } else if (s == 3) {
           DSPGN_PROBE_T(tw);
           wg_wait1();
           DSPGN_PROBE_ADD(PR_WGWAIT, tw);
-          release_stage(w_empty, 1);
-          release_stage(w_empty, 2);
+          release_stage(w_empty, slot_of(kTcStages * c + 1));
+          release_stage(w_empty, slot_of(kTcStages * c + 2));
         }
       }
     }
@@ -509,23 +542,29 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[
   DSPGN_PROBE_T(tw);
   wg_wait0();
   DSPGN_PROBE_ADD(PR_WGWAIT, tw);
-  release_stage(w_empty, 3);
-  phase ^= (uint32_t)(nch & 1);
+  release_stage(w_empty, slot_of(kTcStages * nch - 1));
+  ring_at<RING>(st0, phase, (uint32_t)(kTcStages * nch), stage, phase);
 }
 
-// producer side of the ring: the weight images of one GEMM step, nch chunks of 4 stages of img_bytes each
+// producer side of the ring: the weight images of one GEMM step, nch chunks of 4 stages of img_bytes each, into the ring
+// stages from (stage, phase) on
+template <int RING>
 __device__ __forceinline__ void produce_step(const unsigned char* src, int nch, uint32_t img_bytes, unsigned char* ring,
-                                             uint64_t* w_full, uint64_t* w_empty, uint32_t& phase) {
+                                             uint64_t* w_full, uint64_t* w_empty, uint32_t& stage, uint32_t& phase) {
+  uint32_t st = (RING == kTcStages) ? 0u : stage;             // a 4-stage ring holds exactly one chunk
   for (int c = 0; c < nch; ++c) {
     for (int s = 0; s < kTcStages; ++s) {
+      uint32_t slot, ph;
+      ring_at<RING>(st, phase, (uint32_t)s, slot, ph);
       DSPGN_PROBE_T(te);
-      mbar_wait(&w_empty[s], phase ^ 1);
+      mbar_wait(&w_empty[slot], ph ^ 1);
       DSPGN_PROBE_ADD(PR_WEMPTY, te);
-      mbar_expect_tx(&w_full[s], img_bytes);
-      bulk_g2s(ring + (size_t)s * kTcStageBytes, src + (size_t)(kTcStages * c + s) * img_bytes, img_bytes, &w_full[s]);
+      mbar_expect_tx(&w_full[slot], img_bytes);
+      bulk_g2s(ring + (size_t)slot * kTcStageBytes, src + (size_t)(kTcStages * c + s) * img_bytes, img_bytes, &w_full[slot]);
     }
-    phase ^= 1;
+    ring_at<RING>(st, phase, (uint32_t)kTcStages, st, phase);
   }
+  stage = st;
 }
 
 struct TileRef { int o, row0, slot, mode, tile; };
@@ -560,7 +599,7 @@ __device__ inline int mega_pop(const MegaArgs& q, int n_obj) {
 // SCHED: 0 = one launch per term (static tiles), 1 = persistent kernel, SDF tiles only (SDF-only joint runs, pose-only
 // runs: the tile kind is a compile-time constant), 2 = persistent kernel with the render term (all item kinds)
 template <int SCHED>
-__device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, TcSmemTail& S, int seq, int total_tiles, TileRef& t) {
+__device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, TcSmemTail<SCHED>& S, int seq, int total_tiles, TileRef& t) {
   constexpr bool MEGA = SCHED != 0;
   if (!MEGA) {
     const int tile = blockIdx.x + seq * gridDim.x;
@@ -605,7 +644,8 @@ __device__ inline void mega_push(const MegaArgs& q, int kind, int o, int n) {
 
 // all terms of the object's current iteration are in: solve, update, queue the next iteration (or finish).  Called by
 // the 256 epilogue threads of the CTA that completed the object's last outstanding tile.
-__device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int tid) {
+template <int SCHED>
+__device__ __noinline__ void mega_solve_and_advance(TcSmemTail<SCHED>& S, int o, int tid) {
   const BatchDev& b = S.ctx_b;
   const MegaArgs& q = S.ctx_q;
   const SolveArgs& sv = S.ctx_sv;
@@ -666,13 +706,16 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail& S, int o, int ti
   }
 }
 
+// masks_g (SCHED 1 only): the per-CTA ReLU mask scratch, [grid CTA][kTcMaskLayers][consumer thread]
 template <int SCHED>
-__device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, const MegaArgs& q, const SolveArgs& sv) {
+__device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, const MegaArgs& q, const SolveArgs& sv,
+                                        uint4* __restrict__ masks_g) {
   constexpr bool MEGA = SCHED != 0;
   constexpr bool RENDER = SCHED == 2;
+  constexpr int RING = kTcRing<SCHED>;
   extern __shared__ unsigned char tc_smem_raw[];
   unsigned char* ring = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);   // stays a shared-space pointer
-  TcSmemTail& S = *reinterpret_cast<TcSmemTail*>(ring + (size_t)kTcStages * kTcStageBytes + 2 * (size_t)kTcAloBytes);
+  TcSmemTail<SCHED>& S = *reinterpret_cast<TcSmemTail<SCHED>*>(ring + (size_t)RING * kTcStageBytes + 2 * (size_t)kTcAloBytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   const int total_tiles = MEGA ? 0 : build_tile_prefix(b, a, kTcRows, S.prefix, S.warp_tmp);
@@ -684,7 +727,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
     }
   }
   if (tid == 0) {
-    for (int i = 0; i < kTcStages; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
+    for (int i = 0; i < RING; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
     S.cur_class = -1;
     S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
     if (MEGA) { S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv; }
@@ -697,7 +740,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
     // The producer warpgroup gives its registers to the consumers; only warp 8 lane 0 has work.
     setmaxnreg_dec<kTcProducerRegs>();
     if (warp == 8 && lane == 0) {
-      uint32_t phase = 0;
+      uint32_t stage = 0, phase = 0;
       DSPGN_PROBE_T(tloop);
       for (int seq = 0;; ++seq) {
         if (MEGA) {
@@ -721,8 +764,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD || (!MEGA && tr.mode == MODE_GRIDFWD));
         const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
         for (int s = 0; s < ns; ++s)
-          produce_step(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full,
-                       S.w_empty, phase);
+          produce_step<RING>(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma, ring,
+                             S.w_full, S.w_empty, stage, phase);
       }
       DSPGN_PROBE_ADD(PR_PROD_LOOP, tloop);
     }
@@ -736,9 +779,9 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
     const int qd = lane & 3;                                   // fragment column pair
     const int rl = 16 * (warp & 3) + (lane >> 2);              // fragment rows rl, rl + 8 of the warpgroup
     const int rowA = 64 * grp + rl, rowB = rowA + 8;           // ... as tile rows
-    unsigned char* const alo = ring + (size_t)kTcStages * kTcStageBytes + (size_t)grp * kTcAloBytes;
+    unsigned char* const alo = ring + (size_t)RING * kTcStageBytes + (size_t)grp * kTcAloBytes;
     const uint32_t alo_s = smem_u32(alo), ring_s = smem_u32(ring);
-    uint32_t phase = 0;
+    uint32_t stage = 0, phase = 0;
     float acc[128];
     uint32_t ah[64];
     DSPGN_PROBE_T(tloop);
@@ -896,6 +939,17 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         return (j < 0) ? S.zs[i] : ((unsigned)j < 3u ? S.xr[j * kTcRows + row] : 0.f);
       };
       uint32_t* const maskw = S.maskw + tid;           // word w of layer l: maskw[(4 * l + w) * kTcEpiThreads]
+      // SCHED 1: this thread's masks of layer l in the CTA's global scratch (16 bytes, written once per tile by the
+      // forward step, read once by a backward step)
+      auto mask_g = [&](int l) { return masks_g + ((size_t)blockIdx.x * kTcMaskLayers + l) * kTcEpiThreads + tid; };
+      auto save_mask = [&](int l, const uint32_t (&mw)[4]) {
+        if (SCHED == 1) {
+          *mask_g(l) = make_uint4(mw[0], mw[1], mw[2], mw[3]);
+        } else {
+#pragma unroll
+          for (int w = 0; w < 4; ++w) maskw[(4 * l + w) * kTcEpiThreads] = mw[w];
+        }
+      };
       auto put_operand = [&](int pslot) {
         if (SCHED == 1) store_operand_stsm(acc, ah, alo_s, grp, pslot);
         else store_operand(acc, ah, alo, rl, qd, grp, pslot);
@@ -927,8 +981,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
             acc[e] = on ? w : 0.f;
           }
         }
-#pragma unroll
-        for (int w = 0; w < 4; ++w) maskw[w * kTcEpiThreads] = mw[w];
+        save_mask(0, mw);
         put_operand(-1);
       }
       DSPGN_PROBE_ADD(PR_PRO_L0, tl0);
@@ -943,10 +996,14 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         const int nm = st.n_mma;
         if (MEGA && tid == 0 && s == 0) log_event(q.log, ev_desc(EV_FIRST_MMA, tr.mode, tr.o, tr.tile));
         const int nch = st.k_steps / 4;
+        // SCHED 1: the masks a backward step needs are copied into the staging slot while its GEMM runs.  Each thread
+        // copies and later reads only its own 16 bytes, which it stored itself in the forward pass: cp.async is a weak
+        // memory operation of the issuing thread, ordered after that store, so neither a fence nor a barrier is needed.
+        if (SCHED == 1 && st.kind == TK_BWD_MID) cp_async_16(smem_u32(S.maskw) + 16u * (uint32_t)tid, mask_g(st.mask_layer));
         DSPGN_PROBE_T(tg);
-        if (nm == 80) wg_gemm<80>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
-        else if (nm == 192) wg_gemm<192>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
-        else wg_gemm<256>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), phase, nch);
+        if (nm == 80) wg_gemm<80, RING>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), stage, phase, nch);
+        else if (nm == 192) wg_gemm<192, RING>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), stage, phase, nch);
+        else wg_gemm<256, RING>(acc, ah, alo_s, ring_s, smem_u32(S.w_full), stage, phase, nch);
         DSPGN_PROBE_ADD(PR_GEMM, tg);
         DSPGN_PROBE_T(tepi);
         wg_bar_sync(grp);                                // every MMA of the warpgroup has read the A lo image
@@ -978,8 +1035,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
               else pa = fmaf(fmaxf(w, 0.f), S.wlast[c], pa);
             }
           }
-#pragma unroll
-          for (int w = 0; w < 4; ++w) maskw[(4 * st.layer + w) * kTcEpiThreads] = mw[w];
+          save_mask(st.layer, mw);
           pa += __shfl_xor_sync(0xffffffffu, pa, 1);
           pb += __shfl_xor_sync(0xffffffffu, pb, 1);
           pa += __shfl_xor_sync(0xffffffffu, pa, 2);
@@ -1036,14 +1092,19 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
               acc[e] = (c < k_next) ? t : 0.f;
             }
           }
-#pragma unroll
-          for (int w = 0; w < 4; ++w) maskw[(4 * st.layer + w) * kTcEpiThreads] = mw[w];
+          save_mask(st.layer, mw);
           DSPGN_PROBE_ADD(pk, tval);
           put_operand(pk);
         } else if (st.kind == TK_BWD_MID) {
           uint32_t mw[4];
+          if (SCHED == 1) {
+            cp_async_wait_all();
+            const uint4 m = reinterpret_cast<const uint4*>(S.maskw)[tid];
+            mw[0] = m.x; mw[1] = m.y; mw[2] = m.z; mw[3] = m.w;
+          } else {
 #pragma unroll
-          for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
+            for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
+          }
           if (SCHED == 1) {
             if (st.cat_off == 189 && L == 64 && in0 == 67 && nm == kHid) epi_skip_grad<189, 64>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
             else if (st.cat_off >= 0) epi_skip_grad<0, 0>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
@@ -1229,16 +1290,17 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) k_decoder_tc(BatchDev b, TermArgs a) {
-  tc_body<0>(b, a, MegaArgs{}, SolveArgs{});
+  tc_body<0>(b, a, MegaArgs{}, SolveArgs{}, nullptr);
 }
 // persistent object-pipelined variants: all GN iterations of all objects in ONE launch.
 // k_gn_persistent: SDF tiles only (SDF-only joint runs, pose-only runs); k_gn_persistent_render: joint runs with the
 // render term (ray-sample tiles, scan items, band tiles, SDF tiles)
-__global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv) {
-  tc_body<1>(b, a, q, sv);
+// masks: ReLU mask scratch of kTcMaskLayers x kTcEpiThreads uint4 per CTA of the grid (the grid is at most the SM count)
+__global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv, uint4* masks) {
+  tc_body<1>(b, a, q, sv, masks);
 }
 __global__ void __launch_bounds__(kTcThreads, 1) k_gn_persistent_render(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv) {
-  tc_body<2>(b, a, q, sv);
+  tc_body<2>(b, a, q, sv, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1261,10 +1323,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_tc_selftest(const float* __re
   }
   __syncthreads();
   const int n_img = tc_mma_n(n_mma), nch = tc_pad_k_steps(k_steps) / 4;
-  uint32_t phase = 0;
+  uint32_t stage = 0, phase = 0;
   if (warp >= 8) {
     setmaxnreg_dec<kTcProducerRegs>();
-    if (warp == 8 && lane == 0) produce_step(blob, nch, 64u * (uint32_t)n_img, ring, w_full, w_empty, phase);
+    if (warp == 8 && lane == 0) produce_step<kTcStages>(blob, nch, 64u * (uint32_t)n_img, ring, w_full, w_empty, stage, phase);
     return;
   }
   setmaxnreg_inc<kTcConsumerRegs>();
@@ -1279,9 +1341,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_tc_selftest(const float* __re
     acc[e] = (c < k_steps * 16) ? A[(size_t)((e & 2) ? rowB : rowA) * lda + c] : 0.f;
   }
   store_operand(acc, ah, alo, rl, qd, grp);
-  if (n_img == 80) wg_gemm<80>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), phase, nch);
-  else if (n_img == 192) wg_gemm<192>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), phase, nch);
-  else wg_gemm<256>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), phase, nch);
+  if (n_img == 80) wg_gemm<80, kTcStages>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), stage, phase, nch);
+  else if (n_img == 192) wg_gemm<192, kTcStages>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), stage, phase, nch);
+  else wg_gemm<256, kTcStages>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), stage, phase, nch);
 #pragma unroll
   for (int e = 0; e < 128; ++e) {
     const int c = frag_col(e, qd);
@@ -1393,12 +1455,12 @@ inline void tc_free_decoder(TcDecoderHost& h) {
 }
 
 inline int tc_setup_kernels(std::string& err) {
-  if (cudaFuncSetAttribute(k_decoder_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes) != cudaSuccess) {
+  if (cudaFuncSetAttribute(k_decoder_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes<0>) != cudaSuccess) {
     err = std::string("cudaFuncSetAttribute(k_decoder_tc): ") + cudaGetErrorString(cudaGetLastError());
     return DSPGN_E_CUDA;
   }
-  if (cudaFuncSetAttribute(k_gn_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(k_gn_persistent_render, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes) != cudaSuccess) {
+  if (cudaFuncSetAttribute(k_gn_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes<1>) != cudaSuccess ||
+      cudaFuncSetAttribute(k_gn_persistent_render, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes<2>) != cudaSuccess) {
     err = std::string("cudaFuncSetAttribute(k_gn_persistent): ") + cudaGetErrorString(cudaGetLastError());
     return DSPGN_E_CUDA;
   }
@@ -1415,7 +1477,7 @@ inline int tc_launch_term(const BatchDev& b, const TermArgs& a, int num_sms, lon
                           std::string& err) {
   int grid = (int)std::min<long long>(tiles_upper, num_sms);
   if (grid < 1) grid = 1;
-  k_decoder_tc<<<grid, kTcThreads, kTcSmemBytes, stream>>>(b, a);
+  k_decoder_tc<<<grid, kTcThreads, kTcSmemBytes<0>, stream>>>(b, a);
   (void)err;
   return 0;
 }

@@ -1,6 +1,6 @@
 """Where a tensor-core tile's cycles go, from a probe build of the library (on an H100).
 
-  python tools/tile_probe.py [--workload cfg2_sdf] [--runs 5] [--out DIR]
+  python tools/tile_probe.py [--workload cfg2_sdf] [--runs 5] [--sm-budget N] [--out DIR]
 
 Compiles the library with -DDSPGN_STALL_PROBE into DIR (the shipped library is not touched): lane 0 of consumer warp 0
 of each warpgroup and the producer lane add the clock64 cycles of each part of the persistent tile loop to per-CTA
@@ -8,6 +8,8 @@ counters (dspgn_tc.cuh, ProbeSlot).  Runs the workload `runs` times after a warm
 consumer loop spent in each part, the producer's wait for free ring stages, cycles per tile and per solve, and the card
 (name, power limit, max SM clock) read in the same call.  Writes DIR/tile_probe.json.  The probe's clock reads and
 counter updates add a little work of their own; the shares are what matter, not the absolute time.
+--sm-budget N runs the persistent kernel on N SMs (BatchSolver.debug_sm_budget): half the SMs ask half as much of L2,
+so a ring wait that is L2 contention shrinks with the budget, one that is latency does not.
 """
 import argparse
 import ctypes as C
@@ -57,6 +59,7 @@ def main():
     ap.add_argument("--workload", default="cfg2_sdf")
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--out", default=None, help="directory for the probe build and tile_probe.json (default: temporary)")
+    ap.add_argument("--sm-budget", type=int, default=0, help="SMs of the persistent kernel (default 0: every SM)")
     ap.add_argument("--lib", default=None, help="an existing probe build of this tree to run instead of compiling one")
     args = ap.parse_args()
     out = os.path.abspath(args.out) if args.out else tempfile.mkdtemp(prefix="tile_probe_")
@@ -75,6 +78,7 @@ def main():
         raise SystemExit("one decoder class per run: pick a workload other than " + args.workload)
     opt = Optimizer(os.path.join(ROOT, "tests", "golden", f"decoder_{cls}.npz"), cfg, sdf_only=sdf_only, engine="tc")
     opt.solver.upload(ins)
+    sms = opt.solver.debug_sm_budget(args.sm_budget)
     modes = [0] * len(ins)
     for _ in range(3):
         opt.solver.run_modes(modes)
@@ -100,7 +104,7 @@ def main():
     share["mma_issue_other"] = (s["gemm"] - s["wfull_wait"] - s["wgmma_wait"]) / loop
     share["unaccounted"] = 1.0 - sum(share.values())
     res = {
-        "workload": args.workload, "gpu": gpu, "ctas": ctas, "runs": args.runs, "ms_per_run_probe_build": ms,
+        "workload": args.workload, "gpu": gpu, "sm_budget": sms, "ctas": ctas, "runs": args.runs, "ms_per_run_probe_build": ms,
         "tiles_per_run": s["tiles"] / 2 / args.runs, "solves_per_run": s["solves"] / 2 / args.runs,
         "consumer_share": share,
         "cycles_per_tile": {k: s[k] / s["tiles"] for k in parts + ["gemm"]} | {"loop": loop / s["tiles"]},
