@@ -9,6 +9,7 @@
 #include <new>
 #include <algorithm>
 #include <atomic>
+#include <thread>
 
 #include <cub/device/device_scan.cuh>
 
@@ -176,6 +177,17 @@ struct DspgnSolver {
   long long arena_force_v = 0, arena_force_f = 0;   // dspgn_debug_mesh_arena
   long long host_syncs = 0;          // dspgn_debug_host_syncs
   int sm_force = 0;                  // dspgn_debug_sm_budget (0: the automatic budget, grid_sms)
+  // cooperative stop (dspgn_keyframe_stop): a host-mapped word the kernels read, one generation per stoppable call
+  uint32_t* h_stop = nullptr;        // pinned, mapped; the generation of the last call a stop was requested for
+  uint32_t* d_stop = nullptr;        // its device address
+  std::atomic<uint32_t> stop_live{0};   // generation of the call in flight (0: none); read by dspgn_keyframe_stop
+  uint32_t stop_gen = 0;             // generation of the current / last call
+  const volatile uint8_t* stop_flag = nullptr;   // dspgn_solver_set_stop_flag
+  cudaEvent_t ev_poll = nullptr;     // the waits that poll stop_flag
+  int stop_at_obj = -1, stop_at_iter = -1;       // dspgn_debug_stop_at, for the next stoppable call
+  int call_stop_obj = -1, call_stop_iter = -1;   // ... taken by the call in flight (caller object index)
+  int run_stop_slot = -1;            // ... the resident slot of that object in the chunk being enqueued (-1: not in it)
+  const int* run_pair = nullptr;     // the chunk's pair partners on the device (meshed calls with pairs), else nullptr
 };
 
 namespace {
@@ -201,9 +213,62 @@ int grid_sms(const DspgnSolver* s) {
   return frames ? std::max(s->num_sms - kFrameReserveSms, 1) : s->num_sms;
 }
 
+// ---- cooperative stop (dspgn_keyframe_stop) ------------------------------------------------------------------------
+// A stop of the call in flight: the word takes the call's generation, never an older generation over a newer one (a
+// stop that races with the end of its call cannot cancel the next call's).
+void request_stop(DspgnSolver* s) {
+  const uint32_t g = s->stop_live.load(std::memory_order_acquire);
+  if (g == 0) return;
+  uint32_t cur = __atomic_load_n(s->h_stop, __ATOMIC_RELAXED);
+  while (cur < g && !__atomic_compare_exchange_n(s->h_stop, &cur, g, true, __ATOMIC_RELEASE, __ATOMIC_RELAXED)) {}
+}
+
+void stop_end(DspgnSolver* s) {
+  s->stop_live.store(0, std::memory_order_release);
+  s->call_stop_obj = s->call_stop_iter = -1;
+  s->run_stop_slot = -1;
+  s->run_pair = nullptr;
+}
+
+// The stoppable calls (dspgn_reconstruct_batch, the keyframe calls) hold one for their duration: a generation of their
+// own, live until the call returns; a submitted call keeps it (keep = true) until its wait.  The call takes the test
+// hook of dspgn_debug_stop_at.
+struct StopScope {
+  DspgnSolver* s;
+  bool keep = false;
+  explicit StopScope(DspgnSolver* s_) : s(s_) {
+    s->stop_gen = s->stop_gen + 1;
+    if (s->stop_gen == 0) {            // 2^32 calls: the word may hold a large old generation; no call is in flight
+      __atomic_store_n(s->h_stop, 0u, __ATOMIC_RELAXED);
+      s->stop_gen = 1;
+    }
+    s->call_stop_obj = s->stop_at_obj; s->call_stop_iter = s->stop_at_iter;
+    s->stop_at_obj = s->stop_at_iter = -1;
+    s->stop_live.store(s->stop_gen, std::memory_order_release);
+  }
+  ~StopScope() { if (!keep) stop_end(s); }
+};
+
+// The wait of a solver with a registered stop flag: the event and the flag polled in turn, yielding the core between
+// polls -- a spin like the one a blocking synchronisation does under the runtime's default scheduling.  A timed sleep
+// overshoots by the kernel's timer slack and, on a busy host, by milliseconds (DESIGN §5).
+cudaError_t poll_event(DspgnSolver* s, cudaEvent_t e) {
+  bool raised = false;
+  for (;;) {
+    const cudaError_t q = cudaEventQuery(e);
+    if (q != cudaErrorNotReady) return q;
+    if (!raised && *s->stop_flag != 0) { request_stop(s); raised = true; }
+    std::this_thread::yield();
+  }
+}
+
 // Every wait of the calling thread on the device goes through these (dspgn_debug_host_syncs counts them).
 cudaError_t sync_stream(DspgnSolver* s) {
   ++s->host_syncs;
+  if (s->stop_flag) {
+    const cudaError_t e = cudaEventRecord(s->ev_poll, s->stream);
+    return e != cudaSuccess ? e : poll_event(s, s->ev_poll);
+  }
   return cudaStreamSynchronize(s->stream);
 }
 
@@ -218,7 +283,7 @@ cudaError_t settle_event(DspgnSolver* s, cudaEvent_t e) {
   const cudaError_t q = cudaEventQuery(e);
   if (q != cudaErrorNotReady) return q;
   ++s->host_syncs;
-  return cudaEventSynchronize(e);
+  return s->stop_flag ? poll_event(s, e) : cudaEventSynchronize(e);
 }
 
 #define BUSY(s)                                                                                              \
@@ -421,6 +486,10 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
   CU(cudaEventCreateWithFlags(&s->ev_join, cudaEventDisableTiming));
   CU(cudaEventCreate(&s->ev_run0));
   CU(cudaEventCreate(&s->ev_run1));
+  CU(cudaEventCreateWithFlags(&s->ev_poll, cudaEventDisableTiming));
+  CU(cudaHostAlloc(reinterpret_cast<void**>(&s->h_stop), sizeof(uint32_t), cudaHostAllocMapped));
+  *s->h_stop = 0;
+  CU(cudaHostGetDevicePointer(reinterpret_cast<void**>(&s->d_stop), s->h_stop, 0));
 #undef CU
 #define CU(call)                                                                          \
   do {                                                                                    \
@@ -458,6 +527,8 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   if (s->stream2) cudaStreamDestroy(s->stream2);
   if (s->ev_run0) cudaEventDestroy(s->ev_run0);
   if (s->ev_run1) cudaEventDestroy(s->ev_run1);
+  if (s->ev_poll) cudaEventDestroy(s->ev_poll);
+  if (s->h_stop) cudaFreeHost(s->h_stop);
   delete s;
 }
 
@@ -720,6 +791,10 @@ BatchDev batch_dev(DspgnSolver* s) {
   b.gather = s->gdev;
   const RunTable t = run_table(s->d_run.p, s->n_obj, s->run_table_gated);
   b.modes = t.modes; b.q0_off = t.q0_off; b.link = t.link; b.t_map = t.t_map;
+  // only the runs of a stoppable call can stop, and never those of the multi-GPU exchange
+  const bool stoppable = s->stop_live.load(std::memory_order_relaxed) != 0 && s->gdev.slots == nullptr;
+  b.stop = stoppable ? StopDev{s->d_stop, s->stop_gen, s->run_stop_slot, s->call_stop_iter, s->run_pair}
+                     : StopDev{nullptr, 0u, -1, -1, nullptr};
   return b;
 }
 
@@ -1238,6 +1313,19 @@ int collect_run(DspgnSolver* s, const QueueCounters* hq) {
   if (cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot; else cudaGetLastError();
   return 0;
 }
+
+// The row counters of a stopped run: the run counted every slot's rows for its full iteration count, a STOPPED slot ran
+// iters_done iterations.  Slots n.. are the joint slots of gated objects; woken_added: kf_records counts theirs.
+void uncount_stopped(DspgnSolver* s, const DspgnObjectOut* res, int n, int slots, bool mega, bool woken_added) {
+  const DspgnConfig& c = s->cfg;
+  for (int k = 0; k < slots; ++k) {
+    if (res[k].status != DSPGN_ST_STOPPED || (k >= n && woken_added)) continue;
+    const long long missing = c.num_iterations - res[k].iters_done;
+    const ObjMeta& M = s->h_meta[k];
+    s->ctr.rows_fwd_bwd -= missing * M.n_pts;
+    if (!mega && !c.sdf_only) s->ctr.rows_fwd_only -= missing * M.n_rays * c.num_depth_samples;   // the kernel counts its own
+  }
+}
 }  // namespace
 
 int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
@@ -1260,12 +1348,16 @@ int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
 int dspgn_reconstruct_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out) {
   if (!s || !in || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
   BUSY(s);
+  StopScope stop(s);
   // any number of objects: resident batches of at most kMaxObjScan, one after the other
   for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
     const int n = std::min(kMaxObjScan, n_obj - o0);
     if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
+    s->run_stop_slot = (s->call_stop_obj >= o0 && s->call_stop_obj < o0 + n) ? s->call_stop_obj - o0 : -1;
     if (int rc = dspgn_run_batch(s, 0)) return rc;
+    const bool mega = s->mega_ran;
     if (int rc = dspgn_results(s, out + o0)) return rc;
+    uncount_stopped(s, out + o0, n, n, mega, false);
   }
   return 0;
 }
@@ -1380,11 +1472,9 @@ int kf_enqueue_chunk(DspgnSolver* s, const KfWalk& w, size_t u0, int n, int slot
   std::vector<int32_t> cm;
   for (int k = 0; k < n; ++k) { ins.push_back(w.in[w.order[u0 + k]]); cm.push_back(w.modes[w.order[u0 + k]]); }
   link.assign(n, -1);
-  if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
-    if (int rc = dspgn_upload_batch(s, n, ins.data())) return rc;
-    if (int rc = run_batch_impl(s, cm.data())) return rc;
-  } else {
-    std::vector<float> t_map(16 * (size_t)slots, 0.f);
+  std::vector<float> t_map;
+  if (slots != n) {
+    t_map.assign(16 * (size_t)slots, 0.f);
     for (int k = 0; k < n; ++k) {
       const int o = w.order[u0 + k];
       if (!w.gated(o)) continue;
@@ -1399,26 +1489,39 @@ int kf_enqueue_chunk(DspgnSolver* s, const KfWalk& w, size_t u0, int n, int slot
       for (int r = 0; r < 4; ++r)
         for (int c = 0; c < 4; ++c) t_map[16 * (size_t)k + 4 * r + c] = g.t_cam_obj_map[(size_t)r * g.map_rs + (size_t)c * g.map_cs];
     }
+  }
+  gc = 0;
+  int* d_sel = nullptr;
+  if (w.mesh) {
+    // per slot: its grid in the chunk's block (-1: not a candidate) | the slot of the other hypothesis of its pair.
+    // Uploaded before the run: the pairs are also the objects the call's stop leaves running.
+    const size_t sel_bytes = 4 * 2 * (size_t)slots;
+    if (s->d_mesh_sel.cap < sel_bytes) CU(settle_stream(s));
+    if (s->d_mesh_sel.reserve(sel_bytes) || s->h_mesh_sel.reserve(sel_bytes)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
+    int* sel = s->h_mesh_sel.as<int>();
+    std::fill(sel, sel + 2 * (size_t)slots, -1);
+    for (int k = 0; k < n; ++k) {
+      const int o = w.order[u0 + k];
+      if (!w.candidate(o)) continue;
+      sel[cm[k] == DSPGN_MODE_JOINT ? k : link[k]] = gc;
+      grid_of[o] = g0 + gc++;
+      if (w.paired(o)) sel[(size_t)slots + k] = w.pair[o] > o ? k + 1 : k - 1;
+    }
+    d_sel = s->d_mesh_sel.as<int>();
+    CU(cudaMemcpyAsync(d_sel, sel, sel_bytes, cudaMemcpyHostToDevice, s->stream));
+  }
+  s->run_pair = (d_sel != nullptr && w.pair != nullptr) ? d_sel + slots : nullptr;
+  s->run_stop_slot = -1;
+  for (int k = 0; k < n; ++k)
+    if (w.order[u0 + k] == s->call_stop_obj) s->run_stop_slot = k;
+  if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
+    if (int rc = dspgn_upload_batch(s, n, ins.data())) return rc;
+    if (int rc = run_batch_impl(s, cm.data())) return rc;
+  } else {
     if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
     if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data(), device_wake)) return rc;
   }
-  gc = 0;
   if (!w.mesh) return 0;
-  // per slot: its grid in the chunk's block (-1: not a candidate) | the slot of the other hypothesis of its pair
-  const size_t sel_bytes = 4 * 2 * (size_t)slots;
-  if (s->d_mesh_sel.cap < sel_bytes) CU(settle_stream(s));
-  if (s->d_mesh_sel.reserve(sel_bytes) || s->h_mesh_sel.reserve(sel_bytes)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
-  int* sel = s->h_mesh_sel.as<int>();
-  std::fill(sel, sel + 2 * (size_t)slots, -1);
-  for (int k = 0; k < n; ++k) {
-    const int o = w.order[u0 + k];
-    if (!w.candidate(o)) continue;
-    sel[cm[k] == DSPGN_MODE_JOINT ? k : link[k]] = gc;
-    grid_of[o] = g0 + gc++;
-    if (w.paired(o)) sel[(size_t)slots + k] = w.pair[o] > o ? k + 1 : k - 1;
-  }
-  int* d_sel = s->d_mesh_sel.as<int>();
-  CU(cudaMemcpyAsync(d_sel, sel, sel_bytes, cudaMemcpyHostToDevice, s->stream));
   if (u0 == 0) {                                     // the call-wide query grid of create_voxel_grid
     k_mesh_grid_points<<<(unsigned)((w.R + 255) / 256), 256, 0, s->stream>>>(s->d_grid_pts.as<float>(), 1, w.dim);
     s->ctr.kernel_launches++;
@@ -1451,8 +1554,9 @@ int kf_records(DspgnSolver* s, const KfWalk& w, size_t u0, int n, const std::vec
       r = res[link[k]];
       r.gate = DSPGN_GATE_REJECTED;
       const ObjMeta& M = s->h_meta[link[k]];
-      if (woken_rows >= 1) s->ctr.rows_fwd_bwd += (long long)M.n_pts * s->cfg.num_iterations;
-      if (woken_rows >= 2) s->ctr.rows_fwd_only += (long long)M.n_rays * s->cfg.num_depth_samples * s->cfg.num_iterations;
+      const long long iters = r.status == DSPGN_ST_STOPPED ? r.iters_done : s->cfg.num_iterations;
+      if (woken_rows >= 1) s->ctr.rows_fwd_bwd += (long long)M.n_pts * iters;
+      if (woken_rows >= 2) s->ctr.rows_fwd_only += (long long)M.n_rays * s->cfg.num_depth_samples * iters;
     }
     done += r.mesh == DSPGN_MESH_DONE ? 1 : 0;
   }
@@ -1495,6 +1599,7 @@ int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int3
   KfWalk w;
   if (int rc = kf_walk(s, n_obj, in, modes, gates, mesh, w)) return rc;
   BUSY(s);
+  StopScope stop(s);
   std::vector<int32_t> gV, gF, grid_of(mesh ? n_obj : 0, -1);
   if (mesh) {
     if (int rc = kf_grids(s, w)) return rc;
@@ -1512,6 +1617,7 @@ int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int3
     const bool mega = s->mega_ran;
     res.resize(slots);
     if (int rc = dspgn_results(s, res.data())) return rc;
+    uncount_stopped(s, res.data(), n, slots, mega, mega);
     const int done = kf_records(s, w, u0, n, link, res.data(), out, mega ? 1 : 0);   // the woken slots' SDF rows
     if (gc > 0) {
       s->ctr.rows_fwd_only += (long long)done * w.R;
@@ -1571,6 +1677,7 @@ int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, co
                              "and 2^24 candidate grid rows (the blocking calls take any size)");
   CU(cudaSetDevice(s->device));
   if (!s->ev_flight) CU(cudaEventCreateWithFlags(&s->ev_flight, cudaEventDisableTiming));
+  StopScope stop(s);                                 // kept until the wait on success
   DspgnSolver::Flight& F = s->flight;
   F = DspgnSolver::Flight{};
   F.grid_of.assign(mesh ? n_obj : 0, -1);
@@ -1618,6 +1725,7 @@ int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, co
   F.n_obj = n_obj; F.slots = slots; F.n = (int)u1; F.dim = w.dim; F.n_cand = w.n_cand; F.gc = gc;
   F.order.swap(w.order);
   F.active = true;
+  stop.keep = true;
   return 0;
 }
 
@@ -1638,12 +1746,14 @@ int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices
   if ((n_vertices == nullptr) == F.mesh || (n_faces == nullptr) == F.mesh)
     return fail(DSPGN_E_ARG, "n_vertices and n_faces must be given iff the submitted call had a mesh spec");
   F.active = false;                                  // collected from here on, whatever happens below
+  struct StopEnd { DspgnSolver* s; ~StopEnd() { stop_end(s); } } stop_end_{s};   // the call's stop ends with the wait
   CU(cudaSetDevice(s->device));
   CU(settle_event(s, s->ev_flight));
   s->upload_pending = false;                         // the event follows every copy of the call
   s->run_upload_pending = false;
   const unsigned char* h = s->h_flight.as<unsigned char>();
   if (int rc = collect_run(s, F.mega ? reinterpret_cast<const QueueCounters*>(h + F.o_ctr) : nullptr)) return rc;
+  uncount_stopped(s, reinterpret_cast<const DspgnObjectOut*>(h), F.n, F.slots, F.mega, true);
   KfWalk w;                                          // the walk's bookkeeping (the inputs are not read again)
   w.n_obj = F.n_obj; w.n_cand = F.n_cand; w.dim = F.dim; w.R = (long long)F.dim * F.dim * F.dim; w.mesh = F.mesh;
   w.order.swap(F.order);
@@ -1680,6 +1790,29 @@ int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices
 int dspgn_debug_host_syncs(DspgnSolver* s, int64_t* out) {
   if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
   *out = s->host_syncs;
+  return 0;
+}
+
+int dspgn_keyframe_stop(DspgnSolver* s) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  request_stop(s);
+  return 0;
+}
+
+int dspgn_solver_set_stop_flag(DspgnSolver* s, const volatile uint8_t* flag) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  BUSY(s);
+  s->stop_flag = flag;
+  return 0;
+}
+
+int dspgn_debug_stop_at(DspgnSolver* s, int obj, int iter) {
+  if (!s) return fail(DSPGN_E_ARG, "null solver");
+  const int max_iter = std::max(s->cfg.num_iterations, s->cfg.pose_only_iterations);
+  if (!(obj == -1 && iter == -1) && (obj < 0 || iter < 0 || iter >= max_iter))
+    return fail(DSPGN_E_ARG, "stop_at: obj >= 0 and 0 <= iter < the solver's iteration count, or -1, -1");
+  BUSY(s);
+  s->stop_at_obj = obj; s->stop_at_iter = iter;
   return 0;
 }
 

@@ -45,6 +45,15 @@ __device__ __forceinline__ int record_mesh(const float* results, int o) {
   return reinterpret_cast<const int*>(results + (size_t)o * DSPGN_RESULT_FLOATS)[kRecMeshWord];
 }
 
+// Cooperative stop of a run (dspgn_keyframe_stop): the solver's host-mapped stop word holds the generation of the last
+// call a stop was requested for; the run stops when it holds its own call's generation.
+struct StopDev {
+  unsigned* word;            // host-mapped; nullptr = the run cannot stop (no stoppable call, multi-GPU exchange, debug)
+  unsigned gen;              // generation of the call the run belongs to
+  int dbg_obj, dbg_iter;     // dspgn_debug_stop_at: the resident slot / iteration at whose solve the device raises the stop
+  const int* pair;           // [n_obj] other hypothesis of a mono pair, -1 none (nullptr: no pair in the run)
+};
+
 // The resident batch and its run, as every kernel of the run sees it (one by-value kernel parameter; the persistent
 // kernel keeps a copy in shared memory for its out-of-line solve step).
 struct BatchDev {
@@ -74,6 +83,7 @@ struct BatchDev {
   // joint slot o, -1 otherwise; t_map [n_obj][16] the map's prediction of each gated object
   const int* link;
   const float* t_map;
+  StopDev stop;
 };
 
 struct TermArgs {

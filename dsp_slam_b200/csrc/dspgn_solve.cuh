@@ -205,6 +205,35 @@ __device__ inline int gate_record(float* results, int o, const float* T_init, co
   return g;
 }
 
+// ---- cooperative stop (dspgn_keyframe_stop) -----------------------------------------------------------------------
+// The stop word lives in pinned host memory: a system-scope load sees a host store (or another CTA's) without a fence.
+__device__ __forceinline__ bool stop_seen(const StopDev& s) {
+  unsigned v;
+  asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(s.word) : "memory");
+  return v == s.gen;
+}
+
+// The solve of resident object o at iteration `iter` (one thread, beside the elimination): the test hook raises the stop,
+// then a stoppable object's solve that is not its last reads the word.  1: the object stops after this iteration's
+// update (unless the solve fails).
+__device__ __forceinline__ int stop_check(const StopDev& s, int o, int iter, bool pose_only, bool last_iter) {
+  if (s.word == nullptr) return 0;
+  const bool can = !pose_only && !last_iter && (s.pair == nullptr || s.pair[o] < 0);
+  if (o == s.dbg_obj && iter == s.dbg_iter && (can || pose_only))
+    asm volatile("st.relaxed.sys.global.u32 [%0], %1;" :: "l"(s.word), "r"(s.gen) : "memory");
+  return (can && stop_seen(s)) ? 1 : 0;
+}
+
+// The record of a rejected gated object's joint slot that a stop keeps from waking: its input pose (t_cam_obj_sim3), zero
+// code, no iteration.  One thread.
+__device__ inline void stopped_slot_record(float* results, ObjState* state, const float* T_init, int slot) {
+  float* r = results + (size_t)slot * DSPGN_RESULT_FLOATS;
+  for (int i = 0; i < 16; ++i) r[i] = T_init[16 * (size_t)slot + i];
+  for (int i = 16; i < DSPGN_RESULT_FLOATS; ++i) r[i] = 0.f;
+  reinterpret_cast<int*>(r)[81] = DSPGN_ST_STOPPED;
+  state[slot].status = DSPGN_ST_STOPPED;
+}
+
 // ---- device-side input construction (SURVEY 8 row f4) --------------------------------------------------------------
 // Runs once per upload, in place on the uploaded staging block: ray slots hold (u, v, 1) and become inv_k [u, v, 1]
 // (loss_utils.py:23-37 / LocalMapping_util.cc:378-386); world map points become camera points x_c = R x_w + t
@@ -458,6 +487,7 @@ struct SolveSmem {
   float s_rot[4];                              // J_rot.x, J_rot.z, res_rot, active
   double s_sum[4];                             // sdf loss sum, sdf rows, render loss sum
   int s_flag;
+  int s_stop;                                  // the object observed a stop at the end of this solve
 };
 
 // MEGA = called by the 256 epilogue threads of the persistent decoder kernel (named barrier, other CTAs wrote
@@ -701,6 +731,9 @@ __device__ int solve_object(const BatchDev& b, const SolveArgs& a, const EventLo
   }
   solve_sync<MEGA>();
   SOLVE_EV(4);
+  // the stop word: read by the first thread the elimination leaves idle, so its PCIe round trip runs under the pivots
+  // (the barrier after the elimination publishes it; a failed solve ignores it)
+  if (tid == kElimThreads && !dbg) SM.s_stop = stop_check(b.stop, o, ldv(&st.iters), pose_only, last_iter);
   // ---- Gauss-Jordan elimination of the SPD system, thread i = row i in registers; one barrier per pivot ----------
   if (tid < kElimThreads) {
     // Thread i keeps row i of [H | b] in registers, rotated so that the current pivot column is always index 0: after
@@ -737,7 +770,11 @@ __device__ int solve_object(const BatchDev& b, const SolveArgs& a, const EventLo
   const bool fail = (s_flag != 0);
   if (!pose_only && tid < L && !fail) st.z[tid] = ldv(&st.z[tid]) + prm.lr * xs[tid + 7];
   solve_sync<MEGA>();                        // the result record below reads every z entry
-  if (!pose_only && !fail && !last_iter) refresh_zb0(st, b.decs[b.meta[o].class_id], tid, kSolveThreads);
+  // a stop observed in this solve ends the object as its last iteration would: the same update, the same record but
+  // the status
+  const bool stop = !fail && SM.s_stop != 0;
+  const bool final_solve = last_iter || stop;
+  if (!pose_only && !fail && !final_solve) refresh_zb0(st, b.decs[b.meta[o].class_id], tid, kSolveThreads);
   if (tid == 0) {
     st.loss = loss; st.V = V; st.m = m;
     b.V_count[o] = 0;
@@ -754,10 +791,11 @@ __device__ int solve_object(const BatchDev& b, const SolveArgs& a, const EventLo
       derive_depth_range(st, prm.D);
       st.iters = ldv(&st.iters) + 1;
     }
-    if (last_iter || (MEGA && fail)) write_result(b, o, st);
+    if (stop) { st.status = DSPGN_ST_STOPPED; st.n_iter = st.iters; }   // later launches skip it (k_solve, term_rows)
+    if (final_solve || (MEGA && fail)) write_result(b, o, st);
   }
   SOLVE_EV(6);
-  return (last_iter || fail) ? 1 : 0;
+  return (final_solve || fail) ? 1 : 0;
 }
 
 __global__ void __launch_bounds__(kSolveThreads) k_solve(BatchDev b, SolveArgs a) {
@@ -772,13 +810,18 @@ __global__ void __launch_bounds__(kSolveThreads) k_solve(BatchDev b, SolveArgs a
 }
 
 // Per-iteration schedule of a gated run, between its two phases: the joint slots whose pose-only object was rejected
-// run num_iterations from their k_init state, every other object is finished (its record is final).
+// run num_iterations from their k_init state, every other object is finished (its record is final).  Once the call's
+// stop is observed no slot wakes: a rejected one gets its stopped record.
 __global__ void k_gate_wake(BatchDev b, int n_iter_joint) {
   const int o = blockIdx.x * blockDim.x + threadIdx.x;
   if (o >= b.n_obj) return;
   const int lk = b.link[o];
-  const bool wake = lk >= 0 && b.modes[o] == DSPGN_MODE_JOINT &&
-                    reinterpret_cast<const int*>(b.results + (size_t)lk * DSPGN_RESULT_FLOATS)[85] == DSPGN_GATE_REJECTED;
+  bool wake = lk >= 0 && b.modes[o] == DSPGN_MODE_JOINT &&
+              reinterpret_cast<const int*>(b.results + (size_t)lk * DSPGN_RESULT_FLOATS)[85] == DSPGN_GATE_REJECTED;
+  if (wake && b.stop.word != nullptr && stop_seen(b.stop)) {
+    stopped_slot_record(b.results, b.state, b.T_init, o);
+    wake = false;
+  }
   b.state[o].n_iter = wake ? n_iter_joint : 0;
 }
 

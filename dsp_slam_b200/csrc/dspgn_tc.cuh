@@ -671,9 +671,14 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail<SCHED>& S, int o,
     if (fin) {
       // a gated pose-only object: the map-consistency check on its record; rejected, it wakes its joint slot (k_init
       // left the slot initialised, its iteration-0 counters set and no item queued), kept, the slot is done unrun
-      // (a slot rejected at upload never gets here: its pose-only object was rejected at upload too)
+      // (a slot rejected at upload never gets here: its pose-only object was rejected at upload too); once the call's
+      // stop is observed a rejected slot is not woken but gets its stopped record
       const int slot = (b.link != nullptr && b.state[o].mode == DSPGN_MODE_POSE) ? b.link[o] : -1;
-      const bool wake = slot >= 0 && gate_record(b.results, o, b.T_init, b.t_map) == DSPGN_GATE_REJECTED;
+      bool wake = slot >= 0 && gate_record(b.results, o, b.T_init, b.t_map) == DSPGN_GATE_REJECTED;
+      if (wake && b.stop.word != nullptr && stop_seen(b.stop)) {
+        stopped_slot_record(b.results, b.state, b.T_init, slot);
+        wake = false;
+      }
       __threadfence();                       // the result record before the object counts as done
       atomicAdd(&q.ctr->done_objects, (slot >= 0 && !wake) ? 2 : 1);
       if (wake) {

@@ -354,6 +354,22 @@ class BatchSolver:
         self.n_obj = n
         return self._meshed(out, n, int(voxels_dim), nv, nf, want_sdf)
 
+    def request_stop(self):
+        """dspgn_keyframe_stop: stop the call in flight at the next GN iteration of each stoppable object (the joint
+        objects outside mono pairs); they come back with status _lib.ST_STOPPED.  Callable from any thread while another
+        thread is inside a call on this solver; never blocks; nothing in flight: no effect."""
+        _lib.check(_lib.load().dspgn_keyframe_stop(self.handle))
+
+    def set_stop_flag(self, address):
+        """dspgn_solver_set_stop_flag: the address of a byte the library polls while it waits for the device (a nonzero
+        value requests the stop); None / 0 unregisters it.  The byte must outlive the registration."""
+        _lib.check(_lib.load().dspgn_solver_set_stop_flag(self.handle, C.c_void_p(address or None)))
+
+    def debug_stop_at(self, obj=-1, iteration=-1):
+        """Test hook (dspgn_debug_stop_at): the next stoppable call raises its own stop at the end of object obj's solve
+        of GN iteration `iteration`; -1, -1 clears it."""
+        _lib.check(_lib.load().dspgn_debug_stop_at(self.handle, int(obj), int(iteration)))
+
     def host_syncs(self):
         """dspgn_debug_host_syncs: how often the solver's calls have blocked the calling thread on the device."""
         v = C.c_int64()
@@ -495,6 +511,14 @@ class KeyframeFuture(object):
     def result(self):
         self._settle()
         return self._value
+
+    def stop(self):
+        """Stop the call at the next GN iteration (BatchSolver.request_stop; LocalMapping's mbAbortBA): its stoppable
+        objects that have not finished come back like objects the reference never created (is_good=False, status
+        _lib.ST_STOPPED).  Never blocks; callable from any thread; a settled future: no effect."""
+        owner = self._owner
+        if not self._settled and owner is not None:
+            owner.solver.request_stop()
 
     def _settle(self):
         if self._settled:

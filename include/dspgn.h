@@ -63,6 +63,7 @@ extern "C" {
 #define DSPGN_ST_RENDER_NAN 3  /* optimizer.py:149-150 (no band rows -> NaN loss) */
 #define DSPGN_ST_SOLVE 4       /* normal matrix not positive definite / non-finite step */
 #define DSPGN_ST_BAD_INPUT 5   /* unusable detection (no surface points, too many rays, ...): never evaluated */
+#define DSPGN_ST_STOPPED 6     /* the call was stopped (dspgn_keyframe_stop) before the object's last iteration */
 
 /* kernel schedules of a run (results are bit-identical; the per-iteration schedule exists for debugging / profiling) */
 #define DSPGN_SCHED_AUTO 0
@@ -270,7 +271,8 @@ int dspgn_keyframe_batch_meshed(DspgnSolver* s, int n_obj, const DspgnObjectIn* 
  *           meshes.  Records, counts and meshes are bit-identical to dspgn_keyframe_batch_meshed / _gated.
  * One call in flight per solver: until wait, every other entry point on the solver returns DSPGN_E_BUSY (results_device
  * and gather_device return NULL, gather_close does nothing) and leaves the call intact, except query, wait,
- * dspgn_solver_sync, dspgn_solver_engine and dspgn_debug_host_syncs; dspgn_solver_destroy waits for the call first.
+ * dspgn_keyframe_stop, dspgn_solver_sync, dspgn_solver_engine and dspgn_debug_host_syncs; dspgn_solver_destroy waits for
+ * the call first.
  * Solvers on different streams may each have a call in flight.  The multi-GPU exchange does not apply.
  * SM budget: the persistent kernels fill a whole SM per CTA, so while one runs on every SM no block of another kernel
  * starts anywhere.  While at least one frame handle (DspgnLidarFrame, DspgnMonoFrame) is alive on the solver's device,
@@ -286,6 +288,41 @@ int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices
 /* Debug: the number of times the solver's calls have blocked the calling thread on the device so far (stream and event
  * synchronisations, counted only when the device still had work to finish). */
 int dspgn_debug_host_syncs(DspgnSolver* s, int64_t* out);
+
+/* Cooperative stop of a running keyframe call: LocalMapping's mbAbortBA (src/LocalMapping.cc:165-170, :611, :680), which
+ * CreateNewMapObjects checks before and after each reconstruct_object (src/LocalMapping_util.cc:168-169, 184-185) and
+ * ORB-SLAM hands to g2o as its force-stop flag.
+ *   stoppable objects  the joint objects of dspgn_reconstruct_batch and of the keyframe calls (blocking and submitted),
+ *                      including the joint slot of a gated object, except both hypotheses of a mono pair.  Pose-only
+ *                      objects, pairs and the multi-GPU exchange always run to the end.
+ *   when               a stoppable object reads the stop word once in each solve that is not its last; observed, the
+ *                      stop takes effect after that iteration's update: the object finishes with status
+ *                      DSPGN_ST_STOPPED (a solve that fails keeps its own status), and its record -- status
+ *                      word aside -- is bit-identical to the record of the same call with num_iterations = iters_done.
+ *                      Every other record is the unstopped call's.
+ *   gated objects      the pose-only record and its gate word are always complete.  A REJECTED object whose joint slot
+ *                      would wake after the stop was observed does not run it: its record is DSPGN_ST_STOPPED with
+ *                      iters_done 0, pose t_cam_obj_sim3, code zero, loss / n_valid / n_band 0, gate DSPGN_GATE_REJECTED.
+ *   meshes             a STOPPED candidate is DSPGN_MESH_FAILED (its grid NaN); every other mesh is the unstopped call's.
+ *   return codes       a stopped call returns DSPGN_OK; counters count the rows of the iterations that ran.
+ * dspgn_keyframe_stop  requests the stop of the solver's call in flight (dspgn_reconstruct_batch, dspgn_keyframe_batch*,
+ *                      or a submitted call until its wait returns).  Nothing in flight: no effect -- a stop never reaches a
+ *                      later call (each call has its own generation, which the kernels compare with the stop word).  The one
+ *                      entry point that may be called from any thread while another thread is inside a call on the same
+ *                      solver (never concurrently with dspgn_solver_destroy); it never blocks and never touches the stream.
+ * dspgn_solver_set_stop_flag  registers a caller-owned byte (a C++ bool such as &mbAbortBA; NULL unregisters): while a
+ *                      call waits for the device (the blocking calls' synchronisations, dspgn_keyframe_wait) it polls the
+ *                      byte between cudaEventQuery polls (yielding the core, never a timed sleep), and a nonzero value becomes
+ *                      dspgn_keyframe_stop.  Each such wait counts as one host sync.  No flag: every wait is a plain
+ *                      blocking synchronisation, as before. */
+int dspgn_keyframe_stop(DspgnSolver* s);
+int dspgn_solver_set_stop_flag(DspgnSolver* s, const volatile uint8_t* flag);
+/* Test hook: in the next stoppable call the device raises that call's stop itself in caller object `obj`'s solve of
+ * iteration `iter` (0-based), just before that solve reads the stop word: a stoppable object then ends STOPPED
+ * with iters_done = iter + 1; a pose-only object raises it after any of its iterations, its last included (a gated one
+ * before its verdict wakes the joint slot).  A stoppable object's last solve reads nothing and raises nothing.  -1, -1
+ * clears it; anything else out of range returns DSPGN_E_ARG. */
+int dspgn_debug_stop_at(DspgnSolver* s, int obj, int iter);
 /* Test hook: the mesh arena of the following submits holds max_vertices vertices and max_faces faces (both 0: the
  * automatic size, a per-object estimate that grows with the meshes the solver has seen).  A keyframe whose meshes do not
  * fit is meshed again at the exact size inside dspgn_keyframe_wait: slower, never different. */
