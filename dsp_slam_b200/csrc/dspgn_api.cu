@@ -75,6 +75,7 @@ struct HostBuf {   // pinned staging
 struct DspgnDecoder {
   int device = 0;
   bool has_ln = false;
+  int hid = kHid;            // row stride of the SIMT weight images: kHidWide for a decoder with a layer wider than kHid
   DspgnDecoderSpec spec{};
   DecoderDev dev{};
   std::vector<void*> allocs;
@@ -85,10 +86,12 @@ struct DspgnSolver {
   int device = 0;
   int num_sms = 0;
   int engine = DSPGN_ENGINE_SIMT;
+  int simt_hid = kHid;       // SIMT instantiation of the solver: its widest class's row stride
   DspgnConfig cfg{};
   cudaStream_t stream = nullptr;
   std::vector<DspgnDecoder*> classes;
   DevBuf d_decs;
+  std::vector<void*> wide_allocs;  // kHidWide-stride weight images of the narrow classes of a wide solver
   // resident batch
   int n_obj = 0;
   int tot_pts = 0, tot_rays = 0, tot_fg = 0;
@@ -206,6 +209,14 @@ void count_frame(int device, int delta) {
   if (device >= 0 && device < kMaxDevices) g_live_frames[device].fetch_add(delta, std::memory_order_relaxed);
 }
 
+// rows per tile of the solver's decoder engine (the per-tile partial sums of a term: one slot per tile)
+int tile_rows(const DspgnSolver* s) { return (s->engine == DSPGN_ENGINE_TC) ? kTcRows : simt_rows(s->simt_hid); }
+
+// the SIMT engine's LayerNorm scratch of one grid-sized launch: [CTA][layer][H][rows] (TermArgs.ln_scratch)
+size_t ln_half_floats(const DspgnSolver* s) {
+  return (size_t)s->num_sms * DSPGN_MAX_LINEAR * s->simt_hid * simt_rows(s->simt_hid);
+}
+
 // CTAs of the next grid-sized launch (k_gn_persistent*, k_decoder_tc, k_decoder_simt): at most this many
 int grid_sms(const DspgnSolver* s) {
   if (s->sm_force > 0) return s->sm_force;
@@ -307,8 +318,8 @@ int check_spec(const DspgnDecoderSpec& s) {
   if (s.latent_in_layer != -1 && (s.latent_in_layer < 1 || s.latent_in_layer > s.num_linear - 1))
     return fail(DSPGN_E_ARG, "latent_in_layer must be a layer index >= 1 or -1");
   for (int k = 0; k < s.num_linear; ++k) {
-    if (s.in_dim[k] < 1 || s.in_dim[k] > kHid || s.out_dim[k] < 1 || s.out_dim[k] > kHid)
-      return fail(DSPGN_E_ARG, "layer widths must be in [1,256]");
+    if (s.in_dim[k] < 1 || s.in_dim[k] > kHidWide || s.out_dim[k] < 1 || s.out_dim[k] > kHidWide)
+      return fail(DSPGN_E_ARG, "layer widths must be in [1,512]");
     const int ck = cat_kind_of(s, k);
     if (ck < 0 || ck > 2 || (k == 0 && ck != 0)) return fail(DSPGN_E_ARG, "bad cat_kind");
     if (s.layer_norm[k] != 0 && k == s.num_linear - 1) return fail(DSPGN_E_ARG, "the last layer cannot be normalised");
@@ -373,17 +384,20 @@ int dspgn_decoder_create_ex(const DspgnDecoderSpec* spec, const float* const* W,
   dv.latent_in = (n_cat1 == 1) ? cat1_layer : -1;
   dv.use_tanh = spec->use_tanh != 0; dv.generic = generic ? 1 : 0;
   d->has_ln = false;
+  for (int k = 0; k < nl; ++k)
+    if (spec->in_dim[k] > kHid || spec->out_dim[k] > kHid) d->hid = kHidWide;
+  const int H = d->hid;
   int rc = 0;
   for (int k = 0; k < nl && rc == 0; ++k) {
     const int nin = spec->in_dim[k], nout = spec->out_dim[k];
     dv.in_dim[k] = nin; dv.out_dim[k] = nout;
     const int in_pad = (nin + kKC - 1) / kKC * kKC, out_pad = (nout + kKC - 1) / kKC * kKC;
-    std::vector<float> wf((size_t)in_pad * kHid, 0.f), wb((size_t)out_pad * kHid, 0.f), bb(kHid, 0.f);
+    std::vector<float> wf((size_t)in_pad * H, 0.f), wb((size_t)out_pad * H, 0.f), bb(H, 0.f);
     for (int j = 0; j < nout; ++j) {
       for (int i = 0; i < nin; ++i) {
         const float w = W[k][(size_t)j * nin + i];
-        wf[(size_t)i * kHid + j] = w;
-        wb[(size_t)j * kHid + i] = w;
+        wf[(size_t)i * H + j] = w;
+        wb[(size_t)j * H + i] = w;
       }
       bb[j] = b[k][j];
     }
@@ -391,12 +405,12 @@ int dspgn_decoder_create_ex(const DspgnDecoderSpec* spec, const float* const* W,
     if (!rc) rc = upload_vec(d, wb, &dv.Wb[k]);
     if (!rc) rc = upload_vec(d, bb, &dv.bias[k]);
     if (!rc && k == nl - 1) {
-      std::vector<float> wl(kHid, 0.f);
+      std::vector<float> wl(H, 0.f);
       for (int i = 0; i < nin; ++i) wl[i] = W[k][i];
       rc = upload_vec(d, wl, &dv.w_last);
     }
     if (!rc && spec->layer_norm[k]) {
-      std::vector<float> g(kHid, 0.f), be(kHid, 0.f);
+      std::vector<float> g(H, 0.f), be(H, 0.f);
       for (int j = 0; j < nout; ++j) { g[j] = ln_gamma[k][j]; be[j] = ln_beta[k][j]; }
       rc = upload_vec(d, g, &dv.ln_gamma[k]);
       if (!rc) rc = upload_vec(d, be, &dv.ln_beta[k]);
@@ -450,7 +464,24 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
   s->num_sms = prop.multiProcessorCount;
   for (int c = 0; c < n_classes; ++c) s->classes.push_back(classes[c]);
   std::vector<DecoderDev> decs;
-  for (auto* d : s->classes) decs.push_back(d->dev);
+  for (auto* d : s->classes) s->simt_hid = std::max(s->simt_hid, d->hid);
+  for (auto* d : s->classes) {
+    decs.push_back(d->dev);
+    if (d->hid == s->simt_hid) continue;
+    // a narrow class of a wide solver runs in the wide instantiation: its matrices again at the wider row stride
+    DecoderDev& dv = decs.back();
+    for (int k = 0; k < dv.n_lin; ++k)
+      for (const float** m : {&dv.Wf[k], &dv.Wb[k]}) {
+        const size_t rows = (size_t)((m == &dv.Wf[k] ? dv.in_dim[k] : dv.out_dim[k]) + kKC - 1) / kKC * kKC;
+        void* p = nullptr;
+        CU(cudaMalloc(&p, rows * s->simt_hid * sizeof(float)));
+        s->wide_allocs.push_back(p);
+        CU(cudaMemset(p, 0, rows * s->simt_hid * sizeof(float)));
+        CU(cudaMemcpy2D(p, s->simt_hid * sizeof(float), *m, d->hid * sizeof(float), d->hid * sizeof(float), rows,
+                        cudaMemcpyDeviceToDevice));
+        *m = static_cast<const float*>(p);
+      }
+  }
   if (s->d_decs.reserve(decs.size() * sizeof(DecoderDev))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
   CU(cudaMemcpy(s->d_decs.p, decs.data(), decs.size() * sizeof(DecoderDev), cudaMemcpyHostToDevice));
   bool tc_ok = true;
@@ -464,10 +495,14 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
   }
   if (eng == DSPGN_ENGINE_TC && !tc_ok) { dspgn_solver_destroy(s); return fail(DSPGN_E_ARG, "tensor-core engine unavailable for this decoder shape"); }
   s->engine = eng;
-  CU(cudaFuncSetAttribute(k_decoder_simt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem)));
+  if (s->simt_hid == kHid)
+    CU(cudaFuncSetAttribute(k_decoder_simt<kHid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHid>)));
+  else
+    CU(cudaFuncSetAttribute(k_decoder_simt<kHidWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHidWide>)));
   for (auto* d : s->classes)
-    if (d->has_ln) {      // LayerNorm decoders: per-CTA scratch for the normalised activations (forward -> backward)
-      if (s->d_ln.reserve(4 * (size_t)s->num_sms * DSPGN_MAX_LINEAR * kHid * kTP)) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
+    if (d->has_ln) {      // LayerNorm decoders: per-CTA scratch for the normalised activations (forward -> backward),
+                          // one half for the ray-sample pass, which may run beside the SDF-row pass (launch_terms)
+      if (s->d_ln.reserve(4 * 2 * ln_half_floats(s))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
       break;
     }
   if (eng == DSPGN_ENGINE_TC &&
@@ -511,6 +546,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
                     &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_masks, &s->d_run,
                     &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout, &s->d_mesh_sel}) b->release();
+  for (void* p : s->wide_allocs) cudaFree(p);
   s->h_stage.release();
   s->h_mbase.release();
   s->h_results.release();
@@ -701,7 +737,7 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
   const bool render = !decode_only && !s->cfg.sdf_only;
   if (!decode_only) {
     // per-tile partial sums: one slot per possible tile of each term at the engine's tile height
-    const size_t rows_per_tile = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
+    const size_t rows_per_tile = tile_rows(s);
     const size_t tiles_s = (size_t)tp / rows_per_tile + n_obj + 1, tiles_r = (size_t)ts / rows_per_tile + 2 * (size_t)n_obj + 1;
     bad |= s->d_part_s.reserve(4 * (size_t)kAccStride * tiles_s);
     if (render) bad |= s->d_part_r.reserve(4 * (size_t)kAccStride * tiles_r);
@@ -743,14 +779,15 @@ int launch_term(DspgnSolver* s, const BatchDev& b, const TermArgs& a, long long 
   cudaStream_t st = use_given ? stream : s->stream;
   const bool timed = s->timing && !use_given;
   if (timed) cudaEventRecord(next_event(s), st);
-  const long long tile_rows = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
-  long long tiles = (rows_upper + tile_rows - 1) / tile_rows + s->n_obj;
+  const long long rows = tile_rows(s);
+  long long tiles = (rows_upper + rows - 1) / rows + s->n_obj;
   if (s->engine == DSPGN_ENGINE_TC) {
     if (int rc = tc_launch_term(b, a, grid_sms(s), tiles, st, g_err)) return rc;
   } else {
     int grid = (int)std::min<long long>(tiles, grid_sms(s));
     if (grid < 1) grid = 1;
-    k_decoder_simt<<<grid, kThreads, sizeof(SimtSmem), st>>>(b, a);
+    if (s->simt_hid == kHid) k_decoder_simt<kHid><<<grid, kThreads, sizeof(SimtSmem<kHid>), st>>>(b, a);
+    else k_decoder_simt<kHidWide><<<grid, kThreads, sizeof(SimtSmem<kHidWide>), st>>>(b, a);
   }
   if (timed) cudaEventRecord(next_event(s), st);
   s->ctr.kernel_launches++;
@@ -764,7 +801,7 @@ TermArgs base_term(DspgnSolver* s, int mode) {
   a.pt_active = nullptr; a.cut_iter = -1; a.iter = 0;
   a.part = (mode == MODE_BAND) ? s->d_part_r.as<float>() : (mode == MODE_SDF ? s->d_part_s.as<float>() : nullptr);
   a.tile_base = (mode == MODE_BAND) ? s->d_tbase.as<int>() + s->n_obj : (mode == MODE_SDF ? s->d_tbase.as<int>() : nullptr);
-  a.ln_scratch = s->d_ln.as<float>();
+  a.ln_scratch = s->d_ln.p ? s->d_ln.as<float>() + (mode == MODE_RAYFWD ? ln_half_floats(s) : 0) : nullptr;
   a.dbg_J = nullptr; a.dbg_res = nullptr; a.dbg_obj = -1; a.dbg_P = 0;
   return a;
 }
@@ -933,7 +970,7 @@ SolveArgs base_solve(DspgnSolver* s) {
   SolveArgs v{};
   v.part_s = s->d_part_s.as<float>(); v.part_r = s->d_part_r.as<float>();
   v.base_s = s->d_tbase.as<int>(); v.base_r = s->d_tbase.as<int>() + s->n_obj;
-  v.tile_rows = (s->engine == DSPGN_ENGINE_TC) ? kTcRows : kTP;
+  v.tile_rows = tile_rows(s);
   v.prm = SolverParams{c.k1, c.k2, c.k3, c.k4, c.b1, c.b2, c.lr, c.s_damp, c.code_len, c.num_depth_samples, c.cut_off, c.sdf_only};
   v.dbg_obj = -1; v.dbg_H = nullptr; v.dbg_b = nullptr; v.dbg_dx = nullptr; v.dbg_loss = nullptr;
   return v;

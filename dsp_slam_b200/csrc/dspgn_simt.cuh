@@ -1,6 +1,7 @@
 // fp32 SIMT decoder engine: fused  transform -> DeepSDF forward -> backward-to-input -> Jacobian rows
-// -> per-tile partial sums of J^T J / J^T r  for one 64-row tile per CTA iteration.  This engine is the on-device ground truth
-// (plain FFMA, fp32 accumulation in k order) against which the tensor-core engine is checked.
+// -> per-tile partial sums of J^T J / J^T r  for one tile per CTA iteration (64 rows; 32 for layers wider than 256).
+// This engine is the on-device ground truth (plain FFMA, fp32 accumulation in k order) against which the tensor-core
+// engine is checked.
 //
 // Restates: loss.py:22-43 (SDF term), loss.py:143-150 (band rows of the render term),
 // loss_utils.py:51-103 (decode / input Jacobian), deep_sdf_decoder.py:75-110, optimizer.py:161-167.
@@ -10,23 +11,31 @@
 
 namespace dspgn {
 
-constexpr int kTP = 64;          // rows (points) per tile
 constexpr int kTcRows = 128;     // rows per tile of the tensor-core engine (dspgn_tc.cuh)
 constexpr int kThreads = 256;
-constexpr int kHid = 256;        // max layer width
+constexpr int kHid = 256;        // max layer width of the tensor-core engine and of the narrow SIMT instantiation
+constexpr int kHidWide = 512;    // max layer width of the wide SIMT instantiation (the widest decoder accepted)
+// Rows per tile of the SIMT instantiation for layers up to `hid` wide: 256 threads own 8 features x 8 rows each, so
+// hid x rows = 256 x 64 = 512 x 32.  Shared memory of the wide tile (SimtSmem<512>): activations 64 KB, weight chunks
+// 64 KB, ReLU masks 16 KB, decoder input and its gradient 17 KB, the rest 6 KB -- 168 KB of the 227 KB opt-in.  A 64-row
+// tile at 512 would need 241 KB.
+__host__ __device__ constexpr int simt_rows(int hid) { return hid <= kHid ? 64 : 32; }
+__host__ __device__ constexpr int ilog2(int x) { return x <= 1 ? 0 : 1 + ilog2(x >> 1); }
 constexpr int kKC = 16;          // reduction chunk staged in smem
 constexpr int kMaxObjScan = 1024;
 
 struct DecoderDev {
   int L, n_lin, latent_in, in0;            // in0 = L + 3
   int in_dim[DSPGN_MAX_LINEAR], out_dim[DSPGN_MAX_LINEAR];
-  const float* Wf[DSPGN_MAX_LINEAR];       // forward, reduction-major  [in_pad16][256]:  Wf[i*256+j] = W[j][i]
-  const float* Wb[DSPGN_MAX_LINEAR];       // backward, reduction-major [out_pad16][256]: Wb[i*256+j] = W[i][j]
-  const float* bias[DSPGN_MAX_LINEAR];     // [256] zero padded
-  const float* w_last;                     // [256] last layer row
+  // weight images at the row stride H of the SIMT instantiation that runs the class (256, or 512 in a solver that holds
+  // a class wider than 256); the tensor-core engine reads them at 256
+  const float* Wf[DSPGN_MAX_LINEAR];       // forward, reduction-major  [in_pad16][H]:  Wf[i*H+j] = W[j][i]
+  const float* Wb[DSPGN_MAX_LINEAR];       // backward, reduction-major [out_pad16][H]: Wb[i*H+j] = W[i][j]
+  const float* bias[DSPGN_MAX_LINEAR];     // [max(256, width)] zero padded
+  const float* w_last;                     // [max(256, width)] last layer row
   // optional variants (deep_sdf_decoder.py:41-47,58-63,87-102): SIMT engine only
   int cat_kind[DSPGN_MAX_LINEAR];          // input of layer k = [activations | 0: nothing, 1: decoder input, 2: xyz]
-  const float* ln_gamma[DSPGN_MAX_LINEAR]; // LayerNorm after layer k (nullptr = none), [256] zero padded
+  const float* ln_gamma[DSPGN_MAX_LINEAR]; // LayerNorm after layer k (nullptr = none), [max(256, width)] zero padded
   const float* ln_beta[DSPGN_MAX_LINEAR];
   int use_tanh, generic;                   // generic = any variant in use
   // tensor-core engine images (dspgn_tc.cuh): pre-swizzled fp16 hi/lo weight chunks + step plan
@@ -97,7 +106,7 @@ struct TermArgs {
   float huber_b;
   // persistent kernel with the render term: the band rows' partials / tile bases / Huber threshold (SDF ones above)
   float* part_r; const int* tile_base_r; float huber_b1;
-  float* ln_scratch;         // SIMT engine, LayerNorm decoders: per-CTA [layer][256][kTP] normalised activations
+  float* ln_scratch;         // SIMT engine, LayerNorm decoders: per-CTA [layer][H][rows] normalised activations
   // debug dump of Jacobian rows (external order [pose | code]) for one object
   float* dbg_J; float* dbg_res; int dbg_obj; int dbg_P;
   // MODE_GRIDFWD: query points [grid_rows][3], grid slot of each object (-1: none)
@@ -234,10 +243,12 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// acc[jj][pp] = sum_{i<Kred} Wg[i*256 + 8*jg+jj] * in_s[i*kTP + 8*pg+pp]
+// acc[jj][pp] = sum_{i<Kred} Wg[i*H + 8*jg+jj] * in_s[i*TP + 8*pg+pp]
+template <int H, int TP>
 __device__ __forceinline__ void gemm_rm(const float* __restrict__ Wg, int Kred, const float* __restrict__ in_s,
                                         float* __restrict__ wbuf, float (&acc)[8][8]) {
-  const int tid = threadIdx.x, jg = tid >> 3, pg = tid & 7;
+  constexpr int kLoads = kKC * H / 4 / kThreads;     // 16-byte copies per thread and weight chunk
+  const int tid = threadIdx.x, jg = tid >> ilog2(TP / 8), pg = tid & (TP / 8 - 1);
 #pragma unroll
   for (int a = 0; a < 8; ++a)
 #pragma unroll
@@ -248,28 +259,28 @@ __device__ __forceinline__ void gemm_rm(const float* __restrict__ Wg, int Kred, 
     const float4* src = reinterpret_cast<const float4*>(Wg);
     float4* dst = reinterpret_cast<float4*>(wbuf);
 #pragma unroll
-    for (int q = 0; q < 4; ++q) cp_async16(dst + tid + q * kThreads, src + tid + q * kThreads);
+    for (int q = 0; q < kLoads; ++q) cp_async16(dst + tid + q * kThreads, src + tid + q * kThreads);
     cp_async_commit();
   }
   for (int c = 0; c < nch; ++c) {
     cp_async_wait<0>();
     __syncthreads();                 // chunk c landed for all; everyone is done with chunk c-1's buffer
     if (c + 1 < nch) {
-      const float4* src = reinterpret_cast<const float4*>(Wg + (size_t)(c + 1) * kKC * kHid);
-      float4* dst = reinterpret_cast<float4*>(wbuf + ((c + 1) & 1) * kKC * kHid);
+      const float4* src = reinterpret_cast<const float4*>(Wg + (size_t)(c + 1) * kKC * H);
+      float4* dst = reinterpret_cast<float4*>(wbuf + ((c + 1) & 1) * kKC * H);
 #pragma unroll
-      for (int q = 0; q < 4; ++q) cp_async16(dst + tid + q * kThreads, src + tid + q * kThreads);
+      for (int q = 0; q < kLoads; ++q) cp_async16(dst + tid + q * kThreads, src + tid + q * kThreads);
       cp_async_commit();
     }
-    const float* wb = wbuf + (c & 1) * kKC * kHid + 8 * jg;
-    const float* ib = in_s + (size_t)c * kKC * kTP + 8 * pg;
+    const float* wb = wbuf + (c & 1) * kKC * H + 8 * jg;
+    const float* ib = in_s + (size_t)c * kKC * TP + 8 * pg;
     const int kmax = min(kKC, Kred - c * kKC);
 #pragma unroll 4
     for (int kk = 0; kk < kmax; ++kk) {
-      float4 w0 = *reinterpret_cast<const float4*>(wb + kk * kHid);
-      float4 w1 = *reinterpret_cast<const float4*>(wb + kk * kHid + 4);
-      float4 a0 = *reinterpret_cast<const float4*>(ib + kk * kTP);
-      float4 a1 = *reinterpret_cast<const float4*>(ib + kk * kTP + 4);
+      float4 w0 = *reinterpret_cast<const float4*>(wb + kk * H);
+      float4 w1 = *reinterpret_cast<const float4*>(wb + kk * H + 4);
+      float4 a0 = *reinterpret_cast<const float4*>(ib + kk * TP);
+      float4 a1 = *reinterpret_cast<const float4*>(ib + kk * TP + 4);
       const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
       const float x[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
 #pragma unroll
@@ -281,50 +292,57 @@ __device__ __forceinline__ void gemm_rm(const float* __restrict__ Wg, int Kred, 
   __syncthreads();                   // all reads of in_s / wbuf finished: caller may overwrite in_s
 }
 
+template <int H>
 struct SimtSmem {
-  float act[kHid * kTP];             // feature-major activations / gradients / J rows
-  float inp[(kMaxCode + 4) * kTP];   // decoder input [z | x] rows
-  float gin[(kMaxCode + 4) * kTP];   // d sdf / d(input) collected from the concat layers (latent_in / xyz_in_all)
-  float lnst[DSPGN_MAX_LINEAR * kTP];       // LayerNorm: [layer][p] reciprocal std (the mean is not needed backward)
-  float wbuf[2 * kKC * kHid];
-  uint8_t mask[8 * kHid * 8];        // ReLU masks: [layer][feature][p/8] bit p%8
-  float xo[3 * kTP];
-  float yv[kTP], rr[kTP], rscale[kTP];
-  float red[4 * kTP];
+  static constexpr int TP = simt_rows(H);
+  float act[H * TP];                 // feature-major activations / gradients / J rows
+  float inp[(kMaxCode + 4) * TP];    // decoder input [z | x] rows
+  float gin[(kMaxCode + 4) * TP];    // d sdf / d(input) collected from the concat layers (latent_in / xyz_in_all)
+  float lnst[DSPGN_MAX_LINEAR * TP];        // LayerNorm: [layer][p] reciprocal std (the mean is not needed backward)
+  float wbuf[2 * kKC * H];
+  uint8_t mask[8 * H * (TP / 8)];    // ReLU masks: [layer][feature][p/8] bit p%8
+  float xo[3 * TP];
+  float yv[TP], rr[TP], rscale[TP];
+  float red[kThreads];               // last layer: one partial dot product per thread
   int prefix[kMaxObjScan + 1];
   int warp_tmp[32];
 };
+static_assert(sizeof(SimtSmem<kHidWide>) <= 227 * 1024, "wide SIMT tile exceeds the opt-in shared memory");
 
 // LayerNorm backward (deep_sdf_decoder.py:96-102 through autograd): S.act holds the gradient w.r.t. the LN OUTPUT of
 // `layer` for its n features (already through the ReLU mask); turn it into the gradient w.r.t. the LN input:
 //   g_x = rstd * (gamma g - mean_j(gamma g) - xhat * mean_j(gamma g xhat)).     All threads; caller has synchronised.
-struct SimtSmem;
+template <int TP>
 __device__ inline void simt_ln_backward(float* act, float* red, const float* rstd, const float* __restrict__ gamma,
                                         const float* __restrict__ xhat, int n) {
   const int tid = threadIdx.x;
-  if (tid < kTP) {
+  if (tid < TP) {
     float s1 = 0.f, s2 = 0.f;
     for (int j = 0; j < n; ++j) {
-      const float gg = act[j * kTP + tid] * gamma[j];
+      const float gg = act[j * TP + tid] * gamma[j];
       s1 += gg;
-      s2 = fmaf(gg, xhat[j * kTP + tid], s2);
+      s2 = fmaf(gg, xhat[j * TP + tid], s2);
     }
     red[tid] = s1 / (float)n;
-    red[kTP + tid] = s2 / (float)n;
+    red[TP + tid] = s2 / (float)n;
   }
   __syncthreads();
-  for (int idx = tid; idx < n * kTP; idx += kThreads) {
-    const int j = idx / kTP, p = idx - j * kTP;
+  for (int idx = tid; idx < n * TP; idx += kThreads) {
+    const int j = idx / TP, p = idx - j * TP;
     const float gg = act[idx] * gamma[j];
-    act[idx] = rstd[p] * (gg - red[p] - xhat[idx] * red[kTP + p]);
+    act[idx] = rstd[p] * (gg - red[p] - xhat[idx] * red[TP + p]);
   }
   __syncthreads();
 }
 
+// H: the widest layer of any class of the solver (kHid or kHidWide); every class runs at that instantiation
+template <int H>
 __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermArgs a) {
+  constexpr int kTP = simt_rows(H);
+  constexpr int kNPart = kThreads / kTP;      // last layer: partial dot products per row
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  SimtSmem& S = *reinterpret_cast<SimtSmem*>(smem_raw);
-  const int tid = threadIdx.x, jg = tid >> 3, pg = tid & 7;
+  SimtSmem<H>& S = *reinterpret_cast<SimtSmem<H>*>(smem_raw);
+  const int tid = threadIdx.x, jg = tid >> ilog2(kTP / 8), pg = tid & (kTP / 8 - 1);
   const int total_tiles = build_tile_prefix(b, a, kTP, S.prefix, S.warp_tmp);
 
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -368,7 +386,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
     }
     for (int idx = tid; idx < L * kTP; idx += kThreads) S.inp[idx] = st.z[idx / kTP];
     for (int idx = tid; idx < (kMaxCode + 4) * kTP; idx += kThreads) S.gin[idx] = 0.f;
-    float* const xhat_all = (a.ln_scratch != nullptr) ? a.ln_scratch + (size_t)blockIdx.x * DSPGN_MAX_LINEAR * kHid * kTP : nullptr;
+    float* const xhat_all = (a.ln_scratch != nullptr) ? a.ln_scratch + (size_t)blockIdx.x * DSPGN_MAX_LINEAR * H * kTP : nullptr;
     __syncthreads();
     if (tid < 3 * kTP) S.inp[L * kTP + tid] = S.xo[tid];
     if (a.mode == MODE_RAYFWD) {
@@ -386,7 +404,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
     float acc[8][8];
     // ---- phase 1: forward -------------------------------------------------------------------
     for (int k = 0; k < nl - 1; ++k) {
-      gemm_rm(dec.Wf[k], dec.in_dim[k], (k == 0) ? S.inp : S.act, S.wbuf, acc);
+      gemm_rm<H, kTP>(dec.Wf[k], dec.in_dim[k], (k == 0) ? S.inp : S.act, S.wbuf, acc);
       const int nout = dec.out_dim[k];
       const float* bias = dec.bias[k];
       const float* lng = dec.ln_gamma[k];
@@ -404,7 +422,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
               bits |= (t > 0.f ? 1u : 0u) << pp;
               v[pp] = fmaxf(t, 0.f);
             }
-            S.mask[(k * kHid + j) * 8 + pg] = (uint8_t)bits;
+            S.mask[(k * H + j) * (kTP / 8) + pg] = (uint8_t)bits;
             float4* dst = reinterpret_cast<float4*>(S.act + j * kTP + 8 * pg);
             dst[0] = make_float4(v[0], v[1], v[2], v[3]);
             dst[1] = make_float4(v[4], v[5], v[6], v[7]);
@@ -435,7 +453,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
           S.lnst[k * kTP + tid] = 1.0f / sqrtf(var + 1e-5f);
         }
         __syncthreads();
-        float* xh_out = xhat_all + (size_t)k * kHid * kTP;
+        float* xh_out = xhat_all + (size_t)k * H * kTP;
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j = 8 * jg + jj;
@@ -451,7 +469,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
               bits |= (t > 0.f ? 1u : 0u) << pp;
               v[pp] = fmaxf(t, 0.f);
             }
-            S.mask[(k * kHid + j) * 8 + pg] = (uint8_t)bits;
+            S.mask[(k * H + j) * (kTP / 8) + pg] = (uint8_t)bits;
             float4* dst = reinterpret_cast<float4*>(S.act + j * kTP + 8 * pg);
             dst[0] = make_float4(v[0], v[1], v[2], v[3]);
             dst[1] = make_float4(v[4], v[5], v[6], v[7]);
@@ -469,14 +487,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
     }
     {  // last layer (out = 1) + tanh
       const int kin = dec.in_dim[nl - 1];
-      const int p = tid & (kTP - 1), part = tid >> 6;
-      const int j0 = part * (kHid / 4), j1 = min(kin, j0 + kHid / 4);
+      const int p = tid & (kTP - 1), part = tid >> ilog2(kTP);
+      const int j0 = part * (H / kNPart), j1 = min(kin, j0 + H / kNPart);
       float s = 0.f;
       for (int j = j0; j < j1; ++j) s = fmaf(dec.w_last[j], S.act[j * kTP + p], s);
       S.red[part * kTP + p] = s;
       __syncthreads();
       if (tid < kTP) {
-        float t = ((S.red[tid] + S.red[kTP + tid]) + S.red[2 * kTP + tid]) + S.red[3 * kTP + tid];
+        float t = S.red[tid];
+#pragma unroll
+        for (int q = 1; q < kNPart; ++q) t += S.red[q * kTP + tid];
         t += dec.bias[nl - 1][0];
         float dfac = 1.f;
         if (dec.use_tanh) { t = tanhf(t); dfac = 1.f - t * t; }        // deep_sdf_decoder.py:93-94
@@ -509,7 +529,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
         const int j = idx / kTP, p = idx - j * kTP;
         const float g = S.red[p] * dec.w_last[j];
         if (j < ncl) {
-          const unsigned bit = (S.mask[((nl - 2) * kHid + j) * 8 + (p >> 3)] >> (p & 7)) & 1u;
+          const unsigned bit = (S.mask[((nl - 2) * H + j) * (kTP / 8) + (p >> 3)] >> (p & 7)) & 1u;
           S.act[idx] = bit ? g : 0.f;
         } else {
           S.gin[((ckl == 1 ? 0 : L) + (j - ncl)) * kTP + p] += g;
@@ -517,10 +537,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       }
       __syncthreads();
       if (dec.ln_gamma[nl - 2] != nullptr)
-        simt_ln_backward(S.act, S.red + kTP, S.lnst + (nl - 2) * kTP, dec.ln_gamma[nl - 2], xhat_all + (size_t)(nl - 2) * kHid * kTP, ncl);
+        simt_ln_backward<kTP>(S.act, S.red + kTP, S.lnst + (nl - 2) * kTP, dec.ln_gamma[nl - 2], xhat_all + (size_t)(nl - 2) * H * kTP, ncl);
     }
     for (int k = nl - 2; k >= 0; --k) {
-      gemm_rm(dec.Wb[k], dec.out_dim[k], S.act, S.wbuf, acc);
+      gemm_rm<H, kTP>(dec.Wb[k], dec.out_dim[k], S.act, S.wbuf, acc);
       const int nin = dec.in_dim[k];
       const int ck = dec.cat_kind[k];
       const int ncont = (ck == 1) ? nin - in0 : (ck == 2 ? nin - 3 : nin);   // columns that continue down the chain
@@ -537,7 +557,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
 #pragma unroll
           for (int pp = 0; pp < 8; ++pp) v[pp] += dst[pp];
         } else if (k > 0) {
-          const unsigned bits = S.mask[((k - 1) * kHid + j) * 8 + pg];
+          const unsigned bits = S.mask[((k - 1) * H + j) * (kTP / 8) + pg];
 #pragma unroll
           for (int pp = 0; pp < 8; ++pp) v[pp] = ((bits >> pp) & 1u) ? v[pp] : 0.f;
           dst = S.act + j * kTP + 8 * pg;
@@ -555,7 +575,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       }
       __syncthreads();
       if (k > 0 && dec.ln_gamma[k - 1] != nullptr)      // through the LayerNorm of layer k-1 (its ReLU mask is applied above)
-        simt_ln_backward(S.act, S.red, S.lnst + (k - 1) * kTP, dec.ln_gamma[k - 1], xhat_all + (size_t)(k - 1) * kHid * kTP, ncont);
+        simt_ln_backward<kTP>(S.act, S.red, S.lnst + (k - 1) * kTP, dec.ln_gamma[k - 1], xhat_all + (size_t)(k - 1) * H * kTP, ncont);
     }
     // ---- phase 3: Jacobian rows  J = [code (0..63) | pose (64..70) | 0] ---------------------------
     for (int idx = tid + L * kTP; idx < kMaxCode * kTP; idx += kThreads) S.act[idx] = 0.f;  // code_len < 64

@@ -1402,6 +1402,8 @@ inline int tc_pack_decoder(const DspgnDecoderSpec& spec, const float* const* W, 
   const int nl = spec.num_linear, in0 = spec.latent_size + 3, li = dv->latent_in;
   if (nl != 9 && nl < 3) return 0;
   if (in0 > 80) return 0;
+  for (int k = 0; k < nl; ++k)               // the widest wgmma N is 256 (tc_mma_n): wider layers stay on the SIMT engine
+    if (spec.in_dim[k] > kHid || spec.out_dim[k] > kHid) return 0;
   TcPlan& P = dv->tc_plan;
   std::vector<unsigned char> blob;
   int ns = 0;

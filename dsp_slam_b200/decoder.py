@@ -18,8 +18,10 @@ class DecoderWeights:
     """Folded fp32 weights of one decoder: W[k] (out,in), b[k] (out,), latent size L, and what
     deep_sdf_decoder.py concatenates at each layer's input -- cat_kind[k]: 0 nothing, 1 the decoder input
     (`latent_in`, :87-88), 2 xyz (`xyz_in_all`, :89-90) -- plus the optional LayerNorm (gamma, beta) after layer k
-    (:58-63,96-102) and `use_tanh` (:93-94).  The plain shape (one latent_in layer, nothing else) runs on the
-    tensor-core engine; every other variant on the fp32 SIMT engine."""
+    (:58-63,96-102) and `use_tanh` (:93-94).  Accepted: 3 to 9 linear layers, each at most 512 wide, a latent size of
+    at most 64.  The plain shape (one latent_in layer, nothing else) with every layer at most 256 wide runs on the
+    tensor-core engine; every other decoder -- a variant, or a layer wider than 256 such as DeepSDF's own 8 x 512
+    network -- on the fp32 SIMT engine."""
 
     def __init__(self, W, b, latent_in, latent_size, xyz_in_all=False, use_tanh=False, ln=None):
         self.W = [np.ascontiguousarray(w, dtype=np.float32) for w in W]

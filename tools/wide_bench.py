@@ -1,0 +1,92 @@
+"""Cost of a 512-wide decoder: DeepSDF's own 8 x 512 network (tests/wide_fixtures.py, written to a temporary directory)
+against the 8 x 256 one (decoder_cars.npz), both on the fp32 SIMT engine, and the 8 x 256 decoder on the tensor-core
+engine as context, for
+
+  (a) LocalMapping's reconstruction call: 1 object, 250 points, 250 foreground + 200 background rays, 10 iterations
+      (Optimizer.reconstruct_object)
+  (b) the gated, meshed stereo keyframe of tools/keyframe_bench.py: 6 tracked cars of which 2 fail the map check, 2 new
+      cars, meshes of every object the call creates at voxels_dim --mesh-dim (dspgn_keyframe_batch_meshed)
+
+The legs alternate in one process; each is timed with the host clock around the whole call (it ends in a stream
+sync).  Prints one JSON line: per leg and decoder the median / min / p90 in ms, the ratio of the decoder's
+multiply-adds per row (forward) to the 8 x 256 decoder's, the card's name and power limit.
+
+  python tools/wide_bench.py [--steps K] [--warmup W] [--mesh-dim 32]
+"""
+import argparse
+import json
+import os
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+GOLDEN = os.path.join(ROOT, "tests", "golden")
+DECODERS = [("256_simt", "cars", "simt"), ("512_simt", "wide", "simt"), ("256_tc", "cars", "tc")]
+
+
+def macs_per_row(path):
+    from dsp_slam_b200.decoder import DecoderWeights
+    return sum(int(w.shape[0]) * int(w.shape[1]) for w in DecoderWeights.from_npz(path).W)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--mesh-dim", type=int, default=32)
+    args = ap.parse_args()
+    import torch
+    import __graft_entry__ as g
+    g.build()
+    from dsp_slam_b200 import synth
+    from dsp_slam_b200.optimizer import Optimizer
+    from keyframe_bench import N_NEW, N_TRACKED, gpu_card, keyframe_inputs
+    if not torch.cuda.is_available():
+        raise SystemExit("wide_bench.py needs a CUDA device (no CPU fallback)")
+    cfg, objs, modes = keyframe_inputs()
+    tracked = objs[:N_TRACKED]
+    gates = []
+    for i, o in enumerate(tracked):
+        M = np.array(o["t_cam_obj"], dtype=np.float32)
+        if i < 2:
+            M[0, 3] += np.float32(3.0)
+        gates.append(dict(t_cam_obj_map=M, t_cam_obj_sim3=o["t_cam_obj_sim3"]))
+    gates += [None] * N_NEW
+    one = synth.make_object(1, 250, 250, 200)
+
+    legs = {}
+    import wide_fixtures
+    tmp = tempfile.TemporaryDirectory()
+    path = {"cars": os.path.join(GOLDEN, "decoder_cars.npz"), "wide": wide_fixtures.write("wide", tmp.name)}
+    for label, dec, engine in DECODERS:
+        opt = Optimizer(path[dec], cfg, engine=engine)
+        legs[f"a_localmapping_{label}"] = lambda opt=opt: opt.reconstruct_object(
+            one["t_cam_obj_init"], one["pts"], one["rays"], one["depth"])
+        legs[f"b_keyframe_meshed_{label}"] = lambda s=opt.solver: s.keyframe(objs, modes, gates, voxels_dim=args.mesh_dim)
+    for f in legs.values():
+        for _ in range(args.warmup):
+            f()
+    times = {k: [] for k in legs}
+    for _ in range(args.steps):
+        for k, f in legs.items():
+            t0 = time.perf_counter()
+            f()
+            times[k].append((time.perf_counter() - t0) * 1e3)
+    base = macs_per_row(path["cars"])
+    out = {"metric": "wide_decoder_ms", "steps": args.steps, "mesh_dim": args.mesh_dim,
+           "decoder_macs_ratio": {label: macs_per_row(path[dec]) / base for label, dec, _ in DECODERS},
+           "legs": {k: {"median": float(np.median(v)), "min": float(np.min(v)), "p90": float(np.percentile(v, 90))}
+                    for k, v in times.items()},
+           "gpu": gpu_card()}
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
