@@ -10,7 +10,7 @@ MAX_CODE = 64
 MAX_LINEAR = 12
 RESULT_FLOATS = 88
 
-ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC = 0, 1, 2
+ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC, ENGINE_TC_WIDE = 0, 1, 2, 3
 SCHED_AUTO, SCHED_LAUNCHES, SCHED_PERSISTENT = 0, 1, 2
 MODE_JOINT, MODE_POSE = 0, 1
 GATE_OFF, GATE_KEPT, GATE_REJECTED = 0, 1, 2

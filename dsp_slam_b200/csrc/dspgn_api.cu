@@ -9,6 +9,7 @@
 #include <new>
 #include <algorithm>
 #include <atomic>
+#include <mutex>
 #include <thread>
 
 #include <cub/device/device_scan.cuh>
@@ -17,6 +18,7 @@
 #include "dspgn_simt.cuh"
 #include "dspgn_solve.cuh"
 #include "dspgn_tc.cuh"
+#include "dspgn_tc_wide.cuh"
 #include "dspgn_mesh.cuh"
 #include "dspgn_frame.cuh"
 #include "dspgn_mono.cuh"
@@ -80,6 +82,13 @@ struct DspgnDecoder {
   DecoderDev dev{};
   std::vector<void*> allocs;
   TcDecoderHost tc;
+  // DSPGN_ENGINE_TC_WIDE images, built by the first solver that asks for that engine (tcw_pack_decoder).  Solvers
+  // may be created from one decoder on several host threads: the build runs once, under the mutex, and a declined
+  // shape is recorded so that it is not downloaded again.
+  std::mutex tcw_mu;
+  bool tcw_declined = false;
+  TcDecoderHost tcw;
+  TcPlan tcw_plan{};
 };
 
 struct DspgnSolver {
@@ -121,7 +130,8 @@ struct DspgnSolver {
   bool mega_enabled = true;
   bool compact_rays = true;        // persistent kernel, render term: forward-only tiles over the valid-sample hulls only (env DSPGN_COMPACT_RAYS=0: all n_rays x D samples)
   DevBuf d_ev, d_seg, d_ln, d_vpre;
-  DevBuf d_masks;                  // k_gn_persistent: per-CTA ReLU mask scratch (kTcMaskLayers x kTcEpiThreads uint4 per SM)
+  DevBuf d_masks;                  // k_gn_persistent, k_wide_wgmma: per-CTA ReLU mask scratch (kTcMaskLayers x kTcEpiThreads uint4 per SM)
+  DevBuf d_tcw;                    // DSPGN_ENGINE_TC_WIDE: TcwDecDev of every class
   bool events_on = false;          // env DSPGN_CLK: the persistent kernel writes its event log (dspgn_debug_events)
   HostBuf h_results;
   // counters
@@ -210,7 +220,10 @@ void count_frame(int device, int delta) {
 }
 
 // rows per tile of the solver's decoder engine (the per-tile partial sums of a term: one slot per tile)
-int tile_rows(const DspgnSolver* s) { return (s->engine == DSPGN_ENGINE_TC) ? kTcRows : simt_rows(s->simt_hid); }
+int tile_rows(const DspgnSolver* s) {
+  if (s->engine == DSPGN_ENGINE_TC_WIDE) return kTcwRows;
+  return (s->engine == DSPGN_ENGINE_TC) ? kTcRows : simt_rows(s->simt_hid);
+}
 
 // the SIMT engine's LayerNorm scratch of one grid-sized launch: [CTA][layer][H][rows] (TermArgs.ln_scratch)
 size_t ln_half_floats(const DspgnSolver* s) {
@@ -428,6 +441,7 @@ void dspgn_decoder_destroy(DspgnDecoder* d) {
   cudaSetDevice(d->device);
   for (void* p : d->allocs) cudaFree(p);
   tc_free_decoder(d->tc);
+  tc_free_decoder(d->tcw);
   delete d;
 }
 
@@ -494,6 +508,25 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
     else eng = (tc_ok && tc_engine_default()) ? DSPGN_ENGINE_TC : DSPGN_ENGINE_SIMT;
   }
   if (eng == DSPGN_ENGINE_TC && !tc_ok) { dspgn_solver_destroy(s); return fail(DSPGN_E_ARG, "tensor-core engine unavailable for this decoder shape"); }
+  if (eng == DSPGN_ENGINE_TC_WIDE) {
+    std::vector<TcwDecDev> wd;
+    for (auto* d : s->classes) {
+      std::lock_guard<std::mutex> lock(d->tcw_mu);
+      if (!d->tcw.ok && !d->tcw_declined) {
+        if (int rc = tcw_pack_decoder(d->dev, d->hid, d->tcw, d->tcw_plan, g_err)) { dspgn_solver_destroy(s); return rc; }
+        d->tcw_declined = !d->tcw.ok;
+      }
+      if (d->tcw_declined) {
+        dspgn_solver_destroy(s);
+        return fail(DSPGN_E_ARG, "wide tensor-core engine (DSPGN_ENGINE_TC_WIDE) unavailable for this decoder shape: plain "
+                                 "decoders only (no LayerNorm, xyz_in_all, use_tanh or second latent_in layer)");
+      }
+      wd.push_back(TcwDecDev{reinterpret_cast<const unsigned char*>(d->tcw.blob), d->tcw_plan});
+    }
+    if (s->d_tcw.reserve(wd.size() * sizeof(TcwDecDev))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
+    CU(cudaMemcpy(s->d_tcw.p, wd.data(), wd.size() * sizeof(TcwDecDev), cudaMemcpyHostToDevice));
+    if (int rc = tcw_setup_kernel(g_err)) { dspgn_solver_destroy(s); return rc; }
+  }
   s->engine = eng;
   if (s->simt_hid == kHid)
     CU(cudaFuncSetAttribute(k_decoder_simt<kHid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHid>)));
@@ -505,7 +538,8 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
       if (s->d_ln.reserve(4 * 2 * ln_half_floats(s))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
       break;
     }
-  if (eng == DSPGN_ENGINE_TC &&
+  static_assert(kTcwMaskLayers <= kTcMaskLayers, "d_masks holds kTcMaskLayers layers per CTA, k_wide_wgmma strides by kTcwMaskLayers");
+  if ((eng == DSPGN_ENGINE_TC || eng == DSPGN_ENGINE_TC_WIDE) &&
       s->d_masks.reserve(sizeof(uint4) * (size_t)s->num_sms * kTcMaskLayers * kTcEpiThreads)) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
   if (int rc = tc_setup_kernels(g_err)) { dspgn_solver_destroy(s); return rc; }
   if (const char* m = getenv("DSPGN_MEGA")) s->mega_enabled = (m[0] != '0');
@@ -544,7 +578,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   dspgn_gather_close(s);
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
-                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_masks, &s->d_run,
+                    &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_masks, &s->d_tcw, &s->d_run,
                     &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout, &s->d_mesh_sel}) b->release();
   for (void* p : s->wide_allocs) cudaFree(p);
   s->h_stage.release();
@@ -783,6 +817,8 @@ int launch_term(DspgnSolver* s, const BatchDev& b, const TermArgs& a, long long 
   long long tiles = (rows_upper + rows - 1) / rows + s->n_obj;
   if (s->engine == DSPGN_ENGINE_TC) {
     if (int rc = tc_launch_term(b, a, grid_sms(s), tiles, st, g_err)) return rc;
+  } else if (s->engine == DSPGN_ENGINE_TC_WIDE) {
+    tcw_launch_term(b, a, s->d_tcw.as<TcwDecDev>(), s->d_masks.as<uint4>(), grid_sms(s), tiles, st);
   } else {
     int grid = (int)std::min<long long>(tiles, grid_sms(s));
     if (grid < 1) grid = 1;

@@ -547,8 +547,8 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[128], const uint32_t (&ah)[
 }
 
 // producer side of the ring: the weight images of one GEMM step, nch chunks of 4 stages of img_bytes each, into the ring
-// stages from (stage, phase) on
-template <int RING>
+// stages (STAGE_BYTES apart) from (stage, phase) on
+template <int RING, int STAGE_BYTES = kTcStageBytes>
 __device__ __forceinline__ void produce_step(const unsigned char* src, int nch, uint32_t img_bytes, unsigned char* ring,
                                              uint64_t* w_full, uint64_t* w_empty, uint32_t& stage, uint32_t& phase) {
   uint32_t st = (RING == kTcStages) ? 0u : stage;             // a 4-stage ring holds exactly one chunk
@@ -560,7 +560,7 @@ __device__ __forceinline__ void produce_step(const unsigned char* src, int nch, 
       mbar_wait(&w_empty[slot], ph ^ 1);
       DSPGN_PROBE_ADD(PR_WEMPTY, te);
       mbar_expect_tx(&w_full[slot], img_bytes);
-      bulk_g2s(ring + (size_t)slot * kTcStageBytes, src + (size_t)(kTcStages * c + s) * img_bytes, img_bytes, &w_full[slot]);
+      bulk_g2s(ring + (size_t)slot * STAGE_BYTES, src + (size_t)(kTcStages * c + s) * img_bytes, img_bytes, &w_full[slot]);
     }
     ring_at<RING>(st, phase, (uint32_t)kTcStages, st, phase);
   }

@@ -570,7 +570,7 @@ class Optimizer(object):
         c.pose_only_iterations = int(self.num_iterations_pose_only)
         c.sdf_only = int(bool(sdf_only))
         c.engine = {None: _lib.ENGINE_AUTO, "auto": _lib.ENGINE_AUTO, "simt": _lib.ENGINE_SIMT,
-                    "tc": _lib.ENGINE_TC}[engine]
+                    "tc": _lib.ENGINE_TC, "tc_wide": _lib.ENGINE_TC_WIDE}[engine]
         # kernel schedule (bit-identical results): None/"auto", "launches" (one launch per term per iteration), "persistent"
         c.schedule = {None: _lib.SCHED_AUTO, "auto": _lib.SCHED_AUTO, "launches": _lib.SCHED_LAUNCHES,
                       "persistent": _lib.SCHED_PERSISTENT}[schedule]
@@ -854,7 +854,8 @@ class MeshExtractor(object):
         c.b1 = c.b2 = 0.1; c.lr = 1.0; c.s_damp = 1.0
         c.num_iterations = 1; c.code_len = int(code_len); c.num_depth_samples = 50; c.cut_off = 0.01
         c.pose_only_iterations = 5; c.sdf_only = 1
-        c.engine = {None: _lib.ENGINE_AUTO, "auto": _lib.ENGINE_AUTO, "simt": _lib.ENGINE_SIMT, "tc": _lib.ENGINE_TC}[engine]
+        c.engine = {None: _lib.ENGINE_AUTO, "auto": _lib.ENGINE_AUTO, "simt": _lib.ENGINE_SIMT, "tc": _lib.ENGINE_TC,
+                    "tc_wide": _lib.ENGINE_TC_WIDE}[engine]
         self._dd = dd
         self.solver = BatchSolver([dd], c, device)
 

@@ -1,6 +1,6 @@
 """Cost of a 512-wide decoder: DeepSDF's own 8 x 512 network (tests/wide_fixtures.py, written to a temporary directory)
-against the 8 x 256 one (decoder_cars.npz), both on the fp32 SIMT engine, and the 8 x 256 decoder on the tensor-core
-engine as context, for
+against the 8 x 256 one (decoder_cars.npz), both on the fp32 SIMT engine and on the wide tensor-core engine
+(engine="tc_wide"), and the 8 x 256 decoder on the tensor-core engine as context, for
 
   (a) LocalMapping's reconstruction call: 1 object, 250 points, 250 foreground + 200 background rays, 10 iterations
       (Optimizer.reconstruct_object)
@@ -28,7 +28,8 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-DECODERS = [("256_simt", "cars", "simt"), ("512_simt", "wide", "simt"), ("256_tc", "cars", "tc")]
+DECODERS = [("256_simt", "cars", "simt"), ("512_simt", "wide", "simt"), ("256_tc", "cars", "tc"),
+            ("256_tc_wide", "cars", "tc_wide"), ("512_tc_wide", "wide", "tc_wide")]
 
 
 def macs_per_row(path):
