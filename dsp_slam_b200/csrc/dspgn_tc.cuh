@@ -257,8 +257,10 @@ constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcRing<SCHED> * kTcStageBytes + 
 static_assert(kTcSmemBytes<0> <= 227 * 1024, "k_decoder_tc: shared memory exceeds the 227 KB per block of sm_90");
 static_assert(kTcSmemBytes<1> <= 227 * 1024, "k_gn_persistent: shared memory exceeds the 227 KB per block of sm_90");
 static_assert(kTcSmemBytes<2> <= 227 * 1024, "k_gn_persistent_render: shared memory exceeds the 227 KB per block of sm_90");
-static_assert(offsetof(TcSmemTail<1>, bias) % 8 == 0 && offsetof(TcSmemTail<1>, w0x) % 8 == 0,
-              "the SDF-tile epilogues read bias and W0 column pairs as float2");
+static_assert(offsetof(TcSmemTail<0>, bias) % 8 == 0 && offsetof(TcSmemTail<0>, w0x) % 8 == 0 &&
+              offsetof(TcSmemTail<1>, bias) % 8 == 0 && offsetof(TcSmemTail<1>, w0x) % 8 == 0 &&
+              offsetof(TcSmemTail<2>, bias) % 8 == 0 && offsetof(TcSmemTail<2>, w0x) % 8 == 0,
+              "the epilogues read bias and W0 column pairs as float2");
 static_assert(offsetof(TcSmemTail<1>, maskw) % 16 == 0, "the SDF-tile kernel stages one uint4 of masks per thread");
 
 // ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
@@ -273,37 +275,15 @@ __device__ __forceinline__ int opaque_int(int v) {
 }
 
 // accumulator-shaped values -> A operand of the next GEMM step: hi halves into `ah` (the register A fragment of
-// K-step t is columns [16t, 16t+16) of the accumulator fragment), lo halves into this warpgroup's swizzled image.
-// Ends with the proxy fence and the warpgroup barrier the wgmma reads need.  pslot: probe build only, the step kind's
-// first probe slot (PR_EPI_KIND + 3 * kind), or -1.
-__device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&ah)[64], unsigned char* alo, int rl, int q, int grp,
-                                              int pslot = -1) {
-  DSPGN_PROBE_T(ts);
-#pragma unroll
-  for (int t = 0; t < 16; ++t) {
-#pragma unroll
-    for (int h = 0; h < 4; ++h) {       // h: (rows rl / rl+8) x (columns 16t+2q / 16t+8+2q)
-      uint32_t hi, lo;
-      split_pack(v[8 * t + 2 * h], v[8 * t + 2 * h + 1], hi, lo);
-      ah[4 * t + h] = hi;
-      const int row = rl + 8 * (h & 1), kk = 16 * t + 8 * (h >> 1) + 2 * q;
-      const int off = (kk >> 6) * 8192 + row * 128 + ((((kk & 63) >> 3) ^ (row & 7)) << 4) + (kk & 7) * 2;
-      *reinterpret_cast<uint32_t*>(alo + off) = lo;
-    }
-  }
-  DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 1, ts);
-  DSPGN_PROBE_T(tf);
-  fence_proxy_async();
-  wg_bar_sync(grp);
-  DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 2, tf);
-}
-
-// store_operand of the SDF-tile kernel: the same registers and bytes, the lo image written with 16 stmatrix.x4 instead of
-// 64 scalar stores.  The lo halves of K-step t form an m16k16 fragment whose four 8 x 8 matrices, (rows rl / rl + 8) x
-// (columns 16t.. / 16t+8..), are exactly the values h = 0..3 above; lane l gives the swizzled address of row l % 8 of
-// matrix l / 8.  In that row's 16-byte chunk  ((kk & 63) >> 3) ^ (row & 7)  the K-step enters only as 2(t & 3), so a lane
-// needs one base address and one xor per t.
-__device__ __forceinline__ void store_operand_stsm(const float (&v)[128], uint32_t (&ah)[64], uint32_t alo, int grp, int pslot = -1) {
+// K-step t is columns [16t, 16t+16) of the accumulator fragment), lo halves into this warpgroup's swizzled image `alo`
+// (shared-space address: 4 K chunks of 64 rows x 128 B, 128B swizzle), written with 16 stmatrix.x4.  The lo halves of
+// K-step t form an m16k16 fragment whose four 8 x 8 matrices, (rows rl / rl + 8) x (columns 16t.. / 16t+8..), are
+// exactly the thread's values h = 0..3, v[8t + 2h], v[8t + 2h + 1]; lane l gives the swizzled address of row l % 8 of
+// matrix l / 8.  Column kk of row `row` sits at byte  (kk >> 6) * 8192 + row * 128 + ((((kk & 63) >> 3) ^ (row & 7)) << 4)
+// + (kk & 7) * 2; in that 16-byte chunk the K-step enters only as 2(t & 3), so a lane needs one base address and one
+// xor per t.  Ends with the proxy fence and the warpgroup barrier the wgmma reads need.  pslot: probe build only, the
+// step kind's first probe slot (PR_EPI_KIND + 3 * kind), or -1.
+__device__ __forceinline__ void store_operand(const float (&v)[128], uint32_t (&ah)[64], uint32_t alo, int grp, int pslot = -1) {
   DSPGN_PROBE_T(ts);
   const int lane = threadIdx.x & 31;
   const int srow = 16 * ((threadIdx.x >> 5) & 3) + (lane & 7) + 8 * ((lane >> 3) & 1);
@@ -325,8 +305,7 @@ __device__ __forceinline__ void store_operand_stsm(const float (&v)[128], uint32
   DSPGN_PROBE_ADD_IF(pslot >= 0, pslot + 2, tf);
 }
 
-// ---- epilogue value loops of the SDF-tile kernel (k_gn_persistent).  They give the values of the general loops in
-// tc_body, element by element and in the same order, without a branch per element.  Fragment element e = 4j + h covers
+// ---- epilogue value loops of the tile, without a branch per fragment element.  Fragment element e = 4j + h covers
 // columns 8j + 2q + (h & 1) with q < 4, and n_mma and k_next are multiples of 8: a column is below either bound iff 8j
 // is.  NM / KNEXT are the step's n_mma / k_next at compile time, so for the pairs the 8 x 256 decoders produce every live
 // / zero decision is fixed per j.  NM = KNEXT = 0 is the fallback for other pairs: the runtime values nm / k_next.
@@ -443,8 +422,8 @@ __device__ __forceinline__ void epi_bwd_first(const float (&acc)[128], int qs, i
 }
 
 // layer 0 of a decoder whose first GEMM step takes all 256 of its outputs (k_steps * 16 = out_dim[0] = 256): every
-// column is live, bias (zb0) and the xyz rows of W0 are read as column pairs.  The fmaf order is that of the general
-// loop in tc_body:  bias -> x0 -> x1 -> x2.
+// column is live, bias (zb0) and the xyz rows of W0 are read as column pairs.  The fmaf order is that of the runtime
+// layer-0 loop in tc_body for other shapes:  bias -> x0 -> x1 -> x2.
 __device__ __forceinline__ void epi_layer0_256(float (&acc)[128], uint32_t (&mw)[4], const float* bias, const float* w0x, int qs,
                                                float xa0, float xa1, float xa2, float xb0, float xb1, float xb2) {
 #pragma unroll
@@ -938,11 +917,6 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       DSPGN_PROBE_T(tl0);
       if (tid == 0) S.cur_class = M.class_id;
 
-      // decoder input element i of tile row `row`: [z | x | 0...]
-      auto inp = [&](int i, int row) -> float {
-        const int j = i - L;
-        return (j < 0) ? S.zs[i] : ((unsigned)j < 3u ? S.xr[j * kTcRows + row] : 0.f);
-      };
       uint32_t* const maskw = S.maskw + tid;           // word w of layer l: maskw[(4 * l + w) * kTcEpiThreads]
       // SCHED 1: this thread's masks of layer l in the CTA's global scratch (16 bytes, written once per tile by the
       // forward step, read once by a backward step)
@@ -955,10 +929,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           for (int w = 0; w < 4; ++w) maskw[(4 * l + w) * kTcEpiThreads] = mw[w];
         }
       };
-      auto put_operand = [&](int pslot) {
-        if (SCHED == 1) store_operand_stsm(acc, ah, alo_s, grp, pslot);
-        else store_operand(acc, ah, alo, rl, qd, grp, pslot);
-      };
+      auto put_operand = [&](int pslot) { store_operand(acc, ah, alo_s, grp, pslot); };
 
       // ---- A operand of the first GEMM step (= layer 1): layer 0 on the CUDA cores.  With W0[:, :L] z folded into
       // zb0, layer 0 is 3 FMAs per output:  h0[j] = relu(zb0[j] + W0[j][L..L+2] . x)  (deep_sdf_decoder.py:91,103).
@@ -970,7 +941,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         const float xb0 = S.xr[rowB], xb1 = S.xr[kTcRows + rowB], xb2 = S.xr[2 * kTcRows + rowB];
         const int qs = opaque_int(qd);
         uint32_t mw[4] = {0u, 0u, 0u, 0u};
-        if (SCHED == 1 && kk == kHid && n0out == kHid) {
+        if (kk == kHid && n0out == kHid) {
           epi_layer0_256(acc, mw, S.bias, w0x, qs, xa0, xa1, xa2, xb0, xb1, xb2);
         } else {
 #pragma unroll
@@ -1077,26 +1048,11 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         } else if (st.kind == TK_FWD_HIDDEN) {
           const float* bb = S.bias + st.layer * kHid;
           uint32_t mw[4] = {0u, 0u, 0u, 0u};
-          if (SCHED == 1) {
-            if (nm == 256 && k_next == 256) epi_fwd_hidden<256, 256>(acc, mw, bb, qs, nm, k_next);
-            else if (nm == 192 && k_next == 256) epi_fwd_hidden<192, 256>(acc, mw, bb, qs, nm, k_next);
-            else epi_fwd_hidden<0, 0>(acc, mw, bb, qs, nm, k_next);
-            if (st.cat_off == 189 && L == 64) epi_concat_input<189, 64>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
-            else if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 128; ++e) {
-              const int c = frag_col(e, qs);
-              float t = 0.f;
-              if (c < nm) {
-                const float w = acc[e] + bb[c];
-                mw[e >> 5] |= (w > 0.f ? 1u : 0u) << (e & 31);
-                t = fmaxf(w, 0.f);
-              }
-              if (st.cat_off >= 0 && c >= st.cat_off) t = inp(c - st.cat_off, (e & 2) ? rowB : rowA);   // deep_sdf_decoder.py:87-88
-              acc[e] = (c < k_next) ? t : 0.f;
-            }
-          }
+          if (nm == 256 && k_next == 256) epi_fwd_hidden<256, 256>(acc, mw, bb, qs, nm, k_next);
+          else if (nm == 192 && k_next == 256) epi_fwd_hidden<192, 256>(acc, mw, bb, qs, nm, k_next);
+          else epi_fwd_hidden<0, 0>(acc, mw, bb, qs, nm, k_next);
+          if (st.cat_off == 189 && L == 64) epi_concat_input<189, 64>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
+          else if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
           save_mask(st.layer, mw);
           DSPGN_PROBE_ADD(pk, tval);
           put_operand(pk);
@@ -1110,48 +1066,16 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
 #pragma unroll
             for (int w = 0; w < 4; ++w) mw[w] = maskw[(4 * st.mask_layer + w) * kTcEpiThreads];
           }
-          if (SCHED == 1) {
-            if (st.cat_off == 189 && L == 64 && in0 == 67 && nm == kHid) epi_skip_grad<189, 64>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
-            else if (st.cat_off >= 0) epi_skip_grad<0, 0>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
-            if (nm == 256 && k_next == 256) epi_bwd_mid<256, 256>(acc, mw, nm, k_next);
-            else if (nm == 256 && k_next == 192) epi_bwd_mid<256, 192>(acc, mw, nm, k_next);
-            else epi_bwd_mid<0, 0>(acc, mw, nm, k_next);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 128; ++e) {
-              const int c = frag_col(e, qs);
-              float t = 0.f;
-              if (c < nm) {
-                const float v = acc[e];
-                t = ((mw[e >> 5] >> (e & 31)) & 1u) ? v : 0.f;
-                if (st.cat_off >= 0 && c >= st.cat_off) {      // latent_in skip path -> d/d(input)
-                  const int ii = c - st.cat_off;
-                  if (ii < in0) S.Jp[((e & 2) ? rowB : rowA) * kJpStride + ((ii < L) ? ii : (kMaxCode + ii - L))] = v;
-                  t = 0.f;
-                }
-              }
-              acc[e] = (c < k_next) ? t : 0.f;
-            }
-          }
+          if (st.cat_off == 189 && L == 64 && in0 == 67 && nm == kHid) epi_skip_grad<189, 64>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
+          else if (st.cat_off >= 0) epi_skip_grad<0, 0>(acc, qs, nm, st.cat_off, in0, L, S.Jp, rowA, rowB);
+          if (nm == 256 && k_next == 256) epi_bwd_mid<256, 256>(acc, mw, nm, k_next);
+          else if (nm == 256 && k_next == 192) epi_bwd_mid<256, 192>(acc, mw, nm, k_next);
+          else epi_bwd_mid<0, 0>(acc, mw, nm, k_next);
           DSPGN_PROBE_ADD(pk, tval);
           if (more) put_operand(pk);
         } else {
           // ---- TK_BWD_FIRST: d/d(input) complete -> Jacobian row (loss.py:34-41 / :143-150) -------------
-          if (SCHED == 1) {
-            epi_bwd_first(acc, qs, in0, L, has_skip, S.Jp, S.scr, rowA, rowB);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 128; ++e) {
-              const int c = frag_col(e, qs);
-              if (c < nm && c < in0) {
-                const int row = (e & 2) ? rowB : rowA;
-                float* pj = S.Jp + row * kJpStride + ((c < L) ? c : (kMaxCode + c - L));
-                float g = acc[e];
-                if (has_skip) g += *pj;
-                *pj = g * S.scr[row];                                  // loss.py:145 (de_ds) / inactive rows
-              }
-            }
-          }
+          epi_bwd_first(acc, qs, in0, L, has_skip, S.Jp, S.scr, rowA, rowB);
           DSPGN_PROBE_ADD(pk, tval);
         }
         if (!more || st.kind == TK_BWD_FIRST) {
@@ -1181,7 +1105,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         if (mask_out != nullptr && mode == MODE_SDF && r < nrows)
           mask_out[M.pts_off + row0 + r] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;      // optimizer.py:76-78
         S.rr[r] = huber_weight(fabsf(res), huber_b) * res;
-        if (SCHED == 1) jr[kMaxCode + 7] = S.rr[r];      // the J^T J chains of column block 17 give J^T (rho r) as well
+        jr[kMaxCode + 7] = S.rr[r];                       // the J^T J chains of column block 17 give J^T (rho r) as well
         S.rsc[r] = (mode == MODE_SDF) ? sc : (r < nrows ? 1.f : 0.f);
         if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF && r < nrows) a.dbg_res[row0 + r] = res;
       }
@@ -1228,18 +1152,13 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
             const int rI = 4 * bi + u, cI = 4 * bj + v;
             if (cI >= rI && cI < kMaxCode + 7) accp[tri_index(rI, cI)] = h[u][v];
           }
-        if (SCHED == 1 && bj == 17) {
-          // column 71 holds rho r: the same fmaf chains over p as the J^T r loop below
+        if (bj == 17) {
+          // column 71 holds rho r: J^T (rho r) is  fmaf(J[p][c], rho r[p], .)  over p = 0..127 in order
 #pragma unroll
           for (int u = 0; u < 4; ++u)
             if (4 * bi + u < kMaxCode + 7) accp[kAccB + 4 * bi + u] = h[u][3];
         }
         DSPGN_PROBE_ADD(PR_JTJ_STORE, tjs);
-      } else if (SCHED != 1 && tid < 171 + kMaxCode + 7) {
-        const int c = tid - 171;
-        float sacc = 0.f;
-        for (int p = 0; p < kTcRows; ++p) sacc = fmaf(S.Jp[p * kJpStride + c], S.rr[p], sacc);
-        accp[kAccB + c] = sacc;
       } else if (tid >= 248) {
         // loss and row count: 8 threads x 16 rows, fixed-order combine
         const int k = tid - 248;
@@ -1345,7 +1264,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_tc_selftest(const float* __re
     const int c = frag_col(e, qd);
     acc[e] = (c < k_steps * 16) ? A[(size_t)((e & 2) ? rowB : rowA) * lda + c] : 0.f;
   }
-  store_operand(acc, ah, alo, rl, qd, grp);
+  store_operand(acc, ah, smem_u32(alo), grp);
   if (n_img == 80) wg_gemm<80, kTcStages>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), stage, phase, nch);
   else if (n_img == 192) wg_gemm<192, kTcStages>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), stage, phase, nch);
   else wg_gemm<256, kTcStages>(acc, ah, smem_u32(alo), smem_u32(ring), smem_u32(bars), stage, phase, nch);
