@@ -115,7 +115,7 @@ struct DspgnSolver {
   DevBuf d_sdf, d_bx, d_bs, d_br;
   DevBuf d_dbg;
   DevBuf d_q_flag, d_q_ctr, d_tiles_left, d_obj_iter;   // persistent-kernel work queue
-  int* d_tbase_static = nullptr;   // [n_obj] first 128-row SDF tile of each object (inside the staging block)
+  int* d_tbase_static = nullptr;   // [n_obj] first SDF tile (engine tile height) of each object (inside the staging block)
   int* d_tbase_r_static = nullptr; // [n_obj] first band-tile partial slot of each object (capacity: its ray-sample tiles + 1)
   // per-run object table (layout: run_table)
   DevBuf d_run;
@@ -124,9 +124,8 @@ struct DspgnSolver {
   bool run_upload_pending = false;
   bool run_table_valid = false;    // d_run holds h_run for the resident batch (a repeated run skips the copy)
   bool run_table_gated = false;    // ... and it is the table of a gated run (it has link and t_map)
-  int total_tiles128 = 0;          // SDF tiles of the batch
-  long long total_ray_tiles128 = 0;// ray-sample tiles of the batch
-  int max_tiles128 = 0;            // largest tile count of one term of one object (queue items hold 19 bits)
+  int total_tiles = 0;             // SDF tiles of the batch at the engine's tile height (tile_rows)
+  int max_tiles = 0;               // largest tile count of one term of one object (queue items hold 19 bits)
   bool mega_enabled = true;
   bool compact_rays = true;        // persistent kernel, render term: forward-only tiles over the valid-sample hulls only (env DSPGN_COMPACT_RAYS=0: all n_rays x D samples)
   DevBuf d_ev, d_seg, d_ln, d_vpre;
@@ -696,15 +695,16 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
     int acc = 0, mx = 0;
     long long accr = 0;
     int* hTBr = hTB + n_obj;
+    const int rows = tile_rows(s);
     for (int o = 0; o < n_obj; ++o) {
-      const int nt = (s->h_meta[o].n_pts + kTcRows - 1) / kTcRows;
-      const int ntf = (int)(((long long)s->h_meta[o].n_rays * D + kTcRows - 1) / kTcRows);
+      const int nt = (s->h_meta[o].n_pts + rows - 1) / rows;
+      const int ntf = (int)(((long long)s->h_meta[o].n_rays * D + rows - 1) / rows);
       hTB[o] = acc; hTBr[o] = (int)(accr + o);
       acc += nt; accr += ntf;
       if (nt > mx) mx = nt;
       if (ntf > mx) mx = ntf;
     }
-    s->total_tiles128 = acc; s->total_ray_tiles128 = accr; s->max_tiles128 = mx;
+    s->total_tiles = acc; s->max_tiles = mx;
   }
   for (int o = 0; o < n_obj; ++o) {
     const DspgnObjectIn& I = in[o];
@@ -892,7 +892,7 @@ struct RunPlan {
 int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = false, const int32_t* link = nullptr,
              const float* t_map = nullptr) {
   const DspgnConfig& c = s->cfg;
-  const int n = s->n_obj, D = c.num_depth_samples;
+  const int n = s->n_obj, D = c.num_depth_samples, rows = tile_rows(s);
   p = RunPlan{};
   p.gated = link != nullptr;
   for (int o = 0; o < n; ++o) {
@@ -918,7 +918,7 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
     const int m = modes[o];
     const bool dormant = link && link[o] >= 0 && m == DSPGN_MODE_JOINT;
     const bool r = p.render && m == DSPGN_MODE_JOINT;
-    const long long ntS = (M.n_pts + kTcRows - 1) / kTcRows, ntF = ((long long)M.n_rays * D + kTcRows - 1) / kTcRows;
+    const long long ntS = (M.n_pts + rows - 1) / rows, ntF = ((long long)M.n_rays * D + rows - 1) / rows;
     if (!dormant) {
       p.pts[m] += M.n_pts;
       if (m == DSPGN_MODE_JOINT) p.smp_joint += (long long)M.n_rays * D;
@@ -949,6 +949,7 @@ int launch_init(DspgnSolver* s, const BatchDev& b, const RunPlan& p, const MegaA
   ia.code_len = s->cfg.code_len;
   ia.n_iter_joint = p.iters[DSPGN_MODE_JOINT]; ia.n_iter_pose = p.iters[DSPGN_MODE_POSE];
   ia.n_bad = s->n_bad;
+  ia.tile_rows = tile_rows(s);
   k_init<<<s->n_obj, 128, 0, s->stream>>>(b, ia, q);
   s->ctr.kernel_launches++;
   CU(cudaGetLastError());
@@ -1064,8 +1065,9 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
   s->evs_used = 0;
   CU(cudaEventRecord(s->ev_run0, s->stream));
   const bool render = p.render;
-  const bool mega = s->mega_enabled && s->engine == DSPGN_ENGINE_TC && s->total_tiles128 > 0 &&
-                    s->max_tiles128 <= kItemTileMask && s->n_obj <= kItemObjMask + 1 && p.q_cap < (1LL << 27);
+  const bool wide = s->engine == DSPGN_ENGINE_TC_WIDE;
+  const bool mega = s->mega_enabled && (s->engine == DSPGN_ENGINE_TC || wide) && s->total_tiles > 0 &&
+                    s->max_tiles <= kItemTileMask && s->n_obj <= kItemObjMask + 1 && p.q_cap < (1LL << 27);
   if (mega) {
     // ---- persistent object-pipelined kernel: every GN iteration of every object in ONE launch --------------
     MegaArgs q;
@@ -1080,10 +1082,11 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     if (p.any[DSPGN_MODE_POSE] && p.iters[DSPGN_MODE_POSE] > 5) { a.pt_active = s->d_active.as<uint8_t>(); a.cut_iter = 4; }
     if (q.log.ev) CU(cudaMemsetAsync(q.log.ev, 0, 8, s->stream));
     SolveArgs v = base_solve(s);
-    v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.tile_rows = kTcRows; v.iter_index = 0;
+    v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.iter_index = 0;
     const int grid = grid_sms(s);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
-    if (render) k_gn_persistent_render<<<grid, kTcThreads, kTcSmemBytes<2>, s->stream>>>(b, a, q, v);
+    if (wide) k_wide_persistent<<<grid, kTcThreads, kTcwMegaSmemBytes, s->stream>>>(b, a, q, v, s->d_tcw.as<TcwDecDev>(), s->d_masks.as<uint4>());
+    else if (render) k_gn_persistent_render<<<grid, kTcThreads, kTcSmemBytes<2>, s->stream>>>(b, a, q, v);
     else k_gn_persistent<<<grid, kTcThreads, kTcSmemBytes<1>, s->stream>>>(b, a, q, v, s->d_masks.as<uint4>());
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
     s->ctr.kernel_launches += 1;

@@ -373,6 +373,7 @@ struct InitArgs {
   int code_len;
   int n_iter_joint, n_iter_pose;   // GN iterations of a joint / pose-only object
   int n_bad;                       // objects rejected at upload (they count as done from the start)
+  int tile_rows;                   // rows per tile of the persistent kernel that runs next (its iteration-0 items)
 };
 
 // zb0 = b0 + W0[:, :L] z   (fp32 FMA chain in i order; all threads of the calling CTA / epilogue)
@@ -424,16 +425,17 @@ __global__ void k_init(BatchDev b, InitArgs a, MegaArgs q) {
     if (tid == 0 && link >= 0 && mode == DSPGN_MODE_POSE) gate_record(b.results, o, b.T_init, b.t_map);
   }
   if (mega) {
-    const int ntS = (M.n_pts + kTcRows - 1) / kTcRows;
+    const int rows = a.tile_rows;
+    const int ntS = (M.n_pts + rows - 1) / rows;
     // slots reserved by the host for this object's iteration 0: every ray sample (joint objects of a run with the render
     // term) + every SDF tile
-    const int ntF_cap = (q.render && !M.bad && mode == DSPGN_MODE_JOINT) ? (M.n_rays * b.D + kTcRows - 1) / kTcRows : 0;
+    const int ntF_cap = (q.render && !M.bad && mode == DSPGN_MODE_JOINT) ? (M.n_rays * b.D + rows - 1) / rows : 0;
     int ntF = ntF_cap;
     if (q.vpre != nullptr && ntF_cap > 0) {
       __shared__ int s_wsum[32];
       __syncthreads();                         // T_oc / depth range written by thread 0 above
       const int vh = valid_sample_ranges<false>(M, st, b.rays, b.D, q.vpre + vpre_base(M, o), tid, blockDim.x, s_wsum);
-      ntF = (vh + kTcRows - 1) / kTcRows;
+      ntF = (vh + rows - 1) / rows;
     }
     const int base = b.q0_off[o];
     if (!dormant) {                          // a dormant slot has no reserved slots: its wake pushes these items

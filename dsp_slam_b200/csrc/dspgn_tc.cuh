@@ -251,6 +251,8 @@ struct TcSmemTail {
   BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
   int push_base, push_nF, push_nS, push_o;   // cooperative publication of an object's next-iteration tiles
   float ost[16]; int ost_rows;            // the tile's object: T_oc[12], dmin, dmax, dstep, dfar; rows of its term (counter)
+  // workspace of the solve step (mega_solve_and_advance): the J tile, dead between tiles
+  __device__ SolveSmem& solve_smem() { return *reinterpret_cast<SolveSmem*>(Jp); }
 };
 template <int SCHED>
 constexpr size_t kTcSmemBytes = 1024 + (size_t)kTcRing<SCHED> * kTcStageBytes + 2 * (size_t)kTcAloBytes + sizeof(TcSmemTail<SCHED>);
@@ -574,6 +576,38 @@ __device__ inline int mega_pop(const MegaArgs& q, int n_obj) {
   }
 }
 
+// Persistent kernels: work item number `seq` of this CTA from the CTA-local FIFO its scheduler lane fills (mega_fifo_fill),
+// as a tile of ROWS rows; false once the queue is drained.  SDF_ONLY: every item is an SDF tile (a compile-time kind).
+template <int ROWS, bool SDF_ONLY, class Tail>
+__device__ __forceinline__ bool mega_tile_at(const TermArgs& a, Tail& S, int seq, TileRef& t) {
+  volatile int* pub = &S.fifo_pub;
+  while (*pub <= seq) __nanosleep(64);           // filled by this CTA's scheduler lane, which always terminates (mega_pop)
+  const int item = reinterpret_cast<volatile int*>(S.fifo)[seq & 3];
+  if (item < 0) return false;
+  t.o = (item >> kItemObjShift) & kItemObjMask;
+  t.mode = SDF_ONLY ? MODE_SDF : (item >> kItemKindShift);
+  const int j = item & kItemTileMask;
+  t.tile = j;
+  t.row0 = j * ROWS;
+  t.slot = (t.mode == MODE_BAND) ? a.tile_base_r[t.o] + j : (t.mode == MODE_SDF ? a.tile_base[t.o] + j : 0);
+  return true;
+}
+
+// The scheduler lane of a persistent kernel: pop this CTA's next work item into slot `seq` of the CTA-local FIFO, at most
+// 3 entries ahead of the epilogue warps, and publish it (-1: no more work).
+template <class Tail>
+__device__ __forceinline__ void mega_fifo_fill(const MegaArgs& q, int n_obj, Tail& S, int seq) {
+  DSPGN_PROBE_T(tp);
+  volatile int* es = &S.epi_seq;
+  while (seq - *es >= 3) __nanosleep(64);   // the epilogue warps always make progress (bounded tile work)
+  const int item = mega_pop(q, n_obj);
+  DSPGN_PROBE_ADD(PR_POP, tp);
+  if (item >= 0) log_event(q.log, ev_desc(EV_POPPED, item >> kItemKindShift, (item >> kItemObjShift) & kItemObjMask, item & kItemTileMask));
+  reinterpret_cast<volatile int*>(S.fifo)[seq & 3] = item;
+  __threadfence_block();
+  *reinterpret_cast<volatile int*>(&S.fifo_pub) = seq + 1;
+}
+
 // tile number `seq` of this CTA: static round-robin over the launch's tiles, or the CTA-local FIFO
 // SCHED: 0 = one launch per term (static tiles), 1 = persistent kernel, SDF tiles only (SDF-only joint runs, pose-only
 // runs: the tile kind is a compile-time constant), 2 = persistent kernel with the render term (all item kinds)
@@ -590,17 +624,7 @@ __device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, Tc
     t.mode = a.mode;
     return true;
   } else {
-    volatile int* pub = &S.fifo_pub;
-    while (*pub <= seq) __nanosleep(64);           // filled by this CTA's scheduler lane, which always terminates (mega_pop)
-    const int item = reinterpret_cast<volatile int*>(S.fifo)[seq & 3];
-    if (item < 0) return false;
-    t.o = (item >> kItemObjShift) & kItemObjMask;
-    t.mode = (SCHED == 1) ? MODE_SDF : (item >> kItemKindShift);
-    const int j = item & kItemTileMask;
-    t.tile = j;
-    t.row0 = j * kTcRows;
-    t.slot = (t.mode == MODE_BAND) ? a.tile_base_r[t.o] + j : (t.mode == MODE_SDF ? a.tile_base[t.o] + j : 0);
-    return true;
+    return mega_tile_at<kTcRows, SCHED == 1>(a, S, seq, t);
   }
 }
 
@@ -622,14 +646,15 @@ __device__ inline void mega_push(const MegaArgs& q, int kind, int o, int n) {
 }
 
 // all terms of the object's current iteration are in: solve, update, queue the next iteration (or finish).  Called by
-// the 256 epilogue threads of the CTA that completed the object's last outstanding tile.
-template <int SCHED>
-__device__ __noinline__ void mega_solve_and_advance(TcSmemTail<SCHED>& S, int o, int tid) {
+// the 256 epilogue threads of the CTA that completed the object's last outstanding tile.  ROWS: rows per tile of the
+// kernel; Tail: its shared-memory tail (argument copies, push fields, warp_tmp, solve_smem()).
+template <int ROWS, class Tail>
+__device__ __noinline__ void mega_solve_and_advance(Tail& S, int o, int tid) {
   const BatchDev& b = S.ctx_b;
   const MegaArgs& q = S.ctx_q;
   const SolveArgs& sv = S.ctx_sv;
   __threadfence();
-  SolveSmem& SM = *reinterpret_cast<SolveSmem*>(S.Jp);
+  SolveSmem& SM = S.solve_smem();
   const int it = ldv(q.obj_iter + o);
   const bool render = q.render && b.state[o].mode == DSPGN_MODE_JOINT;     // pose-only objects: SDF tiles only
   if (tid == 0) log_event(q.log, ev_desc(EV_SOLVE_BEGIN, 0, o, it));
@@ -661,15 +686,15 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail<SCHED>& S, int o,
       __threadfence();                       // the result record before the object counts as done
       atomicAdd(&q.ctr->done_objects, (slot >= 0 && !wake) ? 2 : 1);
       if (wake) {
-        const int ntF = ldv(q.ray_left + slot), ntS = (b.meta[slot].n_pts + kTcRows - 1) / kTcRows;
+        const int ntF = ldv(q.ray_left + slot), ntS = (b.meta[slot].n_pts + ROWS - 1) / ROWS;
         base = atomicAdd(&q.ctr->tail, ntF + ntS);
         S.push_nF = ntF; S.push_nS = ntS; S.push_o = slot;
       }
     } else {
       // (no fence in this branch: the tail only reserves slots; state and counters are fenced below, before any slot is published)
       const ObjMeta M = b.meta[o];
-      const int ntS = (M.n_pts + kTcRows - 1) / kTcRows;
-      const int ntF = render ? ((vh >= 0 ? vh : M.n_rays * b.D) + kTcRows - 1) / kTcRows : 0;
+      const int ntS = (M.n_pts + ROWS - 1) / ROWS;
+      const int ntF = render ? ((vh >= 0 ? vh : M.n_rays * b.D) + ROWS - 1) / ROWS : 0;
       *reinterpret_cast<volatile int*>(q.obj_iter + o) = it + 1;
       *reinterpret_cast<volatile int*>(q.pending + o) = ntS + (ntF > 0 ? 1 : 0);
       *reinterpret_cast<volatile int*>(q.ray_left + o) = ntF;
@@ -687,6 +712,83 @@ __device__ __noinline__ void mega_solve_and_advance(TcSmemTail<SCHED>& S, int o,
     epi_bar_sync();                           // ... of every thread, before the first slot is published
     for (int j = tid; j < n; j += kTcEpiThreads)
       *reinterpret_cast<volatile int*>(q.q_flag + base + j) = ((j < nF) ? make_item(MODE_RAYFWD, po, j) : make_item(MODE_SDF, po, j - nF)) + 1;
+  }
+}
+
+// Scan item of a persistent kernel: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141), no GEMM
+// steps.  The CTA that finishes the object's last chunk turns the segment counts into the band-row prefix and queues the
+// band tiles (ROWS rows each); when no SDF tile is outstanding either, it runs the solve step.  256 epilogue threads.
+// k_wide_persistent calls it; tc_body keeps the same steps inline: called from there, k_gn_persistent_render grows to
+// 642 branch regions (BSSY), over the 638 tests/test_tc_sass.py allows it.
+template <int ROWS, class Tail>
+__device__ __forceinline__ void mega_scan_item(Tail& S, const BatchDev& b, const MegaArgs& q, const SolveArgs& sv, const TileRef& tr,
+                                               int tid) {
+  const int o = tr.o;
+  scan_chunk(b, sv.prm.th, q.vpre, q.seg_cnt, o, tr.tile, tid);
+  __threadfence();
+  epi_bar_sync();
+  if (tid == 0) {
+    log_event(q.log, ev_desc(EV_TILE_END, tr.mode, o, tr.tile));
+    *reinterpret_cast<volatile int*>(&S.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
+  }
+  epi_bar_sync();
+  int act = *reinterpret_cast<volatile int*>(&S.last_flag);
+  if (act == 1) {
+    // last chunk of the object: segment prefix -> band row count -> band tiles
+    __threadfence();
+    scan_prefix(b, q.seg_cnt, q.seg_prefix, o, tid, S.warp_tmp);
+    epi_bar_sync();
+    if (tid == 0) {
+      __threadfence();                         // prefix / band_m / band rows before the band tiles are published
+      atomicAdd(&q.ctr->valid_rows_total, (unsigned long long)ldv(b.V_count + o));   // V of this iteration is complete (roofline accounting)
+      const int m = ldv(b.band_m + o);
+      const int ntB = (m + ROWS - 1) / ROWS;
+      atomicAdd(&q.ctr->band_rows_total, m);
+      // the render term's placeholder in `pending` becomes its ntB band tiles BEFORE they can be popped
+      const int left = atomicAdd(q.pending + o, ntB - 1) + ntB - 1;
+      mega_push(q, MODE_BAND, o, ntB);
+      *reinterpret_cast<volatile int*>(&S.last_flag) = (left == 0) ? 2 : 0;
+    }
+    epi_bar_sync();
+    act = *reinterpret_cast<volatile int*>(&S.last_flag);
+  } else act = 0;
+  if (act == 2) mega_solve_and_advance<ROWS>(S, o, tid);
+}
+
+// End of a GEMM tile of a persistent kernel (kind `mode`, tile `tile` of object o, meta M): its partial
+// sums / sdf values go out device-wide, then the object pipeline.  Per object and iteration:  ray-sample tiles (forward
+// only) -> [last one] per-ray scan + band compaction -> band tiles (fwd+bwd) ;  SDF tiles (fwd+bwd) ;  [last SDF / band
+// tile] solve, pose / code update, tiles of the next iteration.  The CTA that finishes the last tile of a stage runs the
+// serial step with its 256 epilogue threads while every other SM keeps working on other objects.
+template <bool RENDER, int ROWS, class Tail>
+__device__ __forceinline__ void mega_tile_end(Tail& S, const MegaArgs& q, const ObjMeta& M, int o, int mode, int tile, int tid) {
+  DSPGN_PROBE_T(tend);
+  __threadfence();                             // this tile's partial sums / sdf values are visible device-wide
+  epi_bar_sync();
+  if (tid == 0) {
+    log_event(q.log, ev_desc(EV_TILE_END, mode, o, tile));
+    int act = 0;
+    if (RENDER && mode == MODE_RAYFWD) { if (atomicSub(q.ray_left + o, 1) == 1) act = 1; }
+    else if (atomicSub(q.pending + o, 1) == 1) act = 2;
+    *reinterpret_cast<volatile int*>(&S.last_flag) = act;
+  }
+  epi_bar_sync();
+  int act = *reinterpret_cast<volatile int*>(&S.last_flag);
+  if (RENDER && act == 1) {
+    // every ray sample of the object has its sdf value: the per-ray scan becomes 64-ray work items of its own
+    if (tid == 0) {
+      const int nch = (M.n_rays + kScanChunkRays - 1) / kScanChunkRays;
+      *reinterpret_cast<volatile int*>(q.scan_left + o) = nch;
+      __threadfence();
+      mega_push(q, kKindScan, o, nch);
+    }
+  }
+  DSPGN_PROBE_ADD(PR_TILE_END, tend);
+  if (act == 2) {
+    DSPGN_PROBE_T(tsv);
+    mega_solve_and_advance<ROWS>(S, o, tid);
+    DSPGN_PROBE_ADD(PR_SOLVE, tsv);
+    DSPGN_PROBE_COUNT(PR_SOLVES);
   }
 }
 
@@ -727,18 +829,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       uint32_t stage = 0, phase = 0;
       DSPGN_PROBE_T(tloop);
       for (int seq = 0;; ++seq) {
-        if (MEGA) {
-          // scheduler: fetch this CTA's next tile into the local FIFO (at most 3 entries ahead of the epilogue)
-          DSPGN_PROBE_T(tp);
-          volatile int* es = &S.epi_seq;
-          while (seq - *es >= 3) __nanosleep(64);   // the epilogue warps always make progress (bounded tile work)
-          const int item = mega_pop(q, b.n_obj);
-          DSPGN_PROBE_ADD(PR_POP, tp);
-          if (item >= 0) log_event(q.log, ev_desc(EV_POPPED, item >> kItemKindShift, (item >> kItemObjShift) & kItemObjMask, item & kItemTileMask));
-          reinterpret_cast<volatile int*>(S.fifo)[seq & 3] = item;
-          __threadfence_block();
-          *reinterpret_cast<volatile int*>(&S.fifo_pub) = seq + 1;
-        }
+        if (MEGA) mega_fifo_fill(q, b.n_obj, S, seq);
         TileRef tr;
         if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
         const int o = tr.o;
@@ -778,6 +869,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = seq + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
       if (RENDER && tr.mode == kKindScan) {
         // ---- scan item: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141); no GEMM steps ----------
+        // (the steps of mega_scan_item, inline: see there)
         const int o = tr.o;
         scan_chunk(b, sv.prm.th, q.vpre, q.seg_cnt, o, tr.tile, tid);
         __threadfence();
@@ -807,7 +899,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           epi_bar_sync();
           act = *reinterpret_cast<volatile int*>(&S.last_flag);
         } else act = 0;
-        if (act == 2) mega_solve_and_advance(S, o, tid);
+        if (act == 2) mega_solve_and_advance<kTcRows>(S, o, tid);
         continue;
       }
       const int o = tr.o, row0 = tr.row0, tile = tr.slot, mode = tr.mode;
@@ -1173,40 +1265,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       }
       }   // !fwd_only
       DSPGN_PROBE_ADD(PR_JTJ, tjtj);
-      if (MEGA) {
-        DSPGN_PROBE_T(tend);
-        // ---- object pipeline.  Per object and iteration:  ray-sample tiles (forward only) -> [last one] per-ray scan +
-        // band compaction -> band tiles (fwd+bwd) ;  SDF tiles (fwd+bwd) ;  [last SDF / band tile] solve, pose / code
-        // update, tiles of the next iteration.  The CTA that finishes the last tile of a stage runs the serial step
-        // with its 256 epilogue threads while every other SM keeps working on other objects.
-        __threadfence();                             // this tile's partial sums / sdf values are visible device-wide
-        epi_bar_sync();
-        if (tid == 0) {
-          log_event(q.log, ev_desc(EV_TILE_END, mode, o, tr.tile));
-          int act = 0;
-          if (RENDER && mode == MODE_RAYFWD) { if (atomicSub(q.ray_left + o, 1) == 1) act = 1; }
-          else if (atomicSub(q.pending + o, 1) == 1) act = 2;
-          *reinterpret_cast<volatile int*>(&S.last_flag) = act;
-        }
-        epi_bar_sync();
-        int act = *reinterpret_cast<volatile int*>(&S.last_flag);
-        if (RENDER && act == 1) {
-          // every ray sample of the object has its sdf value: the per-ray scan becomes 64-ray work items of its own
-          if (tid == 0) {
-            const int nch = (M.n_rays + kScanChunkRays - 1) / kScanChunkRays;
-            *reinterpret_cast<volatile int*>(q.scan_left + o) = nch;
-            __threadfence();
-            mega_push(q, kKindScan, o, nch);
-          }
-        }
-        DSPGN_PROBE_ADD(PR_TILE_END, tend);
-        if (act == 2) {
-          DSPGN_PROBE_T(tsv);
-          mega_solve_and_advance(S, o, tid);
-          DSPGN_PROBE_ADD(PR_SOLVE, tsv);
-          DSPGN_PROBE_COUNT(PR_SOLVES);
-        }
-      }
+      if (MEGA) mega_tile_end<RENDER, kTcRows>(S, q, M, o, mode, tr.tile, tid);
       // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
     }
     DSPGN_PROBE_ADD(PR_LOOP, tloop);

@@ -21,6 +21,7 @@
 // per-tile partial sums k_solve reads (kAccStride per tile), so everything downstream of launch_term is shared with the
 // other engines.  Shared memory: ring 64 KB | A hi 64 KB | A lo 64 KB | TcwSmemTail (J tile, per-row values, plans).
 #pragma once
+#include <type_traits>
 #include "dspgn_tc.cuh"
 
 namespace dspgn {
@@ -38,6 +39,7 @@ struct TcwDecDev {
   TcPlan plan;
 };
 
+template <int SCHED>
 struct TcwSmemTail {
   float Jp[kTcwRows * kJpStride];         // [row][72+4]: J row of each point; cols 0..66 double as latent_in skip gradient
   float bias[kTcwHid];                    // bias of the current forward step, zero padded
@@ -49,7 +51,7 @@ struct TcwSmemTail {
   float ypart[2 * kTcwRows];              // last layer: each warpgroup's half of the per-row dot product
   float zs[kMaxCode + 16];                // latent code of the tile's object (zero padded)
   float ost[16];                          // T_oc[12], dmin, dmax, dstep, dfar of the tile's object
-  int prefix[kMaxObjScan + 1];
+  int prefix[SCHED == 0 ? kMaxObjScan + 1 : 1];   // tile prefix of the per-iteration schedule (unused by SCHED 1)
   int warp_tmp[32];
   // the tile being run: object, first row, rows, class.  The step loop and the tail read them from here after each
   // barrier: held in registers through the epilogues, such tile-wide scalars spill to local memory.
@@ -57,9 +59,30 @@ struct TcwSmemTail {
   uint64_t w_full[kTcwRing], w_empty[kTcwRing];
   TcPlan plans[DSPGN_MAX_CLASSES];
 };
-constexpr size_t kTcwSmemBytes = 1024 + (size_t)kTcwRing * kTcwStageBytes + 2 * (size_t)kTcwAImgBytes + sizeof(TcwSmemTail);
+// The persistent kernel's tail (k_wide_persistent): the same fields, then the tile's kind and index in its term, the
+// CTA-local FIFO, the copies of the kernel arguments for the out-of-line solve step and the publication fields (as in
+// TcSmemTail).  Its solve workspace is the A hi image and the range words of a ray-sample tile's object are staged in the
+// A lo image: both images are dead between tiles (the last GEMM step of a tile retired every MMA that read them).
+struct TcwMegaTail : TcwSmemTail<1> {
+  int t_mode, t_j;
+  int fifo[4]; int fifo_pub; int epi_seq; int last_flag;
+  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
+  int push_base, push_nF, push_nS, push_o;
+  __device__ SolveSmem& solve_smem() {
+    return *reinterpret_cast<SolveSmem*>(reinterpret_cast<unsigned char*>(this) - 2 * (size_t)kTcwAImgBytes);
+  }
+};
+template <int SCHED> using TcwTail = std::conditional_t<SCHED == 0, TcwSmemTail<0>, TcwMegaTail>;
+template <int SCHED>
+constexpr size_t kTcwSmemBytesOf = 1024 + (size_t)kTcwRing * kTcwStageBytes + 2 * (size_t)kTcwAImgBytes + sizeof(TcwTail<SCHED>);
+constexpr size_t kTcwSmemBytes = kTcwSmemBytesOf<0>, kTcwMegaSmemBytes = kTcwSmemBytesOf<1>;
 static_assert(kTcwSmemBytes <= 227 * 1024, "k_wide_wgmma: shared memory exceeds the 227 KB per block of sm_90");
-static_assert(offsetof(TcwSmemTail, bias) % 8 == 0, "epi_fwd_hidden reads bias column pairs as float2");
+static_assert(kTcwMegaSmemBytes <= 227 * 1024, "k_wide_persistent: shared memory exceeds the 227 KB per block of sm_90");
+static_assert(offsetof(TcwSmemTail<0>, bias) % 8 == 0 && offsetof(TcwSmemTail<1>, bias) % 8 == 0,
+              "epi_fwd_hidden reads bias column pairs as float2");
+static_assert(sizeof(SolveSmem) <= kTcwAImgBytes, "k_wide_persistent: the solve workspace overlays the A hi image");
+static_assert(4 * (kScanMaxRays + 1) <= kTcwAImgBytes && 4 * (kScanMaxRays / kSegRays + 1) <= kTcwAImgBytes,
+              "k_wide_persistent: a ray-sample / band tile stages its object's range words in the A lo image");
 
 // accumulator-shaped values of warpgroup grp (columns [256 grp, 256 grp + 256)) -> hi / lo A images of the next step
 __device__ __forceinline__ void tcw_store_operand(const float (&v)[128], unsigned char* ahi, unsigned char* alo, int rl, int q,
@@ -119,16 +142,23 @@ __device__ __forceinline__ void tcw_gemm(float (&acc)[128], uint32_t ahi, uint32
   ring_at<kTcwRing>(stage, phase, (uint32_t)(kTcStages * nch), stage, phase);
 }
 
-__global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermArgs a, const TcwDecDev* __restrict__ wd,
-                                                               uint4* __restrict__ masks_g) {
+// The wide tile loop of both schedules.  SCHED 0 (k_wide_wgmma): one launch per term and iteration, static round-robin
+// over the launch's tiles (a.mode is the tile kind).  SCHED 1 (k_wide_persistent): every GN iteration of every object
+// in one launch, the work items of the device queue (ray-sample, scan, band and SDF items at kTcwRows rows per tile)
+// through the CTA-local FIFO, the solve step and the next iteration's items in the CTA that finishes an object's
+// iteration -- the scheduling of k_gn_persistent_render (dspgn_tc.cuh: mega_*), with this tile.
+template <int SCHED>
+__device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, const TcwDecDev* __restrict__ wd,
+                                         uint4* __restrict__ masks_g, const MegaArgs& q, const SolveArgs& sv) {
+  constexpr bool MEGA = SCHED == 1;
   extern __shared__ unsigned char tcw_smem_raw[];
   unsigned char* ring = tcw_smem_raw + ((1024u - (smem_u32(tcw_smem_raw) & 1023u)) & 1023u);
   unsigned char* const ahi = ring + (size_t)kTcwRing * kTcwStageBytes;
   unsigned char* const alo = ahi + kTcwAImgBytes;
-  TcwSmemTail& S = *reinterpret_cast<TcwSmemTail*>(alo + kTcwAImgBytes);
+  TcwTail<SCHED>& S = *reinterpret_cast<TcwTail<SCHED>*>(alo + kTcwAImgBytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  const int total_tiles = build_tile_prefix(b, a, kTcwRows, S.prefix, S.warp_tmp);
+  const int total_tiles = MEGA ? 0 : build_tile_prefix(b, a, kTcwRows, S.prefix, S.warp_tmp);
   {
     const int nwords = b.n_classes * (int)(sizeof(TcPlan) / 4);
     for (int i = tid; i < nwords; i += kTcThreads) {
@@ -138,23 +168,42 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
   }
   if (tid == 0) {
     for (int i = 0; i < kTcwRing; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
+    if constexpr (MEGA) {
+      S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
+      S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv;
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (warp >= 8) {
-    // ===================== weight producer (warp 8 lane 0) ======================================
+    // ===================== weight producer (warp 8 lane 0; SCHED 1: also the CTA's scheduler) =================
     setmaxnreg_dec<kTcProducerRegs>();
     if (warp == 8 && lane == 0) {
       uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int cls = b.meta[find_object(S.prefix, b.n_obj, tile)].class_id;
-        const TcPlan& plan = S.plans[cls];
-        const bool fwd_only = a.mode == MODE_RAYFWD || a.mode == MODE_PTSFWD || a.mode == MODE_GRIDFWD;
-        const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
-        for (int s = 0; s < ns; ++s)
-          produce_step<kTcwRing, kTcwStageBytes>(wd[cls].blob + plan.step[s].w_off, plan.step[s].k_steps / 4,
-                                                 64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full, S.w_empty, stage, phase);
+      if constexpr (MEGA) {
+        for (int seq = 0;; ++seq) {
+          mega_fifo_fill(q, b.n_obj, S, seq);
+          TileRef tr;
+          if (!mega_tile_at<kTcwRows, false>(a, S, seq, tr)) break;
+          if (tr.mode == kKindScan) continue;                    // no GEMM steps
+          const int cls = b.meta[tr.o].class_id;
+          const TcPlan& plan = S.plans[cls];
+          const int ns = tr.mode == MODE_RAYFWD ? plan.n_fwd : plan.n_steps;
+          for (int s = 0; s < ns; ++s)
+            produce_step<kTcwRing, kTcwStageBytes>(wd[cls].blob + plan.step[s].w_off, plan.step[s].k_steps / 4,
+                                                   64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full, S.w_empty, stage, phase);
+        }
+      } else {
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+          const int cls = b.meta[find_object(S.prefix, b.n_obj, tile)].class_id;
+          const TcPlan& plan = S.plans[cls];
+          const bool fwd_only = a.mode == MODE_RAYFWD || a.mode == MODE_PTSFWD || a.mode == MODE_GRIDFWD;
+          const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
+          for (int s = 0; s < ns; ++s)
+            produce_step<kTcwRing, kTcwStageBytes>(wd[cls].blob + plan.step[s].w_off, plan.step[s].k_steps / 4,
+                                                   64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full, S.w_empty, stage, phase);
+        }
       }
     }
     return;
@@ -170,19 +219,40 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
   const uint32_t ahi_s = smem_u32(ahi), alo_s = smem_u32(alo);
   const uint32_t ring_g = smem_u32(ring) + (uint32_t)grp * (kTcwStageBytes / 2);
   const uint32_t bars = smem_u32(S.w_full);
-  const int mode = a.mode;
-  const bool grid_mode = mode == MODE_GRIDFWD;
-  const bool fwd_only = mode == MODE_RAYFWD || mode == MODE_PTSFWD || grid_mode;
-  const bool pts_mode = mode == MODE_SDF || mode == MODE_PTSFWD || grid_mode;
+  // SCHED 0: the launch's term; SCHED 1: the tile's kind, read from S.t_mode where it is needed
+  const int mode0 = a.mode;
+  const bool grid_mode = !MEGA && mode0 == MODE_GRIDFWD;
+  const bool fwd_only0 = mode0 == MODE_RAYFWD || mode0 == MODE_PTSFWD || grid_mode;
+  const bool pts_mode0 = mode0 == MODE_SDF || mode0 == MODE_PTSFWD || grid_mode;
+  auto tile_mode = [&] { if constexpr (MEGA) return *reinterpret_cast<volatile int*>(&S.t_mode); else return mode0; };
   uint32_t stage = 0, phase = 0;
   float acc[128];
   // The tile index, the tile count (S.prefix[n_obj]) and this thread's tile row are read from shared memory / %tid
   // where they are needed, so that nothing tile-wide stays in registers through the epilogues.
-  for (int tile = blockIdx.x; tile < S.prefix[b.n_obj];) {
+  for (int tile = MEGA ? 0 : blockIdx.x; MEGA || tile < S.prefix[b.n_obj];) {
     // ---- prologue: the object's pose, code and this row's point --------------------------------------------------
     {
-      const int o = find_object(S.prefix, b.n_obj, tile);
-      const int row0 = (tile - S.prefix[o]) * kTcwRows;
+      int o, row0, mode = mode0;
+      if constexpr (MEGA) {
+        // `tile` counts this CTA's work items (the FIFO sequence number)
+        TileRef tr;
+        if (!mega_tile_at<kTcwRows, false>(a, S, tile, tr)) break;
+        if (tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = tile + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
+        if (tr.mode == kKindScan) {
+          mega_scan_item<kTcwRows>(S, b, q, sv, tr, tid);
+          ++tile;
+          continue;
+        }
+        o = tr.o; row0 = tr.row0; mode = tr.mode;
+        if (tid == 0) { S.t_mode = tr.mode; S.t_j = tr.tile; }
+        // `tile` becomes the tile's partial-sum slot (S.t_tile); the sequence number stays in S.epi_seq - 1, which thread
+        // 0 wrote above, before the prologue's barriers, and rewrites only after every thread passed mega_tile_end's
+        tile = tr.slot;
+      } else {
+        o = find_object(S.prefix, b.n_obj, tile);
+        row0 = (tile - S.prefix[o]) * kTcwRows;
+      }
+      const bool pts_mode = MEGA ? mode == MODE_SDF : pts_mode0;
       const ObjMeta& M = b.meta[o];
       const ObjState& ost = b.state[o];
       const int L = b.decs[M.class_id].L;
@@ -190,8 +260,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
       else if (tid < 16) S.ost[tid] = ldv(&ost.dmin + (tid - 12));
       if (tid >= 32 && tid < 32 + kMaxCode + 16) S.zs[tid - 32] = (tid - 32 < L) ? ldv(&ost.z[tid - 32]) : 0.f;
       const uint8_t* mask_in; uint8_t* mask_out;
-      cut_masks(a, ost.mode, a.iter, mask_in, mask_out);
-      const int nrows = min(kTcwRows, term_rows(b, a, o) - row0);
+      cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
+      const int nrows = min(kTcwRows, (MEGA ? (pts_mode ? M.n_pts : mega_rows(b, q, M, o, mode)) : term_rows(b, a, o)) - row0);
+      // SCHED 1: the object's range words for the row -> sample map of a ray-sample or band tile, in the dead A lo image
+      const int* segp = reinterpret_cast<const int*>(alo);
+      int nseg = 0;
+      if constexpr (MEGA) {
+        const bool compact = mode == MODE_RAYFWD && q.vpre != nullptr;
+        if (mode == MODE_BAND) nseg = (M.n_rays + kSegRays - 1) / kSegRays;
+        const int nw = compact ? M.n_rays + 1 : (mode == MODE_BAND ? nseg + 1 : 0);
+        const int* gp = compact ? q.vpre + vpre_base(M, o) : q.seg_prefix + seg_base(M, o);
+        for (int i = tid; i < nw; i += kTcEpiThreads) reinterpret_cast<int*>(alo)[i] = __ldcg(gp + i);
+      }
       epi_bar_sync();      // the previous tile's per-row stages are done with xr / scr and the tile descriptor
       const int r = tile_row();
       if (tid == 0) { S.t_tile = tile; S.t_o = o; S.t_row0 = row0; S.t_nrows = nrows; S.t_cls = M.class_id; }
@@ -204,11 +284,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
           else xform_point(S.ost, pq[0], pq[1], pq[2], x0, x1, x2);
           sc = (grid_mode || mask_in == nullptr || ldv(mask_in + M.pts_off + rr_)) ? 1.f : 0.f;
         } else if (mode == MODE_BAND) {
-          const size_t sidx = (size_t)M.smp_off + rr_;
+          size_t sidx = (size_t)M.smp_off + rr_;
+          if (MEGA) {
+            // band rows live compacted per ray segment: the largest segment whose prefix is <= the row
+            int lo = 0, hi = nseg;
+            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (segp[mid] <= rr_) lo = mid; else hi = mid; }
+            sidx = (size_t)M.smp_off + (size_t)lo * kSegRays * b.D + (size_t)(rr_ - segp[lo]);
+          }
           x0 = __ldcg(b.band_x + 3 * sidx); x1 = __ldcg(b.band_x + 3 * sidx + 1); x2 = __ldcg(b.band_x + 3 * sidx + 2);
           sc = __ldcg(b.band_s + sidx); res_in = __ldcg(b.band_r + sidx);
         } else {
-          const int ray = rr_ / b.D, j = rr_ - ray * b.D;
+          int ray = rr_ / b.D, j = rr_ - ray * b.D;
+          if (MEGA && q.vpre != nullptr) {
+            int lo = 0, hi = M.n_rays;                 // largest ray whose hull starts at or before this row
+            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((segp[mid] >> 7) <= rr_) lo = mid; else hi = mid; }
+            ray = lo; j = (segp[lo] & 127) + (rr_ - (segp[lo] >> 7));
+          }
           const float* rq = b.rays + 3 * (size_t)(M.ray_off + ray);
           const float d = lin_depth(S.ost[12], S.ost[13], S.ost[14], j, b.D);
           xform_point(S.ost, __fmul_rn(rq[0], d), __fmul_rn(rq[1], d), __fmul_rn(rq[2], d), x0, x1, x2);
@@ -242,6 +333,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
     for (int s = 0;; ++s) {
       const int cls = S.t_cls;
       const TcPlan& plan = S.plans[cls];
+      const bool fwd_only = MEGA ? tile_mode() == MODE_RAYFWD : fwd_only0;
       const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
       if (s >= ns) break;
       const DecoderDev& dec = b.decs[cls];
@@ -249,6 +341,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
       const bool more = s + 1 < ns;
       const int k_next = more ? plan.step[s + 1].k_steps * 16 : 0;
       const int nm = st.n_real;
+      if constexpr (MEGA) { if (tid == 0 && s == 0) log_event(q.log, ev_desc(EV_FIRST_MMA, tile_mode(), S.t_o, S.t_j)); }
       // a forward step's bias, read by its epilogue after the barrier below (the previous epilogue's reads ended
       // before the barrier that published this step's operand)
       if (st.kind == TK_FWD_HIDDEN || st.kind == TK_FWD_PENULT) {
@@ -289,12 +382,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
           const float sc = S.scr[r];
           const int o = S.t_o, row0 = S.t_row0, nrows = S.t_nrows;
           const ObjMeta& M = b.meta[o];
+          const int mode = tile_mode();
           if (tid < kTcwRows && r < nrows) {
             const size_t base = (mode == MODE_RAYFWD) ? (size_t)M.smp_off
                                 : (grid_mode ? (size_t)a.grid_slot[o] * a.grid_rows : (size_t)M.pts_off);
             b.sdf[base + row0 + r] = (sc != 0.f) ? S.yrow[r] : INFINITY;
           }
-          if (mode == MODE_RAYFWD) {
+          if (!MEGA && mode == MODE_RAYFWD) {          // (persistent kernel: counted by the scan items, scan_chunk)
             const unsigned bal = __ballot_sync(0xffffffffu, tid < kTcwRows && r < nrows && sc != 0.f);
             if (lane == 0 && bal) atomicAdd(b.V_count + o, __popc(bal));
           }
@@ -331,16 +425,28 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
         epi_bar_sync();
       }
     }
-    if (fwd_only) { tile = S.t_tile + gridDim.x; continue; }
+    if constexpr (MEGA) {
+      if (tile_mode() == MODE_RAYFWD) {
+        // the next sequence number is read before mega_tile_end's barriers: once past them, thread 0 may already have
+        // taken the next item and rewritten S.epi_seq
+        const int next = *reinterpret_cast<volatile int*>(&S.epi_seq);
+        mega_tile_end<true, kTcwRows>(S, q, b.meta[S.t_o], S.t_o, MODE_RAYFWD, S.t_j, tid);
+        tile = next;
+        continue;
+      }
+    } else {
+      if (fwd_only0) { tile = S.t_tile + gridDim.x; continue; }
+    }
     // ---- pose columns, residual (thread = row; needs every d/d(input) column of the row) -----------------------------
     epi_bar_sync();
     const int o = S.t_o, row0 = S.t_row0, nrows = S.t_nrows, r = tile_row();
     const ObjState& ost = b.state[o];
+    const int mode = tile_mode();
     if (tid < kTcwRows) {
       const int L = b.decs[S.t_cls].L;
       const uint8_t* mask_in; uint8_t* mask_out;
-      cut_masks(a, ost.mode, a.iter, mask_in, mask_out);
-      const float huber_b = term_huber(a, mode, ost.mode, a.huber_b);
+      cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
+      const float huber_b = term_huber(a, mode, ost.mode, (MEGA && mode == MODE_BAND) ? a.huber_b1 : a.huber_b);
       const float x0 = S.xr[r], x1 = S.xr[kTcRows + r], x2 = S.xr[2 * kTcRows + r], sc = S.scr[r];
       float* jr = S.Jp + r * kJpStride;
       for (int i = L; i < kMaxCode; ++i) jr[i] = 0.f;
@@ -369,7 +475,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
       }
     }
     // ---- J^T J, J^T (rho r), loss over the 64 rows of the tile (optimizer.py:161-167) ---------------------------------
-    float* accp = a.part + (size_t)S.t_tile * kAccStride;
+    float* accp = ((MEGA && mode == MODE_BAND) ? a.part_r : a.part) + (size_t)S.t_tile * kAccStride;
     if (tid < 171) {
       int bi = 0, rem = tid;
       while (rem >= 18 - bi) { rem -= 18 - bi; ++bi; }
@@ -415,9 +521,26 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermAr
       }
       if (k == 0) { accp[kAccLoss] = sacc; accp[kAccLoss + 1] = n; }
     }
-    // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
-    tile = S.t_tile + gridDim.x;
+    if constexpr (MEGA) {
+      const int next = *reinterpret_cast<volatile int*>(&S.epi_seq);     // before the barriers, as above
+      mega_tile_end<true, kTcwRows>(S, q, b.meta[o], o, mode, S.t_j, tid);
+      tile = next;
+    } else {
+      // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
+      tile = S.t_tile + gridDim.x;
+    }
   }
+}
+
+__global__ void __launch_bounds__(kTcThreads, 1) k_wide_wgmma(BatchDev b, TermArgs a, const TcwDecDev* __restrict__ wd,
+                                                               uint4* __restrict__ masks_g) {
+  tcw_body<0>(b, a, wd, masks_g, MegaArgs{}, SolveArgs{});
+}
+// Persistent object-pipelined variant: all GN iterations of all objects in ONE launch, every item kind (SDF-only and
+// pose-only runs simply queue no ray-sample items).  masks: the ReLU mask scratch, as for k_wide_wgmma.
+__global__ void __launch_bounds__(kTcThreads, 1) k_wide_persistent(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv,
+                                                                       const TcwDecDev* __restrict__ wd, uint4* __restrict__ masks) {
+  tcw_body<1>(b, a, wd, masks, q, sv);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -505,6 +628,10 @@ inline int tcw_pack_decoder(const DecoderDev& dv, int H, TcDecoderHost& h, TcPla
 inline int tcw_setup_kernel(std::string& err) {
   if (cudaFuncSetAttribute(k_wide_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcwSmemBytes) != cudaSuccess) {
     err = std::string("cudaFuncSetAttribute(k_wide_wgmma): ") + cudaGetErrorString(cudaGetLastError());
+    return DSPGN_E_CUDA;
+  }
+  if (cudaFuncSetAttribute(k_wide_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcwMegaSmemBytes) != cudaSuccess) {
+    err = std::string("cudaFuncSetAttribute(k_wide_persistent): ") + cudaGetErrorString(cudaGetLastError());
     return DSPGN_E_CUDA;
   }
   return 0;

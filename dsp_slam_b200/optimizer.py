@@ -572,6 +572,7 @@ class Optimizer(object):
         c.engine = {None: _lib.ENGINE_AUTO, "auto": _lib.ENGINE_AUTO, "simt": _lib.ENGINE_SIMT,
                     "tc": _lib.ENGINE_TC, "tc_wide": _lib.ENGINE_TC_WIDE}[engine]
         # kernel schedule (bit-identical results): None/"auto", "launches" (one launch per term per iteration), "persistent"
+        # (one launch per run; engines "tc" and "tc_wide", the others run "launches")
         c.schedule = {None: _lib.SCHED_AUTO, "auto": _lib.SCHED_AUTO, "launches": _lib.SCHED_LAUNCHES,
                       "persistent": _lib.SCHED_PERSISTENT}[schedule]
         self.solver = BatchSolver(self._dev_decoders, c, device)

@@ -75,7 +75,7 @@ extern "C" {
 #define DSPGN_ENGINE_SIMT 1    /* fp32 FFMA kernels: on-device ground truth */
 #define DSPGN_ENGINE_TC 2      /* wgmma tensor-core kernels, 3-pass split-fp16 (fp32-class accuracy) */
 /* wgmma tensor-core kernel for plain decoders up to 512 wide (DeepSDF's 8 x 512 network; narrower classes too),
- * per-iteration schedule, tensor-core tolerances.  Opt-in only: AUTO never picks it.  Decoders with LayerNorm,
+ * both schedules (the persistent one: k_wide_persistent), tensor-core tolerances.  Opt-in only: AUTO never picks it.  Decoders with LayerNorm,
  * xyz_in_all, use_tanh or more than one latent_in layer are refused with DSPGN_E_ARG. */
 #define DSPGN_ENGINE_TC_WIDE 3
 

@@ -11,7 +11,12 @@ The legs alternate in one process; each is timed with the host clock around the 
 sync).  Prints one JSON line: per leg and decoder the median / min / p90 in ms, the ratio of the decoder's
 multiply-adds per row (forward) to the 8 x 256 decoder's, the card's name and power limit.
 
-  python tools/wide_bench.py [--steps K] [--warmup W] [--mesh-dim 32]
+--schedules instead times the 8 x 512 decoder on engine="tc_wide" under schedule="launches" (k_wide_wgmma per term and
+iteration) against schedule="persistent" (k_wide_persistent, one launch per call), alternated step by step, on (a),
+(b) and (c) a cfg2-sized batch: 32 objects x 2048 points, SDF term only, 10 iterations (Optimizer.reconstruct_batch);
+the card's SM clock is read in the same call.
+
+  python tools/wide_bench.py [--steps K] [--warmup W] [--mesh-dim 32] [--schedules]
 """
 import argparse
 import json
@@ -42,6 +47,7 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--mesh-dim", type=int, default=32)
+    ap.add_argument("--schedules", action="store_true", help="8 x 512 tc_wide: launches against persistent")
     args = ap.parse_args()
     import torch
     import __graft_entry__ as g
@@ -66,7 +72,17 @@ def main():
     import wide_fixtures
     tmp = tempfile.TemporaryDirectory()
     path = {"cars": os.path.join(GOLDEN, "decoder_cars.npz"), "wide": wide_fixtures.write("wide", tmp.name)}
-    for label, dec, engine in DECODERS:
+    if args.schedules:
+        batch = [dict(t_cam_obj=o["t_cam_obj_init"], pts=o["pts"]) for o in synth.make_batch(32, 2048, 0, 0)]
+        cfg_sdf = json.load(open(os.path.join(ROOT, "dsp_slam_b200", "configs", "config_kitti.json")))
+        for sch in ("launches", "persistent"):
+            opt = Optimizer(path["wide"], cfg, engine="tc_wide", schedule=sch)
+            legs[f"a_localmapping_{sch}"] = lambda opt=opt: opt.reconstruct_object(
+                one["t_cam_obj_init"], one["pts"], one["rays"], one["depth"])
+            legs[f"b_keyframe_meshed_{sch}"] = lambda s=opt.solver: s.keyframe(objs, modes, gates, voxels_dim=args.mesh_dim)
+            opt_sdf = Optimizer(path["wide"], cfg_sdf, engine="tc_wide", schedule=sch, sdf_only=True)
+            legs[f"c_cfg2_sdf_{sch}"] = lambda opt=opt_sdf: opt.reconstruct_batch(batch)
+    for label, dec, engine in ([] if args.schedules else DECODERS):
         opt = Optimizer(path[dec], cfg, engine=engine)
         legs[f"a_localmapping_{label}"] = lambda opt=opt: opt.reconstruct_object(
             one["t_cam_obj_init"], one["pts"], one["rays"], one["depth"])
@@ -81,11 +97,17 @@ def main():
             f()
             times[k].append((time.perf_counter() - t0) * 1e3)
     base = macs_per_row(path["cars"])
-    out = {"metric": "wide_decoder_ms", "steps": args.steps, "mesh_dim": args.mesh_dim,
-           "decoder_macs_ratio": {label: macs_per_row(path[dec]) / base for label, dec, _ in DECODERS},
+    out = {"metric": "wide_schedule_ms" if args.schedules else "wide_decoder_ms", "steps": args.steps, "mesh_dim": args.mesh_dim,
            "legs": {k: {"median": float(np.median(v)), "min": float(np.min(v)), "p90": float(np.percentile(v, 90))}
                     for k, v in times.items()},
            "gpu": gpu_card()}
+    if args.schedules:
+        import subprocess
+        q = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True)
+        out["gpu"]["sm_clock"] = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else None
+    else:
+        out["decoder_macs_ratio"] = {label: macs_per_row(path[dec]) / base for label, dec, _ in DECODERS}
     print(json.dumps(out))
 
 
