@@ -19,6 +19,7 @@
 #include "dspgn_solve.cuh"
 #include "dspgn_tc.cuh"
 #include "dspgn_tc_wide.cuh"
+#include "dspgn_simt_persistent.cuh"
 #include "dspgn_mesh.cuh"
 #include "dspgn_frame.cuh"
 #include "dspgn_mono.cuh"
@@ -531,6 +532,7 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
     CU(cudaFuncSetAttribute(k_decoder_simt<kHid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHid>)));
   else
     CU(cudaFuncSetAttribute(k_decoder_simt<kHidWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHidWide>)));
+  if (int rc = simt_setup_kernels(s->simt_hid, g_err)) { dspgn_solver_destroy(s); return rc; }
   for (auto* d : s->classes)
     if (d->has_ln) {      // LayerNorm decoders: per-CTA scratch for the normalised activations (forward -> backward),
                           // one half for the ray-sample pass, which may run beside the SDF-row pass (launch_terms)
@@ -1065,8 +1067,8 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
   s->evs_used = 0;
   CU(cudaEventRecord(s->ev_run0, s->stream));
   const bool render = p.render;
-  const bool wide = s->engine == DSPGN_ENGINE_TC_WIDE;
-  const bool mega = s->mega_enabled && (s->engine == DSPGN_ENGINE_TC || wide) && s->total_tiles > 0 &&
+  const bool wide = s->engine == DSPGN_ENGINE_TC_WIDE, simt = s->engine == DSPGN_ENGINE_SIMT;
+  const bool mega = s->mega_enabled && s->total_tiles > 0 &&
                     s->max_tiles <= kItemTileMask && s->n_obj <= kItemObjMask + 1 && p.q_cap < (1LL << 27);
   if (mega) {
     // ---- persistent object-pipelined kernel: every GN iteration of every object in ONE launch --------------
@@ -1085,7 +1087,9 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     v.base_s = s->d_tbase_static; v.base_r = s->d_tbase_r_static; v.iter_index = 0;
     const int grid = grid_sms(s);
     if (s->timing) cudaEventRecord(next_event(s), s->stream);
-    if (wide) k_wide_persistent<<<grid, kTcThreads, kTcwMegaSmemBytes, s->stream>>>(b, a, q, v, s->d_tcw.as<TcwDecDev>(), s->d_masks.as<uint4>());
+    if (simt && s->simt_hid == kHid) k_simt_persistent<kHid><<<grid, kThreads, sizeof(SimtMegaSmem<kHid>), s->stream>>>(b, a, q, v);
+    else if (simt) k_simt_persistent<kHidWide><<<grid, kThreads, sizeof(SimtMegaSmem<kHidWide>), s->stream>>>(b, a, q, v);
+    else if (wide) k_wide_persistent<<<grid, kTcThreads, kTcwMegaSmemBytes, s->stream>>>(b, a, q, v, s->d_tcw.as<TcwDecDev>(), s->d_masks.as<uint4>());
     else if (render) k_gn_persistent_render<<<grid, kTcThreads, kTcSmemBytes<2>, s->stream>>>(b, a, q, v);
     else k_gn_persistent<<<grid, kTcThreads, kTcSmemBytes<1>, s->stream>>>(b, a, q, v, s->d_masks.as<uint4>());
     if (s->timing) cudaEventRecord(next_event(s), s->stream);

@@ -335,67 +335,95 @@ __device__ inline void simt_ln_backward(float* act, float* red, const float* rst
   __syncthreads();
 }
 
-// H: the widest layer of any class of the solver (kHid or kHidWide); every class runs at that instantiation
-template <int H>
-__global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermArgs a) {
+// What the persistent kernel (dspgn_simt_persistent.cuh) hands a tile beyond its object, first row, partial-sum slot and
+// kind: the values other CTAs write during the run, read cache-bypassing by the kernel and staged in shared memory.
+struct SimtMegaTile {
+  int term_rows;             // rows of the tile's term: SDF points, ray samples (valid-sample hulls) or band rows
+  int iter;                  // the object's current iteration (inlier cut)
+  const float* ost;          // T_oc[12], dmin, dmax, dstep of the object
+  const float* zs;           // its latent code
+  const int* segp;           // range words of a ray-sample tile (vpre) or a band tile (segment prefix)
+  int nseg;                  // band tile: ray segments of the object
+  int seg_samples;           // band tile: ray samples per segment (kSegRays x D)
+  bool compact;              // ray-sample tile rows enumerate the valid-sample hulls (vpre words in segp)
+};
+
+// One tile of the SIMT engine: transform, forward, backward to the input, Jacobian rows and the tile's partial sums into
+// slot `tile` of its term.  Both schedules run it: MEGA = false is k_decoder_simt (one launch per term and iteration,
+// the term is a.mode), MEGA = true is k_simt_persistent (every item kind of the device queue, the kind is `mode_mega`;
+// `mt` carries the object's state as the run last wrote it).  A row's values do not depend on which other rows share
+// its tile.
+template <int H, bool MEGA>
+__device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, const TermArgs& a, const int o, const int row0,
+                                          const int tile, const int mode_mega, const SimtMegaTile& mt) {
   constexpr int kTP = simt_rows(H);
   constexpr int kNPart = kThreads / kTP;      // last layer: partial dot products per row
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  SimtSmem<H>& S = *reinterpret_cast<SimtSmem<H>*>(smem_raw);
   const int tid = threadIdx.x, jg = tid >> ilog2(kTP / 8), pg = tid & (kTP / 8 - 1);
-  const int total_tiles = build_tile_prefix(b, a, kTP, S.prefix, S.warp_tmp);
-
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int o = find_object(S.prefix, b.n_obj, tile);
-    const int row0 = (tile - S.prefix[o]) * kTP;
+  // the tile's kind: the launch's term (read from the argument where it is used, as before the split), or the item's
+  auto tmode = [&] { if constexpr (MEGA) return mode_mega; else return a.mode; };
+  {
     const ObjMeta M = b.meta[o];
     const ObjState& st = b.state[o];
     const DecoderDev& dec = b.decs[M.class_id];
     const int L = dec.L, in0 = dec.in0, nl = dec.n_lin;
-    const int nrows = min(kTP, term_rows(b, a, o) - row0);
+    const int nrows = min(kTP, (MEGA ? mt.term_rows : term_rows(b, a, o)) - row0);
     const int omode = st.mode;
     const uint8_t* mask_in; uint8_t* mask_out;
-    cut_masks(a, omode, a.iter, mask_in, mask_out);
+    cut_masks(a, omode, MEGA ? mt.iter : a.iter, mask_in, mask_out);
 
     // ---- phase 0: points in the object frame, decoder input rows -----------------------------
     if (tid < kTP) {
       const int p = tid, r = row0 + p;
       float x = 0.f, y = 0.f, z = 0.f, sc = 0.f, res = 0.f;
       if (p < nrows) {
-        if (a.mode == MODE_SDF || a.mode == MODE_PTSFWD) {
+        if (tmode() == MODE_SDF || (!MEGA && tmode() == MODE_PTSFWD)) {
           const float* q = b.pts + 3 * (size_t)(M.pts_off + r);
-          xform_point(st.T_oc, q[0], q[1], q[2], x, y, z);
-          sc = (mask_in == nullptr || mask_in[M.pts_off + r]) ? 1.f : 0.f;
-        } else if (a.mode == MODE_GRIDFWD) {
+          xform_point(MEGA ? mt.ost : st.T_oc, q[0], q[1], q[2], x, y, z);
+          sc = (mask_in == nullptr || (MEGA ? __ldcg(mask_in + M.pts_off + r) : mask_in[M.pts_off + r])) ? 1.f : 0.f;
+        } else if (!MEGA && tmode() == MODE_GRIDFWD) {
           const float* q = a.grid + 3 * (size_t)r;
           x = q[0]; y = q[1]; z = q[2]; sc = 1.f;
-        } else if (a.mode == MODE_BAND) {
-          const size_t s = (size_t)M.smp_off + r;
-          x = b.band_x[3 * s]; y = b.band_x[3 * s + 1]; z = b.band_x[3 * s + 2];
-          sc = b.band_s[s]; res = b.band_r[s];
+        } else if (tmode() == MODE_BAND) {
+          if constexpr (MEGA) {
+            // band rows live compacted per ray segment: the largest segment whose prefix is <= the row
+            int lo = 0, hi = mt.nseg;
+            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (mt.segp[mid] <= r) lo = mid; else hi = mid; }
+            const size_t s = (size_t)M.smp_off + (size_t)lo * mt.seg_samples + (size_t)(r - mt.segp[lo]);
+            x = __ldcg(b.band_x + 3 * s); y = __ldcg(b.band_x + 3 * s + 1); z = __ldcg(b.band_x + 3 * s + 2);
+            sc = __ldcg(b.band_s + s); res = __ldcg(b.band_r + s);
+          } else {
+            const size_t s = (size_t)M.smp_off + r;
+            x = b.band_x[3 * s]; y = b.band_x[3 * s + 1]; z = b.band_x[3 * s + 2];
+            sc = b.band_s[s]; res = b.band_r[s];
+          }
         } else {
-          const int ray = r / b.D, j = r - ray * b.D;
+          int ray = r / b.D, j = r - ray * b.D;
+          if (MEGA && mt.compact) {
+            int lo = 0, hi = M.n_rays;                 // largest ray whose hull starts at or before this row
+            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((mt.segp[mid] >> 7) <= r) lo = mid; else hi = mid; }
+            ray = lo; j = (mt.segp[lo] & 127) + (r - (mt.segp[lo] >> 7));
+          }
           const float* q = b.rays + 3 * (size_t)(M.ray_off + ray);
-          const float d = lin_depth(st.dmin, st.dmax, st.dstep, j, b.D);
-          xform_point(st.T_oc, __fmul_rn(q[0], d), __fmul_rn(q[1], d), __fmul_rn(q[2], d), x, y, z);
+          const float d = MEGA ? lin_depth(mt.ost[12], mt.ost[13], mt.ost[14], j, b.D) : lin_depth(st.dmin, st.dmax, st.dstep, j, b.D);
+          xform_point(MEGA ? mt.ost : st.T_oc, __fmul_rn(q[0], d), __fmul_rn(q[1], d), __fmul_rn(q[2], d), x, y, z);
           sc = inside_unit_sphere(x, y, z) ? 1.f : 0.f;                // loss.py:68
         }
       }
       S.xo[p] = x; S.xo[kTP + p] = y; S.xo[2 * kTP + p] = z;
       S.rscale[p] = sc; S.rr[p] = res;
     }
-    for (int idx = tid; idx < L * kTP; idx += kThreads) S.inp[idx] = st.z[idx / kTP];
+    for (int idx = tid; idx < L * kTP; idx += kThreads) S.inp[idx] = MEGA ? mt.zs[idx / kTP] : st.z[idx / kTP];
     for (int idx = tid; idx < (kMaxCode + 4) * kTP; idx += kThreads) S.gin[idx] = 0.f;
     float* const xhat_all = (a.ln_scratch != nullptr) ? a.ln_scratch + (size_t)blockIdx.x * DSPGN_MAX_LINEAR * H * kTP : nullptr;
     __syncthreads();
     if (tid < 3 * kTP) S.inp[L * kTP + tid] = S.xo[tid];
-    if (a.mode == MODE_RAYFWD) {
+    if (tmode() == MODE_RAYFWD) {
       // whole tile outside the unit sphere: nothing to decode
       int any = __syncthreads_or(tid < kTP && S.rscale[tid] != 0.f);
       if (!any) {
         if (tid < nrows) b.sdf[(size_t)M.smp_off + row0 + tid] = INFINITY;
         __syncthreads();
-        continue;
+        return;
       }
     } else {
       __syncthreads();
@@ -506,18 +534,20 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       }
       __syncthreads();
     }
-    if (a.mode == MODE_RAYFWD || a.mode == MODE_PTSFWD || a.mode == MODE_GRIDFWD) {
+    if (tmode() == MODE_RAYFWD || (!MEGA && (tmode() == MODE_PTSFWD || tmode() == MODE_GRIDFWD))) {
       int cnt = 0;
       if (tid < nrows) {
         const bool valid = S.rscale[tid] != 0.f;
-        const size_t base = (a.mode == MODE_RAYFWD) ? (size_t)M.smp_off
-                            : (a.mode == MODE_GRIDFWD ? (size_t)a.grid_slot[o] * a.grid_rows : (size_t)M.pts_off);
+        const size_t base = (tmode() == MODE_RAYFWD) ? (size_t)M.smp_off
+                            : (tmode() == MODE_GRIDFWD ? (size_t)a.grid_slot[o] * a.grid_rows : (size_t)M.pts_off);
         b.sdf[base + row0 + tid] = valid ? S.yv[tid] : INFINITY;
         cnt = valid ? 1 : 0;
       }
-      cnt = __syncthreads_count(cnt);
-      if (tid == 0 && cnt && a.mode == MODE_RAYFWD) atomicAdd(b.V_count + o, cnt);
-      continue;
+      if constexpr (!MEGA) {       // (persistent kernel: V is counted by the scan items, scan_chunk)
+        cnt = __syncthreads_count(cnt);
+        if (tid == 0 && cnt && tmode() == MODE_RAYFWD) atomicAdd(b.V_count + o, cnt);
+      }
+      return;
     }
 
     // ---- phase 2: backward to the input ------------------------------------------------------
@@ -590,16 +620,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       S.act[(kMaxCode + 5) * kTP + p] = x * gy - y * gx;
       S.act[(kMaxCode + 6) * kTP + p] = (omode == DSPGN_MODE_POSE) ? 0.f : (gx * x + gy * y + gz * z);
       S.act[(kMaxCode + 7) * kTP + p] = 0.f;
-      float res = (a.mode == MODE_SDF) ? S.yv[p] : S.rr[p];
+      float res = (tmode() == MODE_SDF) ? S.yv[p] : S.rr[p];
       const float sc = S.rscale[p];
-      if (sc == 0.f && (a.mode == MODE_SDF || p >= nrows)) res = 0.f;
-      if (mask_out != nullptr && a.mode == MODE_SDF && p < nrows)
+      if (sc == 0.f && (tmode() == MODE_SDF || p >= nrows)) res = 0.f;
+      if (mask_out != nullptr && tmode() == MODE_SDF && p < nrows)
         mask_out[M.pts_off + row0 + p] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;   // optimizer.py:76-78
       S.yv[p] = res;                                        // raw residual (debug dump)
-      S.rr[p] = huber_weight(fabsf(res), term_huber(a, a.mode, omode, a.huber_b)) * res;  // loss_utils.py:250-265
+      S.rr[p] = huber_weight(fabsf(res), term_huber(a, tmode(), omode, (MEGA && tmode() == MODE_BAND) ? a.huber_b1 : a.huber_b)) * res;  // loss_utils.py:250-265
     }
     __syncthreads();
-    if (a.dbg_J != nullptr && o == a.dbg_obj && a.mode == MODE_SDF) {
+    if (!MEGA && a.dbg_J != nullptr && o == a.dbg_obj && tmode() == MODE_SDF) {
       const int P = a.dbg_P, npose = (omode == DSPGN_MODE_POSE) ? 6 : 7;
       for (int idx = tid; idx < nrows * P; idx += kThreads) {
         const int p = idx / P, c = idx - p * P;
@@ -609,7 +639,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       if (tid < nrows) a.dbg_res[row0 + tid] = S.yv[tid];
     }
     // ---- phase 4: H += J^T J, b += J^T (rho r), loss += sum (rho r)^2  (optimizer.py:161-167) ----
-    float* accp = a.part + (size_t)tile * kAccStride;
+    float* accp = ((MEGA && tmode() == MODE_BAND) ? a.part_r : a.part) + (size_t)tile * kAccStride;
     if (tid < 171) {
       // upper-triangular 4x4 blocks of the 72x72 matrix: tid -> (bi <= bj)
       int bi = 0, rem = tid;
@@ -652,12 +682,27 @@ __global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermAr
       float s = 0.f, n = 0.f;
       for (int p = 0; p < kTP; ++p) {
         s = fmaf(S.rr[p], S.rr[p], s);
-        n += (a.mode == MODE_SDF) ? S.rscale[p] : (p < nrows ? 1.f : 0.f);
+        n += (tmode() == MODE_SDF) ? S.rscale[p] : (p < nrows ? 1.f : 0.f);
       }
       accp[kAccLoss] = s;
       accp[kAccLoss + 1] = n;
     }
     __syncthreads();
+  }
+}
+
+// H: the widest layer of any class of the solver (kHid or kHidWide); every class runs at that instantiation
+template <int H>
+__global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermArgs a) {
+  constexpr int kTP = simt_rows(H);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SimtSmem<H>& S = *reinterpret_cast<SimtSmem<H>*>(smem_raw);
+  const int total_tiles = build_tile_prefix(b, a, kTP, S.prefix, S.warp_tmp);
+
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int o = find_object(S.prefix, b.n_obj, tile);
+    const int row0 = (tile - S.prefix[o]) * kTP;
+    simt_tile<H, false>(S, b, a, o, row0, tile, 0, SimtMegaTile{});
   }
 }
 

@@ -1,0 +1,96 @@
+// fp32 SIMT engine on the persistent object-pipelined schedule (DESIGN §4.12): every GN iteration of every object in one
+// launch.  The tile is simt_tile (dspgn_simt.cuh), the same code k_decoder_simt runs; the scheduling is that of
+// k_wide_persistent (dspgn_tc.cuh: mega_*) at simt_rows(H) rows per tile.
+//
+// There is no producer warpgroup: thread 0 of the CTA pops the next work item into the CTA-local FIFO between tiles,
+// behind the barriers that end the previous tile, so the CTA holds no queue ticket while it runs a tile.  The scan items
+// and the solve step run on the CTA's 256 threads (named barrier 1, as on the 256 epilogue threads of the tensor-core
+// kernels).
+#pragma once
+#include "dspgn_tc.cuh"
+
+namespace dspgn {
+
+// Shared memory of k_simt_persistent: the SIMT tile, then the object's staged state, the CTA-local FIFO, the copies of
+// the kernel arguments for the out-of-line solve step and the publication fields (as in TcwMegaTail).  The solve
+// workspace and the range words of a ray-sample or band tile both overlay the activation buffer, dead between tiles:
+// a tile first writes it after the barrier that ends its phase 0, the last reader of the range words.
+template <int H>
+struct SimtMegaSmem : SimtSmem<H> {
+  float ost[16];                     // T_oc[12], dmin, dmax, dstep of the tile's object
+  float zs[kMaxCode];                // its latent code
+  int fifo[4]; int fifo_pub; int epi_seq; int last_flag;
+  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
+  int push_base, push_nF, push_nS, push_o;
+  __device__ SolveSmem& solve_smem() { return *reinterpret_cast<SolveSmem*>(this->act); }
+  __device__ int* range_words() { return reinterpret_cast<int*>(this->act); }
+};
+static_assert(sizeof(SimtMegaSmem<kHid>) <= 227 * 1024 && sizeof(SimtMegaSmem<kHidWide>) <= 227 * 1024,
+              "k_simt_persistent: shared memory exceeds the 227 KB per block of sm_90");
+static_assert(sizeof(SolveSmem) <= sizeof(SimtSmem<kHid>::act) && sizeof(SolveSmem) <= sizeof(SimtSmem<kHidWide>::act),
+              "k_simt_persistent: the solve workspace overlays the activation buffer");
+static_assert(4 * (kScanMaxRays + 1) <= sizeof(SimtSmem<kHid>::act) && 4 * (kScanMaxRays + 1) <= sizeof(SimtSmem<kHidWide>::act) &&
+              4 * (kScanMaxRays / kSegRays + 1) <= sizeof(SimtSmem<kHid>::act),
+              "k_simt_persistent: a ray-sample / band tile stages its object's range words in the activation buffer");
+
+// One CTA per SM (grid_sms); the LayerNorm scratch (a.ln_scratch) holds one region per CTA.
+template <int H>
+__global__ void __launch_bounds__(kThreads, 1) k_simt_persistent(BatchDev b, TermArgs a, MegaArgs q, SolveArgs sv) {
+  constexpr int kTP = simt_rows(H);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SimtMegaSmem<H>& S = *reinterpret_cast<SimtMegaSmem<H>*>(smem_raw);
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
+    S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv;
+  }
+  __syncthreads();
+  for (int seq = 0;; ++seq) {
+    // the previous item ended with a barrier of all threads: take the next one (at most one FIFO entry is ever ahead)
+    if (tid == 0) {
+      *reinterpret_cast<volatile int*>(&S.epi_seq) = seq;
+      mega_fifo_fill(q, b.n_obj, S, seq);
+    }
+    TileRef tr;
+    if (!mega_tile_at<kTP, false>(a, S, seq, tr)) break;
+    if (tid == 0) log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile));
+    if (tr.mode == kKindScan) {
+      mega_scan_item<kTP>(S, b, q, sv, tr, tid);
+      continue;
+    }
+    const int o = tr.o, mode = tr.mode;
+    const ObjMeta& M = b.meta[o];
+    const ObjState& st = b.state[o];
+    // the object's pose, depth range and code as the last solve (another CTA) wrote them
+    if (tid < 12) S.ost[tid] = ldv(&st.T_oc[tid]);
+    else if (tid < 15) S.ost[tid] = ldv(&st.dmin + (tid - 12));
+    else if (tid >= 32 && tid < 32 + kMaxCode) S.zs[tid - 32] = ldv(&st.z[tid - 32]);
+    SimtMegaTile mt{};
+    mt.term_rows = (mode == MODE_SDF) ? M.n_pts : mega_rows(b, q, M, o, mode);
+    mt.iter = (a.cut_iter >= 0) ? ldv(q.obj_iter + o) : 0;
+    mt.ost = S.ost; mt.zs = S.zs; mt.segp = S.range_words();
+    mt.compact = mode == MODE_RAYFWD && q.vpre != nullptr;
+    mt.nseg = (mode == MODE_BAND) ? (M.n_rays + kSegRays - 1) / kSegRays : 0;
+    mt.seg_samples = kSegRays * b.D;
+    // the range words of the row -> sample map of a ray-sample or band tile
+    const int nw = mt.compact ? M.n_rays + 1 : (mode == MODE_BAND ? mt.nseg + 1 : 0);
+    const int* gp = mt.compact ? q.vpre + vpre_base(M, o) : q.seg_prefix + seg_base(M, o);
+    for (int i = tid; i < nw; i += kThreads) S.range_words()[i] = __ldcg(gp + i);
+    __syncthreads();
+    simt_tile<H, true>(S, b, a, o, tr.row0, tr.slot, mode, mt);
+    mega_tile_end<true, kTP>(S, q, M, o, mode, tr.tile, tid);
+  }
+}
+
+inline int simt_setup_kernels(int hid, std::string& err) {
+  const cudaError_t e = (hid == kHid)
+      ? cudaFuncSetAttribute(k_simt_persistent<kHid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtMegaSmem<kHid>))
+      : cudaFuncSetAttribute(k_simt_persistent<kHidWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtMegaSmem<kHidWide>));
+  if (e != cudaSuccess) {
+    err = std::string("cudaFuncSetAttribute(k_simt_persistent): ") + cudaGetErrorString(cudaGetLastError());
+    return DSPGN_E_CUDA;
+  }
+  return 0;
+}
+
+}  // namespace dspgn

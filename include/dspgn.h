@@ -68,7 +68,7 @@ extern "C" {
 /* kernel schedules of a run (results are bit-identical; the per-iteration schedule exists for debugging / profiling) */
 #define DSPGN_SCHED_AUTO 0
 #define DSPGN_SCHED_LAUNCHES 1   /* one launch per residual term and solve per GN iteration */
-#define DSPGN_SCHED_PERSISTENT 2 /* one persistent object-pipelined kernel for all iterations (tensor-core engine only) */
+#define DSPGN_SCHED_PERSISTENT 2 /* one persistent object-pipelined kernel for all iterations (every engine) */
 
 /* decoder engines */
 #define DSPGN_ENGINE_AUTO 0
@@ -120,7 +120,7 @@ typedef struct {
   int32_t pose_only_iterations;/* pose_only_optim.num_iterations */
   int32_t sdf_only;            /* 1: skip the render term (BASELINE config 2 "surface-SDF loss") */
   int32_t engine;              /* DSPGN_ENGINE_* */
-  int32_t schedule;            /* DSPGN_SCHED_*: 0 = automatic (persistent kernel on the tensor-core engine) */
+  int32_t schedule;            /* DSPGN_SCHED_*: 0 = automatic (the persistent kernel, on every engine) */
 } DspgnConfig;
 
 /* One detection, host side.  Strides are in elements (floats). */

@@ -13,7 +13,7 @@ Also what a timed 20 us sleep between polls would cost on the same host (one eve
 Every stopped call's records are checked against the unstopped call's: an object that did not stop is bit-identical.
 Prints one JSON line with the card's name, power limit and SM clocks.
 
-  python tools/stop_bench.py [--steps K] [--warmup W] [--legs tc:persistent,simt:launches] [--dim 32]
+  python tools/stop_bench.py [--steps K] [--warmup W] [--legs tc:persistent,simt:launches,simt:persistent] [--dim 32]
                              [--delays-ms 0.5,2,5] [--rejected 2]
 """
 import argparse
@@ -71,7 +71,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--legs", default="tc:persistent,simt:launches")
+    ap.add_argument("--legs", default="tc:persistent,simt:launches,simt:persistent")
     ap.add_argument("--dim", type=int, default=32)
     ap.add_argument("--delays-ms", default="0.5,2,5")
     ap.add_argument("--rejected", type=int, default=2)

@@ -14,9 +14,11 @@ multiply-adds per row (forward) to the 8 x 256 decoder's, the card's name and po
 --schedules instead times the 8 x 512 decoder on engine="tc_wide" under schedule="launches" (k_wide_wgmma per term and
 iteration) against schedule="persistent" (k_wide_persistent, one launch per call), alternated step by step, on (a),
 (b) and (c) a cfg2-sized batch: 32 objects x 2048 points, SDF term only, 10 iterations (Optimizer.reconstruct_batch);
-the card's SM clock is read in the same call.
+the card's SM clock is read in the same call.  --schedules --engine simt times the fp32 SIMT engine the same way
+(k_decoder_simt per term and iteration against k_simt_persistent) on the 8 x 256 decoder (cars), the 8 x 512 one (wide)
+and the LayerNorm / xyz_in_all / use_tanh variant (decoder_variant.npz).
 
-  python tools/wide_bench.py [--steps K] [--warmup W] [--mesh-dim 32] [--schedules]
+  python tools/wide_bench.py [--steps K] [--warmup W] [--mesh-dim 32] [--schedules [--engine tc_wide|simt]]
 """
 import argparse
 import json
@@ -48,6 +50,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--mesh-dim", type=int, default=32)
     ap.add_argument("--schedules", action="store_true", help="8 x 512 tc_wide: launches against persistent")
+    ap.add_argument("--engine", default="tc_wide", choices=["tc_wide", "simt"],
+                    help="--schedules: the engine timed (simt: the cars, wide and variant decoders)")
     args = ap.parse_args()
     import torch
     import __graft_entry__ as g
@@ -71,17 +75,20 @@ def main():
     legs = {}
     import wide_fixtures
     tmp = tempfile.TemporaryDirectory()
-    path = {"cars": os.path.join(GOLDEN, "decoder_cars.npz"), "wide": wide_fixtures.write("wide", tmp.name)}
+    path = {"cars": os.path.join(GOLDEN, "decoder_cars.npz"), "wide": wide_fixtures.write("wide", tmp.name),
+            "variant": os.path.join(GOLDEN, "decoder_variant.npz")}
     if args.schedules:
         batch = [dict(t_cam_obj=o["t_cam_obj_init"], pts=o["pts"]) for o in synth.make_batch(32, 2048, 0, 0)]
         cfg_sdf = json.load(open(os.path.join(ROOT, "dsp_slam_b200", "configs", "config_kitti.json")))
-        for sch in ("launches", "persistent"):
-            opt = Optimizer(path["wide"], cfg, engine="tc_wide", schedule=sch)
-            legs[f"a_localmapping_{sch}"] = lambda opt=opt: opt.reconstruct_object(
-                one["t_cam_obj_init"], one["pts"], one["rays"], one["depth"])
-            legs[f"b_keyframe_meshed_{sch}"] = lambda s=opt.solver: s.keyframe(objs, modes, gates, voxels_dim=args.mesh_dim)
-            opt_sdf = Optimizer(path["wide"], cfg_sdf, engine="tc_wide", schedule=sch, sdf_only=True)
-            legs[f"c_cfg2_sdf_{sch}"] = lambda opt=opt_sdf: opt.reconstruct_batch(batch)
+        for dec in (["wide"] if args.engine == "tc_wide" else ["cars", "wide", "variant"]):
+            for sch in ("launches", "persistent"):
+                tag = sch if args.engine == "tc_wide" else f"{dec}_{sch}"
+                opt = Optimizer(path[dec], cfg, engine=args.engine, schedule=sch)
+                legs[f"a_localmapping_{tag}"] = lambda opt=opt: opt.reconstruct_object(
+                    one["t_cam_obj_init"], one["pts"], one["rays"], one["depth"])
+                legs[f"b_keyframe_meshed_{tag}"] = lambda s=opt.solver: s.keyframe(objs, modes, gates, voxels_dim=args.mesh_dim)
+                opt_sdf = Optimizer(path[dec], cfg_sdf, engine=args.engine, schedule=sch, sdf_only=True)
+                legs[f"c_cfg2_sdf_{tag}"] = lambda opt=opt_sdf: opt.reconstruct_batch(batch)
     for label, dec, engine in ([] if args.schedules else DECODERS):
         opt = Optimizer(path[dec], cfg, engine=engine)
         legs[f"a_localmapping_{label}"] = lambda opt=opt: opt.reconstruct_object(
@@ -97,7 +104,7 @@ def main():
             f()
             times[k].append((time.perf_counter() - t0) * 1e3)
     base = macs_per_row(path["cars"])
-    out = {"metric": "wide_schedule_ms" if args.schedules else "wide_decoder_ms", "steps": args.steps, "mesh_dim": args.mesh_dim,
+    out = {"metric": "wide_schedule_ms" if args.schedules else "wide_decoder_ms", "engine": args.engine if args.schedules else None, "steps": args.steps, "mesh_dim": args.mesh_dim,
            "legs": {k: {"median": float(np.median(v)), "min": float(np.min(v)), "p90": float(np.percentile(v, 90))}
                     for k, v in times.items()},
            "gpu": gpu_card()}
