@@ -202,6 +202,69 @@ __device__ __forceinline__ void cut_masks(const TermArgs& a, int obj_mode, int i
   out = (on && it == a.cut_iter) ? a.pt_active : nullptr;
 }
 
+// ---- per-row stages of every tile body (simt_tile, tc_body, tcw_body) ----------------------------------------------
+// Band row `row` of an object on the persistent schedule: band rows live compacted per ray segment (scan_prefix), so the
+// row is in the largest segment lo whose prefix segp[lo] <= row.  Its sample index, from the object's first sample `base`;
+// seg_samples = ray samples per segment (kSegRays x D).
+__device__ __forceinline__ size_t band_row_sample(const int* segp, int nseg, size_t base, size_t seg_samples, int row) {
+  int lo = 0, hi = nseg;
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (segp[mid] <= row) lo = mid; else hi = mid; }
+  return base + (size_t)lo * seg_samples + (size_t)(row - segp[lo]);
+}
+
+// Ray-sample row `row` of object M: sample j of ray `ray` at depth lin_depth(dmin, dmax, dstep, j), in the object frame
+// through T (T_oc); returns its weight, 1 inside the unit sphere (loss.py:68).  Rows are ray * D + j, or with `compact`
+// they enumerate the valid-sample hulls: hull[ray] = first row << 7 | first sample, and the row belongs to the largest
+// ray whose hull starts at or before it.
+__device__ __forceinline__ float ray_sample_row(const BatchDev& b, const ObjMeta& M, const float* T, float dmin, float dmax,
+                                                float dstep, const int* hull, bool compact, int row, float& x0, float& x1,
+                                                float& x2) {
+  int ray = row / b.D, j = row - ray * b.D;
+  if (compact) {
+    int lo = 0, hi = M.n_rays;
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((hull[mid] >> 7) <= row) lo = mid; else hi = mid; }
+    ray = lo; j = (hull[lo] & 127) + (row - (hull[lo] >> 7));
+  }
+  const float* rq = b.rays + 3 * (size_t)(M.ray_off + ray);
+  const float d = lin_depth(dmin, dmax, dstep, j, b.D);
+  xform_point(T, __fmul_rn(rq[0], d), __fmul_rn(rq[1], d), __fmul_rn(rq[2], d), x0, x1, x2);
+  return inside_unit_sphere(x0, x1, x2) ? 1.f : 0.f;
+}
+
+struct RowTail { float rho_r, n, res; };
+// The end of tile row r's Jacobian row J (column c at J[c * cs]; columns 64..66 hold the input gradient g), thread = row:
+// pose columns  dsdf/dx . [I | -x^ | x] = [g, x cross g, g.x]  at the object-frame point x (loss_utils.py:166-185; no
+// scale column for a pose-only object) and column 71 zeroed; the residual of the row (res: the decoder output of an SDF
+// row, the residual of a band row; 0 for a padded or masked-out row) and the inlier-cut mask of an SDF row at
+// mask_out[mask_base + r] (optimizer.py:76-78).  Returns rho r (loss_utils.py:250-265, threshold huber_b), the row's
+// count in the loss's row count and the raw residual.  (mask_base: the object's first point + the tile's first row;
+// with the row index added here, k_decoder_tc keeps its register allocation.)
+__device__ __forceinline__ RowTail row_tail(float* J, int cs, float x0, float x1, float x2, float g0, float g1, float g2,
+                                            float res, float sc, int r, int nrows, int mode, int omode, float huber_b,
+                                            uint8_t* mask_out, int mask_base) {
+  J[(kMaxCode + 3) * cs] = x1 * g2 - x2 * g1;
+  J[(kMaxCode + 4) * cs] = x2 * g0 - x0 * g2;
+  J[(kMaxCode + 5) * cs] = x0 * g1 - x1 * g0;
+  J[(kMaxCode + 6) * cs] = (omode == DSPGN_MODE_POSE) ? 0.f : (g0 * x0 + g1 * x1 + g2 * x2);
+  J[(kMaxCode + 7) * cs] = 0.f;
+  if (sc == 0.f && (mode == MODE_SDF || r >= nrows)) res = 0.f;
+  if (mask_out != nullptr && mode == MODE_SDF && r < nrows)
+    mask_out[mask_base + r] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;
+  return {huber_weight(fabsf(res), huber_b) * res, (mode == MODE_SDF) ? sc : (r < nrows ? 1.f : 0.f), res};
+}
+
+// Debug hook: rows 0 .. nrows-1 of the tile's Jacobian (row p, column c at J[p * rs + c * cs]) into a.dbg_J at tile row
+// row0, P columns each, pose columns first
+__device__ __forceinline__ void dbg_dump_J(const TermArgs& a, const float* J, int rs, int cs, int row0, int nrows, int omode,
+                                           int tid, int nthreads) {
+  const int P = a.dbg_P, npose = (omode == DSPGN_MODE_POSE) ? 6 : 7;
+  for (int idx = tid; idx < nrows * P; idx += nthreads) {
+    const int p = idx / P, c = idx - p * P;
+    const int ci = (c < npose) ? (kMaxCode + c) : (c - npose);
+    a.dbg_J[(size_t)(row0 + p) * P + c] = J[p * rs + ci * cs];
+  }
+}
+
 // exclusive scan of tiles per object into s_prefix[0..n_obj]; returns total (all threads)
 __device__ inline int build_tile_prefix(const BatchDev& b, const TermArgs& a, int tile_rows, int* s_prefix, int* s_warp) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
@@ -385,10 +448,7 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
           x = q[0]; y = q[1]; z = q[2]; sc = 1.f;
         } else if (tmode() == MODE_BAND) {
           if constexpr (MEGA) {
-            // band rows live compacted per ray segment: the largest segment whose prefix is <= the row
-            int lo = 0, hi = mt.nseg;
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (mt.segp[mid] <= r) lo = mid; else hi = mid; }
-            const size_t s = (size_t)M.smp_off + (size_t)lo * mt.seg_samples + (size_t)(r - mt.segp[lo]);
+            const size_t s = band_row_sample(mt.segp, mt.nseg, M.smp_off, mt.seg_samples, r);
             x = __ldcg(b.band_x + 3 * s); y = __ldcg(b.band_x + 3 * s + 1); z = __ldcg(b.band_x + 3 * s + 2);
             sc = __ldcg(b.band_s + s); res = __ldcg(b.band_r + s);
           } else {
@@ -397,16 +457,8 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
             sc = b.band_s[s]; res = b.band_r[s];
           }
         } else {
-          int ray = r / b.D, j = r - ray * b.D;
-          if (MEGA && mt.compact) {
-            int lo = 0, hi = M.n_rays;                 // largest ray whose hull starts at or before this row
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((mt.segp[mid] >> 7) <= r) lo = mid; else hi = mid; }
-            ray = lo; j = (mt.segp[lo] & 127) + (r - (mt.segp[lo] >> 7));
-          }
-          const float* q = b.rays + 3 * (size_t)(M.ray_off + ray);
-          const float d = MEGA ? lin_depth(mt.ost[12], mt.ost[13], mt.ost[14], j, b.D) : lin_depth(st.dmin, st.dmax, st.dstep, j, b.D);
-          xform_point(MEGA ? mt.ost : st.T_oc, __fmul_rn(q[0], d), __fmul_rn(q[1], d), __fmul_rn(q[2], d), x, y, z);
-          sc = inside_unit_sphere(x, y, z) ? 1.f : 0.f;                // loss.py:68
+          sc = MEGA ? ray_sample_row(b, M, mt.ost, mt.ost[12], mt.ost[13], mt.ost[14], mt.segp, mt.compact, r, x, y, z)
+                    : ray_sample_row(b, M, st.T_oc, st.dmin, st.dmax, st.dstep, nullptr, false, r, x, y, z);
         }
       }
       S.xo[p] = x; S.xo[kTP + p] = y; S.xo[2 * kTP + p] = z;
@@ -611,31 +663,17 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
     for (int idx = tid + L * kTP; idx < kMaxCode * kTP; idx += kThreads) S.act[idx] = 0.f;  // code_len < 64
     if (tid < kTP) {
       const int p = tid;
-      const float gx = S.act[(kMaxCode + 0) * kTP + p], gy = S.act[(kMaxCode + 1) * kTP + p],
-                  gz = S.act[(kMaxCode + 2) * kTP + p];
-      const float x = S.xo[p], y = S.xo[kTP + p], z = S.xo[2 * kTP + p];
-      // dsdf/dx . [I | -x^ | x]  (loss_utils.py:166-185)  ==  [g, x cross g, g.x]
-      S.act[(kMaxCode + 3) * kTP + p] = y * gz - z * gy;
-      S.act[(kMaxCode + 4) * kTP + p] = z * gx - x * gz;
-      S.act[(kMaxCode + 5) * kTP + p] = x * gy - y * gx;
-      S.act[(kMaxCode + 6) * kTP + p] = (omode == DSPGN_MODE_POSE) ? 0.f : (gx * x + gy * y + gz * z);
-      S.act[(kMaxCode + 7) * kTP + p] = 0.f;
-      float res = (tmode() == MODE_SDF) ? S.yv[p] : S.rr[p];
-      const float sc = S.rscale[p];
-      if (sc == 0.f && (tmode() == MODE_SDF || p >= nrows)) res = 0.f;
-      if (mask_out != nullptr && tmode() == MODE_SDF && p < nrows)
-        mask_out[M.pts_off + row0 + p] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;   // optimizer.py:76-78
-      S.yv[p] = res;                                        // raw residual (debug dump)
-      S.rr[p] = huber_weight(fabsf(res), term_huber(a, tmode(), omode, (MEGA && tmode() == MODE_BAND) ? a.huber_b1 : a.huber_b)) * res;  // loss_utils.py:250-265
+      const RowTail t = row_tail(S.act + p, kTP, S.xo[p], S.xo[kTP + p], S.xo[2 * kTP + p], S.act[(kMaxCode + 0) * kTP + p],
+                                 S.act[(kMaxCode + 1) * kTP + p], S.act[(kMaxCode + 2) * kTP + p],
+                                 (tmode() == MODE_SDF) ? S.yv[p] : S.rr[p], S.rscale[p], p, nrows, tmode(), omode,
+                                 term_huber(a, tmode(), omode, (MEGA && tmode() == MODE_BAND) ? a.huber_b1 : a.huber_b),
+                                 mask_out, M.pts_off + row0);
+      S.yv[p] = t.res;                                      // raw residual (debug dump)
+      S.rr[p] = t.rho_r;
     }
     __syncthreads();
     if (!MEGA && a.dbg_J != nullptr && o == a.dbg_obj && tmode() == MODE_SDF) {
-      const int P = a.dbg_P, npose = (omode == DSPGN_MODE_POSE) ? 6 : 7;
-      for (int idx = tid; idx < nrows * P; idx += kThreads) {
-        const int p = idx / P, c = idx - p * P;
-        const int ci = (c < npose) ? (kMaxCode + c) : (c - npose);
-        a.dbg_J[(size_t)(row0 + p) * P + c] = S.act[ci * kTP + p];
-      }
+      dbg_dump_J(a, S.act, 1, kTP, row0, nrows, omode, tid, kThreads);
       if (tid < nrows) a.dbg_res[row0 + tid] = S.yv[tid];
     }
     // ---- phase 4: H += J^T J, b += J^T (rho r), loss += sum (rho r)^2  (optimizer.py:161-167) ----

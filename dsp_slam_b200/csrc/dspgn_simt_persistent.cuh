@@ -11,17 +11,14 @@
 
 namespace dspgn {
 
-// Shared memory of k_simt_persistent: the SIMT tile, then the object's staged state, the CTA-local FIFO, the copies of
-// the kernel arguments for the out-of-line solve step and the publication fields (as in TcwMegaTail).  The solve
-// workspace and the range words of a ray-sample or band tile both overlay the activation buffer, dead between tiles:
-// a tile first writes it after the barrier that ends its phase 0, the last reader of the range words.
+// Shared memory of k_simt_persistent: the SIMT tile, then the object's staged state and the persistent schedule's state.
+// The solve workspace and the range words of a ray-sample or band tile both overlay the activation buffer, dead between
+// tiles: a tile first writes it after the barrier that ends its phase 0, the last reader of the range words.
 template <int H>
 struct SimtMegaSmem : SimtSmem<H> {
-  float ost[16];                     // T_oc[12], dmin, dmax, dstep of the tile's object
+  float ost[15];                     // T_oc[12], dmin, dmax, dstep of the tile's object
   float zs[kMaxCode];                // its latent code
-  int fifo[4]; int fifo_pub; int epi_seq; int last_flag;
-  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
-  int push_base, push_nF, push_nS, push_o;
+  MegaSmem mega;
   __device__ SolveSmem& solve_smem() { return *reinterpret_cast<SolveSmem*>(this->act); }
   __device__ int* range_words() { return reinterpret_cast<int*>(this->act); }
 };
@@ -40,19 +37,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_simt_persistent(BatchDev b, Ter
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SimtMegaSmem<H>& S = *reinterpret_cast<SimtMegaSmem<H>*>(smem_raw);
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
-    S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv;
-  }
+  if (tid == 0) S.mega.init(b, q, sv);
   __syncthreads();
   for (int seq = 0;; ++seq) {
     // the previous item ended with a barrier of all threads: take the next one (at most one FIFO entry is ever ahead)
     if (tid == 0) {
-      *reinterpret_cast<volatile int*>(&S.epi_seq) = seq;
-      mega_fifo_fill(q, b.n_obj, S, seq);
+      *reinterpret_cast<volatile int*>(&S.mega.epi_seq) = seq;
+      mega_fifo_fill(q, b.n_obj, S.mega, seq);
     }
     TileRef tr;
-    if (!mega_tile_at<kTP, false>(a, S, seq, tr)) break;
+    if (!mega_tile_at<kTP, false>(a, S.mega, seq, tr)) break;
     if (tid == 0) log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile));
     if (tr.mode == kKindScan) {
       mega_scan_item<kTP>(S, b, q, sv, tr, tid);
@@ -69,13 +63,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_simt_persistent(BatchDev b, Ter
     mt.term_rows = (mode == MODE_SDF) ? M.n_pts : mega_rows(b, q, M, o, mode);
     mt.iter = (a.cut_iter >= 0) ? ldv(q.obj_iter + o) : 0;
     mt.ost = S.ost; mt.zs = S.zs; mt.segp = S.range_words();
-    mt.compact = mode == MODE_RAYFWD && q.vpre != nullptr;
-    mt.nseg = (mode == MODE_BAND) ? (M.n_rays + kSegRays - 1) / kSegRays : 0;
+    mt.nseg = mega_stage_ranges(q, M, o, mode, S.range_words(), tid, mt.compact);
     mt.seg_samples = kSegRays * b.D;
-    // the range words of the row -> sample map of a ray-sample or band tile
-    const int nw = mt.compact ? M.n_rays + 1 : (mode == MODE_BAND ? mt.nseg + 1 : 0);
-    const int* gp = mt.compact ? q.vpre + vpre_base(M, o) : q.seg_prefix + seg_base(M, o);
-    for (int i = tid; i < nw; i += kThreads) S.range_words()[i] = __ldcg(gp + i);
     __syncthreads();
     simt_tile<H, true>(S, b, a, o, tr.row0, tr.slot, mode, mt);
     mega_tile_end<true, kTP>(S, q, M, o, mode, tr.tile, tid);

@@ -226,6 +226,21 @@ __device__ __forceinline__ void split_pack(float a, float b, uint32_t& hi, uint3
 // ------------------------------------------------------------------------------------------------
 constexpr int kJpStride = 76;             // floats per row of the point-major Jacobian tile (72 + pad, 16B aligned)
 constexpr int kTcMaskLayers = 8;          // hidden layers with a saved ReLU mask (layers 0 .. 7 of the 8 x 256 decoders)
+// Shared-memory state of the persistent schedule (the mega_* helpers), embedded in the tail of every persistent kernel:
+// the CTA-local tile FIFO (scheduler lane -> epilogue threads), the stage-end flag word, the copies of the kernel
+// arguments for the out-of-line solve step and the cooperative publication of an object's next-iteration tiles.
+// Passing references to the kernel parameters themselves would make them address-taken: the compiler then parks all of
+// them in local memory and the tile loop reads its pointers with LDL instead of from the constant bank.
+struct MegaSmem {
+  int fifo[4]; int fifo_pub; int epi_seq; int last_flag;
+  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
+  int push_base, push_nF, push_nS, push_o;
+  // one thread, before the kernel's first barrier
+  __device__ void init(const BatchDev& b, const MegaArgs& q, const SolveArgs& sv) {
+    fifo_pub = 0; epi_seq = 0; last_flag = 0;
+    ctx_b = b; ctx_q = q; ctx_sv = sv;
+  }
+};
 template <int SCHED>
 struct TcSmemTail {
   float Jp[kTcRows * kJpStride];          // [row][72+4]: J row of each point; cols 0..66 double as latent_in skip gradient
@@ -242,15 +257,11 @@ struct TcSmemTail {
   int prefix[SCHED == 1 ? 1 : kMaxObjScan + 1];     // tile prefix of the per-iteration schedule (unused by SCHED 1)
   int warp_tmp[32];
   uint64_t w_full[kTcRing<SCHED>], w_empty[kTcRing<SCHED>];   // adjacent: wg_gemm addresses both from w_full
-  int cur_class;
-  int fifo[4]; int fifo_pub; int epi_seq; int last_flag;   // persistent mode: CTA-local tile FIFO (scheduler = producer warp)
   TcPlan plans[DSPGN_MAX_CLASSES];        // step plans of every decoder class (read by all warp roles)
-  // persistent mode: copies of the kernel arguments for the out-of-line solve step.  Passing references to the kernel
-  // parameters themselves would make them address-taken: the compiler then parks all of them in local memory and the tile
-  // loop reads its pointers with LDL instead of from the constant bank.
-  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
-  int push_base, push_nF, push_nS, push_o;   // cooperative publication of an object's next-iteration tiles
-  float ost[16]; int ost_rows;            // the tile's object: T_oc[12], dmin, dmax, dstep, dfar; rows of its term (counter)
+  int cur_class;
+  int ost_rows;                           // rows of the tile's term (a counter)
+  float ost[16];                          // the tile's object: T_oc[12], dmin, dmax, dstep, dfar
+  MegaSmem mega;                          // persistent mode (scheduler = producer warp)
   // workspace of the solve step (mega_solve_and_advance): the J tile, dead between tiles
   __device__ SolveSmem& solve_smem() { return *reinterpret_cast<SolveSmem*>(Jp); }
 };
@@ -264,6 +275,64 @@ static_assert(offsetof(TcSmemTail<0>, bias) % 8 == 0 && offsetof(TcSmemTail<0>, 
               offsetof(TcSmemTail<2>, bias) % 8 == 0 && offsetof(TcSmemTail<2>, w0x) % 8 == 0,
               "the epilogues read bias and W0 column pairs as float2");
 static_assert(offsetof(TcSmemTail<1>, maskw) % 16 == 0, "the SDF-tile kernel stages one uint4 of masks per thread");
+
+// ---- J^T J, J^T (rho r) and the loss of a J tile of ROWS rows (optimizer.py:161-167) into its partial sums accp.  Row p
+// of the tile: its Jacobian row at Jp[p * kJpStride] with rho r in column 71, rho r in rr[p], its row count in rsc[p].
+// Threads 0..170: one upper-triangular 4 x 4 block of the 72 x 72 product each; column 71 is left out of H, and the
+// chains of column block 17 give J^T (rho r) as  fmaf(J[p][c], rho r[p], .)  over p in order.  Threads 248..255: loss
+// and row count over ROWS / 8 rows each, fixed-order combine.
+template <int ROWS>
+__device__ __forceinline__ void jtile_sums(const float* Jp, const float* rr, const float* rsc, float* accp, int tid) {
+  if (tid < 171) {
+    DSPGN_PROBE_T(tjl);
+    int bi = 0, rem = tid;
+    while (rem >= 18 - bi) { rem -= 18 - bi; ++bi; }
+    const int bj = bi + rem;
+    float h[4][4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+#pragma unroll
+      for (int v = 0; v < 4; ++v) h[u][v] = 0.f;
+    const float* pa = Jp + 4 * bi;
+    const float* pb = Jp + 4 * bj;
+#pragma unroll 4
+    for (int p = 0; p < ROWS; ++p) {
+      const float4 A4 = *reinterpret_cast<const float4*>(pa + p * kJpStride);
+      const float4 B4 = *reinterpret_cast<const float4*>(pb + p * kJpStride);
+      const float av[4] = {A4.x, A4.y, A4.z, A4.w}, bv[4] = {B4.x, B4.y, B4.z, B4.w};
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+#pragma unroll
+        for (int v = 0; v < 4; ++v) h[u][v] = fmaf(av[u], bv[v], h[u][v]);
+    }
+    DSPGN_PROBE_ADD(PR_JTJ_LOOP, tjl);
+    DSPGN_PROBE_T(tjs);
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const int rI = 4 * bi + u, cI = 4 * bj + v;
+        if (cI >= rI && cI < kMaxCode + 7) accp[tri_index(rI, cI)] = h[u][v];
+      }
+    if (bj == 17) {
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+        if (4 * bi + u < kMaxCode + 7) accp[kAccB + 4 * bi + u] = h[u][3];
+    }
+    DSPGN_PROBE_ADD(PR_JTJ_STORE, tjs);
+  } else if (tid >= 248) {
+    constexpr int kPer = ROWS / 8;
+    const int k = tid - 248;
+    float sacc = 0.f, n = 0.f;
+    for (int p = kPer * k; p < kPer * k + kPer; ++p) { sacc = fmaf(rr[p], rr[p], sacc); n += rsc[p]; }
+#pragma unroll
+    for (int d = 1; d < 8; d <<= 1) {
+      sacc += __shfl_down_sync(0xff000000u, sacc, d);
+      n += __shfl_down_sync(0xff000000u, n, d);
+    }
+    if (k == 0) { accp[kAccLoss] = sacc; accp[kAccLoss + 1] = n; }
+  }
+}
 
 // ---- accumulator fragment (m64nNk16, fp32): thread (warp w of the warpgroup, lane l) holds element e of
 // 8-column block j = e >> 2 at row 16w + l/4 (+8 when e & 2), column 8j + 2(l%4) + (e & 1).
@@ -578,8 +647,8 @@ __device__ inline int mega_pop(const MegaArgs& q, int n_obj) {
 
 // Persistent kernels: work item number `seq` of this CTA from the CTA-local FIFO its scheduler lane fills (mega_fifo_fill),
 // as a tile of ROWS rows; false once the queue is drained.  SDF_ONLY: every item is an SDF tile (a compile-time kind).
-template <int ROWS, bool SDF_ONLY, class Tail>
-__device__ __forceinline__ bool mega_tile_at(const TermArgs& a, Tail& S, int seq, TileRef& t) {
+template <int ROWS, bool SDF_ONLY>
+__device__ __forceinline__ bool mega_tile_at(const TermArgs& a, MegaSmem& S, int seq, TileRef& t) {
   volatile int* pub = &S.fifo_pub;
   while (*pub <= seq) __nanosleep(64);           // filled by this CTA's scheduler lane, which always terminates (mega_pop)
   const int item = reinterpret_cast<volatile int*>(S.fifo)[seq & 3];
@@ -595,8 +664,7 @@ __device__ __forceinline__ bool mega_tile_at(const TermArgs& a, Tail& S, int seq
 
 // The scheduler lane of a persistent kernel: pop this CTA's next work item into slot `seq` of the CTA-local FIFO, at most
 // 3 entries ahead of the epilogue warps, and publish it (-1: no more work).
-template <class Tail>
-__device__ __forceinline__ void mega_fifo_fill(const MegaArgs& q, int n_obj, Tail& S, int seq) {
+__device__ __forceinline__ void mega_fifo_fill(const MegaArgs& q, int n_obj, MegaSmem& S, int seq) {
   DSPGN_PROBE_T(tp);
   volatile int* es = &S.epi_seq;
   while (seq - *es >= 3) __nanosleep(64);   // the epilogue warps always make progress (bounded tile work)
@@ -624,7 +692,7 @@ __device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, Tc
     t.mode = a.mode;
     return true;
   } else {
-    return mega_tile_at<kTcRows, SCHED == 1>(a, S, seq, t);
+    return mega_tile_at<kTcRows, SCHED == 1>(a, S.mega, seq, t);
   }
 }
 
@@ -634,6 +702,19 @@ __device__ __forceinline__ int mega_rows(const BatchDev& b, const MegaArgs& q, c
   if (mode == MODE_BAND) return ldv(b.band_m + o);
   if (q.vpre != nullptr) return ldv(q.vpre + vpre_base(M, o) + M.n_rays) >> 7;   // valid-sample hulls only
   return M.n_rays * b.D;
+}
+
+// The object's range words of a ray-sample tile (valid-sample-hull words: ray_sample_row) or a band tile (segment prefix:
+// band_row_sample) into dst, a shared-memory buffer the tile does not use before its first barrier; 256 threads.
+// Returns the band tile's segment count (0 otherwise); `compact`: the ray-sample tile's rows enumerate the hulls.
+__device__ __forceinline__ int mega_stage_ranges(const MegaArgs& q, const ObjMeta& M, int o, int mode, int* dst, int tid,
+                                                 bool& compact) {
+  compact = mode == MODE_RAYFWD && q.vpre != nullptr;
+  const int nseg = (mode == MODE_BAND) ? (M.n_rays + kSegRays - 1) / kSegRays : 0;
+  const int nw = compact ? M.n_rays + 1 : (mode == MODE_BAND ? nseg + 1 : 0);
+  const int* gp = compact ? q.vpre + vpre_base(M, o) : q.seg_prefix + seg_base(M, o);
+  for (int i = tid; i < nw; i += kTcEpiThreads) dst[i] = __ldcg(gp + i);
+  return nseg;
 }
 
 // publish `n` queue items (kind, object, tile 0..n-1): reserve slots, fence (everything the items depend on, incl. the
@@ -647,12 +728,13 @@ __device__ inline void mega_push(const MegaArgs& q, int kind, int o, int n) {
 
 // all terms of the object's current iteration are in: solve, update, queue the next iteration (or finish).  Called by
 // the 256 epilogue threads of the CTA that completed the object's last outstanding tile.  ROWS: rows per tile of the
-// kernel; Tail: its shared-memory tail (argument copies, push fields, warp_tmp, solve_smem()).
+// kernel; Tail: its shared-memory tail (mega, warp_tmp, solve_smem()).
 template <int ROWS, class Tail>
 __device__ __noinline__ void mega_solve_and_advance(Tail& S, int o, int tid) {
-  const BatchDev& b = S.ctx_b;
-  const MegaArgs& q = S.ctx_q;
-  const SolveArgs& sv = S.ctx_sv;
+  MegaSmem& P = S.mega;
+  const BatchDev& b = P.ctx_b;
+  const MegaArgs& q = P.ctx_q;
+  const SolveArgs& sv = P.ctx_sv;
   __threadfence();
   SolveSmem& SM = S.solve_smem();
   const int it = ldv(q.obj_iter + o);
@@ -688,7 +770,7 @@ __device__ __noinline__ void mega_solve_and_advance(Tail& S, int o, int tid) {
       if (wake) {
         const int ntF = ldv(q.ray_left + slot), ntS = (b.meta[slot].n_pts + ROWS - 1) / ROWS;
         base = atomicAdd(&q.ctr->tail, ntF + ntS);
-        S.push_nF = ntF; S.push_nS = ntS; S.push_o = slot;
+        P.push_nF = ntF; P.push_nS = ntS; P.push_o = slot;
       }
     } else {
       // (no fence in this branch: the tail only reserves slots; state and counters are fenced below, before any slot is published)
@@ -699,15 +781,15 @@ __device__ __noinline__ void mega_solve_and_advance(Tail& S, int o, int tid) {
       *reinterpret_cast<volatile int*>(q.pending + o) = ntS + (ntF > 0 ? 1 : 0);
       *reinterpret_cast<volatile int*>(q.ray_left + o) = ntF;
       base = atomicAdd(&q.ctr->tail, ntF + ntS);  // the long chain (rays -> scan -> band -> solve) first, then the SDF tiles
-      S.push_nF = ntF; S.push_nS = ntS; S.push_o = o;
+      P.push_nF = ntF; P.push_nS = ntS; P.push_o = o;
     }
-    S.push_base = base;
+    P.push_base = base;
   }
   epi_bar_sync();
-  const int base = S.push_base;
+  const int base = P.push_base;
   if (base >= 0) {
-    const int nF = S.push_nF, n = nF + S.push_nS;
-    const int po = S.push_o;                  // o, or the joint slot it woke
+    const int nF = P.push_nF, n = nF + P.push_nS;
+    const int po = P.push_o;                  // o, or the joint slot it woke
     __threadfence();                          // this thread's share of the ray range words (thread 0: state, counters)
     epi_bar_sync();                           // ... of every thread, before the first slot is published
     for (int j = tid; j < n; j += kTcEpiThreads)
@@ -729,10 +811,10 @@ __device__ __forceinline__ void mega_scan_item(Tail& S, const BatchDev& b, const
   epi_bar_sync();
   if (tid == 0) {
     log_event(q.log, ev_desc(EV_TILE_END, tr.mode, o, tr.tile));
-    *reinterpret_cast<volatile int*>(&S.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
+    *reinterpret_cast<volatile int*>(&S.mega.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
   }
   epi_bar_sync();
-  int act = *reinterpret_cast<volatile int*>(&S.last_flag);
+  int act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
   if (act == 1) {
     // last chunk of the object: segment prefix -> band row count -> band tiles
     __threadfence();
@@ -747,10 +829,10 @@ __device__ __forceinline__ void mega_scan_item(Tail& S, const BatchDev& b, const
       // the render term's placeholder in `pending` becomes its ntB band tiles BEFORE they can be popped
       const int left = atomicAdd(q.pending + o, ntB - 1) + ntB - 1;
       mega_push(q, MODE_BAND, o, ntB);
-      *reinterpret_cast<volatile int*>(&S.last_flag) = (left == 0) ? 2 : 0;
+      *reinterpret_cast<volatile int*>(&S.mega.last_flag) = (left == 0) ? 2 : 0;
     }
     epi_bar_sync();
-    act = *reinterpret_cast<volatile int*>(&S.last_flag);
+    act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
   } else act = 0;
   if (act == 2) mega_solve_and_advance<ROWS>(S, o, tid);
 }
@@ -770,10 +852,10 @@ __device__ __forceinline__ void mega_tile_end(Tail& S, const MegaArgs& q, const 
     int act = 0;
     if (RENDER && mode == MODE_RAYFWD) { if (atomicSub(q.ray_left + o, 1) == 1) act = 1; }
     else if (atomicSub(q.pending + o, 1) == 1) act = 2;
-    *reinterpret_cast<volatile int*>(&S.last_flag) = act;
+    *reinterpret_cast<volatile int*>(&S.mega.last_flag) = act;
   }
   epi_bar_sync();
-  int act = *reinterpret_cast<volatile int*>(&S.last_flag);
+  int act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
   if (RENDER && act == 1) {
     // every ray sample of the object has its sdf value: the per-ray scan becomes 64-ray work items of its own
     if (tid == 0) {
@@ -815,8 +897,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
   if (tid == 0) {
     for (int i = 0; i < RING; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
     S.cur_class = -1;
-    S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
-    if (MEGA) { S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv; }
+    if (MEGA) S.mega.init(b, q, sv);
     fence_barrier_init();
   }
   __syncthreads();
@@ -829,7 +910,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       uint32_t stage = 0, phase = 0;
       DSPGN_PROBE_T(tloop);
       for (int seq = 0;; ++seq) {
-        if (MEGA) mega_fifo_fill(q, b.n_obj, S, seq);
+        if (MEGA) mega_fifo_fill(q, b.n_obj, S.mega, seq);
         TileRef tr;
         if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
         const int o = tr.o;
@@ -866,7 +947,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
       DSPGN_PROBE_ADD(PR_FIFO, tq);
       DSPGN_PROBE_T(tpro);
-      if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = seq + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
+      if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.mega.epi_seq) = seq + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
       if (RENDER && tr.mode == kKindScan) {
         // ---- scan item: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141); no GEMM steps ----------
         // (the steps of mega_scan_item, inline: see there)
@@ -876,10 +957,10 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
         epi_bar_sync();
         if (tid == 0) {
           log_event(q.log, ev_desc(EV_TILE_END, tr.mode, o, tr.tile));
-          *reinterpret_cast<volatile int*>(&S.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
+          *reinterpret_cast<volatile int*>(&S.mega.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
         }
         epi_bar_sync();
-        int act = *reinterpret_cast<volatile int*>(&S.last_flag);
+        int act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
         if (act == 1) {
           // last chunk of the object: segment prefix -> band row count -> band tiles
           __threadfence();
@@ -894,10 +975,10 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
             // the render term's placeholder in `pending` becomes its ntB band tiles BEFORE they can be popped
             const int left = atomicAdd(q.pending + o, ntB - 1) + ntB - 1;
             mega_push(q, MODE_BAND, o, ntB);
-            *reinterpret_cast<volatile int*>(&S.last_flag) = (left == 0) ? 2 : 0;
+            *reinterpret_cast<volatile int*>(&S.mega.last_flag) = (left == 0) ? 2 : 0;
           }
           epi_bar_sync();
-          act = *reinterpret_cast<volatile int*>(&S.last_flag);
+          act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
         } else act = 0;
         if (act == 2) mega_solve_and_advance<kTcRows>(S, o, tid);
         continue;
@@ -937,24 +1018,10 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       // pose-only inlier cut (optimizer.py:76-78): recorded while iteration `cut_iter` runs, applied afterwards
       const uint8_t* mask_in; uint8_t* mask_out;
       cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
-      const int* segp = nullptr;
-      int nseg = 0;
-      const bool compact = RENDER && mode == MODE_RAYFWD && q.vpre != nullptr;
-      if (compact) {
-        // the object's per-ray range words (<= 8193 ints) in the idle J tile: row -> (ray, sample) by binary search below
-        int* sp = reinterpret_cast<int*>(S.Jp);
-        const int* gp = q.vpre + vpre_base(M, o);
-        for (int i = tid; i <= M.n_rays; i += kTcEpiThreads) sp[i] = __ldcg(gp + i);
-        segp = sp;
-      }
-      if (RENDER && mode == MODE_BAND) {
-        // band rows live compacted per ray segment: stage the object's segment prefix in the idle J tile
-        nseg = (M.n_rays + kSegRays - 1) / kSegRays;
-        int* sp = reinterpret_cast<int*>(S.Jp);
-        const int* gp = q.seg_prefix + seg_base(M, o);
-        for (int i = tid; i <= nseg; i += kTcEpiThreads) sp[i] = __ldcg(gp + i);
-        segp = sp;
-      }
+      // the object's range words (<= 8193 ints) of a ray-sample or band tile in the idle J tile
+      const int* segp = reinterpret_cast<const int*>(S.Jp);
+      bool compact = false;
+      const int nseg = RENDER ? mega_stage_ranges(q, M, o, mode, reinterpret_cast<int*>(S.Jp), tid, compact) : 0;
       // surface points do not depend on anything above: fetch them before the barrier
       int nrows = 0;
       float p0 = 0.f, p1 = 0.f, p2 = 0.f, sc = 0.f;
@@ -982,25 +1049,11 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           xform_point(Toc, p0, p1, p2, x0, x1, x2);
         } else if (mode == MODE_BAND) {
           // band rows were written by the CTAs that ran this object's scan: L2 is the point of coherence
-          size_t sidx = (size_t)M.smp_off + rr_;
-          if (RENDER) {
-            int lo = 0, hi = nseg;                     // largest segment with prefix <= row
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (segp[mid] <= rr_) lo = mid; else hi = mid; }
-            sidx = (size_t)M.smp_off + (size_t)lo * kSegRays * b.D + (size_t)(rr_ - segp[lo]);
-          }
+          const size_t sidx = RENDER ? band_row_sample(segp, nseg, M.smp_off, (size_t)kSegRays * b.D, rr_) : (size_t)M.smp_off + rr_;
           x0 = __ldcg(b.band_x + 3 * sidx); x1 = __ldcg(b.band_x + 3 * sidx + 1); x2 = __ldcg(b.band_x + 3 * sidx + 2);
           sc = __ldcg(b.band_s + sidx); res_in = __ldcg(b.band_r + sidx);
         } else {
-          int ray = rr_ / b.D, j = rr_ - ray * b.D;
-          if (compact) {
-            int lo = 0, hi = M.n_rays;                 // largest ray whose hull starts at or before this row
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((segp[mid] >> 7) <= rr_) lo = mid; else hi = mid; }
-            ray = lo; j = (segp[lo] & 127) + (rr_ - (segp[lo] >> 7));
-          }
-          const float* rq = b.rays + 3 * (size_t)(M.ray_off + ray);
-          const float d = lin_depth(S.ost[12], S.ost[13], S.ost[14], j, b.D);
-          xform_point(Toc, __fmul_rn(rq[0], d), __fmul_rn(rq[1], d), __fmul_rn(rq[2], d), x0, x1, x2);
-          sc = inside_unit_sphere(x0, x1, x2) ? 1.f : 0.f;            // loss.py:68
+          sc = ray_sample_row(b, M, Toc, S.ost[12], S.ost[13], S.ost[14], segp, compact, rr_, x0, x1, x2);
         }
       }
       if (grp == 0) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; S.scr[r] = sc; }
@@ -1185,84 +1238,19 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       if (grp == 0) {
         float* jr = S.Jp + r * kJpStride;
         for (int i = L; i < kMaxCode; ++i) jr[i] = 0.f;
-        const float g0 = jr[kMaxCode], g1 = jr[kMaxCode + 1], g2 = jr[kMaxCode + 2];
-        // dsdf/dx . [I | -x^ | x] = [g, x cross g, g.x]   (loss_utils.py:166-185)
-        jr[kMaxCode + 3] = x1 * g2 - x2 * g1;
-        jr[kMaxCode + 4] = x2 * g0 - x0 * g2;
-        jr[kMaxCode + 5] = x0 * g1 - x1 * g0;
-        jr[kMaxCode + 6] = (ost.mode == DSPGN_MODE_POSE) ? 0.f : (g0 * x0 + g1 * x1 + g2 * x2);
-        jr[kMaxCode + 7] = 0.f;
-        float res = (mode == MODE_SDF) ? yv : res_in;
-        if (sc == 0.f && (mode == MODE_SDF || r >= nrows)) res = 0.f;
-        if (mask_out != nullptr && mode == MODE_SDF && r < nrows)
-          mask_out[M.pts_off + row0 + r] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;      // optimizer.py:76-78
-        S.rr[r] = huber_weight(fabsf(res), huber_b) * res;
-        jr[kMaxCode + 7] = S.rr[r];                       // the J^T J chains of column block 17 give J^T (rho r) as well
-        S.rsc[r] = (mode == MODE_SDF) ? sc : (r < nrows ? 1.f : 0.f);
-        if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF && r < nrows) a.dbg_res[row0 + r] = res;
+        const RowTail t = row_tail(jr, 1, x0, x1, x2, jr[kMaxCode], jr[kMaxCode + 1], jr[kMaxCode + 2],
+                                   (mode == MODE_SDF) ? yv : res_in, sc, r, nrows, mode, ost.mode, huber_b, mask_out,
+                                   M.pts_off + row0);
+        S.rr[r] = t.rho_r;
+        jr[kMaxCode + 7] = t.rho_r;                       // for jtile_sums: J^T (rho r) from the J^T J chains
+        S.rsc[r] = t.n;
+        if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF && r < nrows) a.dbg_res[row0 + r] = t.res;
       }
       epi_bar_sync();
       DSPGN_PROBE_ADD(PR_JTJ_POSE, tjtj);
-      if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF) {
-        const int P = a.dbg_P, npose = (ost.mode == DSPGN_MODE_POSE) ? 6 : 7;
-        for (int idx = tid; idx < nrows * P; idx += kTcEpiThreads) {
-          const int p = idx / P, c = idx - p * P;
-          const int ci = (c < npose) ? (kMaxCode + c) : (c - npose);
-          a.dbg_J[(size_t)(row0 + p) * P + c] = S.Jp[p * kJpStride + ci];
-        }
-      }
-      // ---- J^T J, J^T (rho r), loss over the 128 rows of the tile (optimizer.py:161-167) -------------
-      float* accp = part + (size_t)tile * kAccStride;
-      if (tid < 171) {
-        DSPGN_PROBE_T(tjl);
-        int bi = 0, rem = tid;
-        while (rem >= 18 - bi) { rem -= 18 - bi; ++bi; }
-        const int bj = bi + rem;
-        float h[4][4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-#pragma unroll
-          for (int v = 0; v < 4; ++v) h[u][v] = 0.f;
-        const float* pa = S.Jp + 4 * bi;
-        const float* pb = S.Jp + 4 * bj;
-#pragma unroll 4
-        for (int p = 0; p < kTcRows; ++p) {
-          const float4 A4 = *reinterpret_cast<const float4*>(pa + p * kJpStride);
-          const float4 B4 = *reinterpret_cast<const float4*>(pb + p * kJpStride);
-          const float av[4] = {A4.x, A4.y, A4.z, A4.w}, bv[4] = {B4.x, B4.y, B4.z, B4.w};
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-#pragma unroll
-            for (int v = 0; v < 4; ++v) h[u][v] = fmaf(av[u], bv[v], h[u][v]);
-        }
-        DSPGN_PROBE_ADD(PR_JTJ_LOOP, tjl);
-        DSPGN_PROBE_T(tjs);
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const int rI = 4 * bi + u, cI = 4 * bj + v;
-            if (cI >= rI && cI < kMaxCode + 7) accp[tri_index(rI, cI)] = h[u][v];
-          }
-        if (bj == 17) {
-          // column 71 holds rho r: J^T (rho r) is  fmaf(J[p][c], rho r[p], .)  over p = 0..127 in order
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (4 * bi + u < kMaxCode + 7) accp[kAccB + 4 * bi + u] = h[u][3];
-        }
-        DSPGN_PROBE_ADD(PR_JTJ_STORE, tjs);
-      } else if (tid >= 248) {
-        // loss and row count: 8 threads x 16 rows, fixed-order combine
-        const int k = tid - 248;
-        float sacc = 0.f, n = 0.f;
-        for (int p = 16 * k; p < 16 * k + 16; ++p) { sacc = fmaf(S.rr[p], S.rr[p], sacc); n += S.rsc[p]; }
-#pragma unroll
-        for (int d = 1; d < 8; d <<= 1) {
-          sacc += __shfl_down_sync(0xff000000u, sacc, d);
-          n += __shfl_down_sync(0xff000000u, n, d);
-        }
-        if (k == 0) { accp[kAccLoss] = sacc; accp[kAccLoss + 1] = n; }
-      }
+      if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF)
+        dbg_dump_J(a, S.Jp, kJpStride, 1, row0, nrows, ost.mode, tid, kTcEpiThreads);
+      jtile_sums<kTcRows>(S.Jp, S.rr, S.rsc, part + (size_t)tile * kAccStride, tid);
       }   // !fwd_only
       DSPGN_PROBE_ADD(PR_JTJ, tjtj);
       if (MEGA) mega_tile_end<RENDER, kTcRows>(S, q, M, o, mode, tr.tile, tid);

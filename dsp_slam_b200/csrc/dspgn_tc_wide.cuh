@@ -59,15 +59,13 @@ struct TcwSmemTail {
   uint64_t w_full[kTcwRing], w_empty[kTcwRing];
   TcPlan plans[DSPGN_MAX_CLASSES];
 };
-// The persistent kernel's tail (k_wide_persistent): the same fields, then the tile's kind and index in its term, the
-// CTA-local FIFO, the copies of the kernel arguments for the out-of-line solve step and the publication fields (as in
-// TcSmemTail).  Its solve workspace is the A hi image and the range words of a ray-sample tile's object are staged in the
-// A lo image: both images are dead between tiles (the last GEMM step of a tile retired every MMA that read them).
+// The persistent kernel's tail (k_wide_persistent): the same fields, then the tile's kind and index in its term and the
+// persistent schedule's state.  Its solve workspace is the A hi image and the range words of a ray-sample or band tile's
+// object are staged in the A lo image: both images are dead between tiles (the last GEMM step of a tile retired every MMA
+// that read them).
 struct TcwMegaTail : TcwSmemTail<1> {
   int t_mode, t_j;
-  int fifo[4]; int fifo_pub; int epi_seq; int last_flag;
-  BatchDev ctx_b; MegaArgs ctx_q; SolveArgs ctx_sv;
-  int push_base, push_nF, push_nS, push_o;
+  MegaSmem mega;
   __device__ SolveSmem& solve_smem() {
     return *reinterpret_cast<SolveSmem*>(reinterpret_cast<unsigned char*>(this) - 2 * (size_t)kTcwAImgBytes);
   }
@@ -168,10 +166,7 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
   }
   if (tid == 0) {
     for (int i = 0; i < kTcwRing; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
-    if constexpr (MEGA) {
-      S.fifo_pub = 0; S.epi_seq = 0; S.last_flag = 0;
-      S.ctx_b = b; S.ctx_q = q; S.ctx_sv = sv;
-    }
+    if constexpr (MEGA) S.mega.init(b, q, sv);
     fence_barrier_init();
   }
   __syncthreads();
@@ -183,9 +178,9 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
       uint32_t stage = 0, phase = 0;
       if constexpr (MEGA) {
         for (int seq = 0;; ++seq) {
-          mega_fifo_fill(q, b.n_obj, S, seq);
+          mega_fifo_fill(q, b.n_obj, S.mega, seq);
           TileRef tr;
-          if (!mega_tile_at<kTcwRows, false>(a, S, seq, tr)) break;
+          if (!mega_tile_at<kTcwRows, false>(a, S.mega, seq, tr)) break;
           if (tr.mode == kKindScan) continue;                    // no GEMM steps
           const int cls = b.meta[tr.o].class_id;
           const TcPlan& plan = S.plans[cls];
@@ -236,8 +231,8 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
       if constexpr (MEGA) {
         // `tile` counts this CTA's work items (the FIFO sequence number)
         TileRef tr;
-        if (!mega_tile_at<kTcwRows, false>(a, S, tile, tr)) break;
-        if (tid == 0) { *reinterpret_cast<volatile int*>(&S.epi_seq) = tile + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
+        if (!mega_tile_at<kTcwRows, false>(a, S.mega, tile, tr)) break;
+        if (tid == 0) { *reinterpret_cast<volatile int*>(&S.mega.epi_seq) = tile + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
         if (tr.mode == kKindScan) {
           mega_scan_item<kTcwRows>(S, b, q, sv, tr, tid);
           ++tile;
@@ -264,14 +259,8 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
       const int nrows = min(kTcwRows, (MEGA ? (pts_mode ? M.n_pts : mega_rows(b, q, M, o, mode)) : term_rows(b, a, o)) - row0);
       // SCHED 1: the object's range words for the row -> sample map of a ray-sample or band tile, in the dead A lo image
       const int* segp = reinterpret_cast<const int*>(alo);
-      int nseg = 0;
-      if constexpr (MEGA) {
-        const bool compact = mode == MODE_RAYFWD && q.vpre != nullptr;
-        if (mode == MODE_BAND) nseg = (M.n_rays + kSegRays - 1) / kSegRays;
-        const int nw = compact ? M.n_rays + 1 : (mode == MODE_BAND ? nseg + 1 : 0);
-        const int* gp = compact ? q.vpre + vpre_base(M, o) : q.seg_prefix + seg_base(M, o);
-        for (int i = tid; i < nw; i += kTcEpiThreads) reinterpret_cast<int*>(alo)[i] = __ldcg(gp + i);
-      }
+      bool compact = false;
+      const int nseg = MEGA ? mega_stage_ranges(q, M, o, mode, reinterpret_cast<int*>(alo), tid, compact) : 0;
       epi_bar_sync();      // the previous tile's per-row stages are done with xr / scr and the tile descriptor
       const int r = tile_row();
       if (tid == 0) { S.t_tile = tile; S.t_o = o; S.t_row0 = row0; S.t_nrows = nrows; S.t_cls = M.class_id; }
@@ -284,26 +273,11 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
           else xform_point(S.ost, pq[0], pq[1], pq[2], x0, x1, x2);
           sc = (grid_mode || mask_in == nullptr || ldv(mask_in + M.pts_off + rr_)) ? 1.f : 0.f;
         } else if (mode == MODE_BAND) {
-          size_t sidx = (size_t)M.smp_off + rr_;
-          if (MEGA) {
-            // band rows live compacted per ray segment: the largest segment whose prefix is <= the row
-            int lo = 0, hi = nseg;
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (segp[mid] <= rr_) lo = mid; else hi = mid; }
-            sidx = (size_t)M.smp_off + (size_t)lo * kSegRays * b.D + (size_t)(rr_ - segp[lo]);
-          }
+          const size_t sidx = MEGA ? band_row_sample(segp, nseg, M.smp_off, (size_t)kSegRays * b.D, rr_) : (size_t)M.smp_off + rr_;
           x0 = __ldcg(b.band_x + 3 * sidx); x1 = __ldcg(b.band_x + 3 * sidx + 1); x2 = __ldcg(b.band_x + 3 * sidx + 2);
           sc = __ldcg(b.band_s + sidx); res_in = __ldcg(b.band_r + sidx);
         } else {
-          int ray = rr_ / b.D, j = rr_ - ray * b.D;
-          if (MEGA && q.vpre != nullptr) {
-            int lo = 0, hi = M.n_rays;                 // largest ray whose hull starts at or before this row
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((segp[mid] >> 7) <= rr_) lo = mid; else hi = mid; }
-            ray = lo; j = (segp[lo] & 127) + (rr_ - (segp[lo] >> 7));
-          }
-          const float* rq = b.rays + 3 * (size_t)(M.ray_off + ray);
-          const float d = lin_depth(S.ost[12], S.ost[13], S.ost[14], j, b.D);
-          xform_point(S.ost, __fmul_rn(rq[0], d), __fmul_rn(rq[1], d), __fmul_rn(rq[2], d), x0, x1, x2);
-          sc = inside_unit_sphere(x0, x1, x2) ? 1.f : 0.f;            // loss.py:68
+          sc = ray_sample_row(b, M, S.ost, S.ost[12], S.ost[13], S.ost[14], segp, compact, rr_, x0, x1, x2);
         }
       }
       if (tid < kTcwRows) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; S.scr[r] = sc; S.rin[r] = res_in; }
@@ -404,7 +378,7 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
           }
         }
       } else if (st.kind == TK_FWD_HIDDEN) {
-        // the passes of dspgn_tc.cuh on this warpgroup's columns: bounds and the concat offset relative to c0
+        // the epi_* passes of tc_body on this warpgroup's columns: bounds and the concat offset relative to c0
         uint32_t mw[4] = {0u, 0u, 0u, 0u};
         epi_fwd_hidden<0, 0>(acc, mw, S.bias + c0, qs, nm - c0, k_next - c0);
         if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next - c0, st.cat_off - c0, dec.L, S.zs, S.xr, rowA, rowB);
@@ -429,7 +403,7 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
       if (tile_mode() == MODE_RAYFWD) {
         // the next sequence number is read before mega_tile_end's barriers: once past them, thread 0 may already have
         // taken the next item and rewritten S.epi_seq
-        const int next = *reinterpret_cast<volatile int*>(&S.epi_seq);
+        const int next = *reinterpret_cast<volatile int*>(&S.mega.epi_seq);
         mega_tile_end<true, kTcwRows>(S, q, b.meta[S.t_o], S.t_o, MODE_RAYFWD, S.t_j, tid);
         tile = next;
         continue;
@@ -447,82 +421,22 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
       const uint8_t* mask_in; uint8_t* mask_out;
       cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
       const float huber_b = term_huber(a, mode, ost.mode, (MEGA && mode == MODE_BAND) ? a.huber_b1 : a.huber_b);
-      const float x0 = S.xr[r], x1 = S.xr[kTcRows + r], x2 = S.xr[2 * kTcRows + r], sc = S.scr[r];
       float* jr = S.Jp + r * kJpStride;
       for (int i = L; i < kMaxCode; ++i) jr[i] = 0.f;
-      const float g0 = jr[kMaxCode], g1 = jr[kMaxCode + 1], g2 = jr[kMaxCode + 2];
-      // dsdf/dx . [I | -x^ | x] = [g, x cross g, g.x]   (loss_utils.py:166-185)
-      jr[kMaxCode + 3] = x1 * g2 - x2 * g1;
-      jr[kMaxCode + 4] = x2 * g0 - x0 * g2;
-      jr[kMaxCode + 5] = x0 * g1 - x1 * g0;
-      jr[kMaxCode + 6] = (ost.mode == DSPGN_MODE_POSE) ? 0.f : (g0 * x0 + g1 * x1 + g2 * x2);
-      jr[kMaxCode + 7] = 0.f;
-      float res = (mode == MODE_SDF) ? S.yrow[r] : S.rin[r];
-      if (sc == 0.f && (mode == MODE_SDF || r >= nrows)) res = 0.f;
-      if (mask_out != nullptr && mode == MODE_SDF && r < nrows)
-        mask_out[b.meta[o].pts_off + row0 + r] = (sc != 0.f && fabsf(res) <= 0.05f) ? 1 : 0;      // optimizer.py:76-78
-      S.rr[r] = huber_weight(fabsf(res), huber_b) * res;
-      S.rsc[r] = (mode == MODE_SDF) ? sc : (r < nrows ? 1.f : 0.f);
-      if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF && r < nrows) a.dbg_res[row0 + r] = res;
+      const RowTail t = row_tail(jr, 1, S.xr[r], S.xr[kTcRows + r], S.xr[2 * kTcRows + r], jr[kMaxCode], jr[kMaxCode + 1],
+                                 jr[kMaxCode + 2], (mode == MODE_SDF) ? S.yrow[r] : S.rin[r], S.scr[r], r, nrows, mode,
+                                 ost.mode, huber_b, mask_out, b.meta[o].pts_off + row0);
+      S.rr[r] = t.rho_r;
+      jr[kMaxCode + 7] = t.rho_r;                       // for jtile_sums: J^T (rho r) from the J^T J chains
+      S.rsc[r] = t.n;
+      if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF && r < nrows) a.dbg_res[row0 + r] = t.res;
     }
     epi_bar_sync();
-    if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF) {
-      const int P = a.dbg_P, npose = (ost.mode == DSPGN_MODE_POSE) ? 6 : 7;
-      for (int idx = tid; idx < nrows * P; idx += kTcEpiThreads) {
-        const int p = idx / P, c = idx - p * P;
-        const int ci = (c < npose) ? (kMaxCode + c) : (c - npose);
-        a.dbg_J[(size_t)(row0 + p) * P + c] = S.Jp[p * kJpStride + ci];
-      }
-    }
-    // ---- J^T J, J^T (rho r), loss over the 64 rows of the tile (optimizer.py:161-167) ---------------------------------
-    float* accp = ((MEGA && mode == MODE_BAND) ? a.part_r : a.part) + (size_t)S.t_tile * kAccStride;
-    if (tid < 171) {
-      int bi = 0, rem = tid;
-      while (rem >= 18 - bi) { rem -= 18 - bi; ++bi; }
-      const int bj = bi + rem;
-      float h[4][4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) h[u][v] = 0.f;
-      const float* pa = S.Jp + 4 * bi;
-      const float* pb = S.Jp + 4 * bj;
-#pragma unroll 4
-      for (int p = 0; p < kTcwRows; ++p) {
-        const float4 A4 = *reinterpret_cast<const float4*>(pa + p * kJpStride);
-        const float4 B4 = *reinterpret_cast<const float4*>(pb + p * kJpStride);
-        const float av[4] = {A4.x, A4.y, A4.z, A4.w}, bv[4] = {B4.x, B4.y, B4.z, B4.w};
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-#pragma unroll
-          for (int v = 0; v < 4; ++v) h[u][v] = fmaf(av[u], bv[v], h[u][v]);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const int rI = 4 * bi + u, cI = 4 * bj + v;
-          if (cI >= rI && cI < kMaxCode + 7) accp[tri_index(rI, cI)] = h[u][v];
-        }
-    } else if (tid < 171 + kMaxCode + 7) {
-      const int c = tid - 171;
-      float sacc = 0.f;
-      for (int p = 0; p < kTcwRows; ++p) sacc = fmaf(S.Jp[p * kJpStride + c], S.rr[p], sacc);
-      accp[kAccB + c] = sacc;
-    } else if (tid >= 248) {
-      // loss and row count: 8 threads x 8 rows, fixed-order combine
-      const int k = tid - 248;
-      float sacc = 0.f, n = 0.f;
-      for (int p = 8 * k; p < 8 * k + 8; ++p) { sacc = fmaf(S.rr[p], S.rr[p], sacc); n += S.rsc[p]; }
-#pragma unroll
-      for (int d = 1; d < 8; d <<= 1) {
-        sacc += __shfl_down_sync(0xff000000u, sacc, d);
-        n += __shfl_down_sync(0xff000000u, n, d);
-      }
-      if (k == 0) { accp[kAccLoss] = sacc; accp[kAccLoss + 1] = n; }
-    }
+    if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF)
+      dbg_dump_J(a, S.Jp, kJpStride, 1, row0, nrows, ost.mode, tid, kTcEpiThreads);
+    jtile_sums<kTcwRows>(S.Jp, S.rr, S.rsc, ((MEGA && mode == MODE_BAND) ? a.part_r : a.part) + (size_t)S.t_tile * kAccStride, tid);
     if constexpr (MEGA) {
-      const int next = *reinterpret_cast<volatile int*>(&S.epi_seq);     // before the barriers, as above
+      const int next = *reinterpret_cast<volatile int*>(&S.mega.epi_seq);     // before the barriers, as above
       mega_tile_end<true, kTcwRows>(S, q, b.meta[o], o, mode, S.t_j, tid);
       tile = next;
     } else {
