@@ -298,6 +298,26 @@ __device__ __forceinline__ int find_object(const int* s_prefix, int n_obj, int t
   return lo;
 }
 
+// A tile of kind `mode` runs the decoder forward only (ray-sample, point-forward and grid-forward tiles).  MEGA: the
+// persistent schedule, whose queue kind 3 is a scan item (kKindScan), not MODE_PTSFWD.
+template <bool MEGA>
+__device__ __forceinline__ bool tile_fwd_only(int mode) {
+  return mode == MODE_RAYFWD || (!MEGA && (mode == MODE_PTSFWD || mode == MODE_GRIDFWD));
+}
+// GEMM steps of a tensor-core tile of kind `mode` with step plan p: none for a scan item, the forward steps for a
+// forward-only tile, every step otherwise
+template <bool MEGA>
+__device__ __forceinline__ int tile_steps(const TcPlan& p, int mode) {
+  if (MEGA && mode == kKindScan) return 0;
+  return tile_fwd_only<MEGA>(mode) ? p.n_fwd : p.n_steps;
+}
+
+// The object of the tile being run, staged in shared memory by its prologue (stage_obj, dspgn_tc.cuh)
+struct TileObj {
+  float ost[16];                     // T_oc[12], dmin, dmax, dstep, dfar
+  float zs[kMaxCode + 16];           // latent code, zero padded
+};
+
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
@@ -367,6 +387,7 @@ struct SimtSmem {
   float xo[3 * TP];
   float yv[TP], rr[TP], rscale[TP];
   float red[kThreads];               // last layer: one partial dot product per thread
+  TileObj obj;
   int prefix[kMaxObjScan + 1];
   int warp_tmp[32];
 };
@@ -403,8 +424,6 @@ __device__ inline void simt_ln_backward(float* act, float* red, const float* rst
 struct SimtMegaTile {
   int term_rows;             // rows of the tile's term: SDF points, ray samples (valid-sample hulls) or band rows
   int iter;                  // the object's current iteration (inlier cut)
-  const float* ost;          // T_oc[12], dmin, dmax, dstep of the object
-  const float* zs;           // its latent code
   const int* segp;           // range words of a ray-sample tile (vpre) or a band tile (segment prefix)
   int nseg;                  // band tile: ray segments of the object
   int seg_samples;           // band tile: ray samples per segment (kSegRays x D)
@@ -414,8 +433,8 @@ struct SimtMegaTile {
 // One tile of the SIMT engine: transform, forward, backward to the input, Jacobian rows and the tile's partial sums into
 // slot `tile` of its term.  Both schedules run it: MEGA = false is k_decoder_simt (one launch per term and iteration,
 // the term is a.mode), MEGA = true is k_simt_persistent (every item kind of the device queue, the kind is `mode_mega`;
-// `mt` carries the object's state as the run last wrote it).  A row's values do not depend on which other rows share
-// its tile.
+// `mt` carries the values other CTAs write during the run).  The caller has staged the object in S.obj (stage_obj).  A
+// row's values do not depend on which other rows share its tile.
 template <int H, bool MEGA>
 __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, const TermArgs& a, const int o, const int row0,
                                           const int tile, const int mode_mega, const SimtMegaTile& mt) {
@@ -441,7 +460,7 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
       if (p < nrows) {
         if (tmode() == MODE_SDF || (!MEGA && tmode() == MODE_PTSFWD)) {
           const float* q = b.pts + 3 * (size_t)(M.pts_off + r);
-          xform_point(MEGA ? mt.ost : st.T_oc, q[0], q[1], q[2], x, y, z);
+          xform_point(S.obj.ost, q[0], q[1], q[2], x, y, z);
           sc = (mask_in == nullptr || (MEGA ? __ldcg(mask_in + M.pts_off + r) : mask_in[M.pts_off + r])) ? 1.f : 0.f;
         } else if (!MEGA && tmode() == MODE_GRIDFWD) {
           const float* q = a.grid + 3 * (size_t)r;
@@ -457,14 +476,14 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
             sc = b.band_s[s]; res = b.band_r[s];
           }
         } else {
-          sc = MEGA ? ray_sample_row(b, M, mt.ost, mt.ost[12], mt.ost[13], mt.ost[14], mt.segp, mt.compact, r, x, y, z)
-                    : ray_sample_row(b, M, st.T_oc, st.dmin, st.dmax, st.dstep, nullptr, false, r, x, y, z);
+          sc = ray_sample_row(b, M, S.obj.ost, S.obj.ost[12], S.obj.ost[13], S.obj.ost[14], mt.segp, MEGA && mt.compact, r, x,
+                              y, z);
         }
       }
       S.xo[p] = x; S.xo[kTP + p] = y; S.xo[2 * kTP + p] = z;
       S.rscale[p] = sc; S.rr[p] = res;
     }
-    for (int idx = tid; idx < L * kTP; idx += kThreads) S.inp[idx] = MEGA ? mt.zs[idx / kTP] : st.z[idx / kTP];
+    for (int idx = tid; idx < L * kTP; idx += kThreads) S.inp[idx] = S.obj.zs[idx / kTP];
     for (int idx = tid; idx < (kMaxCode + 4) * kTP; idx += kThreads) S.gin[idx] = 0.f;
     float* const xhat_all = (a.ln_scratch != nullptr) ? a.ln_scratch + (size_t)blockIdx.x * DSPGN_MAX_LINEAR * H * kTP : nullptr;
     __syncthreads();
@@ -586,7 +605,7 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
       }
       __syncthreads();
     }
-    if (tmode() == MODE_RAYFWD || (!MEGA && (tmode() == MODE_PTSFWD || tmode() == MODE_GRIDFWD))) {
+    if (tile_fwd_only<MEGA>(tmode())) {
       int cnt = 0;
       if (tid < nrows) {
         const bool valid = S.rscale[tid] != 0.f;
@@ -726,21 +745,6 @@ __device__ __forceinline__ void simt_tile(SimtSmem<H>& S, const BatchDev& b, con
       accp[kAccLoss + 1] = n;
     }
     __syncthreads();
-  }
-}
-
-// H: the widest layer of any class of the solver (kHid or kHidWide); every class runs at that instantiation
-template <int H>
-__global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermArgs a) {
-  constexpr int kTP = simt_rows(H);
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  SimtSmem<H>& S = *reinterpret_cast<SimtSmem<H>*>(smem_raw);
-  const int total_tiles = build_tile_prefix(b, a, kTP, S.prefix, S.warp_tmp);
-
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int o = find_object(S.prefix, b.n_obj, tile);
-    const int row0 = (tile - S.prefix[o]) * kTP;
-    simt_tile<H, false>(S, b, a, o, row0, tile, 0, SimtMegaTile{});
   }
 }
 

@@ -1,23 +1,22 @@
-// fp32 SIMT engine on the persistent object-pipelined schedule (DESIGN §4.12): every GN iteration of every object in one
-// launch.  The tile is simt_tile (dspgn_simt.cuh), the same code k_decoder_simt runs; the scheduling is that of
-// k_wide_persistent (dspgn_tc.cuh: mega_*) at simt_rows(H) rows per tile.
+// The kernels of the fp32 SIMT engine: k_decoder_simt on the per-iteration schedule (one launch per term and iteration)
+// and k_simt_persistent on the persistent object-pipelined schedule (DESIGN §4.12, every GN iteration of every object in
+// one launch).  Both run the tile simt_tile (dspgn_simt.cuh) on the tiles of the shared tile source (tile_at,
+// dspgn_tc.cuh); the persistent kernel starts each work item with the shared prologue of the tensor-core kernels
+// (mega_item_begin) at simt_rows(H) rows per tile.
 //
-// There is no producer warpgroup: thread 0 of the CTA pops the next work item into the CTA-local FIFO between tiles,
-// behind the barriers that end the previous tile, so the CTA holds no queue ticket while it runs a tile.  The scan items
-// and the solve step run on the CTA's 256 threads (named barrier 1, as on the 256 epilogue threads of the tensor-core
-// kernels).
+// k_simt_persistent has no producer warpgroup: thread 0 of the CTA pops the next work item into the CTA-local FIFO
+// between tiles, behind the barriers that end the previous tile, so the CTA holds no queue ticket while it runs a tile.
+// The scan items and the solve step run on the CTA's 256 threads (named barrier 1, as on the 256 epilogue threads of the
+// tensor-core kernels).
 #pragma once
 #include "dspgn_tc.cuh"
 
 namespace dspgn {
 
-// Shared memory of k_simt_persistent: the SIMT tile, then the object's staged state and the persistent schedule's state.
-// The solve workspace and the range words of a ray-sample or band tile both overlay the activation buffer, dead between
+// Shared memory of k_simt_persistent: the SIMT tile, then the persistent schedule's state.  The solve workspace and the range words of a ray-sample or band tile both overlay the activation buffer, dead between
 // tiles: a tile first writes it after the barrier that ends its phase 0, the last reader of the range words.
 template <int H>
 struct SimtMegaSmem : SimtSmem<H> {
-  float ost[15];                     // T_oc[12], dmin, dmax, dstep of the tile's object
-  float zs[kMaxCode];                // its latent code
   MegaSmem mega;
   __device__ SolveSmem& solve_smem() { return *reinterpret_cast<SolveSmem*>(this->act); }
   __device__ int* range_words() { return reinterpret_cast<int*>(this->act); }
@@ -29,6 +28,23 @@ static_assert(sizeof(SolveSmem) <= sizeof(SimtSmem<kHid>::act) && sizeof(SolveSm
 static_assert(4 * (kScanMaxRays + 1) <= sizeof(SimtSmem<kHid>::act) && 4 * (kScanMaxRays + 1) <= sizeof(SimtSmem<kHidWide>::act) &&
               4 * (kScanMaxRays / kSegRays + 1) <= sizeof(SimtSmem<kHid>::act),
               "k_simt_persistent: a ray-sample / band tile stages its object's range words in the activation buffer");
+
+// H: the widest layer of any class of the solver (kHid or kHidWide); every class runs at that instantiation
+template <int H>
+__global__ void __launch_bounds__(kThreads, 1) k_decoder_simt(BatchDev b, TermArgs a) {
+  constexpr int kTP = simt_rows(H);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SimtSmem<H>& S = *reinterpret_cast<SimtSmem<H>*>(smem_raw);
+  build_tile_prefix(b, a, kTP, S.prefix, S.warp_tmp);
+  for (int seq = 0;; ++seq) {
+    TileRef tr;
+    if (!tile_at<kTP, 0>(b, a, S, seq, tr)) break;
+    // (the previous tile ended with a barrier of all threads, after its last read of S.obj)
+    stage_obj(S.obj, b.state[tr.o], b.decs[b.meta[tr.o].class_id].L, threadIdx.x);
+    __syncthreads();
+    simt_tile<H, false>(S, b, a, tr.o, tr.row0, tr.slot, tr.mode, SimtMegaTile{});
+  }
+}
 
 // One CTA per SM (grid_sms); the LayerNorm scratch (a.ln_scratch) holds one region per CTA.
 template <int H>
@@ -46,23 +62,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_simt_persistent(BatchDev b, Ter
       mega_fifo_fill(q, b.n_obj, S.mega, seq);
     }
     TileRef tr;
-    if (!mega_tile_at<kTP, false>(a, S.mega, seq, tr)) break;
-    if (tid == 0) log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile));
-    if (tr.mode == kKindScan) {
-      mega_scan_item<kTP>(S, b, q, sv, tr, tid);
-      continue;
-    }
+    if (!tile_at<kTP, 2>(b, a, S, seq, tr)) break;
+    SimtMegaTile mt{};
+    // (publishes seq again: the scheduler is thread 0 itself, which pops item seq + 1 only after this item's barriers)
+    if (!mega_item_begin<kTP>(S, b, a, q, sv, tr, seq, tid, mt.iter, mt.term_rows)) continue;
     const int o = tr.o, mode = tr.mode;
     const ObjMeta& M = b.meta[o];
-    const ObjState& st = b.state[o];
-    // the object's pose, depth range and code as the last solve (another CTA) wrote them
-    if (tid < 12) S.ost[tid] = ldv(&st.T_oc[tid]);
-    else if (tid < 15) S.ost[tid] = ldv(&st.dmin + (tid - 12));
-    else if (tid >= 32 && tid < 32 + kMaxCode) S.zs[tid - 32] = ldv(&st.z[tid - 32]);
-    SimtMegaTile mt{};
-    mt.term_rows = (mode == MODE_SDF) ? M.n_pts : mega_rows(b, q, M, o, mode);
-    mt.iter = (a.cut_iter >= 0) ? ldv(q.obj_iter + o) : 0;
-    mt.ost = S.ost; mt.zs = S.zs; mt.segp = S.range_words();
+    mt.segp = S.range_words();
     mt.nseg = mega_stage_ranges(q, M, o, mode, S.range_words(), tid, mt.compact);
     mt.seg_samples = kSegRays * b.D;
     __syncthreads();

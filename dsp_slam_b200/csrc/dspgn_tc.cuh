@@ -250,7 +250,7 @@ struct TcSmemTail {
   float bias[9 * kHid];
   float wlast[kHid];
   float w0x[3 * kHid];                    // xyz rows of the layer-0 matrix (the latent rows are folded into ObjState.zb0)
-  float zs[kMaxCode + 16];                // latent code of the tile's object (zero padded)
+  TileObj obj;                            // the tile's object (stage_obj)
   float xr[3 * kTcRows];                  // object-frame point of every row
   float rr[kTcRows], rsc[kTcRows];
   float yrow[kTcRows], scr[kTcRows];      // decoder output and row weight (0 = inactive row) of every row
@@ -259,8 +259,6 @@ struct TcSmemTail {
   uint64_t w_full[kTcRing<SCHED>], w_empty[kTcRing<SCHED>];   // adjacent: wg_gemm addresses both from w_full
   TcPlan plans[DSPGN_MAX_CLASSES];        // step plans of every decoder class (read by all warp roles)
   int cur_class;
-  int ost_rows;                           // rows of the tile's term (a counter)
-  float ost[16];                          // the tile's object: T_oc[12], dmin, dmax, dstep, dfar
   MegaSmem mega;                          // persistent mode (scheduler = producer warp)
   // workspace of the solve step (mega_solve_and_advance): the J tile, dead between tiles
   __device__ SolveSmem& solve_smem() { return *reinterpret_cast<SolveSmem*>(Jp); }
@@ -617,6 +615,34 @@ __device__ __forceinline__ void produce_step(const unsigned char* src, int nch, 
   stage = st;
 }
 
+// producer side of a tile: the weight images of the first ns GEMM steps of plan (tile_steps), from the class's blob
+template <int RING, int STAGE_BYTES = kTcStageBytes>
+__device__ __forceinline__ void produce_tile(const unsigned char* blob, const TcPlan& plan, int ns, unsigned char* ring,
+                                             uint64_t* w_full, uint64_t* w_empty, uint32_t& stage, uint32_t& phase) {
+  for (int s = 0; s < ns; ++s)
+    produce_step<RING, STAGE_BYTES>(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma,
+                                    ring, w_full, w_empty, stage, phase);
+}
+
+// the step plans of the batch's n_classes decoder classes into shared memory (plan_of(c): class c's plan in global
+// memory); all kTcThreads threads
+template <class PlanOf>
+__device__ __forceinline__ void stage_plans(TcPlan* dst, int n_classes, PlanOf plan_of, int tid) {
+  constexpr int kWords = (int)(sizeof(TcPlan) / 4);
+  for (int i = tid; i < n_classes * kWords; i += kTcThreads)
+    reinterpret_cast<int*>(&dst[i / kWords])[i % kWords] = reinterpret_cast<const int*>(&plan_of(i / kWords))[i % kWords];
+}
+
+// The tile's object into shared memory: pose and depth range (threads 0..15), latent code zero padded (threads
+// 0 .. kMaxCode + 15).  On the persistent schedule the last solve (another CTA) wrote them: read cache-bypassing
+// once per tile and shared.  As 12 + 3 loads in every thread they were ~130 requests per tile for the same two L2 lines
+// -- and on few-object batches every SM asks for them at the same moment.
+__device__ __forceinline__ void stage_obj(TileObj& d, const ObjState& st, int L, int tid) {
+  if (tid < 12) d.ost[tid] = ldv(&st.T_oc[tid]);
+  else if (tid < 16) d.ost[tid] = ldv(&st.dmin + (tid - 12));
+  if (tid < kMaxCode + 16) d.zs[tid] = (tid < L) ? ldv(&st.z[tid]) : 0.f;
+}
+
 struct TileRef { int o, row0, slot, mode, tile; };
 
 // pop one work item for this CTA (persistent mode); -1 = no more work anywhere
@@ -645,23 +671,6 @@ __device__ inline int mega_pop(const MegaArgs& q, int n_obj) {
   }
 }
 
-// Persistent kernels: work item number `seq` of this CTA from the CTA-local FIFO its scheduler lane fills (mega_fifo_fill),
-// as a tile of ROWS rows; false once the queue is drained.  SDF_ONLY: every item is an SDF tile (a compile-time kind).
-template <int ROWS, bool SDF_ONLY>
-__device__ __forceinline__ bool mega_tile_at(const TermArgs& a, MegaSmem& S, int seq, TileRef& t) {
-  volatile int* pub = &S.fifo_pub;
-  while (*pub <= seq) __nanosleep(64);           // filled by this CTA's scheduler lane, which always terminates (mega_pop)
-  const int item = reinterpret_cast<volatile int*>(S.fifo)[seq & 3];
-  if (item < 0) return false;
-  t.o = (item >> kItemObjShift) & kItemObjMask;
-  t.mode = SDF_ONLY ? MODE_SDF : (item >> kItemKindShift);
-  const int j = item & kItemTileMask;
-  t.tile = j;
-  t.row0 = j * ROWS;
-  t.slot = (t.mode == MODE_BAND) ? a.tile_base_r[t.o] + j : (t.mode == MODE_SDF ? a.tile_base[t.o] + j : 0);
-  return true;
-}
-
 // The scheduler lane of a persistent kernel: pop this CTA's next work item into slot `seq` of the CTA-local FIFO, at most
 // 3 entries ahead of the epilogue warps, and publish it (-1: no more work).
 __device__ __forceinline__ void mega_fifo_fill(const MegaArgs& q, int n_obj, MegaSmem& S, int seq) {
@@ -676,23 +685,33 @@ __device__ __forceinline__ void mega_fifo_fill(const MegaArgs& q, int n_obj, Meg
   *reinterpret_cast<volatile int*>(&S.fifo_pub) = seq + 1;
 }
 
-// tile number `seq` of this CTA: static round-robin over the launch's tiles, or the CTA-local FIFO
-// SCHED: 0 = one launch per term (static tiles), 1 = persistent kernel, SDF tiles only (SDF-only joint runs, pose-only
-// runs: the tile kind is a compile-time constant), 2 = persistent kernel with the render term (all item kinds)
-template <int SCHED>
-__device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, TcSmemTail<SCHED>& S, int seq, int total_tiles, TileRef& t) {
-  constexpr bool MEGA = SCHED != 0;
-  if (!MEGA) {
+// Work item number `seq` of this CTA as a tile of ROWS rows; false once there is none.  SCHED 0: one launch per term,
+// static round-robin over the launch's tiles (S.prefix: the block's tile prefix, build_tile_prefix; the kind is a.mode).
+// Persistent kernels: the CTA-local FIFO (S.mega) its scheduler lane fills (mega_fifo_fill); SCHED 1 = SDF tiles only
+// (SDF-only joint runs, pose-only runs: the kind is a compile-time constant), SCHED 2 = every item kind.
+template <int ROWS, int SCHED, class Tail>
+__device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, Tail& S, int seq, TileRef& t) {
+  if constexpr (SCHED == 0) {
     const int tile = blockIdx.x + seq * gridDim.x;
-    if (tile >= total_tiles) return false;
+    if (tile >= S.prefix[b.n_obj]) return false;
     t.o = find_object(S.prefix, b.n_obj, tile);
     t.tile = tile - S.prefix[t.o];
-    t.row0 = t.tile * kTcRows;
+    t.row0 = t.tile * ROWS;
     t.slot = tile;
     t.mode = a.mode;
     return true;
   } else {
-    return mega_tile_at<kTcRows, SCHED == 1>(a, S.mega, seq, t);
+    volatile int* pub = &S.mega.fifo_pub;
+    while (*pub <= seq) __nanosleep(64);         // filled by this CTA's scheduler lane, which always terminates (mega_pop)
+    const int item = reinterpret_cast<volatile int*>(S.mega.fifo)[seq & 3];
+    if (item < 0) return false;
+    t.o = (item >> kItemObjShift) & kItemObjMask;
+    t.mode = SCHED == 1 ? MODE_SDF : (item >> kItemKindShift);
+    const int j = item & kItemTileMask;
+    t.tile = j;
+    t.row0 = j * ROWS;
+    t.slot = (t.mode == MODE_BAND) ? a.tile_base_r[t.o] + j : (t.mode == MODE_SDF ? a.tile_base[t.o] + j : 0);
+    return true;
   }
 }
 
@@ -800,8 +819,6 @@ __device__ __noinline__ void mega_solve_and_advance(Tail& S, int o, int tid) {
 // Scan item of a persistent kernel: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141), no GEMM
 // steps.  The CTA that finishes the object's last chunk turns the segment counts into the band-row prefix and queues the
 // band tiles (ROWS rows each); when no SDF tile is outstanding either, it runs the solve step.  256 epilogue threads.
-// k_wide_persistent calls it; tc_body keeps the same steps inline: called from there, k_gn_persistent_render grows to
-// 642 branch regions (BSSY), over the 638 tests/test_tc_sass.py allows it.
 template <int ROWS, class Tail>
 __device__ __forceinline__ void mega_scan_item(Tail& S, const BatchDev& b, const MegaArgs& q, const SolveArgs& sv, const TileRef& tr,
                                                int tid) {
@@ -835,6 +852,28 @@ __device__ __forceinline__ void mega_scan_item(Tail& S, const BatchDev& b, const
     act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
   } else act = 0;
   if (act == 2) mega_solve_and_advance<ROWS>(S, o, tid);
+}
+
+// Start of work item tr on the epilogue threads of a persistent kernel (ROWS rows per tile).  Thread 0 publishes `pub`
+// as the epilogue's FIFO position (S.mega.epi_seq) and logs the item.  A scan item runs here: false, no GEMM tile.
+// Otherwise the object goes to S.obj (stage_obj; read after the caller's next barrier), `iter` is the object's
+// iteration (the inline cut) and `rows` the rows of the tile's term.
+template <int ROWS, class Tail>
+__device__ __forceinline__ bool mega_item_begin(Tail& S, const BatchDev& b, const TermArgs& a, const MegaArgs& q,
+                                                const SolveArgs& sv, const TileRef& tr, int pub, int tid, int& iter, int& rows) {
+  if (tid == 0) {
+    *reinterpret_cast<volatile int*>(&S.mega.epi_seq) = pub;
+    log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile));
+  }
+  if (tr.mode == kKindScan) {
+    mega_scan_item<ROWS>(S, b, q, sv, tr, tid);
+    return false;
+  }
+  const ObjMeta& M = b.meta[tr.o];
+  stage_obj(S.obj, b.state[tr.o], b.decs[M.class_id].L, tid);
+  iter = (a.cut_iter >= 0) ? ldv(q.obj_iter + tr.o) : a.iter;
+  rows = mega_rows(b, q, M, tr.o, tr.mode);
+  return true;
 }
 
 // End of a GEMM tile of a persistent kernel (kind `mode`, tile `tile` of object o, meta M): its partial
@@ -886,14 +925,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
   TcSmemTail<SCHED>& S = *reinterpret_cast<TcSmemTail<SCHED>*>(ring + (size_t)RING * kTcStageBytes + 2 * (size_t)kTcAloBytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  const int total_tiles = MEGA ? 0 : build_tile_prefix(b, a, kTcRows, S.prefix, S.warp_tmp);
-  {
-    const int nwords = b.n_classes * (int)(sizeof(TcPlan) / 4);
-    for (int i = tid; i < nwords; i += kTcThreads) {
-      const int c = i / (int)(sizeof(TcPlan) / 4), w = i % (int)(sizeof(TcPlan) / 4);
-      reinterpret_cast<int*>(&S.plans[c])[w] = reinterpret_cast<const int*>(&b.decs[c].tc_plan)[w];
-    }
-  }
+  if (!MEGA) build_tile_prefix(b, a, kTcRows, S.prefix, S.warp_tmp);
+  stage_plans(S.plans, b.n_classes, [&](int c) -> const TcPlan& { return b.decs[c].tc_plan; }, tid);
   if (tid == 0) {
     for (int i = 0; i < RING; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
     S.cur_class = -1;
@@ -912,16 +945,10 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
       for (int seq = 0;; ++seq) {
         if (MEGA) mega_fifo_fill(q, b.n_obj, S.mega, seq);
         TileRef tr;
-        if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
-        const int o = tr.o;
-        const int cls = b.meta[o].class_id;
-        const TcPlan& plan = S.plans[cls];
-        const unsigned char* blob = b.decs[cls].tc_blob;
-        const bool fwd_only = (tr.mode == MODE_RAYFWD || tr.mode == MODE_PTSFWD || (!MEGA && tr.mode == MODE_GRIDFWD));
-        const int ns = (RENDER && tr.mode == kKindScan) ? 0 : (fwd_only ? plan.n_fwd : plan.n_steps);
-        for (int s = 0; s < ns; ++s)
-          produce_step<RING>(blob + plan.step[s].w_off, plan.step[s].k_steps / 4, 64u * (uint32_t)plan.step[s].n_mma, ring,
-                             S.w_full, S.w_empty, stage, phase);
+        if (!tile_at<kTcRows, SCHED>(b, a, S, seq, tr)) break;
+        const int cls = b.meta[tr.o].class_id;
+        produce_tile<RING>(b.decs[cls].tc_blob, S.plans[cls], tile_steps<MEGA>(S.plans[cls], tr.mode), ring, S.w_full, S.w_empty,
+                           stage, phase);
       }
       DSPGN_PROBE_ADD(PR_PROD_LOOP, tloop);
     }
@@ -944,102 +971,62 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
     for (int seq = 0;; ++seq) {
       TileRef tr;
       DSPGN_PROBE_T(tq);
-      if (!tile_at<SCHED>(b, a, S, seq, total_tiles, tr)) break;
+      if (!tile_at<kTcRows, SCHED>(b, a, S, seq, tr)) break;
       DSPGN_PROBE_ADD(PR_FIFO, tq);
       DSPGN_PROBE_T(tpro);
-      if (MEGA && tid == 0) { *reinterpret_cast<volatile int*>(&S.mega.epi_seq) = seq + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
-      if (RENDER && tr.mode == kKindScan) {
-        // ---- scan item: occupancy scan / rendered depth / band rows of 64 rays (loss.py:84-141); no GEMM steps ----------
-        // (the steps of mega_scan_item, inline: see there)
-        const int o = tr.o;
-        scan_chunk(b, sv.prm.th, q.vpre, q.seg_cnt, o, tr.tile, tid);
-        __threadfence();
-        epi_bar_sync();
-        if (tid == 0) {
-          log_event(q.log, ev_desc(EV_TILE_END, tr.mode, o, tr.tile));
-          *reinterpret_cast<volatile int*>(&S.mega.last_flag) = (atomicSub(q.scan_left + o, 1) == 1) ? 1 : 0;
-        }
-        epi_bar_sync();
-        int act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
-        if (act == 1) {
-          // last chunk of the object: segment prefix -> band row count -> band tiles
-          __threadfence();
-          scan_prefix(b, q.seg_cnt, q.seg_prefix, o, tid, S.warp_tmp);
-          epi_bar_sync();
-          if (tid == 0) {
-            __threadfence();                         // prefix / band_m / band rows before the band tiles are published
-            atomicAdd(&q.ctr->valid_rows_total, (unsigned long long)ldv(b.V_count + o));   // V of this iteration is complete (roofline accounting)
-            const int m = ldv(b.band_m + o);
-            const int ntB = (m + kTcRows - 1) / kTcRows;
-            atomicAdd(&q.ctr->band_rows_total, m);
-            // the render term's placeholder in `pending` becomes its ntB band tiles BEFORE they can be popped
-            const int left = atomicAdd(q.pending + o, ntB - 1) + ntB - 1;
-            mega_push(q, MODE_BAND, o, ntB);
-            *reinterpret_cast<volatile int*>(&S.mega.last_flag) = (left == 0) ? 2 : 0;
-          }
-          epi_bar_sync();
-          act = *reinterpret_cast<volatile int*>(&S.mega.last_flag);
-        } else act = 0;
-        if (act == 2) mega_solve_and_advance<kTcRows>(S, o, tid);
-        continue;
+      // ---- prologue, phase A: everything that comes from global memory, then ONE barrier ------------------------------
+      int iter = a.iter, term_n = 0;
+      if constexpr (MEGA) {
+        if (!mega_item_begin<kTcRows>(S, b, a, q, sv, tr, seq + 1, tid, iter, term_n)) continue;
+      } else {
+        stage_obj(S.obj, b.state[tr.o], b.decs[b.meta[tr.o].class_id].L, tid);
+        term_n = term_rows(b, a, tr.o);
       }
       const int o = tr.o, row0 = tr.row0, tile = tr.slot, mode = tr.mode;
-      const ObjMeta M = b.meta[o];
+      const ObjMeta& M = b.meta[o];
       const ObjState& ost = b.state[o];
       const DecoderDev& dec = b.decs[M.class_id];
       const TcPlan& plan = S.plans[M.class_id];
       const int L = dec.L, in0 = dec.in0, n_lin = dec.n_lin;
       const bool has_skip = dec.latent_in >= 0;
       const bool grid_mode = !MEGA && mode == MODE_GRIDFWD;
-      const bool fwd_only = (mode == MODE_RAYFWD || mode == MODE_PTSFWD || grid_mode);
-      const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
+      const bool fwd_only = (mode == MODE_RAYFWD || mode == MODE_PTSFWD || grid_mode);   // (a scan item never gets here)
+      const int ns = tile_steps<MEGA>(plan, mode);
       const float huber_b = term_huber(a, mode, ost.mode, (RENDER && mode == MODE_BAND) ? a.huber_b1 : a.huber_b);
       float* const part = (RENDER && mode == MODE_BAND) ? a.part_r : a.part;
-      // ---- prologue, phase A: everything that comes from global memory, then ONE barrier ------------------------------
-      // The pose / depth range of this object may have been rewritten by another CTA's solve: read (cache-bypassing) once
-      // per tile by 16 threads and shared through smem.  As 12 + 3 loads in every thread they were ~130 requests per tile
-      // for the same two L2 lines -- and on few-object batches every SM asks for them at the same moment.
-      if (tid < 12) S.ost[tid] = ldv(&ost.T_oc[tid]);
-      else if (tid < 16) S.ost[tid] = ldv(&ost.dmin + (tid - 12));          // dmin, dmax, dstep, dfar
       const bool pts_mode = (mode == MODE_SDF || mode == MODE_PTSFWD || grid_mode);
-      if (MEGA && !pts_mode && tid == 16) S.ost_rows = mega_rows(b, q, M, o, mode);   // band / ray-sample rows: a counter
 
-      // per-class constants in smem (bias, last row, xyz rows of layer 0), the tile's latent code
+      // per-class constants in smem (bias, last row, xyz rows of layer 0)
       if (S.cur_class != M.class_id) {
         for (int i = tid; i < n_lin * kHid; i += kTcEpiThreads) S.bias[i] = dec.bias[i / kHid][i % kHid];
         for (int i = tid; i < kHid; i += kTcEpiThreads) S.wlast[i] = dec.w_last[i];
         const float* __restrict__ w0g = dec.Wf[0] + (size_t)L * kHid;   // rows L..L+2 of the reduction-major layer-0 matrix
         for (int i = tid; i < 3 * kHid; i += kTcEpiThreads) S.w0x[i] = w0g[i];
       }
-      if (tid < kMaxCode + 16) S.zs[tid] = (tid < L) ? ldv(&ost.z[tid]) : 0.f;
       // layer 0 with the latent part folded into a per-object bias (ObjState.zb0, refreshed by k_init / the solve step);
       // written after the per-class reload above, read after the barriers below
       S.bias[tid] = ldv(&ost.zb0[tid]);
       // pose-only inlier cut (optimizer.py:76-78): recorded while iteration `cut_iter` runs, applied afterwards
       const uint8_t* mask_in; uint8_t* mask_out;
-      cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
+      cut_masks(a, ost.mode, iter, mask_in, mask_out);
       // the object's range words (<= 8193 ints) of a ray-sample or band tile in the idle J tile
       const int* segp = reinterpret_cast<const int*>(S.Jp);
       bool compact = false;
       const int nseg = RENDER ? mega_stage_ranges(q, M, o, mode, reinterpret_cast<int*>(S.Jp), tid, compact) : 0;
       // surface points do not depend on anything above: fetch them before the barrier
-      int nrows = 0;
+      const int nrows = min(kTcRows, term_n - row0);
       float p0 = 0.f, p1 = 0.f, p2 = 0.f, sc = 0.f;
-      if (pts_mode) {
-        nrows = min(kTcRows, (MEGA ? M.n_pts : term_rows(b, a, o)) - row0);
-        if (r < nrows) {
-          const float* pq = grid_mode ? a.grid + 3 * (size_t)(row0 + r) : b.pts + 3 * (size_t)(M.pts_off + row0 + r);
-          p0 = pq[0]; p1 = pq[1]; p2 = pq[2];
-          sc = (grid_mode || mask_in == nullptr || ldv(mask_in + M.pts_off + row0 + r)) ? 1.f : 0.f;
-        }
+      if (pts_mode && r < nrows) {
+        const float* pq = grid_mode ? a.grid + 3 * (size_t)(row0 + r) : b.pts + 3 * (size_t)(M.pts_off + row0 + r);
+        p0 = pq[0]; p1 = pq[1]; p2 = pq[2];
+        sc = (grid_mode || mask_in == nullptr || ldv(mask_in + M.pts_off + row0 + r)) ? 1.f : 0.f;
       }
       epi_bar_sync();      // (per-iteration schedule: Jp / rr of the previous tile are not written before the barrier further down;
                            //  persistent schedule: the previous tile ended with a barrier, its J tile is dead)
       // ---- phase B: this row's point in the object frame ----------------------------------------------------------------
       float Toc[12];
 #pragma unroll
-      for (int i = 0; i < 12; ++i) Toc[i] = S.ost[i];
-      if (!pts_mode) nrows = min(kTcRows, (MEGA ? S.ost_rows : term_rows(b, a, o)) - row0);
+      for (int i = 0; i < 12; ++i) Toc[i] = S.obj.ost[i];
       float x0 = 0.f, x1 = 0.f, x2 = 0.f, res_in = 0.f;
       if (r < nrows) {
         const int rr_ = row0 + r;
@@ -1053,7 +1040,7 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           x0 = __ldcg(b.band_x + 3 * sidx); x1 = __ldcg(b.band_x + 3 * sidx + 1); x2 = __ldcg(b.band_x + 3 * sidx + 2);
           sc = __ldcg(b.band_s + sidx); res_in = __ldcg(b.band_r + sidx);
         } else {
-          sc = ray_sample_row(b, M, Toc, S.ost[12], S.ost[13], S.ost[14], segp, compact, rr_, x0, x1, x2);
+          sc = ray_sample_row(b, M, Toc, S.obj.ost[12], S.obj.ost[13], S.obj.ost[14], segp, compact, rr_, x0, x1, x2);
         }
       }
       if (grp == 0) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; S.scr[r] = sc; }
@@ -1196,8 +1183,8 @@ __device__ __forceinline__ void tc_body(const BatchDev& b, const TermArgs& a, co
           if (nm == 256 && k_next == 256) epi_fwd_hidden<256, 256>(acc, mw, bb, qs, nm, k_next);
           else if (nm == 192 && k_next == 256) epi_fwd_hidden<192, 256>(acc, mw, bb, qs, nm, k_next);
           else epi_fwd_hidden<0, 0>(acc, mw, bb, qs, nm, k_next);
-          if (st.cat_off == 189 && L == 64) epi_concat_input<189, 64>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
-          else if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next, st.cat_off, L, S.zs, S.xr, rowA, rowB);
+          if (st.cat_off == 189 && L == 64) epi_concat_input<189, 64>(acc, qs, k_next, st.cat_off, L, S.obj.zs, S.xr, rowA, rowB);
+          else if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next, st.cat_off, L, S.obj.zs, S.xr, rowA, rowB);
           save_mask(st.layer, mw);
           DSPGN_PROBE_ADD(pk, tval);
           put_operand(pk);

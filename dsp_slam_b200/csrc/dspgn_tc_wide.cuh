@@ -49,13 +49,13 @@ struct TcwSmemTail {
   // band-row residual
   float rr[kTcwRows], rsc[kTcwRows], scr[kTcwRows], yrow[kTcwRows], rin[kTcwRows];
   float ypart[2 * kTcwRows];              // last layer: each warpgroup's half of the per-row dot product
-  float zs[kMaxCode + 16];                // latent code of the tile's object (zero padded)
-  float ost[16];                          // T_oc[12], dmin, dmax, dstep, dfar of the tile's object
+  TileObj obj;                            // the tile's object (stage_obj)
   int prefix[SCHED == 0 ? kMaxObjScan + 1 : 1];   // tile prefix of the per-iteration schedule (unused by SCHED 1)
   int warp_tmp[32];
-  // the tile being run: object, first row, rows, class.  The step loop and the tail read them from here after each
-  // barrier: held in registers through the epilogues, such tile-wide scalars spill to local memory.
-  int t_tile, t_o, t_row0, t_nrows, t_cls;
+  // the tile being run: CTA sequence number, partial-sum slot, object, first row, rows, class.  The step loop and the
+  // tail read them from here after each barrier: held in registers through the epilogues, such tile-wide scalars spill
+  // to local memory.
+  int t_seq, t_tile, t_o, t_row0, t_nrows, t_cls;
   uint64_t w_full[kTcwRing], w_empty[kTcwRing];
   TcPlan plans[DSPGN_MAX_CLASSES];
 };
@@ -149,6 +149,7 @@ template <int SCHED>
 __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, const TcwDecDev* __restrict__ wd,
                                          uint4* __restrict__ masks_g, const MegaArgs& q, const SolveArgs& sv) {
   constexpr bool MEGA = SCHED == 1;
+  constexpr int SRC = MEGA ? 2 : 0;             // tile_at: static tiles, or every item kind from the FIFO
   extern __shared__ unsigned char tcw_smem_raw[];
   unsigned char* ring = tcw_smem_raw + ((1024u - (smem_u32(tcw_smem_raw) & 1023u)) & 1023u);
   unsigned char* const ahi = ring + (size_t)kTcwRing * kTcwStageBytes;
@@ -156,14 +157,8 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
   TcwTail<SCHED>& S = *reinterpret_cast<TcwTail<SCHED>*>(alo + kTcwAImgBytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  const int total_tiles = MEGA ? 0 : build_tile_prefix(b, a, kTcwRows, S.prefix, S.warp_tmp);
-  {
-    const int nwords = b.n_classes * (int)(sizeof(TcPlan) / 4);
-    for (int i = tid; i < nwords; i += kTcThreads) {
-      const int c = i / (int)(sizeof(TcPlan) / 4), w = i % (int)(sizeof(TcPlan) / 4);
-      reinterpret_cast<int*>(&S.plans[c])[w] = reinterpret_cast<const int*>(&wd[c].plan)[w];
-    }
-  }
+  if (!MEGA) build_tile_prefix(b, a, kTcwRows, S.prefix, S.warp_tmp);
+  stage_plans(S.plans, b.n_classes, [&](int c) -> const TcPlan& { return wd[c].plan; }, tid);
   if (tid == 0) {
     for (int i = 0; i < kTcwRing; ++i) { mbar_init(&S.w_full[i], 1); mbar_init(&S.w_empty[i], 8); }
     if constexpr (MEGA) S.mega.init(b, q, sv);
@@ -176,29 +171,13 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
     setmaxnreg_dec<kTcProducerRegs>();
     if (warp == 8 && lane == 0) {
       uint32_t stage = 0, phase = 0;
-      if constexpr (MEGA) {
-        for (int seq = 0;; ++seq) {
-          mega_fifo_fill(q, b.n_obj, S.mega, seq);
-          TileRef tr;
-          if (!mega_tile_at<kTcwRows, false>(a, S.mega, seq, tr)) break;
-          if (tr.mode == kKindScan) continue;                    // no GEMM steps
-          const int cls = b.meta[tr.o].class_id;
-          const TcPlan& plan = S.plans[cls];
-          const int ns = tr.mode == MODE_RAYFWD ? plan.n_fwd : plan.n_steps;
-          for (int s = 0; s < ns; ++s)
-            produce_step<kTcwRing, kTcwStageBytes>(wd[cls].blob + plan.step[s].w_off, plan.step[s].k_steps / 4,
-                                                   64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full, S.w_empty, stage, phase);
-        }
-      } else {
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-          const int cls = b.meta[find_object(S.prefix, b.n_obj, tile)].class_id;
-          const TcPlan& plan = S.plans[cls];
-          const bool fwd_only = a.mode == MODE_RAYFWD || a.mode == MODE_PTSFWD || a.mode == MODE_GRIDFWD;
-          const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
-          for (int s = 0; s < ns; ++s)
-            produce_step<kTcwRing, kTcwStageBytes>(wd[cls].blob + plan.step[s].w_off, plan.step[s].k_steps / 4,
-                                                   64u * (uint32_t)plan.step[s].n_mma, ring, S.w_full, S.w_empty, stage, phase);
-        }
+      for (int seq = 0;; ++seq) {
+        if constexpr (MEGA) mega_fifo_fill(q, b.n_obj, S.mega, seq);
+        TileRef tr;
+        if (!tile_at<kTcwRows, SRC>(b, a, S, seq, tr)) break;
+        const int cls = b.meta[tr.o].class_id;
+        produce_tile<kTcwRing, kTcwStageBytes>(wd[cls].blob, S.plans[cls], tile_steps<MEGA>(S.plans[cls], tr.mode), ring, S.w_full,
+                                               S.w_empty, stage, phase);
       }
     }
     return;
@@ -222,62 +201,50 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
   auto tile_mode = [&] { if constexpr (MEGA) return *reinterpret_cast<volatile int*>(&S.t_mode); else return mode0; };
   uint32_t stage = 0, phase = 0;
   float acc[128];
-  // The tile index, the tile count (S.prefix[n_obj]) and this thread's tile row are read from shared memory / %tid
+  // The sequence number, the tile count (S.prefix[n_obj]) and this thread's tile row are read from shared memory / %tid
   // where they are needed, so that nothing tile-wide stays in registers through the epilogues.
-  for (int tile = MEGA ? 0 : blockIdx.x; MEGA || tile < S.prefix[b.n_obj];) {
+  for (int seq = 0;; ++seq) {
     // ---- prologue: the object's pose, code and this row's point --------------------------------------------------
     {
-      int o, row0, mode = mode0;
+      TileRef tr;
+      if (!tile_at<kTcwRows, SRC>(b, a, S, seq, tr)) break;
+      int iter = a.iter, term_n = 0;
       if constexpr (MEGA) {
-        // `tile` counts this CTA's work items (the FIFO sequence number)
-        TileRef tr;
-        if (!mega_tile_at<kTcwRows, false>(a, S.mega, tile, tr)) break;
-        if (tid == 0) { *reinterpret_cast<volatile int*>(&S.mega.epi_seq) = tile + 1; log_event(q.log, ev_desc(EV_TILE_BEGIN, tr.mode, tr.o, tr.tile)); }
-        if (tr.mode == kKindScan) {
-          mega_scan_item<kTcwRows>(S, b, q, sv, tr, tid);
-          ++tile;
-          continue;
-        }
-        o = tr.o; row0 = tr.row0; mode = tr.mode;
+        if (!mega_item_begin<kTcwRows>(S, b, a, q, sv, tr, seq + 1, tid, iter, term_n)) continue;
         if (tid == 0) { S.t_mode = tr.mode; S.t_j = tr.tile; }
-        // `tile` becomes the tile's partial-sum slot (S.t_tile); the sequence number stays in S.epi_seq - 1, which thread
-        // 0 wrote above, before the prologue's barriers, and rewrites only after every thread passed mega_tile_end's
-        tile = tr.slot;
       } else {
-        o = find_object(S.prefix, b.n_obj, tile);
-        row0 = (tile - S.prefix[o]) * kTcwRows;
+        stage_obj(S.obj, b.state[tr.o], b.decs[b.meta[tr.o].class_id].L, tid);
+        term_n = term_rows(b, a, tr.o);
       }
+      const int o = tr.o, row0 = tr.row0, mode = tr.mode;
       const bool pts_mode = MEGA ? mode == MODE_SDF : pts_mode0;
       const ObjMeta& M = b.meta[o];
       const ObjState& ost = b.state[o];
       const int L = b.decs[M.class_id].L;
-      if (tid < 12) S.ost[tid] = ldv(&ost.T_oc[tid]);
-      else if (tid < 16) S.ost[tid] = ldv(&ost.dmin + (tid - 12));
-      if (tid >= 32 && tid < 32 + kMaxCode + 16) S.zs[tid - 32] = (tid - 32 < L) ? ldv(&ost.z[tid - 32]) : 0.f;
       const uint8_t* mask_in; uint8_t* mask_out;
-      cut_masks(a, ost.mode, (MEGA && a.cut_iter >= 0) ? ldv(q.obj_iter + o) : a.iter, mask_in, mask_out);
-      const int nrows = min(kTcwRows, (MEGA ? (pts_mode ? M.n_pts : mega_rows(b, q, M, o, mode)) : term_rows(b, a, o)) - row0);
+      cut_masks(a, ost.mode, iter, mask_in, mask_out);
+      const int nrows = min(kTcwRows, term_n - row0);
       // SCHED 1: the object's range words for the row -> sample map of a ray-sample or band tile, in the dead A lo image
       const int* segp = reinterpret_cast<const int*>(alo);
       bool compact = false;
       const int nseg = MEGA ? mega_stage_ranges(q, M, o, mode, reinterpret_cast<int*>(alo), tid, compact) : 0;
       epi_bar_sync();      // the previous tile's per-row stages are done with xr / scr and the tile descriptor
       const int r = tile_row();
-      if (tid == 0) { S.t_tile = tile; S.t_o = o; S.t_row0 = row0; S.t_nrows = nrows; S.t_cls = M.class_id; }
+      if (tid == 0) { S.t_seq = seq; S.t_tile = tr.slot; S.t_o = o; S.t_row0 = row0; S.t_nrows = nrows; S.t_cls = M.class_id; }
       float x0 = 0.f, x1 = 0.f, x2 = 0.f, res_in = 0.f, sc = 0.f;
       if (r < nrows) {
         const int rr_ = row0 + r;
         if (pts_mode) {
           const float* pq = grid_mode ? a.grid + 3 * (size_t)rr_ : b.pts + 3 * (size_t)(M.pts_off + rr_);
           if (grid_mode) { x0 = pq[0]; x1 = pq[1]; x2 = pq[2]; }
-          else xform_point(S.ost, pq[0], pq[1], pq[2], x0, x1, x2);
+          else xform_point(S.obj.ost, pq[0], pq[1], pq[2], x0, x1, x2);
           sc = (grid_mode || mask_in == nullptr || ldv(mask_in + M.pts_off + rr_)) ? 1.f : 0.f;
         } else if (mode == MODE_BAND) {
           const size_t sidx = MEGA ? band_row_sample(segp, nseg, M.smp_off, (size_t)kSegRays * b.D, rr_) : (size_t)M.smp_off + rr_;
           x0 = __ldcg(b.band_x + 3 * sidx); x1 = __ldcg(b.band_x + 3 * sidx + 1); x2 = __ldcg(b.band_x + 3 * sidx + 2);
           sc = __ldcg(b.band_s + sidx); res_in = __ldcg(b.band_r + sidx);
         } else {
-          sc = ray_sample_row(b, M, S.ost, S.ost[12], S.ost[13], S.ost[14], segp, compact, rr_, x0, x1, x2);
+          sc = ray_sample_row(b, M, S.obj.ost, S.obj.ost[12], S.obj.ost[13], S.obj.ost[14], segp, compact, rr_, x0, x1, x2);
         }
       }
       if (tid < kTcwRows) { S.xr[r] = x0; S.xr[kTcRows + r] = x1; S.xr[2 * kTcRows + r] = x2; S.scr[r] = sc; S.rin[r] = res_in; }
@@ -290,7 +257,7 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
           const int j = kk + u - L;
-          v[u] = (j < 0) ? S.zs[kk + u] : ((unsigned)j < 3u ? S.xr[j * kTcRows + row] : 0.f);
+          v[u] = (j < 0) ? S.obj.zs[kk + u] : ((unsigned)j < 3u ? S.xr[j * kTcRows + row] : 0.f);
         }
         uint32_t hi, lo;
         split_pack(v[0], v[1], hi, lo);
@@ -308,7 +275,7 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
       const int cls = S.t_cls;
       const TcPlan& plan = S.plans[cls];
       const bool fwd_only = MEGA ? tile_mode() == MODE_RAYFWD : fwd_only0;
-      const int ns = fwd_only ? plan.n_fwd : plan.n_steps;
+      const int ns = tile_steps<MEGA>(plan, tile_mode());
       if (s >= ns) break;
       const DecoderDev& dec = b.decs[cls];
       const TcStep st = plan.step[s];
@@ -381,7 +348,7 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
         // the epi_* passes of tc_body on this warpgroup's columns: bounds and the concat offset relative to c0
         uint32_t mw[4] = {0u, 0u, 0u, 0u};
         epi_fwd_hidden<0, 0>(acc, mw, S.bias + c0, qs, nm - c0, k_next - c0);
-        if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next - c0, st.cat_off - c0, dec.L, S.zs, S.xr, rowA, rowB);
+        if (st.cat_off >= 0) epi_concat_input<0, 0>(acc, qs, k_next - c0, st.cat_off - c0, dec.L, S.obj.zs, S.xr, rowA, rowB);
         if (!fwd_only) mg[st.layer * kTcEpiThreads] = make_uint4(mw[0], mw[1], mw[2], mw[3]);
       } else if (st.kind == TK_BWD_MID) {
         const uint4 m4 = mg[st.mask_layer * kTcEpiThreads];
@@ -399,17 +366,11 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
         epi_bar_sync();
       }
     }
-    if constexpr (MEGA) {
-      if (tile_mode() == MODE_RAYFWD) {
-        // the next sequence number is read before mega_tile_end's barriers: once past them, thread 0 may already have
-        // taken the next item and rewritten S.epi_seq
-        const int next = *reinterpret_cast<volatile int*>(&S.mega.epi_seq);
-        mega_tile_end<true, kTcwRows>(S, q, b.meta[S.t_o], S.t_o, MODE_RAYFWD, S.t_j, tid);
-        tile = next;
-        continue;
-      }
-    } else {
-      if (fwd_only0) { tile = S.t_tile + gridDim.x; continue; }
+    // (the tile descriptor is rewritten after the first barrier of the next tile's prologue)
+    if (MEGA ? tile_mode() == MODE_RAYFWD : fwd_only0) {
+      seq = S.t_seq;
+      if constexpr (MEGA) mega_tile_end<true, kTcwRows>(S, q, b.meta[S.t_o], S.t_o, MODE_RAYFWD, S.t_j, tid);
+      continue;
     }
     // ---- pose columns, residual (thread = row; needs every d/d(input) column of the row) -----------------------------
     epi_bar_sync();
@@ -435,14 +396,9 @@ __device__ __forceinline__ void tcw_body(const BatchDev& b, const TermArgs& a, c
     if (a.dbg_J != nullptr && o == a.dbg_obj && mode == MODE_SDF)
       dbg_dump_J(a, S.Jp, kJpStride, 1, row0, nrows, ost.mode, tid, kTcEpiThreads);
     jtile_sums<kTcwRows>(S.Jp, S.rr, S.rsc, ((MEGA && mode == MODE_BAND) ? a.part_r : a.part) + (size_t)S.t_tile * kAccStride, tid);
-    if constexpr (MEGA) {
-      const int next = *reinterpret_cast<volatile int*>(&S.mega.epi_seq);     // before the barriers, as above
-      mega_tile_end<true, kTcwRows>(S, q, b.meta[o], o, mode, S.t_j, tid);
-      tile = next;
-    } else {
-      // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
-      tile = S.t_tile + gridDim.x;
-    }
+    seq = S.t_seq;
+    // the next tile's prologue starts with epi_bar_sync(): Jp / rr are not rewritten before it
+    if constexpr (MEGA) mega_tile_end<true, kTcwRows>(S, q, b.meta[o], o, mode, S.t_j, tid);
   }
 }
 
