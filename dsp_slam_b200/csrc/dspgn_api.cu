@@ -6,6 +6,7 @@
 #include <cmath>
 #include <string>
 #include <vector>
+#include <memory>
 #include <new>
 #include <algorithm>
 #include <atomic>
@@ -41,37 +42,26 @@ int fail(int code, const std::string& msg) { g_err = msg; return code; }
       return fail(DSPGN_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_));      \
   } while (0)
 
-struct DevBuf {
+// A buffer that only grows, in device memory (DevBuf) or pinned host memory (HostBuf)
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct Buf {
   void* p = nullptr;
   size_t cap = 0;
   int reserve(size_t bytes) {
     if (bytes <= cap) return 0;
-    if (p) cudaFree(p);
+    if (p) Free(p);
     p = nullptr; cap = 0;
     size_t want = bytes + bytes / 4 + 256;
-    if (cudaMalloc(&p, want) != cudaSuccess) { cudaGetLastError(); return -1; }
+    if (Alloc(&p, want) != cudaSuccess) { cudaGetLastError(); return -1; }
     cap = want;
     return 0;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  void release() { if (p) Free(p); p = nullptr; cap = 0; }
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-struct HostBuf {   // pinned staging
-  void* p = nullptr;
-  size_t cap = 0;
-  int reserve(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (p) cudaFreeHost(p);
-    p = nullptr; cap = 0;
-    size_t want = bytes + bytes / 4 + 256;
-    if (cudaMallocHost(&p, want) != cudaSuccess) { cudaGetLastError(); return -1; }
-    cap = want;
-    return 0;
-  }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-  template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
+using DevBuf = Buf<cudaMalloc, cudaFree>;
+using HostBuf = Buf<cudaMallocHost, cudaFreeHost>;   // pinned staging
 
 }  // namespace
 
@@ -159,7 +149,6 @@ struct DspgnSolver {
     HostBuf h_out;
     int bound_n = -1;
   } gather;
-  GatherDev gdev{};                  // exchange arguments of the run being enqueued (slots == nullptr: off)
   // mesh calls (dspgn_mesh_batch): query points and scan workspace of one chunk, the grids of the whole call
   DevBuf d_grid_pts, d_mgrid, d_mws, d_mscan_tmp, d_mout;
   HostBuf h_mbase;
@@ -199,8 +188,6 @@ struct DspgnSolver {
   cudaEvent_t ev_poll = nullptr;     // the waits that poll stop_flag
   int stop_at_obj = -1, stop_at_iter = -1;       // dspgn_debug_stop_at, for the next stoppable call
   int call_stop_obj = -1, call_stop_iter = -1;   // ... taken by the call in flight (caller object index)
-  int run_stop_slot = -1;            // ... the resident slot of that object in the chunk being enqueued (-1: not in it)
-  const int* run_pair = nullptr;     // the chunk's pair partners on the device (meshed calls with pairs), else nullptr
 };
 
 namespace {
@@ -250,8 +237,6 @@ void request_stop(DspgnSolver* s) {
 void stop_end(DspgnSolver* s) {
   s->stop_live.store(0, std::memory_order_release);
   s->call_stop_obj = s->call_stop_iter = -1;
-  s->run_stop_slot = -1;
-  s->run_pair = nullptr;
 }
 
 // The stoppable calls (dspgn_reconstruct_batch, the keyframe calls) hold one for their duration: a generation of their
@@ -310,6 +295,39 @@ cudaError_t settle_event(DspgnSolver* s, cudaEvent_t e) {
   return s->stop_flag ? poll_event(s, e) : cudaEventSynchronize(e);
 }
 
+// ---- a run's counters and timing (dspgn_counters) ------------------------------------------------------------------
+// Every call that enqueues device work of its own (the runs, dspgn_decode_sdf, the mesh calls, the debug system hook)
+// brackets it with run_begin .. run_end: the counters, the timed-launch event pools and ev_run0 / ev_run1 then describe
+// that call.
+int run_begin(DspgnSolver* s) {
+  s->ctr = DspgnCounters{};
+  s->band_rows_pending = false;
+  s->ev_used = 0;
+  s->evs_used = 0;
+  CU(cudaEventRecord(s->ev_run0, s->stream));
+  return 0;
+}
+
+int run_end(DspgnSolver* s) {
+  CU(cudaEventRecord(s->ev_run1, s->stream));
+  return 0;
+}
+
+// The last run's device times, once its events have completed: decoder_ms and solve_ms from the event pairs of the
+// timed launches (dspgn_enable_timing), total_ms from ev_run0 to ev_run1.
+void read_timings(DspgnSolver* s) {
+  float tot = 0.f;
+  if (cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) != cudaSuccess) { cudaGetLastError(); return; }
+  s->ctr.total_ms = tot;
+  auto pairs = [](const std::vector<cudaEvent_t>& ev, size_t used) {
+    float sum = 0.f;
+    for (size_t i = 0; i + 1 < used; i += 2) { float ms = 0.f; cudaEventElapsedTime(&ms, ev[i], ev[i + 1]); sum += ms; }
+    return sum;
+  };
+  s->ctr.decoder_ms = pairs(s->ev, s->ev_used);
+  s->ctr.solve_ms = pairs(s->ev_solve, s->evs_used);
+}
+
 #define BUSY(s)                                                                                              \
   do {                                                                                                       \
     if ((s) && (s)->flight.active)                                                                           \
@@ -353,6 +371,18 @@ int upload_vec(DspgnDecoder* d, const std::vector<float>& h, const float** out) 
   return 0;
 }
 
+// The device of a new decoder or frame handle: present, an sm_90 part, and made current
+int check_device(int device) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPGN_E_NOGPU, "no CUDA device"); }
+  if (device < 0 || device >= ndev) return fail(DSPGN_E_ARG, "bad device index");
+  CU(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CU(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -371,13 +401,7 @@ int dspgn_decoder_create_ex(const DspgnDecoderSpec* spec, const float* const* W,
   for (int k = 0; k < spec->num_linear && k < DSPGN_MAX_LINEAR; ++k)
     if (spec->layer_norm[k] && (!ln_gamma || !ln_beta || !ln_gamma[k] || !ln_beta[k])) return fail(DSPGN_E_ARG, "LayerNorm parameters missing");
   if (int rc = check_spec(*spec)) return rc;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPGN_E_NOGPU, "no CUDA device"); }
-  if (device < 0 || device >= ndev) return fail(DSPGN_E_ARG, "bad device index");
-  CU(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+  if (int rc = check_device(device)) return rc;
   DspgnDecoder* d = new (std::nothrow) DspgnDecoder();
   if (!d) return fail(DSPGN_E_ALLOC, "oom");
   d->device = device;
@@ -458,19 +482,10 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
     // slices code[:code_len]; the reference itself needs code_len == latent size for its decoder input)
   }
   CU(cudaSetDevice(device));
-  DspgnSolver* s = new (std::nothrow) DspgnSolver();
-  if (!s) return fail(DSPGN_E_ALLOC, "oom");
   // every failure below releases the half-built solver (events, streams, device buffers)
-#undef CU
-#define CU(call)                                                                          \
-  do {                                                                                    \
-    cudaError_t e_ = (call);                                                              \
-    if (e_ != cudaSuccess) {                                                              \
-      const int rc_ = fail(DSPGN_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-      dspgn_solver_destroy(s);                                                            \
-      return rc_;                                                                         \
-    }                                                                                     \
-  } while (0)
+  std::unique_ptr<DspgnSolver, decltype(&dspgn_solver_destroy)> owner(new (std::nothrow) DspgnSolver(), dspgn_solver_destroy);
+  DspgnSolver* s = owner.get();
+  if (!s) return fail(DSPGN_E_ALLOC, "oom");
   s->device = device;
   s->cfg = *cfg;
   cudaDeviceProp prop;
@@ -496,7 +511,7 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
         *m = static_cast<const float*>(p);
       }
   }
-  if (s->d_decs.reserve(decs.size() * sizeof(DecoderDev))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
+  if (s->d_decs.reserve(decs.size() * sizeof(DecoderDev))) return fail(DSPGN_E_ALLOC, "cudaMalloc");
   CU(cudaMemcpy(s->d_decs.p, decs.data(), decs.size() * sizeof(DecoderDev), cudaMemcpyHostToDevice));
   bool tc_ok = true;
   for (auto* d : s->classes) tc_ok = tc_ok && d->tc.ok;
@@ -507,47 +522,45 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
     else if (e && !strcmp(e, "tc")) eng = DSPGN_ENGINE_TC;
     else eng = (tc_ok && tc_engine_default()) ? DSPGN_ENGINE_TC : DSPGN_ENGINE_SIMT;
   }
-  if (eng == DSPGN_ENGINE_TC && !tc_ok) { dspgn_solver_destroy(s); return fail(DSPGN_E_ARG, "tensor-core engine unavailable for this decoder shape"); }
+  if (eng == DSPGN_ENGINE_TC && !tc_ok) return fail(DSPGN_E_ARG, "tensor-core engine unavailable for this decoder shape");
   if (eng == DSPGN_ENGINE_TC_WIDE) {
     std::vector<TcwDecDev> wd;
     for (auto* d : s->classes) {
       std::lock_guard<std::mutex> lock(d->tcw_mu);
       if (!d->tcw.ok && !d->tcw_declined) {
-        if (int rc = tcw_pack_decoder(d->dev, d->hid, d->tcw, d->tcw_plan, g_err)) { dspgn_solver_destroy(s); return rc; }
+        if (int rc = tcw_pack_decoder(d->dev, d->hid, d->tcw, d->tcw_plan, g_err)) return rc;
         d->tcw_declined = !d->tcw.ok;
       }
-      if (d->tcw_declined) {
-        dspgn_solver_destroy(s);
+      if (d->tcw_declined)
         return fail(DSPGN_E_ARG, "wide tensor-core engine (DSPGN_ENGINE_TC_WIDE) unavailable for this decoder shape: plain "
                                  "decoders only (no LayerNorm, xyz_in_all, use_tanh or second latent_in layer)");
-      }
       wd.push_back(TcwDecDev{reinterpret_cast<const unsigned char*>(d->tcw.blob), d->tcw_plan});
     }
-    if (s->d_tcw.reserve(wd.size() * sizeof(TcwDecDev))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
+    if (s->d_tcw.reserve(wd.size() * sizeof(TcwDecDev))) return fail(DSPGN_E_ALLOC, "cudaMalloc");
     CU(cudaMemcpy(s->d_tcw.p, wd.data(), wd.size() * sizeof(TcwDecDev), cudaMemcpyHostToDevice));
-    if (int rc = tcw_setup_kernel(g_err)) { dspgn_solver_destroy(s); return rc; }
+    if (int rc = tcw_setup_kernel(g_err)) return rc;
   }
   s->engine = eng;
   if (s->simt_hid == kHid)
     CU(cudaFuncSetAttribute(k_decoder_simt<kHid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHid>)));
   else
     CU(cudaFuncSetAttribute(k_decoder_simt<kHidWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SimtSmem<kHidWide>)));
-  if (int rc = simt_setup_kernels(s->simt_hid, g_err)) { dspgn_solver_destroy(s); return rc; }
+  if (int rc = simt_setup_kernels(s->simt_hid, g_err)) return rc;
   for (auto* d : s->classes)
     if (d->has_ln) {      // LayerNorm decoders: per-CTA scratch for the normalised activations (forward -> backward),
                           // one half for the ray-sample pass, which may run beside the SDF-row pass (launch_terms)
-      if (s->d_ln.reserve(4 * 2 * ln_half_floats(s))) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
+      if (s->d_ln.reserve(4 * 2 * ln_half_floats(s))) return fail(DSPGN_E_ALLOC, "cudaMalloc");
       break;
     }
   static_assert(kTcwMaskLayers <= kTcMaskLayers, "d_masks holds kTcMaskLayers layers per CTA, k_wide_wgmma strides by kTcwMaskLayers");
   if ((eng == DSPGN_ENGINE_TC || eng == DSPGN_ENGINE_TC_WIDE) &&
-      s->d_masks.reserve(sizeof(uint4) * (size_t)s->num_sms * kTcMaskLayers * kTcEpiThreads)) { dspgn_solver_destroy(s); return fail(DSPGN_E_ALLOC, "cudaMalloc"); }
-  if (int rc = tc_setup_kernels(g_err)) { dspgn_solver_destroy(s); return rc; }
+      s->d_masks.reserve(sizeof(uint4) * (size_t)s->num_sms * kTcMaskLayers * kTcEpiThreads)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
+  if (int rc = tc_setup_kernels(g_err)) return rc;
   if (const char* m = getenv("DSPGN_MEGA")) s->mega_enabled = (m[0] != '0');
   if (const char* m = getenv("DSPGN_COMPACT_RAYS")) s->compact_rays = (m[0] != '0');   // A/B switch of the valid-sample hulls
   if (cfg->schedule == DSPGN_SCHED_LAUNCHES) s->mega_enabled = false;
   else if (cfg->schedule == DSPGN_SCHED_PERSISTENT) s->mega_enabled = true;
-  else if (cfg->schedule != DSPGN_SCHED_AUTO) { dspgn_solver_destroy(s); return fail(DSPGN_E_ARG, "bad schedule"); }
+  else if (cfg->schedule != DSPGN_SCHED_AUTO) return fail(DSPGN_E_ARG, "bad schedule");
   s->events_on = getenv("DSPGN_CLK") != nullptr;
   CU(cudaEventCreateWithFlags(&s->ev_upload, cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(&s->ev_run_upload, cudaEventDisableTiming));
@@ -560,14 +573,7 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
   CU(cudaHostAlloc(reinterpret_cast<void**>(&s->h_stop), sizeof(uint32_t), cudaHostAllocMapped));
   *s->h_stop = 0;
   CU(cudaHostGetDevicePointer(reinterpret_cast<void**>(&s->d_stop), s->h_stop, 0));
-#undef CU
-#define CU(call)                                                                          \
-  do {                                                                                    \
-    cudaError_t e_ = (call);                                                              \
-    if (e_ != cudaSuccess)                                                                \
-      return fail(DSPGN_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_));      \
-  } while (0)
-  *out = s;
+  *out = owner.release();
   return 0;
 }
 
@@ -629,16 +635,21 @@ int dspgn_enable_timing(DspgnSolver* s, int on) {
 int dspgn_counters(DspgnSolver* s, DspgnCounters* out) {
   if (!s || !out) return fail(DSPGN_E_ARG, "null argument");
   BUSY(s);
-  // device time of the last run's kernels, if they have finished (events on the solver's stream)
-  float tot = 0.f;
-  if (s->ev_run0 && s->ev_run1 && cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot;
-  else cudaGetLastError();
+  read_timings(s);
   *out = s->ctr;
   return 0;
 }
 
 // ---------------------------------------------------------------------------------------------
 namespace {
+
+// The SDF tiles and ray-sample tiles of one object at `rows` rows per tile.  k_init counts an object's tiles by the
+// same rule on the device, at InitArgs.tile_rows (ntS, ntF_cap): the two must agree, for k_init seeds the iteration-0
+// queue slots that plan_run reserves.
+struct ObjTiles { long long sdf, smp; };
+ObjTiles obj_tiles(const ObjMeta& M, int D, int rows) {
+  return ObjTiles{(M.n_pts + rows - 1) / rows, ((long long)M.n_rays * D + rows - 1) / rows};
+}
 
 // decode_only: forward-only use (dspgn_decode_sdf) -- no J^T J partials, no band buffers.
 // grid_dim > 0 (mesh calls, decode_only): every object's points are the dim^3 query grid, written on the device into a
@@ -699,8 +710,8 @@ int upload_batch_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, bool d
     int* hTBr = hTB + n_obj;
     const int rows = tile_rows(s);
     for (int o = 0; o < n_obj; ++o) {
-      const int nt = (s->h_meta[o].n_pts + rows - 1) / rows;
-      const int ntf = (int)(((long long)s->h_meta[o].n_rays * D + rows - 1) / rows);
+      const ObjTiles t = obj_tiles(s->h_meta[o], D, rows);
+      const int nt = (int)t.sdf, ntf = (int)t.smp;
       hTB[o] = acc; hTBr[o] = (int)(accr + o);
       acc += nt; accr += ntf;
       if (nt > mx) mx = nt;
@@ -853,9 +864,18 @@ RunTable run_table(void* base, int n, bool gated) {
   return RunTable{p, p + n, gated ? p + 2 * n : nullptr, gated ? reinterpret_cast<float*>(p + 3 * n) : nullptr};
 }
 
+// What the caller of a run passes its kernels besides the resident batch: the multi-GPU exchange slots
+// (dspgn_run_batch_gather) and, for a chunk of a stoppable call, the chunk's slot of the call's stop hook and the pair
+// partners of its slots on the device (meshed calls with pairs).
+struct RunArgs {
+  GatherDev gather{};                // slots == nullptr: no exchange
+  int stop_slot = -1;                // resident slot of call_stop_obj (-1: not in this chunk)
+  const int* pair = nullptr;
+};
+
 // The resident batch and its run table as the kernels see them.  Call after plan_run (it may move d_run) and after
 // every buffer reservation of the run.
-BatchDev batch_dev(DspgnSolver* s) {
+BatchDev batch_dev(DspgnSolver* s, const RunArgs& r) {
   BatchDev b{};
   b.meta = s->d_meta; b.state = s->d_state.as<ObjState>(); b.decs = s->d_decs.as<DecoderDev>();
   b.n_obj = s->n_obj; b.n_classes = (int)s->classes.size(); b.D = s->cfg.num_depth_samples;
@@ -863,12 +883,12 @@ BatchDev batch_dev(DspgnSolver* s) {
   b.sdf = s->d_sdf.as<float>(); b.band_x = s->d_bx.as<float>(); b.band_s = s->d_bs.as<float>(); b.band_r = s->d_br.as<float>();
   b.band_m = s->d_m.as<int>(); b.V_count = s->d_V.as<int>();
   b.results = s->d_results.as<float>();
-  b.gather = s->gdev;
+  b.gather = r.gather;
   const RunTable t = run_table(s->d_run.p, s->n_obj, s->run_table_gated);
   b.modes = t.modes; b.q0_off = t.q0_off; b.link = t.link; b.t_map = t.t_map;
   // only the runs of a stoppable call can stop, and never those of the multi-GPU exchange
-  const bool stoppable = s->stop_live.load(std::memory_order_relaxed) != 0 && s->gdev.slots == nullptr;
-  b.stop = stoppable ? StopDev{s->d_stop, s->stop_gen, s->run_stop_slot, s->call_stop_iter, s->run_pair}
+  const bool stoppable = s->stop_live.load(std::memory_order_relaxed) != 0 && r.gather.slots == nullptr;
+  b.stop = stoppable ? StopDev{s->d_stop, s->stop_gen, r.stop_slot, s->call_stop_iter, r.pair}
                      : StopDev{nullptr, 0u, -1, -1, nullptr};
   return b;
 }
@@ -920,7 +940,7 @@ int plan_run(DspgnSolver* s, const int32_t* modes, RunPlan& p, bool unlimited = 
     const int m = modes[o];
     const bool dormant = link && link[o] >= 0 && m == DSPGN_MODE_JOINT;
     const bool r = p.render && m == DSPGN_MODE_JOINT;
-    const long long ntS = (M.n_pts + rows - 1) / rows, ntF = ((long long)M.n_rays * D + rows - 1) / rows;
+    const auto [ntS, ntF] = obj_tiles(M, D, rows);
     if (!dormant) {
       p.pts[m] += M.n_pts;
       if (m == DSPGN_MODE_JOINT) p.smp_joint += (long long)M.n_rays * D;
@@ -1015,6 +1035,30 @@ SolveArgs base_solve(DspgnSolver* s) {
   return v;
 }
 
+// The solve of GN iteration v.iter_index (per-iteration schedule), timed in ev_solve when timing is on
+int launch_solve(DspgnSolver* s, const BatchDev& b, const SolveArgs& v) {
+  if (s->timing) {
+    if (s->evs_used + 2 > s->ev_solve.size()) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); s->ev_solve.push_back(e0); s->ev_solve.push_back(e1); }
+    cudaEventRecord(s->ev_solve[s->evs_used], s->stream);
+  }
+  k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(b, v);
+  if (s->timing) { cudaEventRecord(s->ev_solve[s->evs_used + 1], s->stream); s->evs_used += 2; }
+  s->ctr.kernel_launches++;
+  CU(cudaGetLastError());
+  return 0;
+}
+
+// GN iterations 0 .. n_iters - 1 of plan p on the per-iteration schedule: each one's terms, then its solve
+int gn_iterations(DspgnSolver* s, const BatchDev& b, const RunPlan& p, int n_iters) {
+  for (int e = 0; e < n_iters; ++e) {
+    if (int rc = launch_terms(s, b, p, e)) return rc;
+    SolveArgs v = base_solve(s);
+    v.iter_index = e;
+    if (int rc = launch_solve(s, b, v)) return rc;
+  }
+  return 0;
+}
+
 // The persistent kernel's work queue for the run: reserves its buffers and builds its MegaArgs (k_init seeds it, the
 // kernel runs on it).
 int mega_args(DspgnSolver* s, const RunPlan& p, MegaArgs& q) {
@@ -1053,19 +1097,15 @@ namespace {
 // phase after a readback of the verdicts, or (device_wake, a submitted call) as a second phase enqueued for every gated
 // slot: k_gate_wake reads the verdicts itself and the slots it does not wake have n_iter 0, so they contribute no rows
 // (term_rows) and k_solve skips them -- the same records.  Their rows are counted when the records come back.
-int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = nullptr, const float* t_map = nullptr,
-                   bool device_wake = false) {
+int run_batch_impl(DspgnSolver* s, const int32_t* modes, const RunArgs& ra, const int32_t* link = nullptr,
+                   const float* t_map = nullptr, bool device_wake = false) {
   CU(cudaSetDevice(s->device));
   RunPlan p;
   if (int rc = plan_run(s, modes, p, false, link, t_map)) return rc;
-  const BatchDev b = batch_dev(s);
+  const BatchDev b = batch_dev(s, ra);
   const int max_iters = std::max(p.any[DSPGN_MODE_JOINT] ? p.iters[DSPGN_MODE_JOINT] : 0,
                                  p.any[DSPGN_MODE_POSE] ? p.iters[DSPGN_MODE_POSE] : 0);
-  s->ctr = DspgnCounters{};
-  s->band_rows_pending = false;
-  s->ev_used = 0;
-  s->evs_used = 0;
-  CU(cudaEventRecord(s->ev_run0, s->stream));
+  if (int rc = run_begin(s)) return rc;
   const bool render = p.render;
   const bool wide = s->engine == DSPGN_ENGINE_TC_WIDE, simt = s->engine == DSPGN_ENGINE_SIMT;
   const bool mega = s->mega_enabled && s->total_tiles > 0 &&
@@ -1098,27 +1138,10 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     s->band_rows_pending = render;           // band rows and valid ray samples are counted by the kernel (dspgn_results)
     s->mega_ran = true;
     CU(cudaGetLastError());
-    CU(cudaEventRecord(s->ev_run1, s->stream));
-    return 0;
+    return run_end(s);
   }
   if (int rc = launch_init(s, b, p)) return rc;
-  auto iterate = [&](const RunPlan& pl, int n_iters) -> int {
-    for (int e = 0; e < n_iters; ++e) {
-      if (int rc = launch_terms(s, b, pl, e)) return rc;
-      SolveArgs v = base_solve(s);
-      v.iter_index = e;
-      if (s->timing) {
-        if (s->evs_used + 2 > s->ev_solve.size()) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); s->ev_solve.push_back(e0); s->ev_solve.push_back(e1); }
-        cudaEventRecord(s->ev_solve[s->evs_used], s->stream);
-      }
-      k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(b, v);
-      if (s->timing) { cudaEventRecord(s->ev_solve[s->evs_used + 1], s->stream); s->evs_used += 2; }
-      s->ctr.kernel_launches++;
-      CU(cudaGetLastError());
-    }
-    return 0;
-  };
-  if (int rc = iterate(p, max_iters)) return rc;
+  if (int rc = gn_iterations(s, b, p, max_iters)) return rc;
   if (p.any_dormant && device_wake) {
     RunPlan pb = p;
     pb.any[DSPGN_MODE_POSE] = false; pb.any[DSPGN_MODE_JOINT] = true;
@@ -1126,7 +1149,7 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
     k_gate_wake<<<(s->n_obj + 127) / 128, 128, 0, s->stream>>>(b, p.iters[DSPGN_MODE_JOINT]);
     s->ctr.kernel_launches++;
     CU(cudaGetLastError());
-    if (int rc = iterate(pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
+    if (int rc = gn_iterations(s, b, pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
   } else if (p.any_dormant) {
     // second phase: the verdicts of the first (record gate words) decide which joint slots run
     const int n = s->n_obj;
@@ -1147,20 +1170,19 @@ int run_batch_impl(DspgnSolver* s, const int32_t* modes, const int32_t* link = n
       k_gate_wake<<<(n + 127) / 128, 128, 0, s->stream>>>(b, p.iters[DSPGN_MODE_JOINT]);
       s->ctr.kernel_launches++;
       CU(cudaGetLastError());
-      if (int rc = iterate(pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
+      if (int rc = gn_iterations(s, b, pb, pb.iters[DSPGN_MODE_JOINT])) return rc;
     }
   }
-  CU(cudaEventRecord(s->ev_run1, s->stream));
-  return 0;
+  return run_end(s);
 }
 
-// dspgn_run_batch / dspgn_run_batch_gather: every object in `mode`
-int run_uniform(DspgnSolver* s, int mode) {
+// dspgn_run_batch / dspgn_run_batch_gather / the whole-batch calls: every object in `mode`
+int run_uniform(DspgnSolver* s, int mode, const RunArgs& ra) {
   if (!s) return fail(DSPGN_E_ARG, "null solver");
   if (s->n_obj < 1) return fail(DSPGN_E_ARG, "no batch uploaded");
   if (mode != DSPGN_MODE_JOINT && mode != DSPGN_MODE_POSE) return fail(DSPGN_E_ARG, "mode must be 0 or 1");
   const std::vector<int32_t> modes(s->n_obj, mode);
-  return run_batch_impl(s, modes.data());
+  return run_batch_impl(s, modes.data(), ra);
 }
 
 // call-level misuse of the per-object entry points: modes outside {0, 1}; a pose-only object without a code or with
@@ -1204,8 +1226,7 @@ int gather_layout(DspgnSolver* s, int n_slots, int world, int rank) {
 
 int dspgn_run_batch(DspgnSolver* s, int mode) {
   BUSY(s);
-  if (s) s->gdev = GatherDev{};
-  return run_uniform(s, mode);
+  return run_uniform(s, mode, RunArgs{});
 }
 
 int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes) {
@@ -1213,8 +1234,7 @@ int dspgn_run_batch_modes(DspgnSolver* s, const int32_t* modes) {
   BUSY(s);
   if (s->n_obj < 1) return fail(DSPGN_E_ARG, "no batch uploaded");
   if (int rc = check_modes(s, modes, s->n_obj, nullptr)) return rc;
-  s->gdev = GatherDev{};
-  return run_batch_impl(s, modes);
+  return run_batch_impl(s, modes, RunArgs{});
 }
 
 // ---- multi-GPU result exchange ----------------------------------------------------------------------------------
@@ -1269,7 +1289,6 @@ void dspgn_gather_close(DspgnSolver* s) {
   }
   G.base = nullptr; G.active = false; G.owner = false; G.bound_n = -1;
   G.d_slot_of.release(); G.d_local.release(); G.h_out.release();
-  s->gdev = GatherDev{};
 }
 
 int dspgn_gather_bind(DspgnSolver* s, const int32_t* slots, int n) {
@@ -1297,12 +1316,8 @@ int dspgn_run_batch_gather(DspgnSolver* s, int mode, int seq) {
   if (!G.active || G.bound_n < 0) return fail(DSPGN_E_ARG, "gather not bound for the resident batch");
   CU(cudaSetDevice(s->device));
   const GatherDev g = gather_dev(s, seq);
-  if (G.bound_n > 0) {
-    s->gdev = g;
-    const int rc = run_uniform(s, mode);
-    s->gdev = GatherDev{};
-    if (rc) return rc;
-  }
+  if (G.bound_n > 0)
+    if (int rc = run_uniform(s, mode, RunArgs{g})) return rc;
   k_gather_publish<<<1, 32, 0, s->stream>>>(g, G.bound_n == 0 ? 1 : 0);
   if (G.rank == 0) k_gather_wait<<<1, 32 * ((G.world + 31) / 32), 0, s->stream>>>(g);
   s->ctr.kernel_launches += (G.rank == 0) ? 2 : 1;
@@ -1370,27 +1385,16 @@ const float* dspgn_results_device(DspgnSolver* s) {
 
 namespace {
 // The host side of a run's end, once its records and (persistent kernel) queue counters hq are on the host: the kernel's
-// row totals and abort flag, and the timings.
+// row totals and abort flag.
 int collect_run(DspgnSolver* s, const QueueCounters* hq) {
-  if (hq) {
-    s->mega_ran = false;
-    if (s->band_rows_pending) {              // roofline accounting: what the reference decodes (loss.py:77-78, :143-144)
-      s->ctr.rows_fwd_bwd += hq->band_rows_total;                 // band rows of all iterations
-      s->ctr.rows_fwd_only += (long long)hq->valid_rows_total;    // V: ray samples inside the unit sphere, all iterations
-    }
-    s->band_rows_pending = false;
-    if (hq->abort_flag) return fail(DSPGN_E_CUDA, "persistent kernel: a work-queue wait timed out (aborted softly; results incomplete)");
+  if (!hq) return 0;
+  s->mega_ran = false;
+  if (s->band_rows_pending) {                // roofline accounting: what the reference decodes (loss.py:77-78, :143-144)
+    s->ctr.rows_fwd_bwd += hq->band_rows_total;                 // band rows of all iterations
+    s->ctr.rows_fwd_only += (long long)hq->valid_rows_total;    // V: ray samples inside the unit sphere, all iterations
   }
-  if (s->timing) {
-    float dec = 0.f;
-    for (size_t i = 0; i + 1 < s->ev_used; i += 2) { float ms = 0.f; cudaEventElapsedTime(&ms, s->ev[i], s->ev[i + 1]); dec += ms; }
-    s->ctr.decoder_ms = dec;
-    float sv = 0.f;
-    for (size_t i = 0; i + 1 < s->evs_used; i += 2) { float ms = 0.f; cudaEventElapsedTime(&ms, s->ev_solve[i], s->ev_solve[i + 1]); sv += ms; }
-    s->ctr.solve_ms = sv;
-  }
-  float tot = 0.f;
-  if (cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot; else cudaGetLastError();
+  s->band_rows_pending = false;
+  if (hq->abort_flag) return fail(DSPGN_E_CUDA, "persistent kernel: a work-queue wait timed out (aborted softly; results incomplete)");
   return 0;
 }
 
@@ -1425,21 +1429,30 @@ int dspgn_results(DspgnSolver* s, DspgnObjectOut* out) {
   return collect_run(s, mega ? &hq : nullptr);
 }
 
+namespace {
+// dspgn_reconstruct_batch / dspgn_estimate_pose_batch: any number of objects in `mode`, as resident batches of at most
+// kMaxObjScan one after the other, each collected before the next.  `stoppable`: the call holds a StopScope; each
+// batch takes the stop hook's object if it has it, and a stopped object's rows come off the counters.
+int whole_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out, int mode, bool stoppable) {
+  for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
+    const int n = std::min(kMaxObjScan, n_obj - o0);
+    if (int rc = upload_batch_impl(s, n, in + o0, false)) return rc;
+    RunArgs ra;
+    if (stoppable && s->call_stop_obj >= o0 && s->call_stop_obj < o0 + n) ra.stop_slot = s->call_stop_obj - o0;
+    if (int rc = run_uniform(s, mode, ra)) return rc;
+    const bool mega = s->mega_ran;
+    if (int rc = dspgn_results(s, out + o0)) return rc;
+    if (stoppable) uncount_stopped(s, out + o0, n, n, mega, false);
+  }
+  return 0;
+}
+}  // namespace
+
 int dspgn_reconstruct_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out) {
   if (!s || !in || !out || n_obj < 1) return fail(DSPGN_E_ARG, "bad argument");
   BUSY(s);
   StopScope stop(s);
-  // any number of objects: resident batches of at most kMaxObjScan, one after the other
-  for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
-    const int n = std::min(kMaxObjScan, n_obj - o0);
-    if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
-    s->run_stop_slot = (s->call_stop_obj >= o0 && s->call_stop_obj < o0 + n) ? s->call_stop_obj - o0 : -1;
-    if (int rc = dspgn_run_batch(s, 0)) return rc;
-    const bool mega = s->mega_ran;
-    if (int rc = dspgn_results(s, out + o0)) return rc;
-    uncount_stopped(s, out + o0, n, n, mega, false);
-  }
-  return 0;
+  return whole_batch(s, n_obj, in, out, DSPGN_MODE_JOINT, true);
 }
 
 int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out) {
@@ -1447,13 +1460,7 @@ int dspgn_estimate_pose_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in
   BUSY(s);
   for (int o = 0; o < n_obj; ++o)
     if (!in[o].code || !(in[o].scale > 0.f)) return fail(DSPGN_E_ARG, "estimate_pose needs a code and a positive scale per object");
-  for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
-    const int n = std::min(kMaxObjScan, n_obj - o0);
-    if (int rc = dspgn_upload_batch(s, n, in + o0)) return rc;
-    if (int rc = dspgn_run_batch(s, 1)) return rc;
-    if (int rc = dspgn_results(s, out + o0)) return rc;
-  }
-  return 0;
+  return whole_batch(s, n_obj, in, out, DSPGN_MODE_POSE, false);
 }
 
 namespace {
@@ -1547,7 +1554,6 @@ int kf_grids(DspgnSolver* s, const KfWalk& w) {
 // gc: grids of the chunk; grid_of[o]: the call-wide grid of each candidate object.
 int kf_enqueue_chunk(DspgnSolver* s, const KfWalk& w, size_t u0, int n, int slots, int g0, bool device_wake,
                      std::vector<int32_t>& link, int& gc, std::vector<int32_t>& grid_of) {
-  s->gdev = GatherDev{};
   std::vector<DspgnObjectIn> ins;
   std::vector<int32_t> cm;
   for (int k = 0; k < n; ++k) { ins.push_back(w.in[w.order[u0 + k]]); cm.push_back(w.modes[w.order[u0 + k]]); }
@@ -1590,23 +1596,23 @@ int kf_enqueue_chunk(DspgnSolver* s, const KfWalk& w, size_t u0, int n, int slot
     d_sel = s->d_mesh_sel.as<int>();
     CU(cudaMemcpyAsync(d_sel, sel, sel_bytes, cudaMemcpyHostToDevice, s->stream));
   }
-  s->run_pair = (d_sel != nullptr && w.pair != nullptr) ? d_sel + slots : nullptr;
-  s->run_stop_slot = -1;
+  RunArgs ra;
+  ra.pair = (d_sel != nullptr && w.pair != nullptr) ? d_sel + slots : nullptr;
   for (int k = 0; k < n; ++k)
-    if (w.order[u0 + k] == s->call_stop_obj) s->run_stop_slot = k;
+    if (w.order[u0 + k] == s->call_stop_obj) ra.stop_slot = k;
   if (slots == n) {                                  // no gate in the chunk: the plain keyframe run
     if (int rc = dspgn_upload_batch(s, n, ins.data())) return rc;
-    if (int rc = run_batch_impl(s, cm.data())) return rc;
+    if (int rc = run_batch_impl(s, cm.data(), ra)) return rc;
   } else {
     if (int rc = dspgn_upload_batch(s, slots, ins.data())) return rc;
-    if (int rc = run_batch_impl(s, cm.data(), link.data(), t_map.data(), device_wake)) return rc;
+    if (int rc = run_batch_impl(s, cm.data(), ra, link.data(), t_map.data(), device_wake)) return rc;
   }
   if (!w.mesh) return 0;
   if (u0 == 0) {                                     // the call-wide query grid of create_voxel_grid
     k_mesh_grid_points<<<(unsigned)((w.R + 255) / 256), 256, 0, s->stream>>>(s->d_grid_pts.as<float>(), 1, w.dim);
     s->ctr.kernel_launches++;
   }
-  BatchDev b = batch_dev(s);
+  BatchDev b = batch_dev(s, ra);
   k_mesh_select<<<slots, 128, 0, s->stream>>>(b, d_sel, d_sel + slots);
   s->ctr.kernel_launches++;
   CU(cudaGetLastError());
@@ -1912,6 +1918,21 @@ int dspgn_debug_sm_budget(DspgnSolver* s, int n, int32_t* current) {
   return 0;
 }
 
+namespace {
+// The forward decode of the `rows` points of a resident batch uploaded decode_only, into sdf
+int decode_points(DspgnSolver* s, float* sdf, long long rows) {
+  const std::vector<int32_t> joint(s->n_obj, DSPGN_MODE_JOINT);
+  RunPlan p;
+  if (int rc = plan_run(s, joint.data(), p)) return rc;
+  BatchDev b = batch_dev(s, RunArgs{});
+  b.sdf = sdf;
+  if (int rc = launch_init(s, b, p)) return rc;
+  if (int rc = launch_term(s, b, base_term(s, MODE_PTSFWD), rows)) return rc;
+  s->ctr.rows_fwd_only += rows;
+  return 0;
+}
+}  // namespace
+
 int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const float* x, int n, int x_rs, int x_cs,
                      float* sdf_out) {
   if (!s || !code || !x || !sdf_out || n < 1) return fail(DSPGN_E_ARG, "bad argument");
@@ -1924,16 +1945,9 @@ int dspgn_decode_sdf(DspgnSolver* s, int class_id, const float* code, const floa
   in.code = code; in.scale = 1.f; in.class_id = class_id;
   if (int rc = upload_batch_impl(s, 1, &in, true)) return rc;      // forward only: no J^T J partial / band buffers
   if (s->d_sdf.reserve(4 * (size_t)n)) return fail(DSPGN_E_ALLOC, "cudaMalloc");
-  s->ctr = DspgnCounters{};
-  s->ev_used = 0;
-  s->gdev = GatherDev{};
-  const int32_t joint = DSPGN_MODE_JOINT;
-  RunPlan p;
-  if (int rc = plan_run(s, &joint, p)) return rc;
-  const BatchDev b = batch_dev(s);
-  if (int rc = launch_init(s, b, p)) return rc;
-  if (int rc = launch_term(s, b, base_term(s, MODE_PTSFWD), n)) return rc;
-  s->ctr.rows_fwd_only += n;
+  if (int rc = run_begin(s)) return rc;
+  if (int rc = decode_points(s, s->d_sdf.as<float>(), n)) return rc;
+  if (int rc = run_end(s)) return rc;
   CU(cudaMemcpyAsync(sdf_out, s->d_sdf.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, s->stream));
   CU(sync_stream(s));
   return 0;
@@ -2033,14 +2047,10 @@ int mesh_impl(DspgnSolver* s, int n, int dim, const float* codes, int code_strid
   s->mesh_v.clear(); s->mesh_f.clear(); s->mesh_grid_of.clear();
   if (s->d_mgrid.cap < 4 * (size_t)n * R) CU(settle_stream(s));
   if (s->d_mgrid.reserve(4 * (size_t)n * R)) return fail(DSPGN_E_ALLOC, "grid allocation failed");
-  s->ctr = DspgnCounters{};
-  s->ev_used = 0;
-  s->gdev = GatherDev{};
-  CU(cudaEventRecord(s->ev_run0, s->stream));
+  if (int rc = run_begin(s)) return rc;
   if (sdf_in) CU(cudaMemcpyAsync(s->d_mgrid.p, sdf_in, 4 * (size_t)n * R, cudaMemcpyHostToDevice, s->stream));
   const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   std::vector<DspgnObjectIn> ins;
-  const std::vector<int32_t> joint(per_chunk, DSPGN_MODE_JOINT);
   for (int o0 = 0; o0 < n; o0 += per_chunk) {
     const int nc = std::min(per_chunk, n - o0);
     float* grid = s->d_mgrid.as<float>() + (size_t)o0 * R;
@@ -2053,26 +2063,13 @@ int mesh_impl(DspgnSolver* s, int n, int dim, const float* codes, int code_strid
         I.code = codes + (size_t)(o0 + k) * code_stride; I.scale = 1.f; I.class_id = class_ids ? class_ids[o0 + k] : 0;
       }
       if (int rc = upload_batch_impl(s, nc, ins.data(), true, dim)) return rc;
-      RunPlan p;
-      if (int rc = plan_run(s, joint.data(), p)) return rc;
-      BatchDev b = batch_dev(s);
-      b.sdf = grid;
-      if (int rc = launch_init(s, b, p)) return rc;
-      if (int rc = launch_term(s, b, base_term(s, MODE_PTSFWD), (long long)nc * R)) return rc;
-      s->ctr.rows_fwd_only += (long long)nc * R;
+      if (int rc = decode_points(s, grid, (long long)nc * R)) return rc;
     }
     const MeshGrid g{grid, nc, dim, R, C, 2.0 / (dim - 1)};
     if (int rc = mesh_chunk(s, g, n_vertices + o0, n_faces + o0)) return rc;
   }
-  CU(cudaEventRecord(s->ev_run1, s->stream));
+  if (int rc = run_end(s)) return rc;
   CU(sync_stream(s));
-  if (s->timing) {
-    float dec = 0.f;
-    for (size_t i = 0; i + 1 < s->ev_used; i += 2) { float ms = 0.f; cudaEventElapsedTime(&ms, s->ev[i], s->ev[i + 1]); dec += ms; }
-    s->ctr.decoder_ms = dec;
-  }
-  float tot = 0.f;
-  if (cudaEventElapsedTime(&tot, s->ev_run0, s->ev_run1) == cudaSuccess) s->ctr.total_ms = tot; else cudaGetLastError();
   s->mesh_n = n; s->mesh_dim = dim;
   return 0;
 }
@@ -2136,19 +2133,10 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
   if (dJ.reserve(4 * ((size_t)npts * P + npts))) return fail(DSPGN_E_ALLOC, "cudaMalloc");
   float* dJp = dJ.as<float>();
   float* dres = dJp + (size_t)npts * P;
-  s->ctr = DspgnCounters{};
-  s->ev_used = 0;
-  s->gdev = GatherDev{};
-  const BatchDev bd = batch_dev(s);
-  int rc = launch_init(s, bd, p);
-  for (int e = 0; e < iter && !rc; ++e) {            // advance the whole batch `iter` GN iterations (per-iteration schedule)
-    rc = launch_terms(s, bd, p, e);
-    if (rc) break;
-    SolveArgs v = base_solve(s);
-    v.iter_index = e;
-    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(bd, v);
-    if (cudaGetLastError() != cudaSuccess) rc = fail(DSPGN_E_CUDA, "k_solve launch failed");
-  }
+  const BatchDev bd = batch_dev(s, RunArgs{});
+  int rc = run_begin(s);
+  if (!rc) rc = launch_init(s, bd, p);
+  if (!rc) rc = gn_iterations(s, bd, p, iter);       // advance the whole batch `iter` GN iterations (per-iteration schedule)
   if (!rc) rc = launch_terms(s, bd, p, iter, dJp, dres, obj, P);
   if (!rc) {
     SolveArgs v = base_solve(s);
@@ -2156,8 +2144,8 @@ int dspgn_debug_system_iter(DspgnSolver* s, int obj, int mode, int iter, float* 
     v.dbg_obj = obj; v.dbg_H = d; v.dbg_b = d + kPMax * kPMax; v.dbg_dx = v.dbg_b + kPMax; v.dbg_loss = v.dbg_dx + kPMax;
     v.iter_index = iter;
     cudaMemsetAsync(d, 0, 4 * ((size_t)kPMax * kPMax + 2 * kPMax + 8), s->stream);
-    k_solve<<<s->n_obj, kSolveThreads, 0, s->stream>>>(bd, v);
-    if (cudaGetLastError() != cudaSuccess) rc = fail(DSPGN_E_CUDA, "k_solve launch failed");
+    rc = launch_solve(s, bd, v);
+    if (!rc) rc = run_end(s);
     if (!rc) {
       cudaMemcpyAsync(H, v.dbg_H, 4 * (size_t)P * P, cudaMemcpyDeviceToHost, s->stream);
       cudaMemcpyAsync(b, v.dbg_b, 4 * (size_t)P, cudaMemcpyDeviceToHost, s->stream);
@@ -2241,20 +2229,17 @@ int dspgn_debug_stall_probe(int device, unsigned long long* out, int reset) {
 
 }  // extern "C"
 
-// ---- LiDAR keyframe detections (dspgn_frame.cuh) ----
+// ---- frame handles: what DspgnLidarFrame and DspgnMonoFrame share ----
 
-struct DspgnLidarFrame {
+namespace {
+
+struct FrameCore {
   int device = 0;
-  DspgnLidarSpec spec{};
   cudaStream_t stream = nullptr;
   cudaStream_t own = nullptr;  // the handle's non-blocking stream (the default), so LocalMapping's work never orders it
   HostBuf h_in, h_out;        // pinned: staged inputs, downloaded outputs
   DevBuf d_in, d_work, d_out;
-  int n_boxes = 0;            // of the last run
-  std::vector<DspgnLidarBoxOut> last;
 };
-
-namespace {
 
 size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
@@ -2269,6 +2254,72 @@ int frame_stream(cudaStream_t* out) {
   }
   return 0;
 }
+
+// A new handle on its own stream, counted as a live frame of the device (grid_sms) until frame_destroy
+template <class F, class Spec>
+int frame_create(const Spec& spec, int device, F** out) {
+  if (int rc = check_device(device)) return rc;
+  F* f = new (std::nothrow) F();
+  if (!f) return fail(DSPGN_E_ALLOC, "oom");
+  f->device = device;
+  f->spec = spec;
+  if (int rc = frame_stream(&f->own)) {
+    delete f;
+    return rc;
+  }
+  f->stream = f->own;
+  count_frame(device, 1);
+  *out = f;
+  return 0;
+}
+
+template <class F>
+void frame_destroy(F* f) {
+  if (!f) return;
+  cudaSetDevice(f->device);
+  cudaStreamSynchronize(f->stream);
+  f->h_in.release(); f->h_out.release();
+  f->d_in.release(); f->d_work.release(); f->d_out.release();
+  if (f->own) cudaStreamDestroy(f->own);
+  count_frame(f->device, -1);
+  delete f;
+}
+
+int frame_set_stream(FrameCore* f, void* cuda_stream) {
+  if (!f) return fail(DSPGN_E_ARG, "null frame");
+  f->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+  return 0;
+}
+
+// every mask's box (l, t, r, b) inside the image
+int check_bboxes(const int32_t* bboxes, int n_masks, int img_w, int img_h) {
+  for (int m = 0; m < n_masks; ++m) {
+    const int32_t* bb = bboxes + 4 * m;
+    if (!(0 <= bb[0] && bb[0] <= bb[2] && bb[2] <= img_w && 0 <= bb[1] && bb[1] <= bb[3] && bb[3] <= img_h))
+      return fail(DSPGN_E_ARG, "bbox " + std::to_string(m) + " outside 0 <= l <= r <= img_w, 0 <= t <= b <= img_h");
+  }
+  return 0;
+}
+
+// the masks of img_h x img_w bytes each into the staging block at dst, each padded with zeros to mstride bytes
+void stage_masks(unsigned char* dst, const uint8_t* masks, int n_masks, size_t hw, size_t mstride) {
+  for (int m = 0; m < n_masks; ++m) {
+    memcpy(dst + m * mstride, masks + m * hw, hw);
+    memset(dst + m * mstride + hw, 0, mstride - hw);
+  }
+}
+
+}  // namespace
+
+// ---- LiDAR keyframe detections (dspgn_frame.cuh) ----
+
+struct DspgnLidarFrame : FrameCore {
+  DspgnLidarSpec spec{};
+  int n_boxes = 0;            // of the last run
+  std::vector<DspgnLidarBoxOut> last;
+};
+
+namespace {
 
 // the output block of a run: header, points [box][num_max][3], rays [box][num_max + 200][3]
 struct FrameOutLayout {
@@ -2290,43 +2341,12 @@ int dspgn_lidar_frame_create(const DspgnLidarSpec* spec, int device, DspgnLidarF
   if (spec->img_h < 1 || spec->img_h > 4096 || spec->img_w < 1 || spec->img_w > 4096) return fail(DSPGN_E_ARG, "image size must be in [1,4096]^2");
   if (spec->num_lidar_max < 1 || spec->num_lidar_max > kFrameMaxLidar) return fail(DSPGN_E_ARG, "num_lidar_max must be in [1,4096]");
   if (spec->downsample_ratio < 1) return fail(DSPGN_E_ARG, "downsample_ratio must be >= 1");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPGN_E_NOGPU, "no CUDA device"); }
-  if (device < 0 || device >= ndev) return fail(DSPGN_E_ARG, "bad device index");
-  CU(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only");
-  DspgnLidarFrame* f = new (std::nothrow) DspgnLidarFrame();
-  if (!f) return fail(DSPGN_E_ALLOC, "oom");
-  f->device = device;
-  f->spec = *spec;
-  if (int rc = frame_stream(&f->own)) {
-    delete f;
-    return rc;
-  }
-  f->stream = f->own;
-  count_frame(device, 1);
-  *out = f;
-  return 0;
+  return frame_create(*spec, device, out);
 }
 
-void dspgn_lidar_frame_destroy(DspgnLidarFrame* f) {
-  if (!f) return;
-  cudaSetDevice(f->device);
-  cudaStreamSynchronize(f->stream);
-  f->h_in.release(); f->h_out.release();
-  f->d_in.release(); f->d_work.release(); f->d_out.release();
-  if (f->own) cudaStreamDestroy(f->own);
-  count_frame(f->device, -1);
-  delete f;
-}
+void dspgn_lidar_frame_destroy(DspgnLidarFrame* f) { frame_destroy(f); }
 
-int dspgn_lidar_frame_set_stream(DspgnLidarFrame* f, void* cuda_stream) {
-  if (!f) return fail(DSPGN_E_ARG, "null frame");
-  f->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  return 0;
-}
+int dspgn_lidar_frame_set_stream(DspgnLidarFrame* f, void* cuda_stream) { return frame_set_stream(f, cuda_stream); }
 
 int dspgn_lidar_frame_run(DspgnLidarFrame* f, const float* scan, int n_points, const DspgnLidarBox* boxes, int n_boxes,
                           const uint8_t* masks, const int32_t* bboxes, int n_masks, DspgnLidarBoxOut* out) {
@@ -2337,11 +2357,7 @@ int dspgn_lidar_frame_run(DspgnLidarFrame* f, const float* scan, int n_points, c
   if (n_masks < 0 || n_masks > kFrameMaxMasks) return fail(DSPGN_E_ARG, "n_masks must be in [0, 64]");
   if ((n_points > 0 && !scan) || (n_boxes > 0 && (!boxes || !out)) || (n_masks > 0 && (!masks || !bboxes)))
     return fail(DSPGN_E_ARG, "null pointer where data is required");
-  for (int m = 0; m < n_masks; ++m) {
-    const int32_t* bb = bboxes + 4 * m;
-    if (!(0 <= bb[0] && bb[0] <= bb[2] && bb[2] <= sp.img_w && 0 <= bb[1] && bb[1] <= bb[3] && bb[3] <= sp.img_h))
-      return fail(DSPGN_E_ARG, "bbox " + std::to_string(m) + " outside 0 <= l <= r <= img_w, 0 <= t <= b <= img_h");
-  }
+  if (int rc = check_bboxes(bboxes, n_masks, sp.img_w, sp.img_h)) return rc;
   CU(cudaSetDevice(f->device));
   f->n_boxes = n_boxes;
   f->last.assign(n_boxes, DspgnLidarBoxOut{0, -1, -1, 0});
@@ -2372,11 +2388,7 @@ int dspgn_lidar_frame_run(DspgnLidarFrame* f, const float* scan, int n_points, c
   }
   if (n_masks) memcpy(h + o_bb, bboxes, 16 * (size_t)n_masks);
   if (n_points) memcpy(h + o_scan, scan, 16 * (size_t)n_points);
-  const size_t hw = (size_t)sp.img_h * sp.img_w;
-  for (int m = 0; m < n_masks; ++m) {
-    memcpy(h + o_mask + m * mstride, masks + m * hw, hw);
-    memset(h + o_mask + m * mstride + hw, 0, mstride - hw);
-  }
+  stage_masks(h + o_mask, masks, n_masks, (size_t)sp.img_h * sp.img_w, mstride);
   FrameParams P{};
   memcpy(P.K, sp.k, sizeof(P.K));
   memcpy(P.inv_k, sp.inv_k, sizeof(P.inv_k));
@@ -2446,13 +2458,8 @@ int dspgn_lidar_frame_results(DspgnLidarFrame* f, float* points, float* depth, f
 
 // ---- A monocular keyframe's detection (dspgn_mono.cuh) ----
 
-struct DspgnMonoFrame {
-  int device = 0;
+struct DspgnMonoFrame : FrameCore {
   DspgnMonoSpec spec{};
-  cudaStream_t stream = nullptr;
-  cudaStream_t own = nullptr;  // the handle's non-blocking stream (the default), as DspgnLidarFrame's
-  HostBuf h_in, h_out;
-  DevBuf d_in, d_work, d_out;
   int n_kp_blocks = 0;         // of the last run
   DspgnMonoOut last{-1, 0, -1, 0};
 };
@@ -2480,43 +2487,12 @@ int dspgn_mono_frame_create(const DspgnMonoSpec* spec, int device, DspgnMonoFram
   if (spec->downsample_ratio < 1) return fail(DSPGN_E_ARG, "downsample_ratio must be >= 1");
   if (spec->mask_erosion < 0 || spec->mask_erosion > kMonoMaxErosion) return fail(DSPGN_E_ARG, "mask_erosion must be in [0,63]");
   if (!(spec->k[0] != 0.0 && spec->k[4] != 0.0)) return fail(DSPGN_E_ARG, "fx and fy must be nonzero");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPGN_E_NOGPU, "no CUDA device"); }
-  if (device < 0 || device >= ndev) return fail(DSPGN_E_ARG, "bad device index");
-  CU(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0) return fail(DSPGN_E_NOGPU, "libdspgn is built for sm_90a (H100) only");
-  DspgnMonoFrame* f = new (std::nothrow) DspgnMonoFrame();
-  if (!f) return fail(DSPGN_E_ALLOC, "oom");
-  f->device = device;
-  f->spec = *spec;
-  if (int rc = frame_stream(&f->own)) {
-    delete f;
-    return rc;
-  }
-  f->stream = f->own;
-  count_frame(device, 1);
-  *out = f;
-  return 0;
+  return frame_create(*spec, device, out);
 }
 
-void dspgn_mono_frame_destroy(DspgnMonoFrame* f) {
-  if (!f) return;
-  cudaSetDevice(f->device);
-  cudaStreamSynchronize(f->stream);
-  f->h_in.release(); f->h_out.release();
-  f->d_in.release(); f->d_work.release(); f->d_out.release();
-  if (f->own) cudaStreamDestroy(f->own);
-  count_frame(f->device, -1);
-  delete f;
-}
+void dspgn_mono_frame_destroy(DspgnMonoFrame* f) { frame_destroy(f); }
 
-int dspgn_mono_frame_set_stream(DspgnMonoFrame* f, void* cuda_stream) {
-  if (!f) return fail(DSPGN_E_ARG, "null frame");
-  f->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  return 0;
-}
+int dspgn_mono_frame_set_stream(DspgnMonoFrame* f, void* cuda_stream) { return frame_set_stream(f, cuda_stream); }
 
 int dspgn_mono_frame_run(DspgnMonoFrame* f, const uint8_t* masks, const int32_t* bboxes, int n_masks,
                          const float* keypoints, int n_kp, DspgnMonoOut* out) {
@@ -2526,11 +2502,7 @@ int dspgn_mono_frame_run(DspgnMonoFrame* f, const uint8_t* masks, const int32_t*
   if (n_kp < 0 || n_kp > (1 << 20)) return fail(DSPGN_E_ARG, "n_kp must be in [0, 2^20]");
   if (!out || (n_masks > 0 && (!masks || !bboxes)) || (n_kp > 0 && !keypoints))
     return fail(DSPGN_E_ARG, "null pointer where data is required");
-  for (int m = 0; m < n_masks; ++m) {
-    const int32_t* bb = bboxes + 4 * m;
-    if (!(0 <= bb[0] && bb[0] <= bb[2] && bb[2] <= sp.img_w && 0 <= bb[1] && bb[1] <= bb[3] && bb[3] <= sp.img_h))
-      return fail(DSPGN_E_ARG, "bbox " + std::to_string(m) + " outside 0 <= l <= r <= img_w, 0 <= t <= b <= img_h");
-  }
+  if (int rc = check_bboxes(bboxes, n_masks, sp.img_w, sp.img_h)) return rc;
   for (int i = 0; i < n_kp; ++i) {       // cv::Mat::at reads ((int)y, (int)x): both truncations inside the image
     const float x = keypoints[2 * i], y = keypoints[2 * i + 1];
     if (!(x > -1.f && x < (float)sp.img_w && y > -1.f && y < (float)sp.img_h))
@@ -2554,11 +2526,7 @@ int dspgn_mono_frame_run(DspgnMonoFrame* f, const uint8_t* masks, const int32_t*
   unsigned char* h = f->h_in.as<unsigned char>();
   memcpy(h, bboxes, 16 * (size_t)n_masks);
   if (n_kp) memcpy(h + o_kp, keypoints, 8 * (size_t)n_kp);
-  const size_t hw = (size_t)sp.img_h * sp.img_w;
-  for (int m = 0; m < n_masks; ++m) {
-    memcpy(h + o_mask + m * mstride, masks + m * hw, hw);
-    memset(h + o_mask + m * mstride + hw, 0, mstride - hw);
-  }
+  stage_masks(h + o_mask, masks, n_masks, (size_t)sp.img_h * sp.img_w, mstride);
   FrameParams A{};                         // the LiDAR call's area blocks: n_boxes = 0, one block per mask
   A.n_masks = n_masks;
   A.mask_stride = (long long)mstride;
