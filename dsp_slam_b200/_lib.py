@@ -15,6 +15,7 @@ SCHED_AUTO, SCHED_LAUNCHES, SCHED_PERSISTENT = 0, 1, 2
 MODE_JOINT, MODE_POSE = 0, 1
 GATE_OFF, GATE_KEPT, GATE_REJECTED = 0, 1, 2
 MESH_OFF, MESH_DONE, MESH_FAILED, MESH_LOST = 0, 1, 2, 3
+INFO_OK, INFO_NONE = 0, 1
 ST_OK, ST_SDF_NAN, ST_RENDER_FEW, ST_RENDER_NAN, ST_SOLVE, ST_BAD_INPUT, ST_STOPPED = 0, 1, 2, 3, 4, 5, 6
 E_ARG, E_CUDA, E_NOGPU, E_ALLOC, E_PEER, E_BUSY = -1, -2, -3, -4, -5, -6
 IPC_HANDLE_BYTES = 64
@@ -142,6 +143,7 @@ SYMBOLS = [
                                         C.POINTER(MeshSpec)]),
     ("dspgn_keyframe_query", C.c_int, [_VP]),
     ("dspgn_keyframe_wait", C.c_int, [_VP, C.POINTER(ObjectOut), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    ("dspgn_pose_information", C.c_int, [_VP, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32)]),
     ("dspgn_debug_host_syncs", C.c_int, [_VP, C.POINTER(C.c_int64)]),
     ("dspgn_keyframe_stop", C.c_int, [_VP]),
     ("dspgn_solver_set_stop_flag", C.c_int, [_VP, _VP]),

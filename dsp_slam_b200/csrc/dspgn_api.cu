@@ -169,6 +169,7 @@ struct DspgnSolver {
     long long cap_v = 0, cap_f = 0;  // mesh arena (vertices | faces)
     size_t o_ctr = 0, o_base = 0, o_arena = 0;   // h_flight: records | queue counters | mesh bases | arena
     std::vector<int> order;          // walk order of the objects
+    std::vector<float> pose_scale;   // KfWalk::pose_scale
     std::vector<int32_t> link, grid_of;
     MeshGrid g{};
     uint8_t* mask = nullptr; int* vscan = nullptr; int* fscan = nullptr;   // the chunk's scans, kept for an overflow
@@ -188,6 +189,14 @@ struct DspgnSolver {
   cudaEvent_t ev_poll = nullptr;     // the waits that poll stop_flag
   int stop_at_obj = -1, stop_at_iter = -1;       // dspgn_debug_stop_at, for the next stoppable call
   int call_stop_obj = -1, call_stop_iter = -1;   // ... taken by the call in flight (caller object index)
+  // pose information (dspgn_pose_information) of the last call that returned records: the solve keeps the last
+  // linearisation of each of the call's slots in d_lin (lin_floats(code_len) floats per slot, every chunk of the call)
+  DevBuf d_lin;
+  int lin_base = -1;                 // d_lin slot of the resident chunk's slot 0; -1: the runs keep no linearisation
+  bool info_valid = false;           // info_items describes the last call (set when its records are complete)
+  std::vector<InfoItem> info_items;  // per object of that call
+  DevBuf d_info;                     // dspgn_pose_information: items | info | status
+  HostBuf h_info;
 };
 
 namespace {
@@ -300,6 +309,7 @@ cudaError_t settle_event(DspgnSolver* s, cudaEvent_t e) {
 // brackets it with run_begin .. run_end: the counters, the timed-launch event pools and ev_run0 / ev_run1 then describe
 // that call.
 int run_begin(DspgnSolver* s) {
+  s->info_valid = false;             // the pose information belongs to the last call, and this is a new one
   s->ctr = DspgnCounters{};
   s->band_rows_pending = false;
   s->ev_used = 0;
@@ -586,7 +596,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   for (DevBuf* b : {&s->d_decs, &s->d_stage, &s->d_state, &s->d_part_s, &s->d_part_r, &s->d_tbase, &s->d_V, &s->d_m, &s->d_results, &s->d_active,
                     &s->d_sdf, &s->d_bx, &s->d_bs, &s->d_br, &s->d_dbg, &s->d_q_flag, &s->d_q_ctr,
                     &s->d_tiles_left, &s->d_obj_iter, &s->d_ev, &s->d_seg, &s->d_ln, &s->d_vpre, &s->d_masks, &s->d_tcw, &s->d_run,
-                    &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout, &s->d_mesh_sel}) b->release();
+                    &s->d_grid_pts, &s->d_mgrid, &s->d_mws, &s->d_mscan_tmp, &s->d_mout, &s->d_mesh_sel, &s->d_lin, &s->d_info}) b->release();
   for (void* p : s->wide_allocs) cudaFree(p);
   s->h_stage.release();
   s->h_mbase.release();
@@ -594,6 +604,7 @@ void dspgn_solver_destroy(DspgnSolver* s) {
   s->h_run.release();
   s->h_mesh_sel.release();
   s->h_flight.release();
+  s->h_info.release();
   if (s->ev_flight) cudaEventDestroy(s->ev_flight);
   for (auto e : s->ev) cudaEventDestroy(e);
   for (auto e : s->ev_solve) cudaEventDestroy(e);
@@ -890,7 +901,40 @@ BatchDev batch_dev(DspgnSolver* s, const RunArgs& r) {
   const bool stoppable = s->stop_live.load(std::memory_order_relaxed) != 0 && r.gather.slots == nullptr;
   b.stop = stoppable ? StopDev{s->d_stop, s->stop_gen, r.stop_slot, s->call_stop_iter, r.pair}
                      : StopDev{nullptr, 0u, -1, -1, nullptr};
+  b.lin = s->lin_base >= 0 ? s->d_lin.as<float>() + (size_t)s->lin_base * lin_floats(s->cfg.code_len) : nullptr;
   return b;
+}
+
+// ---- pose information (dspgn_pose_information) ----------------------------------------------------------------------
+// A call that returns records keeps the last linearisation of each of its `slots` slots (all chunks) in d_lin, the chunk
+// at lin_base; the scope ends it.  d_lin grows like the batch's other buffers (d_results: no settle, cudaFree waits).
+struct LinScope {
+  DspgnSolver* s;
+  explicit LinScope(DspgnSolver* s_) : s(s_) {}
+  ~LinScope() { s->lin_base = -1; }
+  int begin(size_t slots, size_t n_obj) {
+    s->info_valid = false;
+    s->info_items.assign(n_obj, InfoItem{-1, 0, 0.0});
+    if (s->d_lin.reserve(4 * (size_t)lin_floats(s->cfg.code_len) * slots)) return fail(DSPGN_E_ALLOC, "linearisation buffer allocation failed");
+    s->lin_base = 0;
+    return 0;
+  }
+};
+
+// The item of a record from call slot `slot`; pose_scale > 0: a pose-only record whose solver pose carried that scale
+// (estimate_pose_cam_obj's argument), else a joint record, whose scale is cbrt(det R) of its pose as
+// SetPoseMeasurementSim3 takes it.  Only a record whose final update came from a completed solve has a linearisation.
+InfoItem info_item(const DspgnSolver* s, const DspgnObjectOut& r, int slot, float pose_scale) {
+  InfoItem it{-1, 0, 0.0};
+  if ((r.status != DSPGN_ST_OK && r.status != DSPGN_ST_STOPPED) || r.iters_done < 1) return it;
+  const float* T = r.t_cam_obj;
+  const double det = (double)T[0] * ((double)T[5] * T[10] - (double)T[6] * T[9]) -
+                     (double)T[1] * ((double)T[4] * T[10] - (double)T[6] * T[8]) +
+                     (double)T[2] * ((double)T[4] * T[9] - (double)T[5] * T[8]);
+  it.slot = slot;
+  it.P = pose_scale > 0.f ? 6 : 7 + s->cfg.code_len;
+  it.s = pose_scale > 0.f ? (double)pose_scale : std::cbrt(det);
+  return it;
 }
 
 // What a run does with the resident batch, given one mode per object: iteration counts and row counters per mode, and
@@ -1434,16 +1478,22 @@ namespace {
 // kMaxObjScan one after the other, each collected before the next.  `stoppable`: the call holds a StopScope; each
 // batch takes the stop hook's object if it has it, and a stopped object's rows come off the counters.
 int whole_batch(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, DspgnObjectOut* out, int mode, bool stoppable) {
+  LinScope lin(s);
+  if (int rc = lin.begin(n_obj, n_obj)) return rc;
   for (int o0 = 0; o0 < n_obj; o0 += kMaxObjScan) {
     const int n = std::min(kMaxObjScan, n_obj - o0);
     if (int rc = upload_batch_impl(s, n, in + o0, false)) return rc;
     RunArgs ra;
     if (stoppable && s->call_stop_obj >= o0 && s->call_stop_obj < o0 + n) ra.stop_slot = s->call_stop_obj - o0;
+    s->lin_base = o0;
     if (int rc = run_uniform(s, mode, ra)) return rc;
     const bool mega = s->mega_ran;
     if (int rc = dspgn_results(s, out + o0)) return rc;
     if (stoppable) uncount_stopped(s, out + o0, n, n, mega, false);
+    for (int k = o0; k < o0 + n; ++k)
+      s->info_items[k] = info_item(s, out[k], k, mode == DSPGN_MODE_POSE ? in[k].scale : 0.f);
   }
+  s->info_valid = true;
   return 0;
 }
 }  // namespace
@@ -1484,6 +1534,7 @@ struct KfWalk {
   int n_obj = 0, dim = 0, n_cand = 0;
   long long R = 0;                   // grid rows of one candidate
   std::vector<int> order;            // every object once, the flipped hypothesis j right after its map-pose hypothesis i < j
+  std::vector<float> pose_scale;     // per object: the scale of a pose-only object, 0 for a joint one (info_item)
   bool gated(int o) const { return gates != nullptr && gates[o].gate != 0; }
   bool paired(int o) const { return pair != nullptr && pair[o] >= 0; }
   bool candidate(int o) const { return modes[o] == DSPGN_MODE_JOINT || gated(o); }
@@ -1515,7 +1566,9 @@ int kf_walk(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int32_t* m
   }
   w.R = mesh ? (long long)w.dim * w.dim * w.dim : 0;
   w.order.reserve(n_obj);
+  w.pose_scale.assign(n_obj, 0.f);
   for (int o = 0; o < n_obj; ++o) {
+    if (modes[o] == DSPGN_MODE_POSE) w.pose_scale[o] = in[o].scale;
     w.n_cand += w.candidate(o) ? 1 : 0;
     if (w.paired(o) && w.pair[o] < o) continue;
     w.order.push_back(o);
@@ -1629,16 +1682,20 @@ int kf_enqueue_chunk(DspgnSolver* s, const KfWalk& w, size_t u0, int n, int slot
 
 // The chunk's records (res, one per slot) into the caller's out in object order; a rejected gated object gets its joint
 // slot's record.  woken_rows: the woken slots' rows are not in the counters yet (1: SDF rows, 2: also ray-sample rows,
-// when the run had the render term).  Returns the number of DSPGN_MESH_DONE records.
+// when the run had the render term).  Each object's pose information item names the call slot (lin_base + resident
+// slot) its record came from.  Returns the number of DSPGN_MESH_DONE records.
 int kf_records(DspgnSolver* s, const KfWalk& w, size_t u0, int n, const std::vector<int32_t>& link,
-               const DspgnObjectOut* res, DspgnObjectOut* out, int woken_rows) {
+               const DspgnObjectOut* res, DspgnObjectOut* out, int woken_rows, int lin_base) {
   int done = 0;
   for (int k = 0; k < n; ++k) {
-    DspgnObjectOut& r = out[w.order[u0 + k]];
+    const int o = w.order[u0 + k];
+    DspgnObjectOut& r = out[o];
     r = res[k];
+    if (link[k] < 0 || res[k].gate != DSPGN_GATE_REJECTED) s->info_items[o] = info_item(s, r, lin_base + k, w.pose_scale[o]);
     if (link[k] >= 0 && res[k].gate == DSPGN_GATE_REJECTED) {
       r = res[link[k]];
       r.gate = DSPGN_GATE_REJECTED;
+      s->info_items[o] = info_item(s, r, lin_base + link[k], 0.f);
       const ObjMeta& M = s->h_meta[link[k]];
       const long long iters = r.status == DSPGN_ST_STOPPED ? r.iters_done : s->cfg.num_iterations;
       if (woken_rows >= 1) s->ctr.rows_fwd_bwd += (long long)M.n_pts * iters;
@@ -1686,6 +1743,10 @@ int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int3
   if (int rc = kf_walk(s, n_obj, in, modes, gates, mesh, w)) return rc;
   BUSY(s);
   StopScope stop(s);
+  LinScope lin(s);
+  size_t call_slots = n_obj;                           // a gated object's joint run takes a slot of its own
+  for (int o = 0; o < n_obj; ++o) call_slots += w.gated(o) ? 1 : 0;
+  if (int rc = lin.begin(call_slots, n_obj)) return rc;
   std::vector<int32_t> gV, gF, grid_of(mesh ? n_obj : 0, -1);
   if (mesh) {
     if (int rc = kf_grids(s, w)) return rc;
@@ -1694,17 +1755,20 @@ int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int3
   std::vector<int32_t> link;
   std::vector<DspgnObjectOut> res;
   int g0 = 0;                                          // grids of the chunks before this one
+  int lin_base = 0;                                    // call slots of the chunks before this one
   for (size_t u0 = 0; u0 < w.order.size();) {
     int slots = 0;
     const size_t u1 = kf_chunk_end(w, u0, slots);
     const int n = (int)(u1 - u0);
     int gc = 0;                                        // grids of this chunk
+    s->lin_base = lin_base;
     if (int rc = kf_enqueue_chunk(s, w, u0, n, slots, g0, false, link, gc, grid_of)) return rc;
     const bool mega = s->mega_ran;
     res.resize(slots);
     if (int rc = dspgn_results(s, res.data())) return rc;
     uncount_stopped(s, res.data(), n, slots, mega, mega);
-    const int done = kf_records(s, w, u0, n, link, res.data(), out, mega ? 1 : 0);   // the woken slots' SDF rows
+    const int done = kf_records(s, w, u0, n, link, res.data(), out, mega ? 1 : 0, lin_base);   // the woken slots' SDF rows
+    lin_base += slots;
     if (gc > 0) {
       s->ctr.rows_fwd_only += (long long)done * w.R;
       const MeshGrid g{s->d_mgrid.as<float>() + (size_t)g0 * w.R, gc, w.dim, w.R, (long long)(w.dim - 1) * (w.dim - 1) * (w.dim - 1), 2.0 / (w.dim - 1)};
@@ -1714,6 +1778,7 @@ int keyframe_impl(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, const int3
     u0 = u1;
   }
   if (mesh) kf_meshes(s, w, grid_of, gV, gF, n_vertices, n_faces);
+  s->info_valid = true;
   return 0;
 }
 
@@ -1764,6 +1829,8 @@ int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, co
   CU(cudaSetDevice(s->device));
   if (!s->ev_flight) CU(cudaEventCreateWithFlags(&s->ev_flight, cudaEventDisableTiming));
   StopScope stop(s);                                 // kept until the wait on success
+  LinScope lin(s);
+  if (int rc = lin.begin(slots, n_obj)) return rc;
   DspgnSolver::Flight& F = s->flight;
   F = DspgnSolver::Flight{};
   F.grid_of.assign(mesh ? n_obj : 0, -1);
@@ -1810,6 +1877,7 @@ int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, co
   F.render = !s->cfg.sdf_only;
   F.n_obj = n_obj; F.slots = slots; F.n = (int)u1; F.dim = w.dim; F.n_cand = w.n_cand; F.gc = gc;
   F.order.swap(w.order);
+  F.pose_scale.swap(w.pose_scale);
   F.active = true;
   stop.keep = true;
   return 0;
@@ -1843,9 +1911,10 @@ int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices
   KfWalk w;                                          // the walk's bookkeeping (the inputs are not read again)
   w.n_obj = F.n_obj; w.n_cand = F.n_cand; w.dim = F.dim; w.R = (long long)F.dim * F.dim * F.dim; w.mesh = F.mesh;
   w.order.swap(F.order);
+  w.pose_scale.swap(F.pose_scale);
   const int done = kf_records(s, w, 0, F.n, F.link, reinterpret_cast<const DspgnObjectOut*>(h), out,
-                              F.mega ? 1 : (F.render ? 2 : 1));
-  if (!F.mesh) return 0;
+                              F.mega ? 1 : (F.render ? 2 : 1), 0);
+  if (!F.mesh) { s->info_valid = true; return 0; }
   std::vector<int32_t> gV(F.n_cand, 0), gF(F.n_cand, 0);
   s->mesh_v.clear(); s->mesh_f.clear();
   if (F.gc > 0) {
@@ -1870,6 +1939,32 @@ int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices
     }
   }
   kf_meshes(s, w, F.grid_of, gV, gF, n_vertices, n_faces);
+  s->info_valid = true;
+  return 0;
+}
+
+int dspgn_pose_information(DspgnSolver* s, int n, double* info, int32_t* info_status) {
+  if (!s || !info || !info_status) return fail(DSPGN_E_ARG, "null argument");
+  BUSY(s);
+  if (!s->info_valid) return fail(DSPGN_E_ARG, "the solver's last call returned no records (or there was none)");
+  if (n != (int)s->info_items.size()) return fail(DSPGN_E_ARG, "n must equal the object count of the solver's last call");
+  CU(cudaSetDevice(s->device));
+  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t o_info = al(sizeof(InfoItem) * (size_t)n), o_st = al(o_info + 36 * sizeof(double) * (size_t)n),
+               total = o_st + 4 * (size_t)n;
+  if (s->h_info.reserve(total) || s->d_info.reserve(total)) return fail(DSPGN_E_ALLOC, "pose information allocation failed");
+  unsigned char* h = s->h_info.as<unsigned char>();
+  unsigned char* d = s->d_info.as<unsigned char>();
+  memcpy(h, s->info_items.data(), sizeof(InfoItem) * (size_t)n);
+  CU(cudaMemcpyAsync(d, h, sizeof(InfoItem) * (size_t)n, cudaMemcpyHostToDevice, s->stream));
+  k_pose_information<<<n, kInfoThreads, 0, s->stream>>>(s->d_lin.as<float>(), lin_floats(s->cfg.code_len),
+                                                         reinterpret_cast<const InfoItem*>(d), reinterpret_cast<double*>(d + o_info),
+                                                         reinterpret_cast<int*>(d + o_st));
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(h + o_info, d + o_info, total - o_info, cudaMemcpyDeviceToHost, s->stream));
+  CU(sync_stream(s));
+  memcpy(info, h + o_info, 36 * sizeof(double) * (size_t)n);
+  memcpy(info_status, h + o_st, 4 * (size_t)n);
   return 0;
 }
 

@@ -93,6 +93,9 @@ struct BatchDev {
   const int* link;
   const float* t_map;
   StopDev stop;
+  // the last linearisation of every slot (dspgn_pose_information): H without damping, packed upper triangle of the slot's
+  // own P x P system, (7 + code_len)(8 + code_len) / 2 floats per slot; nullptr = the run keeps none
+  float* lin;
 };
 
 struct TermArgs {

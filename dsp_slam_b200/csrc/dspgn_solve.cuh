@@ -474,6 +474,10 @@ __device__ __forceinline__ int ext_to_int(int e, int npose, int L) {
   return (e < npose) ? (kMaxCode + e) : (e - npose);
 }
 
+// BatchDev::lin: floats per slot at code length L, and entry (r, c), r <= c, of a slot's P x P system (external order)
+__host__ __device__ __forceinline__ int lin_floats(int L) { return (7 + L) * (8 + L) / 2; }
+__host__ __device__ __forceinline__ int lin_index(int r, int c, int P) { return r * P - (r * (r - 1)) / 2 + (c - r); }
+
 __device__ __forceinline__ void write_result(const BatchDev& b, int o, const ObjState& st) {
   write_record(b.results, b.gather, o, st, b.meta[o].scale);
 }
@@ -725,6 +729,23 @@ __device__ int solve_object(const BatchDev& b, const SolveArgs& a, const EventLo
     else As[j * kAsStride + kPMax] = (float)v;           // b_j -> augmented column
   }
   solve_sync<MEGA>();
+  // this iteration's H without the damping overwrites the slot's last linearisation (every successful assembly, so the
+  // buffer holds the system of the iteration the record's final update came from).  A pass of its own over the
+  // assembled rows, warp per row: written inside the assembly loop above, the store measured slower on every run,
+  // including the runs that keep nothing.  The damping comes off the fp32 entry in fp64: at most half an ulp of the
+  // damped entry (with scale_damping 100, 4e-6 on the scale diagonal).
+  if (b.lin != nullptr && !dbg) {
+    float* lin = b.lin + (size_t)o * lin_floats(L);
+    const int lane = tid & 31;
+    for (int r = tid >> 5; r < P; r += kSolveThreads / 32) {
+      float* row = lin + lin_index(r, r, P) - r;
+      for (int c = r + lane; c < P; c += 32) {
+        const double damp = pose_only ? (r == c ? 1e-2 : 0.0)
+                                      : (r == c && r < 7 ? (r == 6 ? 1.0 + (double)prm.s_damp : 1.0) : 0.0);
+        row[c] = (float)((double)As[r * kAsStride + c] - damp);
+      }
+    }
+  }
 
   // padding rows/columns P..70 (pose-only: P = 6): identity, zero right-hand side
   for (int idx = tid; idx < kPMax * (kPMax + 1); idx += kSolveThreads) {
@@ -855,6 +876,72 @@ __global__ void k_mesh_select(BatchDev b, const int* grid_slot, const int* pair)
   }
   __syncthreads();
   if (s_word == DSPGN_MESH_DONE) refresh_zb0(b.state[o], b.decs[b.meta[o].class_id], tid, blockDim.x);
+}
+
+// ---- pose information of a record (dspgn_pose_information, DESIGN §4.13) -------------------------------------------
+// One per object of the call: the BatchDev::lin slot its record came from (-1: no valid linearisation), that slot's P (6
+// pose-only, 7 + L joint) and the scale s of the map into the object edge's tangent space.
+struct InfoItem { int slot; int P; double s; };
+constexpr int kInfoThreads = 128;
+
+// One CTA per object, fp64.  The Schur complement of the slot's H onto the six pose coordinates (scale and code
+// eliminated, last index first), a Cholesky test of that 6x6 block, then the map from the library's left perturbation
+// delta = [rho | phi] of T_obj_cam to the edge's e = [omega | upsilon] (Z exp(e)): delta = (-upsilon / s, -omega), so
+// Lambda[a][b] = f_a f_b M[p_a][p_b] with p = (3, 4, 5, 0, 1, 2), f = (-1, -1, -1, -1/s, -1/s, -1/s).
+__global__ void __launch_bounds__(kInfoThreads) k_pose_information(const float* lin, int stride, const InfoItem* items,
+                                                                   double* info, int* status) {
+  __shared__ double A[kPMax][kPMax + 1];       // lower triangle (i >= j) of the system being reduced
+  __shared__ int s_ok;
+  const int o = blockIdx.x, tid = threadIdx.x;
+  const InfoItem it = items[o];
+  double* out = info + 36 * (size_t)o;
+  const int P = it.P;
+  if (tid == 0) s_ok = it.slot >= 0 && (P == 6 || (P > 7 && P <= kPMax)) && it.s > 0.0 && isfinite(it.s);
+  __syncthreads();
+  if (s_ok) {
+    const float* h = lin + (size_t)it.slot * stride;
+    for (int e = tid; e < P * P; e += kInfoThreads) {
+      const int i = e / P, j = e - i * P;
+      if (j <= i) A[i][j] = (double)h[lin_index(j, i, P)];
+    }
+    __syncthreads();
+    for (int k = P - 1; k >= 6; --k) {
+      const double d = A[k][k];                  // the same shared value in every thread: a uniform exit
+      if (!(d > 0.0) || !isfinite(d)) { if (tid == 0) s_ok = 0; break; }
+      for (int e = tid; e < k * k; e += kInfoThreads) {
+        const int i = e / k, j = e - i * k;
+        if (j <= i) A[i][j] -= A[k][i] * A[k][j] / d;
+      }
+      __syncthreads();
+    }
+    __syncthreads();
+    if (tid == 0 && s_ok) {                      // positive definite: Cholesky of the marginal 6x6 block
+      double Lc[6][6];
+      for (int i = 0; i < 6 && s_ok; ++i)
+        for (int j = 0; j <= i; ++j) {
+          double v = A[i][j];
+          for (int q = 0; q < j; ++q) v -= Lc[i][q] * Lc[j][q];
+          if (i == j) {
+            if (!(v > 0.0) || !isfinite(v)) { s_ok = 0; break; }
+            Lc[i][i] = sqrt(v);
+          } else {
+            Lc[i][j] = v / Lc[j][j];
+          }
+        }
+    }
+    __syncthreads();
+  }
+  if (tid < 36) {
+    const int a = tid / 6, c = tid - a * 6;
+    double v = 0.0;
+    if (s_ok) {
+      const int pa = a < 3 ? a + 3 : a - 3, pc = c < 3 ? c + 3 : c - 3;
+      const double fa = a < 3 ? -1.0 : -1.0 / it.s, fc = c < 3 ? -1.0 : -1.0 / it.s;
+      v = fa * fc * A[max(pa, pc)][min(pa, pc)];
+    }
+    out[tid] = v;
+  }
+  if (tid == 0) status[o] = s_ok ? DSPGN_INFO_OK : DSPGN_INFO_NONE;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -119,6 +119,7 @@ class BatchSolver:
         self.device = device
         self._keep = None
         self.n_obj = 0
+        self._records_n = 0      # objects of the last call that returned records (pose_information)
 
     @property
     def engine(self):
@@ -246,14 +247,14 @@ class BatchSolver:
         arr, keep = self._pack(objs)
         out = (_lib.ObjectOut * len(objs))()
         _lib.check(_lib.load().dspgn_reconstruct_batch(self.handle, len(objs), arr, out))
-        self.n_obj = len(objs)
+        self.n_obj = self._records_n = len(objs)
         return out
 
     def estimate_pose(self, objs):
         arr, keep = self._pack(objs)
         out = (_lib.ObjectOut * len(objs))()
         _lib.check(_lib.load().dspgn_estimate_pose_batch(self.handle, len(objs), arr, out))
-        self.n_obj = len(objs)
+        self.n_obj = self._records_n = len(objs)
         return out
 
     def keyframe(self, objs, modes, gates=None, voxels_dim=None, pairs=None, want_sdf=False):
@@ -273,13 +274,13 @@ class BatchSolver:
         if voxels_dim is not None:
             nv, nf = (C.c_int32 * n)(), (C.c_int32 * n)()
             _lib.check(lib.dspgn_keyframe_batch_meshed(self.handle, n, arr, m, g, C.byref(spec), out, nv, nf))
-            self.n_obj = n
+            self.n_obj = self._records_n = n
             return self._meshed(out, n, int(voxels_dim), nv, nf, want_sdf)
         if g is None:
             _lib.check(lib.dspgn_keyframe_batch(self.handle, n, arr, m, out))
         else:
             _lib.check(lib.dspgn_keyframe_batch_gated(self.handle, n, arr, m, g, out))
-        self.n_obj = n
+        self.n_obj = self._records_n = n
         return out
 
     def _keyframe_args(self, objs, modes, gates, voxels_dim, pairs):
@@ -347,12 +348,26 @@ class BatchSolver:
         lib = _lib.load()
         if voxels_dim is None:
             _lib.check(lib.dspgn_keyframe_wait(self.handle, out, None, None))
-            self.n_obj = n
+            self.n_obj = self._records_n = n
             return out
         nv, nf = (C.c_int32 * n)(), (C.c_int32 * n)()
         _lib.check(lib.dspgn_keyframe_wait(self.handle, out, nv, nf))
-        self.n_obj = n
+        self.n_obj = self._records_n = n
         return self._meshed(out, n, int(voxels_dim), nv, nf, want_sdf)
+
+    def pose_information(self):
+        """dspgn_pose_information: the pose information of every record of the last call that returned records
+        (reconstruct, estimate_pose, keyframe, keyframe_wait), in that call's object order.  Returns (info (n, 6, 6)
+        float64, status (n,) int32): info in the tangent space of DSP-SLAM's object-camera edge (EdgeSE3LieAlgebra,
+        e = [omega, upsilon], the pose Z exp(e) about the record's pose Z with its scale divided out), in the units of
+        the record's system: a joint record's row means carry k1 / k2, a pose-only record's do not (multiply it by k2 for
+        the joint scale); status _lib.INFO_OK or _lib.INFO_NONE (zeros).  Read on demand: the calls' records are unchanged."""
+        n = self._records_n
+        info = np.zeros((max(n, 1), 6, 6), np.float64)
+        status = np.zeros(max(n, 1), np.int32)
+        _lib.check(_lib.load().dspgn_pose_information(self.handle, n, info.ctypes.data_as(C.POINTER(C.c_double)),
+                                                      status.ctypes.data_as(C.POINTER(C.c_int32))))
+        return info[:n], status[:n]
 
     def request_stop(self):
         """dspgn_keyframe_stop: stop the call in flight at the next GN iteration of each stoppable object (the joint
@@ -722,6 +737,14 @@ class Optimizer(object):
             r.flipped = bool(flip)
             kept.append(r)
         return kept
+
+    def pose_information(self):
+        """The pose information of the last solver call (BatchSolver.pose_information), one 6x6 matrix per object the
+        call ran, in its order: reconstruct_batch / estimate_pose_batch: objs; keyframe_batch: new_objects, then
+        tracked_objects (a rejected detection's entry is its joint run's); reconstruct_mono_batch: every hypothesis, the
+        map pose before the flipped one.  An outstanding KeyframeFuture is collected first."""
+        self._collect()
+        return self.solver.pose_information()
 
     def estimate_pose_batch(self, objs, return_status=False):
         """Batched estimate_pose_cam_obj.  Failed objects keep their input pose; return_status=True also returns

@@ -289,6 +289,29 @@ int dspgn_keyframe_submit(DspgnSolver* s, int n_obj, const DspgnObjectIn* in, co
                           const DspgnGateIn* gates /* or NULL */, const DspgnMeshSpec* mesh /* or NULL */);
 int dspgn_keyframe_query(DspgnSolver* s);
 int dspgn_keyframe_wait(DspgnSolver* s, DspgnObjectOut* out, int32_t* n_vertices, int32_t* n_faces);
+/* The pose information of every record of the solver's last completed call that returned records --
+ * dspgn_reconstruct_batch, dspgn_estimate_pose_batch, dspgn_keyframe_batch, _gated, _meshed or dspgn_keyframe_wait --
+ * in the call's object order (both hypotheses of a mono pair, every chunk of a call longer than 1024 objects), for the
+ * object-camera edges of DSP-SLAM's joint bundle adjustment (EdgeSE3LieAlgebra, measurement det->SE3Tco).
+ * Every solve keeps its object's normal matrix H without the damping (the code and rotation priors included); for each
+ * record this takes H of the iteration the record's pose came from (a stopped object: its last completed iteration; a
+ * gated object: the pose-only solve when KEPT, the joint run's when REJECTED), eliminates scale and code (Schur
+ * complement, fp64), and maps the 6x6 result from the solver's left perturbation of T_obj_cam into the edge's tangent
+ * space: e = [omega, upsilon] (g2o SE3Quat::log order) with the perturbed pose Z exp(e), Z = the record's pose with its
+ * scale divided out of the rotation (SetPoseMeasurementSim3 / SE3).  DESIGN.md §4.13 derives the map.
+ *   info         n x 36 doubles, row-major 6x6 per object, in the units of the system the record came from: a joint
+ *                record's residuals are row means weighted by k1 (render) and k2 (SDF), plus the code and rotation
+ *                priors (optimizer.py:155-184); a pose-only record's are the plain SDF row mean, no k2 and no prior
+ *                (optimizer.py:68-70).  Multiply a pose-only record's info by k2 to put it on the joint records' scale;
+ *   info_status  DSPGN_INFO_OK, or DSPGN_INFO_NONE (zeros in info): the record has no valid linearisation (status not
+ *                DSPGN_ST_OK / DSPGN_ST_STOPPED, or no completed iteration), or the marginal system is not positive
+ *                definite.
+ * n must equal the call's object count; after a call without records (mesh, decode, the split-phase and multi-GPU runs)
+ * or before any call: DSPGN_E_ARG.  DSPGN_E_BUSY while a submitted call is in flight.  Never part of the calls above:
+ * it enqueues one kernel and its copies of its own and waits for them. */
+#define DSPGN_INFO_OK 0
+#define DSPGN_INFO_NONE 1
+int dspgn_pose_information(DspgnSolver* s, int n, double* info /* n x 36, row-major */, int32_t* info_status /* n */);
 /* Debug: the number of times the solver's calls have blocked the calling thread on the device so far (stream and event
  * synchronisations, counted only when the device still had work to finish). */
 int dspgn_debug_host_syncs(DspgnSolver* s, int64_t* out);

@@ -2,6 +2,8 @@
 
   python tools/ab_bench.py BASE_DIR [--workload cfg2_sdf ...] [--repeats 3] [--steps K] [--warmup W] [--out DIR]
 
+Workload "keyframe" runs tools/keyframe_bench.py (the whole keyframe calls, legs a-d) instead of bench.py; for bench.py
+workloads the end-to-end call's time is reported beside the device time per step (under "figures").
 BASE_DIR is an unpacked copy of the baseline commit, e.g.  git archive <commit> | tar -x -C ab_base  (ab_base/ is
 ignored).  Both trees are built first (their own __graft_entry__.build()).  Then, per workload and repeat, bench.py runs
 in the baseline tree and in this tree alternately, each with --dump-outputs, so slow drift of the card (clocks, other
@@ -24,8 +26,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def run_bench(tree, workload, steps, warmup, dump):
-    cmd = [sys.executable, "bench.py", "--gpus", "1", "--steps", str(steps), "--warmup", str(warmup),
-           "--workload", workload, "--dump-outputs", dump]
+    if workload == "keyframe":          # tools/keyframe_bench.py: the whole keyframe calls, host clock per call
+        cmd = [sys.executable, os.path.join("tools", "keyframe_bench.py"), "--steps", str(10 * steps), "--warmup",
+               str(warmup), "--mesh-dims", "", "--dump-outputs", dump]
+    else:
+        cmd = [sys.executable, "bench.py", "--gpus", "1", "--steps", str(steps), "--warmup", str(warmup),
+               "--workload", workload, "--dump-outputs", dump]
     p = subprocess.run(cmd, cwd=tree, capture_output=True, text=True)
     if p.returncode != 0:
         raise RuntimeError(f"bench.py failed in {tree} ({workload}):\n{p.stdout[-2000:]}\n{p.stderr[-4000:]}")
@@ -34,7 +40,15 @@ def run_bench(tree, workload, steps, warmup, dump):
 
 
 def load_dump(d):
-    return {os.path.basename(f)[:-4]: np.load(f) for f in sorted(glob.glob(os.path.join(d, "*.npy")))}
+    return {os.path.relpath(f, d)[:-4]: np.load(f) for f in sorted(glob.glob(os.path.join(d, "**", "*.npy"), recursive=True))}
+
+
+def step_ms(j):
+    """The timed figures of one run: bench.py's device time per step and its end-to-end call (Optimizer.reconstruct_batch,
+    host clock), or keyframe_bench.py's median per-call time of each leg."""
+    if "legs" in j:
+        return {k: v["median_ms"] for k, v in j["legs"].items() if isinstance(v, dict) and "median_ms" in v}
+    return {"ms_per_step": j["ms_per_step"], "e2e_ms_per_step": (j.get("e2e") or {}).get("ms_per_step")}
 
 
 def compare(a, b):
@@ -88,12 +102,17 @@ def main():
                 runs[side].append((run_bench(trees[side], wl, args.steps, args.warmup, dump), dump))
         ref = load_dump(runs["new"][0][1])
         checks = [compare(ref, load_dump(d)) for side in ("base", "new") for _, d in runs[side]]
-        ms = {s: [j["ms_per_step"] for j, _ in runs[s]] for s in runs}
-        med = {s: statistics.median(v) for s, v in ms.items()}
+        figs = {s: [step_ms(j) for j, _ in runs[s]] for s in runs}
+        names = [k for k, v in figs["new"][0].items() if v is not None]
+        ms = {k: {s: [f[k] for f in figs[s]] for s in runs} for k in names}
+        med = {k: {s: statistics.median(v) for s, v in ms[k].items()} for k in names}
+        first = names[0]
         res = {
             "workload": wl, "gpu": gpu,
-            "ms_per_step": ms, "median_ms": med, "speedup": med["base"] / med["new"],
-            "spread_ms": {s: max(v) - min(v) for s, v in ms.items()},
+            "ms_per_step": ms[first], "median_ms": med[first], "speedup": med[first]["base"] / med[first]["new"],
+            "spread_ms": {s: max(v) - min(v) for s, v in ms[first].items()},
+            "figures": {k: {"median_ms": med[k], "speedup": med[k]["base"] / med[k]["new"],
+                            "spread_ms": {s: max(v) - min(v) for s, v in ms[k].items()}, "ms": ms[k]} for k in names},
             "outputs_equal": all(c[0] for c in checks), "max_abs_delta": max(c[1] for c in checks),
             "fields_differing": sorted(set(f for c in checks for f in c[2])),
             "clocks": {s: [j.get("clocks") for j, _ in runs[s]] for s in runs},
