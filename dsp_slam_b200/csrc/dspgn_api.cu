@@ -483,7 +483,8 @@ int dspgn_solver_create(const DspgnConfig* cfg, DspgnDecoder* const* classes, in
                         DspgnSolver** out) {
   if (!cfg || !classes || !out) return fail(DSPGN_E_ARG, "null argument");
   if (n_classes < 1 || n_classes > DSPGN_MAX_CLASSES) return fail(DSPGN_E_ARG, "n_classes must be in [1,4]");
-  if (cfg->num_depth_samples < 2 || cfg->num_depth_samples > 64) return fail(DSPGN_E_ARG, "num_depth_samples must be in [2,64]");
+  if (cfg->num_depth_samples < 2 || cfg->num_depth_samples > kMaxDepthSamples)
+    return fail(DSPGN_E_ARG, "num_depth_samples must be in [2,256]");
   if (cfg->num_iterations < 1) return fail(DSPGN_E_ARG, "num_iterations must be >= 1");
   for (int c = 0; c < n_classes; ++c) {
     if (!classes[c] || classes[c]->device != device) return fail(DSPGN_E_ARG, "decoder/device mismatch");

@@ -111,6 +111,13 @@ __device__ __forceinline__ float lin_depth(float dmin, float dmax, float step, i
   return (j < D / 2) ? __fmaf_rn(step, (float)j, dmin) : __fmaf_rn(-step, (float)(D - 1 - j), dmax);
 }
 
+// Depth samples per ray (DspgnConfig::num_depth_samples) in [2, kMaxDepthSamples].
+constexpr int kMaxDepthSamples = 256;
+// Range words of the valid-sample hulls (dspgn_solve.cuh: valid_sample_ranges): (row prefix << kRangeSampleBits) | first
+// sample.  The field holds every first sample of D <= 256 and leaves 23 bits of prefix for n_rays * D <= 8192 * 256.
+constexpr int kRangeSampleBits = 8, kRangeSampleMask = (1 << kRangeSampleBits) - 1;
+static_assert(kMaxDepthSamples - 1 <= kRangeSampleMask, "a first sample must fit the range word's sample field");
+
 __device__ __forceinline__ void xform_point(const float* __restrict__ T, float px, float py, float pz,
                                             float& ox, float& oy, float& oz) {
   // loss.py:31-32: products rounded, then summed left to right, then + t (as torch does it)

@@ -175,7 +175,8 @@ struct MegaArgs {
   int* scan_left;            // [n_obj] scan items (64-ray chunks) of the current iteration still running
   int* seg_cnt; int* seg_prefix;   // band rows kept per 8-ray segment / their exclusive prefix per object (dspgn_solve.cuh)
   int* obj_iter;             // [n_obj] current iteration of each object
-  int* vpre;                 // per ray: (exclusive prefix of the valid-sample hulls << 7) | first valid sample, n_rays + 1
+  int* vpre;                 // per ray: (exclusive prefix of the valid-sample hulls << kRangeSampleBits) | first valid
+                             // sample, n_rays + 1
                              // entries per object at ray_off + o (dspgn_solve.cuh: valid_sample_ranges); nullptr = the
                              // forward-only tiles enumerate all n_rays * D samples
   EventLog log;
@@ -217,16 +218,16 @@ __device__ __forceinline__ size_t band_row_sample(const int* segp, int nseg, siz
 
 // Ray-sample row `row` of object M: sample j of ray `ray` at depth lin_depth(dmin, dmax, dstep, j), in the object frame
 // through T (T_oc); returns its weight, 1 inside the unit sphere (loss.py:68).  Rows are ray * D + j, or with `compact`
-// they enumerate the valid-sample hulls: hull[ray] = first row << 7 | first sample, and the row belongs to the largest
-// ray whose hull starts at or before it.
+// they enumerate the valid-sample hulls: hull[ray] = first row << kRangeSampleBits | first sample, and the row belongs
+// to the largest ray whose hull starts at or before it.
 __device__ __forceinline__ float ray_sample_row(const BatchDev& b, const ObjMeta& M, const float* T, float dmin, float dmax,
                                                 float dstep, const int* hull, bool compact, int row, float& x0, float& x1,
                                                 float& x2) {
   int ray = row / b.D, j = row - ray * b.D;
   if (compact) {
     int lo = 0, hi = M.n_rays;
-    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((hull[mid] >> 7) <= row) lo = mid; else hi = mid; }
-    ray = lo; j = (hull[lo] & 127) + (row - (hull[lo] >> 7));
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if ((hull[mid] >> kRangeSampleBits) <= row) lo = mid; else hi = mid; }
+    ray = lo; j = (hull[lo] & kRangeSampleMask) + (row - (hull[lo] >> kRangeSampleBits));
   }
   const float* rq = b.rays + 3 * (size_t)(M.ray_off + ray);
   const float d = lin_depth(dmin, dmax, dstep, j, b.D);

@@ -282,7 +282,8 @@ __global__ void k_build_inputs(BuildArgs a) {
 // Along a ray they are one run of consecutive samples (a line meets a ball in a segment) -- 70 % of the n_rays * D samples
 // on the real SLAM shape, 80-93 % on the BASELINE configs -- so the forward-only tiles of the persistent kernel enumerate
 // only the hull [first valid, last valid] of every ray:
-//   vpre[ray] = (exclusive prefix of the hull lengths << 7) | first valid sample,   vpre[n_rays] = total << 7.
+//   vpre[ray] = (exclusive prefix of the hull lengths << kRangeSampleBits) | first valid sample,
+//   vpre[n_rays] = total << kRangeSampleBits.
 // Sample positions and the inside test are the tile prologue's own (lin_depth, xform_point, inside_unit_sphere), so a hull
 // contains exactly the samples the full enumeration marks valid; the prologue still tests every row it is given.
 // Only the samples next to the two ends of a hull are actually tested: the chord of the ray inside the unit ball
@@ -361,11 +362,11 @@ __device__ inline int valid_sample_ranges(const ObjMeta& M, const ObjState& st, 
     vpre_sync<NAMED_BAR>();
     int woff = 0, tot = 0;
     for (int w = 0; w < nw; ++w) { const int v = s_wsum[w]; if (w < warp) woff += v; tot += v; }
-    if (ray < M.n_rays) vp[ray] = ((carry + woff + x - cnt) << 7) | first;
+    if (ray < M.n_rays) vp[ray] = ((carry + woff + x - cnt) << kRangeSampleBits) | first;
     carry += tot;
     vpre_sync<NAMED_BAR>();
   }
-  if (tid == 0) vp[M.n_rays] = carry << 7;
+  if (tid == 0) vp[M.n_rays] = carry << kRangeSampleBits;
   return carry;
 }
 
@@ -951,6 +952,8 @@ __global__ void __launch_bounds__(kInfoThreads) k_pose_information(const float* 
 // order torch.where yields, and deterministic.  th: the occupancy cut-off (SolverParams::th).
 constexpr int kScanThreads = 1024;
 constexpr int kScanMaxRays = 8192;
+static_assert((long long)kScanMaxRays * kMaxDepthSamples <= (1LL << (31 - kRangeSampleBits)),
+              "an object's sample count must fit the range word's prefix field");
 
 // pose / depth range of the object being scanned, read once per thread (cache-bypassing: in the persistent kernel
 // another CTA's solve wrote it)
@@ -1043,15 +1046,16 @@ __device__ __forceinline__ void ray_scan(const BatchDev& b, const float th, cons
   ray_scan_vals(b, th, M, st, ray, lane, s, keep, de_ds, res);
 }
 
-// write the kept samples of one ray as band rows (x_o, de/ds, residual) starting at row `base` (ray, sample order)
+// write the kept samples of one ray as band rows (x_o, de/ds, residual) starting at row `base` (ray, sample order);
+// the two slots hold samples j0 + lane and j0 + lane + 32
 __device__ __forceinline__ int ray_emit(const BatchDev& b, const ObjMeta& M, const ScanState& st, int ray, int lane,
-                                        const bool keep[2], const float de_ds[2], float res, size_t base) {
+                                        const bool keep[2], const float de_ds[2], float res, size_t base, int j0 = 0) {
   const unsigned b0 = __ballot_sync(0xffffffffu, keep[0]), b1 = __ballot_sync(0xffffffffu, keep[1]);
   const float* q = b.rays + 3 * (size_t)(M.ray_off + ray);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     if (!keep[h]) continue;
-    const int j = lane + 32 * h;
+    const int j = j0 + lane + 32 * h;
     const int pos = (h == 0 ? __popc(b0 & ((1u << lane) - 1u)) : __popc(b0) + __popc(b1 & ((1u << lane) - 1u)));
     const float d = lin_depth(st.dmin, st.dmax, st.dstep, j, b.D);
     float x, y, z;
@@ -1062,6 +1066,103 @@ __device__ __forceinline__ int ray_emit(const BatchDev& b, const ObjMeta& M, con
     b.band_r[row] = res;
   }
   return __popc(b0) + __popc(b1);
+}
+
+// ---- long rays (D > 64): the same render term, walked in windows of 64 samples -------------------------------------
+// Window w holds samples 64w + lane + 32h in ray_scan_vals' two-slot lane layout; D is the same for every ray of a call,
+// so the choice between the two paths is warp-uniform.  Two passes over the windows, each reloading the window's sdf
+// values from L2 (no register array grows with D):
+//   forward: the running transmittance Tc (product of 1 - o over the earlier windows; loss.py:99), each lane's part of
+//            the rendered depth (loss.py:100-114), T at the last sample and the finite-value count; lane w keeps window
+//            w's Tc and its sum of T.  The suffix sum after each window (sum of T over the later windows) is then carried
+//            backwards across those lane words (loss.py:118-122).
+//   emit:    each window's scan again from its Tc, its suffix sums from that carry, then the band test, de/ds and the
+//            rows (loss.py:125-141) at the ray's running row count, so rows stay in (ray, sample) order.
+constexpr int kLongWin = 64, kLongMaxWin = kMaxDepthSamples / kLongWin;
+static_assert(kLongMaxWin <= 32, "one lane word per window");
+
+// one window: occupancies, T = Tc x the inclusive product scan of 1 - o, and the window's suffix sums of T (samples < D)
+__device__ __forceinline__ void long_window(const float th, int D, int j0, int lane, float Tc, const float s[2], float o[2],
+                                            float T[2], float S[2]) {
+  float t[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    o[h] = (j0 + lane + 32 * h < D) ? occupancy(s[h], th) : 0.f;
+    t[h] = 1.f - o[h];
+  }
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const float y0 = __shfl_up_sync(0xffffffffu, t[0], d), y1 = __shfl_up_sync(0xffffffffu, t[1], d);
+    if (lane >= d) { t[0] *= y0; t[1] *= y1; }
+  }
+  t[1] *= __shfl_sync(0xffffffffu, t[0], 31);
+  T[0] = Tc * t[0]; T[1] = Tc * t[1];
+  float u0 = (j0 + lane < D) ? T[0] : 0.f, u1 = (j0 + lane + 32 < D) ? T[1] : 0.f;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const float y0 = __shfl_down_sync(0xffffffffu, u0, d), y1 = __shfl_down_sync(0xffffffffu, u1, d);
+    if (lane + d < 32) { u0 += y0; u1 += y1; }
+  }
+  S[0] = u0 + __shfl_sync(0xffffffffu, u1, 0); S[1] = u1;
+}
+
+// One long ray: its sdf values are samples [first, first + cnt) at b.sdf + M.smp_off + p (the n_rays x D layout is
+// p = ray * D, first = 0, cnt = D).  Adds the ray's finite values to nvalid; with `emit`, writes its kept samples as band
+// rows from row `base`.  Returns the kept count.  All 32 lanes.
+__device__ inline int long_ray(const BatchDev& b, const float th, const ObjMeta& M, const ScanState& st, int ray, int lane,
+                               int p, int first, int cnt, bool emit, size_t base, int& nvalid) {
+  const int D = b.D, nwin = (D + kLongWin - 1) / kLongWin;
+  float s[2], o[2], T[2], S[2];
+  float Tc = 1.f, du = 0.f, Tlast = 0.f, wTc = 0.f, wsum = 0.f;   // wTc / wsum: lane w holds window w's
+#pragma unroll 1
+  for (int w = 0; w < nwin; ++w) {
+    const int j0 = w * kLongWin;
+    ray_load_compact(b, M, p, first - j0, cnt, lane, s);
+    nvalid += __popc(__ballot_sync(0xffffffffu, s[0] != INFINITY)) + __popc(__ballot_sync(0xffffffffu, s[1] != INFINITY));
+    long_window(th, D, j0, lane, Tc, s, o, T, S);
+    float Tprev0 = __shfl_up_sync(0xffffffffu, T[0], 1), Tprev1 = __shfl_up_sync(0xffffffffu, T[1], 1);
+    const float mid = __shfl_sync(0xffffffffu, T[0], 31);
+    if (lane == 0) { Tprev0 = Tc; Tprev1 = mid; }
+    if (j0 + lane < D) du += lin_depth(st.dmin, st.dmax, st.dstep, j0 + lane, D) * (o[0] * Tprev0);
+    if (j0 + lane + 32 < D) du += lin_depth(st.dmin, st.dmax, st.dstep, j0 + lane + 32, D) * (o[1] * Tprev1);
+    const int jl = D - 1 - j0;                                // T_{D-1}, in the last window
+    if (jl < kLongWin) Tlast = __shfl_sync(0xffffffffu, (jl >= 32) ? T[1] : T[0], jl & 31);
+    const float sum = __shfl_sync(0xffffffffu, S[0], 0);
+    if (lane == w) { wTc = Tc; wsum = sum; }
+    Tc = __shfl_sync(0xffffffffu, T[1], 31);
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) du += __shfl_xor_sync(0xffffffffu, du, d);
+  du += st.dfar * Tlast;
+  const float dobs = (ray < M.n_fg) ? b.depth_fg[M.fg_off + ray] : st.dfar;   // optimizer.py:126
+  const float res = fminf(fmaxf(dobs - du, -0.3f), 0.3f);                    // loss.py:136-141
+  float wsuf = 0.f, carry = 0.f;                            // lane w: sum of T over the windows after w
+#pragma unroll 1
+  for (int w = nwin - 1; w >= 0; --w) {
+    if (lane == w) wsuf = carry;
+    carry += __shfl_sync(0xffffffffu, wsum, w);
+  }
+  const float delta_d = (st.dmax - st.dmin) / (float)(D - 1);
+  const float do_ds = -1.0f / (2.0f * th);
+  int count = 0;
+#pragma unroll 1
+  for (int w = 0; w < nwin; ++w) {
+    const int j0 = w * kLongWin;
+    ray_load_compact(b, M, p, first - j0, cnt, lane, s);
+    long_window(th, D, j0, lane, __shfl_sync(0xffffffffu, wTc, w), s, o, T, S);
+    const float after = __shfl_sync(0xffffffffu, wsuf, w);
+    bool keep[2]; float de_ds[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const bool band = (s[h] > -th) && (s[h] < th);    // loss.py:88 (strict); inf never passes
+      const float de_do = (S[h] + after) / (1.f - o[h]);
+      keep[h] = band && (de_do > 1e-2f);                // loss.py:125
+      de_ds[h] = de_do * delta_d * do_ds;               // loss.py:128-130
+    }
+    if (emit) count += ray_emit(b, M, st, ray, lane, keep, de_ds, res, base + count, j0);
+    else count += __popc(__ballot_sync(0xffffffffu, keep[0])) + __popc(__ballot_sync(0xffffffffu, keep[1]));
+  }
+  return count;
 }
 
 // ---- persistent kernel: the scan as parallel work items --------------------------------------------------------------
@@ -1083,15 +1184,34 @@ __device__ inline void scan_chunk(const BatchDev& b, const float th, const int* 
   if (ray0 >= M.n_rays) return;
   ScanState st;
   load_scan_state(b.state[o], st);
-  float sv[kSegRays][2];
   // compact sdf layout: lanes 0..8 fetch the segment's 9 range words once
   int vw = 0;
   if (vpre != nullptr && lane <= kSegRays && ray0 + lane <= M.n_rays) vw = __ldcg(vpre + vpre_base(M, o) + ray0 + lane);
+  const size_t base = (size_t)M.smp_off + (size_t)ray0 * b.D;
+  if (b.D > kLongWin) {                                    // long rays: one ray at a time, rows at the segment's head
+    int nvalid = 0, count = 0;
+#pragma unroll 1
+    for (int i = 0; i < kSegRays; ++i) {
+      const int v0 = __shfl_sync(0xffffffffu, vw, i), v1 = __shfl_sync(0xffffffffu, vw, i + 1);
+      const int ray = ray0 + i;
+      if (ray >= M.n_rays) break;                          // warp-uniform
+      const int p = vpre != nullptr ? v0 >> kRangeSampleBits : ray * b.D;
+      const int first = vpre != nullptr ? v0 & kRangeSampleMask : 0;
+      const int cnt = vpre != nullptr ? (v1 >> kRangeSampleBits) - (v0 >> kRangeSampleBits) : b.D;
+      count += long_ray(b, th, M, st, ray, lane, p, first, cnt, true, base + count, nvalid);
+    }
+    if (lane == 0 && nvalid != 0) atomicAdd(b.V_count + o, nvalid);
+    if (lane == 0) seg_cnt[seg_base(M, o) + seg] = count;
+    return;
+  }
+  float sv[kSegRays][2];
 #pragma unroll
   for (int i = 0; i < kSegRays; ++i) {
     const int v0 = __shfl_sync(0xffffffffu, vw, i), v1 = __shfl_sync(0xffffffffu, vw, i + 1);
     if (ray0 + i < M.n_rays) {
-      if (vpre != nullptr) ray_load_compact(b, M, v0 >> 7, v0 & 127, (v1 >> 7) - (v0 >> 7), lane, sv[i]);
+      if (vpre != nullptr)
+        ray_load_compact(b, M, v0 >> kRangeSampleBits, v0 & kRangeSampleMask,
+                         (v1 >> kRangeSampleBits) - (v0 >> kRangeSampleBits), lane, sv[i]);
       else ray_load(b, M, ray0 + i, lane, sv[i]);
     } else { sv[i][0] = INFINITY; sv[i][1] = INFINITY; }
   }
@@ -1103,7 +1223,6 @@ __device__ inline void scan_chunk(const BatchDev& b, const float th, const int* 
     nvalid += __popc(__ballot_sync(0xffffffffu, sv[i][0] != INFINITY)) + __popc(__ballot_sync(0xffffffffu, sv[i][1] != INFINITY));
   if (lane == 0 && nvalid != 0) atomicAdd(b.V_count + o, nvalid);
   int count = 0;
-  const size_t base = (size_t)M.smp_off + (size_t)ray0 * b.D;
 #pragma unroll
   for (int i = 0; i < kSegRays; ++i) {
     if (ray0 + i >= M.n_rays) break;                       // warp-uniform
@@ -1146,10 +1265,17 @@ __device__ inline void scan_object(const BatchDev& b, const float th, const int 
   ScanState st;
   load_scan_state(b.state[o], st);
   const int N = M.n_rays;
+  const bool long_rays = b.D > kLongWin;
   bool keep[2]; float de_ds[2]; float res;
+  int nvalid = 0;                                          // (V is counted by the ray-sample tiles on this schedule)
   for (int ray = warp; ray < N; ray += nw) {
-    ray_scan(b, th, M, st, ray, lane, keep, de_ds, res);
-    const int c = __popc(__ballot_sync(0xffffffffu, keep[0])) + __popc(__ballot_sync(0xffffffffu, keep[1]));
+    int c;
+    if (long_rays) {
+      c = long_ray(b, th, M, st, ray, lane, ray * b.D, 0, b.D, false, 0, nvalid);
+    } else {
+      ray_scan(b, th, M, st, ray, lane, keep, de_ds, res);
+      c = __popc(__ballot_sync(0xffffffffu, keep[0])) + __popc(__ballot_sync(0xffffffffu, keep[1]));
+    }
     if (lane == 0) s_cnt[ray] = c;
   }
   __syncthreads();
@@ -1171,6 +1297,10 @@ __device__ inline void scan_object(const BatchDev& b, const float th, const int 
   }
   if (tid == 0) b.band_m[o] = carry;
   for (int ray = warp; ray < N; ray += nw) {
+    if (long_rays) {
+      long_ray(b, th, M, st, ray, lane, ray * b.D, 0, b.D, true, (size_t)M.smp_off + s_cnt[ray], nvalid);
+      continue;
+    }
     ray_scan(b, th, M, st, ray, lane, keep, de_ds, res);
     ray_emit(b, M, st, ray, lane, keep, de_ds, res, (size_t)M.smp_off + s_cnt[ray]);
   }

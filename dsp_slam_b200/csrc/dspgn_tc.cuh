@@ -719,7 +719,7 @@ __device__ __forceinline__ bool tile_at(const BatchDev& b, const TermArgs& a, Ta
 __device__ __forceinline__ int mega_rows(const BatchDev& b, const MegaArgs& q, const ObjMeta& M, int o, int mode) {
   if (mode == MODE_SDF) return M.n_pts;
   if (mode == MODE_BAND) return ldv(b.band_m + o);
-  if (q.vpre != nullptr) return ldv(q.vpre + vpre_base(M, o) + M.n_rays) >> 7;   // valid-sample hulls only
+  if (q.vpre != nullptr) return ldv(q.vpre + vpre_base(M, o) + M.n_rays) >> kRangeSampleBits;   // valid-sample hulls only
   return M.n_rays * b.D;
 }
 

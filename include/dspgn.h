@@ -115,7 +115,7 @@ typedef struct {
   float s_damp;                /* joint_optim.scale_damping */
   int32_t num_iterations;      /* joint_optim.num_iterations */
   int32_t code_len;            /* 32 or 64 (<= latent_size of the decoders) */
-  int32_t num_depth_samples;   /* D, <= 64 */
+  int32_t num_depth_samples;   /* D, 2..256 (n_rays * D <= 8192 * 256 per object) */
   float cut_off;               /* cut_off_threshold */
   int32_t pose_only_iterations;/* pose_only_optim.num_iterations */
   int32_t sdf_only;            /* 1: skip the render term (BASELINE config 2 "surface-SDF loss") */
